@@ -906,7 +906,10 @@ int builder_index_elements(Builder* b, uint32_t layer_m, uint32_t ef, uint64_t a
     if (plan.smem == 0) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "max_search too large");
     const uint64_t first = reinsert ? 0 : already;
     const uint64_t total = num - first;
-    const size_t max_batch = 4096;
+    // test knob: GRANNE_B200_BUILD_MAX_BATCH=1 makes every insertion see all earlier links, i.e. the reference's
+    // `singlethreaded` build order (read on every call so that one process can switch it)
+    size_t max_batch = 4096;
+    if (const char* e = std::getenv("GRANNE_B200_BUILD_MAX_BATCH")) max_batch = (size_t)std::max(1, std::atoi(e));
     int rc = builder_reserve(b, max_batch, ef, num);
     if (rc) return rc;
     GB_CUDA(cudaMemsetAsync(b->d_locks, 0, num * sizeof(int), stream));
