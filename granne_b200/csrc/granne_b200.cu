@@ -910,6 +910,12 @@ int builder_index_elements(Builder* b, uint32_t layer_m, uint32_t ef, uint64_t a
     // `singlethreaded` build order (read on every call so that one process can switch it)
     size_t max_batch = 4096;
     if (const char* e = std::getenv("GRANNE_B200_BUILD_MAX_BATCH")) max_batch = (size_t)std::max(1, std::atoi(e));
+    // test knob: GRANNE_B200_BUILD_LINK_WARPS caps the warps that link a batch in (default num_sms x 8).  At 1 the work
+    // counter hands out the members in batch order, so a batched build is deterministic.  The prune pass needs no cap:
+    // each warp there writes only its own node's row.
+    uint64_t link_warps = (uint64_t)h->num_sms * 8;
+    if (const char* e = std::getenv("GRANNE_B200_BUILD_LINK_WARPS"))
+        link_warps = std::min<uint64_t>(link_warps, (uint64_t)std::max(1, std::atoi(e)));
     int rc = builder_reserve(b, max_batch, ef, num);
     if (rc) return rc;
     GB_CUDA(cudaMemsetAsync(b->d_locks, 0, num * sizeof(int), stream));
@@ -945,7 +951,7 @@ int builder_index_elements(Builder* b, uint32_t layer_m, uint32_t ef, uint64_t a
         L.a.tile_rows = plan.tile_rows;
         L.a.work_counter = b->d_counter;
         L.a.num_nodes = (uint32_t)num;
-        L.grid = (unsigned)std::min<uint64_t>(bsz, (uint64_t)h->num_sms * 8);
+        L.grid = (unsigned)std::min<uint64_t>(bsz, link_warps);
         if ((rc = DistDispatch::call(d, L))) return rc;
         pos += bsz;
     }

@@ -229,10 +229,14 @@ int granne_b200_decode_layer(const void* index_bytes, size_t index_len, uint64_t
  * insertions of a layer issued in batches (the reference issues them through rayon, :773-783).  Candidate search is
  * the same kernel that serves granne_b200_search_batch; select_neighbors / connect_nodes / add_and_limit_neighbors run
  * as device kernels with the reference's exact arithmetic.  As with the reference's default (multi-threaded) build the
- * graph depends on the interleaving of concurrent insertions, and the default batched build is checked through recall.
- * With the environment variable GRANNE_B200_BUILD_MAX_BATCH=1 (default 4096: the largest insertion batch) every
- * insertion sees all earlier links; that sequential build is checked byte for byte against the oracle's single-threaded
- * build, which follows the reference's `singlethreaded` order. */
+ * graph depends on the interleaving of concurrent insertions.  Two environment variables, read on every build call,
+ * make it deterministic for testing:
+ *   GRANNE_B200_BUILD_MAX_BATCH (default 4096) caps the insertion batch; at 1 every insertion sees all earlier links,
+ *     and the build equals the oracle's single-threaded one (the reference's `singlethreaded` order) byte for byte.
+ *   GRANNE_B200_BUILD_LINK_WARPS (default num_sms x 8) caps the warps that link a batch in; at 1 the batched build
+ *     equals the oracle's model of this batch schedule byte for byte.
+ * The default concurrent link phase also equals that model exactly when no row overflows and no selection drops a
+ * candidate; with overflow it is checked through row invariants and recall. */
 
 /* BuildConfig (src/index/mod.rs:198-291); granne_b200_build_config_default() fills the reference defaults (:220-231). */
 typedef struct granne_b200_build_config {

@@ -37,6 +37,7 @@
 #include <queue>
 #include <string>
 #include <thread>
+#include <unordered_map>
 #include <utility>
 #include <vector>
 
@@ -873,16 +874,30 @@ struct SpinLocks {
     }
 };
 
+// What the batched model (Builder::index_batches) did: the conditions under which its image is order-independent, and
+// evidence that a case really exercises batches, overflowing connects and contended rows.
+struct BuildCounters {
+    std::atomic<u64> batches{0};
+    std::atomic<u64> max_batch{0};
+    std::atomic<u64> connect_present{0};     // connect_nodes found j already in the row
+    std::atomic<u64> connect_overflow{0};    // connect_nodes found the row full and went to add_and_limit_neighbors
+    std::atomic<u64> nontrivial_selects{0};  // select_neighbors with more candidates than its limit (link or prune)
+    std::atomic<u64> max_batch_in_links{0};  // most reverse links one node received within one batch
+};
+
 struct Builder {
     const Elements* elements;
     BuildConfig config;
     Index ix;  // fixed-width layers, width = config.num_neighbors (index/mod.rs:394)
+    size_t max_batch = 0;               // > 0: the product's batch schedule (index_batches) instead of the reference's
+    BuildCounters* counters = nullptr;  // set together with max_batch
 
     using Cand = std::pair<u64, float>;
 
     // index/mod.rs:849-883
     std::vector<Cand> select_neighbors(std::vector<Cand> candidates, size_t max_neighbors) const {
         if (candidates.size() <= max_neighbors) return candidates;
+        if (counters) counters->nontrivial_selects.fetch_add(1, std::memory_order_relaxed);
         std::vector<Cand> neighbors;
         Query e;
         for (auto& c : candidates) {
@@ -925,20 +940,27 @@ struct Builder {
                 break;
             }
         if (free_pos < w) {
+            if (counters && node[free_pos] == (u32)j) counters->connect_present.fetch_add(1, std::memory_order_relaxed);
             node[free_pos] = (u32)j;
         } else {
+            if (counters) counters->connect_overflow.fetch_add(1, std::memory_order_relaxed);
             Cand ex(j, d);
             add_and_limit_neighbors(node, w, i, &ex, 1, w);
         }
         locks.unlock(i);
     }
 
-    // index/mod.rs:805-846
-    void index_element(const BuildConfig& cfg, size_t num_prev_layers, std::vector<u32>& layer, size_t idx,
-                       SpinLocks& locks) const {
+    // index_element (index/mod.rs:805-846) in two halves: the search half only reads the layer, the link half writes it.
+    // The sequential / threaded build runs them back to back; build_batched runs the search halves of a whole batch
+    // against one snapshot of the layer and then the link halves in batch order.
+    static constexpr float EPS100 = 100.0f * 1.1920929e-07f;  // NotNan::new(100.0 * f32::EPSILON) (:813,829)
+
+    bool is_zero(size_t idx) const { return elements->dist(idx, idx) > EPS100; }  // :812-815
+
+    // :816-822: candidates = search_for_neighbors(layer, prev_layers.search(e,1,1), e, max_search) without idx itself
+    std::vector<Cand> search_element(const BuildConfig& cfg, size_t num_prev_layers, const std::vector<u32>& layer,
+                                     size_t idx, SpinLocks& locks) const {
         const size_t w = ix.width;
-        const float EPS100 = 100.0f * 1.1920929e-07f;
-        if (elements->dist(idx, idx) > EPS100) return;  // do not index zero elements
         Query element;
         elements->get(idx, &element);
         u64 entrypoint = 0;
@@ -957,8 +979,16 @@ struct Builder {
         std::vector<Cand> candidates;
         for (auto& c : found)
             if (c.first != idx) candidates.push_back(c);
+        return candidates;
+    }
+
+    // :824-845: select, the dead-duplicate rule, the own row (initialize_node or connect_nodes), the reverse links.
+    // Returns the selected neighbours (empty when the element stays unconnected).
+    std::vector<Cand> link_element(const BuildConfig& cfg, std::vector<u32>& layer, size_t idx,
+                                   const std::vector<Cand>& candidates, SpinLocks& locks) const {
+        const size_t w = ix.width;
         auto neighbors = select_neighbors(candidates, cfg.num_neighbors);
-        if (neighbors.size() > cfg.num_neighbors / 2 && neighbors[cfg.num_neighbors / 2].second < EPS100) return;
+        if (neighbors.size() > cfg.num_neighbors / 2 && neighbors[cfg.num_neighbors / 2].second < EPS100) return {};
         locks.lock(idx);
         bool empty = layer[idx * w] == UNUSED;
         if (empty) {  // initialize_node :886-895
@@ -968,6 +998,61 @@ struct Builder {
         if (!empty)
             for (auto& n : neighbors) connect_nodes(&layer[idx * w], w, idx, n.first, n.second, locks);
         for (auto& n : neighbors) connect_nodes(&layer[n.first * w], w, n.first, idx, n.second, locks);
+        return neighbors;
+    }
+
+    void index_element(const BuildConfig& cfg, size_t num_prev_layers, std::vector<u32>& layer, size_t idx,
+                       SpinLocks& locks) const {
+        if (is_zero(idx)) return;  // do not index zero elements
+        link_element(cfg, layer, idx, search_element(cfg, num_prev_layers, layer, idx, locks), locks);
+    }
+
+    // NOT a reference behaviour: a restatement of the PRODUCT's batch schedule (builder_index_elements in
+    // granne_b200/csrc/granne_b200.cu) with its link phase serialized, so that the GPU build can be checked exactly.
+    // Per batch: bsz = min(max_batch, max(1, present / 16), remaining), present = the layer's length when reinserting,
+    // else the nodes linked before the batch; ids ascend from `first` (insertion) or descend from the last node
+    // (reinsertion).  Every member searches the layer as it was before the batch (in parallel: nothing is written
+    // during that phase), then the members are linked one after another in batch order, like the product's link kernel
+    // when its work counter hands out members to a single warp.
+    void index_batches(const BuildConfig& cfg, size_t num_prev_layers, std::vector<u32>& layer, size_t first,
+                       bool reinsert, int threads) const {
+        const size_t nrows = layer.size() / ix.width;
+        const size_t total = nrows - first;
+        SpinLocks unlocked;  // the search phase only reads, the link phase is sequential
+        std::vector<size_t> ids;
+        std::vector<std::vector<Cand>> cands;
+        std::unordered_map<size_t, u64> in_links;
+        for (size_t pos = 0; pos < total;) {
+            const size_t present = reinsert ? nrows : first + pos;
+            const size_t bsz = std::min(std::min(max_batch, std::max<size_t>(1, present / 16)), total - pos);
+            ids.resize(bsz);
+            for (size_t k = 0; k < bsz; ++k) ids[k] = reinsert ? nrows - 1 - pos - k : first + pos + k;
+            cands.assign(bsz, {});
+            auto search = [&](size_t b, size_t e) {
+                for (size_t k = b; k < e; ++k)
+                    if (!is_zero(ids[k])) cands[k] = search_element(cfg, num_prev_layers, layer, ids[k], unlocked);
+            };
+            const size_t nt = std::min<size_t>(std::max(threads, 1), bsz / 16 + 1);
+            if (nt <= 1) {
+                search(0, bsz);
+            } else {
+                std::vector<std::thread> ts;
+                const size_t per = (bsz + nt - 1) / nt;
+                for (size_t t = 0; t < nt; ++t) ts.emplace_back(search, std::min(bsz, per * t), std::min(bsz, per * (t + 1)));
+                for (auto& t : ts) t.join();
+            }
+            in_links.clear();
+            for (size_t k = 0; k < bsz; ++k) {
+                if (is_zero(ids[k])) continue;  // do not index zero elements
+                for (auto& n : link_element(cfg, layer, ids[k], cands[k], unlocked)) {
+                    const u64 c = ++in_links[n.first];
+                    if (c > counters->max_batch_in_links) counters->max_batch_in_links = c;
+                }
+            }
+            counters->batches += 1;
+            if (bsz > counters->max_batch) counters->max_batch = bsz;
+            pos += bsz;
+        }
     }
 
     // index/mod.rs:716-802
@@ -981,8 +1066,10 @@ struct Builder {
             layer.resize(num_elements * w, UNUSED);
         size_t nrows = layer.size() / w;
         SpinLocks locks;
-        locks.init(nrows, threads > 1);
-        if (threads <= 1) {
+        locks.init(nrows, threads > 1 && max_batch == 0);
+        if (max_batch > 0) {
+            index_batches(cfg, num_prev_layers, layer, reinsert ? 0 : already, reinsert, threads);
+        } else if (threads <= 1) {
             if (reinsert)
                 for (size_t i = nrows; i-- > 0;) index_element(cfg, num_prev_layers, layer, i, locks);
             else
@@ -1519,7 +1606,36 @@ void* orc_builder_new(void* elements, uint64_t num_neighbors, uint64_t max_searc
     b->ix.width = num_neighbors;
     return b;
 }
-void orc_builder_free(void* p) { delete (Builder*)p; }
+void orc_builder_free(void* p) {
+    auto* b = (Builder*)p;
+    delete b->counters;
+    delete b;
+}
+// max_batch > 0: later build_partial calls follow the product's batch schedule (Builder::index_batches), not the
+// reference's order; 0 switches back.  The counters accumulate over the builder's life.
+void orc_builder_set_max_batch(void* p, uint64_t max_batch) {
+    auto* b = (Builder*)p;
+    b->max_batch = max_batch;
+    if (!b->counters) b->counters = new BuildCounters();
+}
+// out[6] = {batches, largest batch, connects that found j present, connects that overflowed, non-trivial selects,
+// most reverse links into one node within one batch}
+void orc_builder_counters(void* p, uint64_t* out) {
+    const BuildCounters* c = ((Builder*)p)->counters;
+    if (!c) {
+        std::fill(out, out + 6, 0);
+        return;
+    }
+    out[0] = c->batches, out[1] = c->max_batch, out[2] = c->connect_present, out[3] = c->connect_overflow;
+    out[4] = c->nontrivial_selects, out[5] = c->max_batch_in_links;
+}
+// the distances add_and_limit_neighbors sorts a row by (:938): dist(ids[k], element idx)
+void orc_elements_dists(void* p, uint64_t idx, const uint32_t* ids, uint64_t n, float* out) {
+    auto* e = (Elements*)p;
+    Query q;
+    e->get(idx, &q);
+    for (uint64_t k = 0; k < n; ++k) out[k] = e->dist_to_element(ids[k], q);
+}
 // build_partial(num_elements) exactly (0 indexes nothing); returns 1 where the reference panics
 // ("Cannot index fewer elements than already in index", :379-382).
 int orc_builder_build_partial(void* p, uint64_t num_elements, int threads) {

@@ -86,6 +86,9 @@ def lib():
         "orc_builder_free": (None, [vp]),
         "orc_builder_from_index": (vp, [vp, vp, u64, u64, f32, i32, i64]),
         "orc_builder_build_partial": (i32, [vp, u64, i32]),
+        "orc_builder_set_max_batch": (None, [vp, u64]),
+        "orc_builder_counters": (None, [vp, vp]),
+        "orc_elements_dists": (None, [vp, u64, vp, u64, vp]),
         "orc_builder_get_index": (vp, [vp]),
         "orc_entrypoint_trail": (None, [vp, vp, u64, u64, vp]),
         "orc_compute_order": (None, [vp, vp, vp, i32]),
@@ -315,6 +318,15 @@ class Elements:
             return np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_int8)), shape=(n, self.dim)).copy()
         return np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_float)), shape=(n, self.dim)).copy()
 
+    def dists(self, idx, ids):
+        """dist(ids[k], element idx) for every k: the distances a builder sorts node idx's row by
+        (index/mod.rs:938)."""
+        ids = np.ascontiguousarray(ids, dtype=np.uint32)
+        out = np.zeros(ids.size, dtype=np.float32)
+        if ids.size:
+            lib().orc_elements_dists(self._h, idx, _ptr(ids), ids.size, _ptr(out))
+        return out
+
     def dist_to_element(self, idx, raw_query, already_element=False):
         q = _f32(raw_query)
         return np.float32(lib().orc_elements_dist_to(self._h, idx, _ptr(q), int(already_element)))
@@ -495,14 +507,32 @@ class GranneBuilder:
         return b
 
     # stateful use, like the reference's builder: build_partial(n) continues from what is already indexed
-    def build_partial(self, num_elements, threads=1):
-        """Builder::build_partial (index/mod.rs:374-402); returns the index built so far (get_index)."""
+    def build_partial(self, num_elements, threads=1, max_batch=0):
+        """Builder::build_partial (index/mod.rs:374-402); returns the index built so far (get_index).
+        max_batch > 0 follows the product's batch schedule instead (see build_batched)."""
         if getattr(self, "_b", None) is None:
             m, ef, mult, re, exp = self.cfg
             self._b = lib().orc_builder_new(self.elements._h, m, ef, mult, int(re), exp)
+        lib().orc_builder_set_max_batch(self._b, max_batch)
         if lib().orc_builder_build_partial(self._b, num_elements, threads) != 0:
             raise ValueError(lib().orc_last_error().decode())
         return Granne(lib().orc_builder_get_index(self._b), self.elements)
+
+    def build_batched(self, max_batch, threads=1):
+        """NOT a reference behaviour: the product's batched build (granne_b200.cu builder_index_elements) with its
+        link phase serialized.  Each batch of up to `max_batch` insertions searches one snapshot of the layer, then its
+        members are linked one after another in batch order.  `threads` only spreads the searches of a batch; the image
+        does not depend on it.  Returns the index; counters() tells what the build did."""
+        return self.build_partial(len(self.elements), threads, max_batch)
+
+    def counters(self):
+        """What the batched builds of this builder did so far (build_batched / build_partial with max_batch)."""
+        out = np.zeros(6, dtype=np.uint64)
+        if getattr(self, "_b", None) is not None:
+            lib().orc_builder_counters(self._b, _ptr(out))
+        keys = ("batches", "max_batch", "connect_present", "connect_overflow", "nontrivial_selects",
+                "max_batch_in_links")
+        return {k: int(v) for k, v in zip(keys, out)}
 
     def __del__(self):
         try:

@@ -4,12 +4,13 @@ the oracle's threads=1 build byte for byte.  This checks select_neighbors, initi
 add_and_limit_neighbors, the final prune pass, the zero-element skip (:813), the dead duplicate rule (:826-832), half M
 on upper layers (:665-668) and half max_search when reinserting (:698-699) exactly, not through recall.
 
-The default batched build is nondeterministic and stays covered by the recall tests in test_builder_gpu.py."""
+The default batched build is checked against the oracle's model of the batch schedule in test_builder_batched_gpu.py."""
 import numpy as np
 import pytest
 
 import granne_b200
 from helpers.data import random_sum_embeddings, random_vectors
+from helpers.index_image import assert_same_index
 
 pytestmark = pytest.mark.gpu
 
@@ -25,23 +26,6 @@ def _lib():
 @pytest.fixture(autouse=True)
 def _sequential(monkeypatch):
     monkeypatch.setenv("GRANNE_B200_BUILD_MAX_BATCH", "1")  # read by the library on every build call
-
-
-def assert_same_index(oracle, image, ref, el, what=""):
-    """image (GPU builder) == ref (oracle Granne) byte for byte; on a mismatch name the first differing list."""
-    want = ref.to_bytes()
-    if image == want:
-        return
-    # compare both as loaded from their files (sorted lists; a built index keeps insertion order)
-    got, ref = oracle.Granne.from_bytes(image, el), oracle.Granne.from_bytes(want, el)
-    assert got.num_layers() == ref.num_layers(), "%s: %d layers, oracle %d" % (what, got.num_layers(), ref.num_layers())
-    for layer in range(ref.num_layers()):
-        assert got.layer_len(layer) == ref.layer_len(layer), "%s: layer %d length" % (what, layer)
-        for i in range(ref.layer_len(layer)):
-            a, b = got.get_neighbors(i, layer), ref.get_neighbors(i, layer)
-            assert a == b, "%s: layer %d node %d: gpu %s, oracle %s" % (what, layer, i, a, b)
-    pytest.fail("%s: every neighbour list agrees but the index images differ (%d vs %d bytes)"
-                % (what, len(image), len(want)))
 
 
 def build_both(oracle, kind, el, emb_bytes=None, **cfg):
