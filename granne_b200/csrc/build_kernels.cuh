@@ -194,37 +194,12 @@ __device__ __forceinline__ void connect_nodes(const DeviceIndex& ix, WarpCtx& c,
     add_and_limit(ix, c, dist, s, rows, stride, node_width, i, true, j, d, (int)node_width);
 }
 
-template <class Dist>
+// The search context (SmemLayout) followed by the link scratch (link_scratch_bytes).
 __device__ __forceinline__ void setup_ctx(const DeviceIndex& ix, WarpCtx& c, LinkScratch& s, unsigned char* smem_raw,
                                           uint32_t stg_rows, uint32_t stg_row_bytes, uint32_t tile_rows,
                                           uint32_t cand_cap, uint32_t node_width = 32) {
     c.lane = threadIdx.x;
-    unsigned char* sp = smem_raw;
-    c.tile = reinterpret_cast<float*>(sp);
-    c.ids = reinterpret_cast<uint32_t*>(sp + tile_bytes_for_rows(tile_rows) - kIdScratchBytes);
-    sp += tile_bytes_for_rows(tile_rows);
-    c.bar = smem_u32(sp);
-    c.phase = 0;
-    c.pol_stream = make_policy_evict_first();
-    c.pol_keep = make_policy_evict_last();
-    sp += 16;
-    const uint32_t qbytes = (ix.kind == kAngularI8) ? ix.row_stride : ((ix.dim + 3u) & ~3u) * 4u;
-    c.qs = reinterpret_cast<float*>(sp);
-    sp += (qbytes + 15u) & ~15u;
-    c.xs = reinterpret_cast<float*>(sp);
-    if (ix.kind == kSumEmbeddings) sp += (qbytes + 15u) & ~15u;
-    c.stg = nullptr;
-    c.stg_rows = stg_rows;
-    c.stg_row_bytes = stg_row_bytes;
-    if (stg_rows) {
-        sp = smem_raw + (((size_t)(sp - smem_raw) + 127u) & ~(size_t)127u);
-        c.stg = sp;
-        sp += (size_t)stg_rows * stg_row_bytes;
-    }
-    if (Dist::kMbar) {
-        if (c.lane == 0) mbar_init(c.bar, 1);
-        __syncwarp();
-    }
+    unsigned char* sp = place_warp_smem(c, smem_raw, ix, tile_rows, stg_rows, stg_row_bytes);
     c.status = 0;
     c.q_norm_i8 = 0;
     c.n_dist = c.n_expand = c.n_nbr = 0;
@@ -255,7 +230,7 @@ __global__ void __launch_bounds__(32) build_link_kernel(const DeviceIndex ix, co
     WarpCtx c;
     LinkScratch s;
     const uint32_t cand_cap = link_cand_cap(a.cand_stride, a.node_width);
-    setup_ctx<Dist>(ix, c, s, smem_raw, a.stg_rows, a.stg_row_bytes, a.tile_rows, cand_cap, a.node_width);
+    setup_ctx(ix, c, s, smem_raw, a.stg_rows, a.stg_row_bytes, a.tile_rows, cand_cap, a.node_width);
     Dist dist;
     const int lane = c.lane;
     while (true) {
@@ -327,7 +302,7 @@ __global__ void __launch_bounds__(32) build_prune_kernel(const DeviceIndex ix, c
     extern __shared__ __align__(16) unsigned char smem_raw[];
     WarpCtx c;
     LinkScratch s;
-    setup_ctx<Dist>(ix, c, s, smem_raw, a.stg_rows, a.stg_row_bytes, a.tile_rows, link_cand_cap(0, a.node_width),
+    setup_ctx(ix, c, s, smem_raw, a.stg_rows, a.stg_row_bytes, a.tile_rows, link_cand_cap(0, a.node_width),
                     a.node_width);
     Dist dist;
     while (true) {
@@ -357,7 +332,7 @@ __global__ void __launch_bounds__(32) pair_distance_kernel(const DeviceIndex ix,
     extern __shared__ __align__(16) unsigned char smem_raw[];
     WarpCtx c;
     LinkScratch s;
-    setup_ctx<Dist>(ix, c, s, smem_raw, a.stg_rows, a.stg_row_bytes, a.tile_rows, 8);
+    setup_ctx(ix, c, s, smem_raw, a.stg_rows, a.stg_row_bytes, a.tile_rows, 8);
     Dist dist;
     SearchArgs q{};
     q.queries = a.queries;
@@ -399,6 +374,8 @@ __global__ void __launch_bounds__(32) make_elements_kernel(const float* __restri
         __syncwarp();
         for (uint32_t i = lane; i < dim; i += 32) row_s[i] = src[i];
         __syncwarp();
+        // The same arithmetic as quantize_i8 and normalize_f32, spelled out: through those helpers this kernel needs 7
+        // more registers.
         if (kind == kAngularI8) {
             float mx = 0.0f;
             for (uint32_t i = lane; i < dim; i += 32) mx = fmaxf(mx, fabsf(row_s[i]));

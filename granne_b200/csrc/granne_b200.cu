@@ -156,6 +156,43 @@ int dev_alloc(Handle* h, T** out, size_t count) {
     return GRANNE_B200_OK;
 }
 
+// Which distance engine serves an index: calls f.template run<Dist>() for the engine of `d`'s element kind and chunk
+// count (d.full = dim / 32) — DistF32<full> for the chunk counts it is compiled for, DistF32Generic for every other
+// f32 width.  This is the only place that decides it; the row layout (stage_dense) and the launch plan (make_plan)
+// follow from the engine it picks (fixed_f32_chunks).
+struct DistDispatch {
+    template <class F>
+    static int call(const gb::DeviceIndex& d, F&& f) {
+        switch (d.kind) {
+            case gb::kAngularI8: return f.template run<gb::DistI8>();
+            case gb::kSumEmbeddings: return f.template run<gb::DistSum>();
+            default: break;
+        }
+        switch (d.full) {
+            case 0: return f.template run<gb::DistF32<0>>();
+            case 1: return f.template run<gb::DistF32<1>>();
+            case 2: return f.template run<gb::DistF32<2>>();
+            case 3: return f.template run<gb::DistF32<3>>();
+            case 4: return f.template run<gb::DistF32<4>>();
+            case 6: return f.template run<gb::DistF32<6>>();
+            case 8: return f.template run<gb::DistF32<8>>();
+            default: return f.template run<gb::DistF32Generic>();
+        }
+    }
+};
+
+// FULL of the DistF32<FULL> engine that serves `d`, or -1 when an engine for any width does (DistF32Generic, DistI8,
+// DistSum).
+template <class Dist>
+constexpr int kFixedChunks = -1;
+template <int FULL>
+constexpr int kFixedChunks<gb::DistF32<FULL>> = FULL;
+struct FixedChunksProbe {
+    template <class Dist>
+    int run() const { return kFixedChunks<Dist>; }
+};
+int fixed_f32_chunks(const gb::DeviceIndex& d) { return DistDispatch::call(d, FixedChunksProbe{}); }
+
 // Uploads `nrows` dense rows in slabs through a temporary device buffer and re-lays them out on the device.
 int stage_dense(Handle* h, const uint8_t* host_rows, uint64_t nrows, uint32_t dim, bool is_i8,
                 bool device_src = false) {
@@ -189,8 +226,9 @@ int stage_dense(Handle* h, const uint8_t* host_rows, uint64_t nrows, uint32_t di
         if (tmp) GB_CUDA(cudaFree(tmp));
     } else {
         const uint32_t full = d.full;
-        const bool templated = (full <= 4 || full == 6 || full == 8) && h->dev.kind == gb::kAngularF32;
-        d.vec_group = !templated || full == 0 ? 1 : (full % 4 == 0 ? 4 : (full % 2 == 0 ? 2 : 1));
+        // DistF32<full> reads rows lane-permuted in groups of V = DistF32<full>::V chunks; the other engines read the
+        // natural layout (V = 1 permutes nothing)
+        d.vec_group = fixed_f32_chunks(d) > 0 ? (full % 4 == 0 ? 4 : (full % 2 == 0 ? 2 : 1)) : 1;
         d.row_stride = (dim + 3u) & ~3u;
         float* dst = nullptr;
         int rc = dev_alloc(h, &dst, (size_t)nrows * d.row_stride);
@@ -353,26 +391,12 @@ struct LaunchPlan {
     uint32_t list_cap, vis_slots, vis_upper;
     uint32_t vis_retry;  // visited slots per CTA of the retry pass
     int rows;           // fast list rows R (capacity 32*R), 0 = generic list
-    uint32_t stg_rows;  // candidate rows per bulk-copy batch (staged distance engines only)
+    uint32_t stg_rows;  // candidate rows per staged batch (0: the engine loads rows directly)
     uint32_t stg_row_bytes;
-    uint32_t tile_rows;  // ordered-sum tile rows: 8 staged f32, 32 generic f32, 0 for i8 / embeddings
-    size_t base_smem;   // tile + mbarrier + query (+ embeddings scratch) + staging
+    uint32_t tile_rows;  // ordered-sum tile rows: one per staged row (f32), 8 embeddings, 32 direct loads, 0 for i8
+    size_t base_smem;   // gb::SmemLayout::end: tile + id scratch + reserved + query (+ embeddings scratch) + staging
     size_t smem;        // fast pass total
-    bool staged;
 };
-
-bool is_templated_f32(const gb::DeviceIndex& d) {
-    // DistF32<FULL> with FULL > 0 (see dispatch_search)
-    return d.kind == gb::kAngularF32 && d.full > 0 && !(d.vec_group == 1 && d.full > 4) &&
-           (d.full <= 4 || d.full == 6 || d.full == 8);
-}
-bool is_generic_f32_staged(const gb::DeviceIndex& d) {
-    // DistF32Generic stages rows of up to 8 KB (dim < 2080); wider rows load directly
-    return d.kind == gb::kAngularF32 && !is_templated_f32(d) && d.full >= 1 && d.full <= 64;
-}
-bool is_staged_kind(const gb::DeviceIndex& d) {
-    return d.kind == gb::kAngularI8 || is_templated_f32(d) || is_generic_f32_staged(d);
-}
 
 LaunchPlan make_plan(const Handle* h, uint32_t max_search) {
     const gb::DeviceIndex& d = h->dev;
@@ -392,37 +416,37 @@ LaunchPlan make_plan(const Handle* h, uint32_t max_search) {
     const uint64_t cap_slots = 1ull << 20;
     p.vis_retry = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(want * 8, want), std::max<uint64_t>(cap_slots, want));
     want = std::min<uint64_t>(want * h->vis_scale.load(), std::max<uint64_t>(cap_slots, want));
-    const uint32_t qbytes = (d.kind == gb::kAngularI8) ? d.row_stride : ((d.dim + 3u) & ~3u) * 4u;
-    p.staged = is_staged_kind(d);
-    p.tile_rows = d.kind == gb::kAngularI8 ? 0u : ((p.staged || d.kind == gb::kSumEmbeddings) ? 8u : 32u);
-    const bool generic_staged = is_generic_f32_staged(d);
-    if (is_templated_f32(d))  // the ordered-sum tile has one row per staged candidate row of a batch
-        p.tile_rows = std::min<uint32_t>(8u, std::max<uint32_t>(4, ((unsigned)GB_STG_BYTES / (d.full * 128u)) & ~3u));
-    size_t base = gb::tile_bytes_for_rows(p.tile_rows) + 16 + ((qbytes + 15u) & ~15u) * (d.kind == gb::kSumEmbeddings ? 2 : 1);
+    // the staging tile and the ordered-sum tile of the engine that serves the index
+    const int fixed_chunks = fixed_f32_chunks(d);
     p.stg_rows = 0;
     p.stg_row_bytes = 0;
-    if (d.kind == gb::kSumEmbeddings) {
-        // staging tile = the summed vectors of a batch of candidates (one row each)
-        p.stg_row_bytes = ((d.dim + 3u) & ~3u) * 4u;
-        p.stg_rows = std::min<uint32_t>(8u, std::max<uint32_t>(4, (8192u / p.stg_row_bytes) & ~3u));
-        base = ((base + 127) & ~size_t(127)) + (size_t)p.stg_rows * p.stg_row_bytes;
-    }
-    if (p.staged && d.kind == gb::kAngularI8) {
-        // DistI8: the staging tile is a set of 512-byte pass slots (32 lanes x one 16-byte chunk each)
+    if (d.kind == gb::kAngularI8) {
+        // DistI8: no ordered sums; the staging tile is a set of 512-byte pass slots (32 lanes x one 16-byte chunk each)
+        p.tile_rows = 0;
         p.stg_row_bytes = 512;
         p.stg_rows = std::max<uint32_t>(2, (unsigned)GB_STG_BYTES / 512u);
-        base = ((base + 127) & ~size_t(127)) + (size_t)p.stg_rows * p.stg_row_bytes;
-    } else if (generic_staged) {
-        const uint32_t row_bytes = d.full * 128u;
-        p.stg_row_bytes = row_bytes;
-        p.stg_rows = std::min<uint32_t>(8u, std::max<uint32_t>(2, (unsigned)(2 * GB_STG_BYTES) / row_bytes));
-        base = ((base + 127) & ~size_t(127)) + (size_t)p.stg_rows * row_bytes;
-    } else if (p.staged) {
-        const uint32_t row_bytes = d.full * 128u;
-        p.stg_row_bytes = row_bytes;
-        p.stg_rows = std::min<uint32_t>(8u, std::max<uint32_t>(4, ((unsigned)GB_STG_BYTES / row_bytes) & ~3u));
-        base = ((base + 127) & ~size_t(127)) + (size_t)p.stg_rows * row_bytes;
+    } else if (d.kind == gb::kSumEmbeddings) {
+        // DistSum: the staging tile holds the summed vectors of a batch of candidates (one row each)
+        p.tile_rows = 8;
+        p.stg_row_bytes = ((d.dim + 3u) & ~3u) * 4u;
+        p.stg_rows = std::min<uint32_t>(8u, std::max<uint32_t>(4, (8192u / p.stg_row_bytes) & ~3u));
+    } else if (fixed_chunks > 0) {
+        // DistF32<full>: the ordered-sum tile has one row per staged candidate row of a batch
+        p.stg_row_bytes = d.full * 128u;
+        p.stg_rows = std::min<uint32_t>(8u, std::max<uint32_t>(4, ((unsigned)GB_STG_BYTES / p.stg_row_bytes) & ~3u));
+        p.tile_rows = p.stg_rows;
+    } else if (fixed_chunks < 0 && d.full <= 64) {
+        // DistF32Generic stages rows of up to 8 KB (dim < 2080), at most 8 (the tile rows) per batch
+        p.tile_rows = 8;
+        p.stg_row_bytes = d.full * 128u;
+        p.stg_rows = std::min<uint32_t>(8u, std::max<uint32_t>(2, (unsigned)(2 * GB_STG_BYTES) / p.stg_row_bytes));
+    } else {
+        // DistF32<0> (dim < 32) and DistF32Generic on wider rows load directly; the generic engine then parks the lane
+        // partials of up to 32 candidates in the tile
+        p.tile_rows = 32;
     }
+    const size_t base =
+        gb::SmemLayout<size_t>(0, d.kind, d.dim, d.row_stride, p.tile_rows, p.stg_rows, p.stg_row_bytes).end;
     p.base_smem = base;
     const size_t budget = h->smem_optin;
     if (p.rows) {
@@ -555,42 +579,26 @@ int launch_kernels(Handle* h, Workspace* w, gb::SearchArgs a, const LaunchPlan& 
     return GRANNE_B200_OK;
 }
 
-template <class Dist>
-int launch_search(Handle* h, Workspace* w, const gb::SearchArgs& a, const LaunchPlan& plan, cudaStream_t stream,
-                  const gb::DeviceIndex& dv) {
-    switch (plan.rows) {
-        case 3: return launch_kernels<Dist, 3>(h, w, a, plan, stream, dv);
-        case 7: return launch_kernels<Dist, 7>(h, w, a, plan, stream, dv);
-        case 15: return launch_kernels<Dist, 15>(h, w, a, plan, stream, dv);
-        case 31: return launch_kernels<Dist, 31>(h, w, a, plan, stream, dv);
-        default: return launch_kernels<Dist, 0>(h, w, a, plan, stream, dv);
+// The search passes for the engine DistDispatch picks.  `d`: the staged index the kernels see — the handle's own, or a
+// private view of it (compute_order searches single layers without touching the shared handle)
+struct SearchLaunch {
+    Handle* h;
+    Workspace* w;
+    const gb::SearchArgs& a;
+    const LaunchPlan& plan;
+    cudaStream_t stream;
+    const gb::DeviceIndex& d;
+    template <class Dist>
+    int run() {
+        switch (plan.rows) {
+            case 3: return launch_kernels<Dist, 3>(h, w, a, plan, stream, d);
+            case 7: return launch_kernels<Dist, 7>(h, w, a, plan, stream, d);
+            case 15: return launch_kernels<Dist, 15>(h, w, a, plan, stream, d);
+            case 31: return launch_kernels<Dist, 31>(h, w, a, plan, stream, d);
+            default: return launch_kernels<Dist, 0>(h, w, a, plan, stream, d);
+        }
     }
-}
-
-// `d`: the staged index the kernels see — the handle's own, or a private view of it (compute_order searches single
-// layers without touching the shared handle)
-int dispatch_search(Handle* h, Workspace* w, const gb::SearchArgs& a, const LaunchPlan& plan, cudaStream_t stream,
-                    const gb::DeviceIndex& d) {
-    switch (d.kind) {
-        case gb::kAngularI8:
-            return launch_search<gb::DistI8>(h, w, a, plan, stream, d);
-        case gb::kSumEmbeddings:
-            return launch_search<gb::DistSum>(h, w, a, plan, stream, d);
-        default:
-            break;
-    }
-    if (d.vec_group == 1 && d.full > 4) return launch_search<gb::DistF32Generic>(h, w, a, plan, stream, d);
-    switch (d.full) {
-        case 0: return launch_search<gb::DistF32<0>>(h, w, a, plan, stream, d);
-        case 1: return launch_search<gb::DistF32<1>>(h, w, a, plan, stream, d);
-        case 2: return launch_search<gb::DistF32<2>>(h, w, a, plan, stream, d);
-        case 3: return launch_search<gb::DistF32<3>>(h, w, a, plan, stream, d);
-        case 4: return launch_search<gb::DistF32<4>>(h, w, a, plan, stream, d);
-        case 6: return launch_search<gb::DistF32<6>>(h, w, a, plan, stream, d);
-        case 8: return launch_search<gb::DistF32<8>>(h, w, a, plan, stream, d);
-        default: return launch_search<gb::DistF32Generic>(h, w, a, plan, stream, d);
-    }
-}
+};
 
 // ---- workspace pool -----------------------------------------------------------------------------------------------
 int ws_acquire(Handle* h, Workspace** out) {
@@ -770,7 +778,8 @@ int enqueue_search(Handle* h, Workspace* w, const void* d_queries, size_t nq, in
     a.stg_row_bytes = plan.stg_row_bytes;
     a.tile_rows = plan.tile_rows;
     a.vis_global = nullptr;
-    rc = dispatch_search(h, w, a, plan, stream, view ? *view : h->dev);
+    const gb::DeviceIndex& dv = view ? *view : h->dev;
+    rc = DistDispatch::call(dv, SearchLaunch{h, w, a, plan, stream, dv});
     if (rc) return rc;
     GB_CUDA(cudaMemcpyAsync(w->h_retried, w->d_retried, 8, cudaMemcpyDeviceToHost, stream));
     return GRANNE_B200_OK;
@@ -785,29 +794,6 @@ int error_from_bits(int bits) {
 }
 
 // ---- GranneBuilder (src/index/mod.rs:295-531, 645-960) on the device ---------------------------------------------
-struct DistDispatch {
-    // calls f.template run<Dist>() for the distance engine that serves `d` (same mapping as dispatch_search)
-    template <class F>
-    static int call(const gb::DeviceIndex& d, F&& f) {
-        switch (d.kind) {
-            case gb::kAngularI8: return f.template run<gb::DistI8>();
-            case gb::kSumEmbeddings: return f.template run<gb::DistSum>();
-            default: break;
-        }
-        if (d.vec_group == 1 && d.full > 4) return f.template run<gb::DistF32Generic>();
-        switch (d.full) {
-            case 0: return f.template run<gb::DistF32<0>>();
-            case 1: return f.template run<gb::DistF32<1>>();
-            case 2: return f.template run<gb::DistF32<2>>();
-            case 3: return f.template run<gb::DistF32<3>>();
-            case 4: return f.template run<gb::DistF32<4>>();
-            case 6: return f.template run<gb::DistF32<6>>();
-            case 8: return f.template run<gb::DistF32<8>>();
-            default: return f.template run<gb::DistF32Generic>();
-        }
-    }
-};
-
 struct PairLaunch {
     Handle* h;
     gb::PairArgs a;
@@ -920,7 +906,7 @@ int builder_index_elements(Builder* b, uint32_t layer_m, uint32_t ef, uint64_t a
     if (rc) return rc;
     GB_CUDA(cudaMemsetAsync(b->d_locks, 0, num * sizeof(int), stream));
     const size_t link_smem = plan.base_smem + gb::link_scratch_bytes(gb::link_cand_cap(ef, b->cfg.num_neighbors),
-                                                                      b->cfg.num_neighbors) + 64;
+                                                                      b->cfg.num_neighbors);
     uint64_t pos = 0;
     while (pos < total) {
         // nodes already linked into this layer: a batch never exceeds 1/16 of them (its members do not see each other)
@@ -958,7 +944,7 @@ int builder_index_elements(Builder* b, uint32_t layer_m, uint32_t ef, uint64_t a
     // limit number of neighbors (:794-797)
     GB_CUDA(cudaMemsetAsync(b->d_counter, 0, 16, stream));
     LinkLaunch P{h, {}, plan.base_smem + gb::link_scratch_bytes(gb::link_cand_cap(0, b->cfg.num_neighbors),
-                                                               b->cfg.num_neighbors) + 64, 0, stream, true};
+                                                               b->cfg.num_neighbors), 0, stream, true};
     P.a.rows = rows;
     P.a.stride = b->stride;
     P.a.node_width = b->cfg.num_neighbors;
@@ -1709,7 +1695,7 @@ int granne_b200_compute_distances(int element_kind, const float* a, const float*
         GB_CUDA(cudaMalloc(&d_err, 4));
         GB_CUDA(cudaMemcpy(d_a, a, (size_t)n * dim * 4, cudaMemcpyHostToDevice));
         GB_CUDA(cudaMemset(d_err, 0, 4));
-        PairLaunch L{h.get(), {}, plan.base_smem + gb::link_scratch_bytes(8, 32) + 64, 0, nullptr};
+        PairLaunch L{h.get(), {}, plan.base_smem + gb::link_scratch_bytes(8, 32), 0, nullptr};
         L.a.queries = d_a;
         L.a.n = (uint32_t)n;
         L.a.out = d_out;

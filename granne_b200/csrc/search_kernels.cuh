@@ -9,14 +9,14 @@
 //     split u32 arrays Ld (distance bits | expanded flag) / Li (ids), capacity 32*R; slow pass (search_layer): 64-bit
 //     keys in a global-memory workspace, for the rare query whose plateau of equal distances overflows the fast list;
 //   * an exact visited set (the reference's FxHashSet): fast pass = a bucketed table in global memory that stays L2
-//     resident (8 ids per 32-byte bucket, one sector read per neighbour, no atomics — the warp is the only writer);
+//     resident (4 ids per 16-byte bucket, one 128-bit load per neighbour, no atomics — the warp is the only writer);
 //     slow pass = open addressing with CAS in the global workspace;
-//   * an 8-row x 36-float tile in shared memory used to reproduce the reference's strictly ordered 32-lane
-//     partial-sum reduction, plus a staging tile for candidate rows.
-// Candidate rows are gathered from HBM with 1-D bulk copies (cp.async.bulk -> UBLKCP, completion on an mbarrier with
-// expect_tx), all rows of a batch in flight at once; the f32 row layout in HBM is lane-permuted so that lane i reads
-// its accumulator chunks with 128-bit shared loads.  Element rows use an L2 evict_first policy, adjacency rows and the
-// visited table evict_last; the adjacency row of the runner-up candidate is fetched speculatively while the current
+//   * a tile of up to 32 rows x 36 floats in shared memory used to reproduce the reference's strictly ordered 32-lane
+//     partial-sum reduction, plus a staging tile for candidate rows (layout: SmemLayout).
+// Candidate rows are gathered from HBM into the staging tile with per-lane cp.async (each lane copies only the bytes it
+// reads back, so no cross-lane barrier is needed), all rows of a batch in flight at once; the f32 row layout in HBM is
+// lane-permuted so that lane i reads its accumulator chunks with 128-bit shared loads.  The visited table uses an L2
+// evict_last policy; the adjacency row of the runner-up candidate is fetched speculatively while the current
 // expansion's distances are computed.
 //
 // Exactness (bit-identical ids AND f32 distances, identical n_dist / n_expand counters):
@@ -40,7 +40,7 @@
 #define GB_MIN_BLOCKS 24  // resident one-warp CTAs per SM the fast kernel is register-limited to (tuning knob)
 #endif
 #ifndef GB_STG_BYTES
-#define GB_STG_BYTES 4096  // staging tile per warp for bulk-copied candidate rows (tuning knob)
+#define GB_STG_BYTES 4096  // staging tile per warp for gathered candidate rows (tuning knob)
 #endif
 
 namespace granne_b200 {
@@ -61,6 +61,44 @@ __host__ __device__ constexpr uint32_t tile_bytes_for_rows(uint32_t rows) {
 
 enum ElementKind : int { kAngularF32 = 0, kAngularI8 = 1, kSumEmbeddings = 2 };
 enum QueryFormat : int { kQueryRawF32 = 0, kQueryElement = 1, kQueryById = 2 };  // ById: builder only (u32 ids)
+
+// Shared-memory layout of one warp in the dynamic window: the host sizes every launch from it, the build kernels place
+// their pointers with it (place_warp_smem), and search_kernel spells out the same walk:
+//   tile (ordered-sum rows) + id scratch | reserved 16 bytes | qs | xs (embeddings only) | staging tile | end
+// qs holds the query (f32 dim rounded up to 4 floats, or the row_stride bytes of an i8 row), xs one element of the same
+// size; both start on 16-byte boundaries, the staging tile (stg_rows x stg_row_bytes) on a 128-byte boundary.  Behind
+// `end` each kernel appends its own: the fast list, or the generic list and visited set (search_kernel), or the link
+// scratch (build kernels).
+// The layout is walked from `base` in the address type P: the host walks byte offsets (P = size_t, base = 0), the
+// kernels walk their shared window (P = unsigned char*, base = smem_raw), so that every pointer is smem_raw + offset
+// and the compiler keeps the accesses in the shared address space (LDS/STS with 32-bit addresses).
+template <class P>
+struct SmemLayout {
+    // Once held the mbarrier of a bulk-copy gather.  Kept because moving the offsets behind it reschedules the search
+    // kernels, which run at their register cap; removing it needs a measurement of its own.
+    static constexpr uint32_t kReservedBytes = 16;
+    P ids, qs, xs, stg, end;  // stg = P() without a staging tile
+
+    __host__ __device__ __forceinline__ SmemLayout(P base, int kind, uint32_t dim, uint32_t row_stride,
+                                                   uint32_t tile_rows, uint32_t stg_rows, uint32_t stg_row_bytes) {
+        P sp = base;  // the tile starts at base
+        ids = sp + tile_bytes_for_rows(tile_rows) - kIdScratchBytes;
+        sp += tile_bytes_for_rows(tile_rows);
+        sp += kReservedBytes;
+        const uint32_t slot_bytes = (kind == kAngularI8) ? row_stride : ((dim + 3u) & ~3u) * 4u;
+        qs = sp;
+        sp += (slot_bytes + 15u) & ~15u;
+        xs = sp;
+        if (kind == kSumEmbeddings) sp += (slot_bytes + 15u) & ~15u;
+        stg = P();
+        if (stg_rows) {
+            sp = base + (((size_t)(sp - base) + 127u) & ~(size_t)127u);
+            stg = sp;
+            sp += (size_t)stg_rows * stg_row_bytes;
+        }
+        end = sp;
+    }
+};
 
 // per-query status bits (device side)
 constexpr int kStatusOverflow = 1;   // workspace too small for an exact answer -> slow path
@@ -111,7 +149,7 @@ struct SearchArgs {
     uint32_t vis_slots;       // visited slots for the bottom layer
     uint32_t vis_slots_upper; // visited slots for the max_search = 1 descents
     uint32_t* vis_global;     // fast pass: one table of vis_slots u32 per CTA in global memory (L2 resident)
-    uint32_t stg_rows;        // candidate rows per bulk-copy batch (0 = this element kind loads directly)
+    uint32_t stg_rows;        // candidate rows per staged batch (0 = this element kind loads directly)
     uint32_t stg_row_bytes;   // bytes of one staged row (f32: 128*FULL, i8: row_stride)
     uint32_t tile_rows;       // rows of the ordered-sum tile (8 for the staged f32 engine, 32 generic, 0 unused)
     uint32_t* out_ids;
@@ -152,19 +190,7 @@ __device__ __forceinline__ unsigned lanemask_lt() {
     return m;
 }
 
-// Streaming 128-bit / 32-bit loads of candidate rows: read-only path, do not pollute L1 (each row is used once).
-__device__ __forceinline__ float4 ldg_row_f4(const float* p) {
-    float4 v;
-    asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0,%1,%2,%3}, [%4];"
-                 : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
-                 : "l"(p));
-    return v;
-}
-__device__ __forceinline__ float2 ldg_row_f2(const float* p) {
-    float2 v;
-    asm volatile("ld.global.nc.L1::no_allocate.v2.f32 {%0,%1}, [%2];" : "=f"(v.x), "=f"(v.y) : "l"(p));
-    return v;
-}
+// Streaming 32-bit loads of candidate rows: read-only path, do not pollute L1 (each row is used once).
 __device__ __forceinline__ float ldg_row_f1(const float* p) {
     float v;
     asm volatile("ld.global.nc.L1::no_allocate.f32 %0, [%1];" : "=f"(v) : "l"(p));
@@ -194,12 +220,9 @@ struct WarpCtx {
     uint32_t* ids;     // 32 u32 scratch for compacting candidate ids (always shared)
     float* qs;         // query, natural layout: f32[dim] (or i8 words for ANGULAR_INT), shared
     float* xs;         // EMBEDDINGS scratch f32[dim], shared
-    unsigned char* stg;  // staging tile for bulk-copied candidate rows (shared, 128-byte aligned)
+    unsigned char* stg;  // staging tile for gathered candidate rows (shared, 128-byte aligned)
     uint32_t stg_rows;   // rows that fit in the staging tile (<= 16)
     uint32_t stg_row_bytes;
-    uint32_t bar;        // shared-space address of the mbarrier the bulk copies signal
-    uint32_t phase;      // its current phase parity
-    unsigned long long pol_stream;  // L2 policy evict_first: candidate rows are read once per query
     unsigned long long pol_keep;    // L2 policy evict_last: the per-warp visited tables are re-read all the time
     int lane;
     int status;
@@ -207,45 +230,26 @@ struct WarpCtx {
     uint32_t n_dist, n_expand, n_nbr;
 };
 
-// ---- mbarrier + 1-D bulk copy (TMA, UBLKCP) helpers ----------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    uint32_t ok;
-    do {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(ok)
-            : "r"(bar), "r"(parity)
-            : "memory");
-    } while (!ok);
-}
-// global -> shared, `bytes` multiple of 16, both addresses 16-byte aligned; completion is counted on `bar`.
-__device__ __forceinline__ void bulk_copy_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar,
-                                              unsigned long long policy) {
-    asm volatile(
-        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(dst),
-        "l"(src), "r"(bytes), "r"(bar), "l"(policy)
-        : "memory");
-}
-__device__ __forceinline__ unsigned long long make_policy_evict_first() {
-    unsigned long long p;
-    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
-    return p;
-}
 __device__ __forceinline__ unsigned long long make_policy_evict_last() {
     unsigned long long p;
     asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
     return p;
+}
+
+// Points the warp's shared buffers into smem_raw as SmemLayout places them; returns the first byte behind them.
+__device__ __forceinline__ unsigned char* place_warp_smem(WarpCtx& c, unsigned char* smem_raw, const DeviceIndex& ix,
+                                                          uint32_t tile_rows, uint32_t stg_rows, uint32_t stg_row_bytes) {
+    const SmemLayout<unsigned char*> L(smem_raw, ix.kind, ix.dim, ix.row_stride, tile_rows, stg_rows, stg_row_bytes);
+    c.tile = reinterpret_cast<float*>(smem_raw);
+    c.ids = reinterpret_cast<uint32_t*>(L.ids);
+    c.pol_keep = make_policy_evict_last();
+    c.qs = reinterpret_cast<float*>(L.qs);
+    c.xs = reinterpret_cast<float*>(L.xs);
+    c.stg = L.stg;
+    c.stg_rows = stg_rows;
+    c.stg_row_bytes = stg_row_bytes;
+    return L.end;
 }
 
 // ---- per-lane asynchronous copies (cp.async -> LDGSTS): global -> shared without staging registers ----------------
@@ -276,22 +280,91 @@ __device__ __forceinline__ float ordered_lane_sum_bcast(float p) {
     return r;
 }
 
+// The same ordered sum for the 32 lane partials of one candidate parked in row `trow` of the tile (the lane that
+// owns the candidate sums; 16-byte aligned rows, one LDS.128 per four partials).
+__device__ __forceinline__ float ordered_tile_sum(const float* tile, int trow) {
+    float r = 0.0f;
+    const float4* t = reinterpret_cast<const float4*>(tile + trow * kTileStride);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+        const float4 v = t[i];
+        r = __fadd_rn(r, v.x);
+        r = __fadd_rn(r, v.y);
+        r = __fadd_rn(r, v.z);
+        r = __fadd_rn(r, v.w);
+    }
+    return r;
+}
+
+// normalize_f32 (math.rs:124-150) of x[0..dim) in place, all lanes: norm = sqrt(dot(x, x)) with dot_product_f32's
+// order (lane FMA over the full chunks, ordered 32-lane sum, FMA tail); if norm > 0 { x[i] /= norm }.
+__device__ __forceinline__ void normalize_f32(float* x, int dim, int full, int lane) {
+    float p = 0.0f;
+    for (int ch = 0; ch < full; ++ch) {
+        const float v = x[ch * 32 + lane];
+        p = __fmaf_rn(v, v, p);
+    }
+    float r = ordered_lane_sum_bcast(p);
+    for (int t = full * 32; t < dim; ++t) {
+        const float v = x[t];
+        r = __fmaf_rn(v, v, r);
+    }
+    const float norm = __fsqrt_rn(r);
+    __syncwarp();  // every lane has finished reading the un-normalised tail before anyone overwrites it
+    if (norm > 0.0f)
+        for (int i = lane; i < dim; i += 32) x[i] = __fdiv_rn(x[i], norm);
+    __syncwarp();
+}
+
+// angular_int::Vector::quantize (angular_int.rs:28-45) of x[0..dim) into dst, all lanes: max |x|, then x * 127 / max
+// truncated toward zero and clamped to i8 (NaN -> 0).  Sets kStatusNotFinite in *status if x holds a NaN (the
+// reference's NotNan max fails on it).
+__device__ __forceinline__ void quantize_i8(const float* x, int8_t* dst, int dim, int lane, int* status) {
+    float mx = 0.0f;
+    bool bad = false;
+    for (int i = lane; i < dim; i += 32) {
+        const float v = x[i];
+        if (v != v) bad = true;
+        mx = fmaxf(mx, fabsf(v));
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(kFullMask, mx, o));
+    if (__any_sync(kFullMask, bad)) *status |= kStatusNotFinite;
+    for (int i = lane; i < dim; i += 32) {
+        const float vi = __fdiv_rn(__fmul_rn(x[i], 127.0f), mx);
+        int q;
+        if (vi != vi)
+            q = 0;
+        else if (vi >= 127.0f)
+            q = 127;
+        else if (vi <= -128.0f)
+            q = -128;
+        else
+            q = (int)vi;  // truncation toward zero
+        dst[i] = (int8_t)q;
+    }
+}
+
+// Position of element e < 32*full in a lane-permuted f32 row (permute_rows_f32_kernel): chunk ch = g*V + v, lane i
+// lands at g*32*V + i*V + v.  The tail (e >= 32*full) stays in place.
+__device__ __forceinline__ uint32_t permuted_offset(uint32_t e, uint32_t V) {
+    const uint32_t ch = e / 32, i = e % 32, g = ch / V, vv = ch % V;
+    return g * 32 * V + i * V + vv;
+}
+
 // ------------------------------------------------------------------------------------------------------------------
 // distance engines.  Contract: on entry lane j (< k) holds candidate id `my_id`; returns d_j in lane j.
 // ------------------------------------------------------------------------------------------------------------------
 
 // ANGULAR f32, compile-time chunk count FULL (dim = 32*FULL + tail).  Query chunk values live in registers.
-// Candidate rows are fetched with 1-D bulk copies (cp.async.bulk -> UBLKCP): lane b issues the copy of row b of the
-// batch into the staging tile and one mbarrier collects all completions, so a whole batch of rows is in flight with
-// one instruction per row and no data registers.  Rows are lane-permuted in HBM (permute_rows_f32_kernel) so that lane
-// i then reads its share of G*V chunks with conflict-free LDS.128/64/32.
+// Candidate rows are gathered into the staging tile with per-lane cp.async (see dists), a whole batch of rows in flight
+// at once and no data registers held.  Rows are lane-permuted in HBM (permute_rows_f32_kernel) so that lane i copies
+// and then reads its share of G*V chunks with conflict-free LDS.128/64/32.
 template <int FULL>
 struct DistF32 {
     static constexpr int V = (FULL % 4 == 0) ? 4 : ((FULL % 2 == 0) ? 2 : 1);
     static constexpr int G = FULL / V;
     static constexpr int NQ = FULL > 0 ? FULL : 1;
-    static constexpr bool kStaged = FULL > 0;  // candidate rows pass through the shared staging tile
-    static constexpr bool kMbar = false;        // ... with cp.async groups, not an mbarrier
     float q[NQ];
 
     __device__ __forceinline__ void load_query(const DeviceIndex& ix, const WarpCtx& c) {
@@ -325,17 +398,7 @@ struct DistF32 {
     // in tile row `trow` (ignored when FULL == 0).
     __device__ __forceinline__ float ordered_finish(const DeviceIndex& ix, WarpCtx& c, uint32_t id, int trow) const {
         float r = 0.0f;
-        if (FULL > 0) {
-            const float4* t = reinterpret_cast<const float4*>(c.tile + trow * kTileStride);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const float4 v = t[i];
-                r = __fadd_rn(r, v.x);
-                r = __fadd_rn(r, v.y);
-                r = __fadd_rn(r, v.z);
-                r = __fadd_rn(r, v.w);
-            }
-        }
+        if (FULL > 0) r = ordered_tile_sum(c.tile, trow);
         const int tail = ix.tail;
         if (tail) {
             const float* row = reinterpret_cast<const float*>(static_cast<const char*>(ix.vectors) +
@@ -417,21 +480,10 @@ struct DistF32 {
 // back for its accumulator chunk[l], and the ordered 32-lane sums of a batch run through the 8-row tile.  Rows too
 // wide for the staging tile (stg_rows == 0) load directly.
 struct DistF32Generic {
-    static constexpr bool kStaged = false;
-    static constexpr bool kMbar = false;
     __device__ __forceinline__ void load_query(const DeviceIndex&, const WarpCtx&) {}
 
     static __device__ __forceinline__ float ordered_finish(const DeviceIndex& ix, WarpCtx& c, uint32_t id, int trow) {
-        float r = 0.0f;
-        const float4* t = reinterpret_cast<const float4*>(c.tile + trow * kTileStride);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-            const float4 v = t[i];
-            r = __fadd_rn(r, v.x);
-            r = __fadd_rn(r, v.y);
-            r = __fadd_rn(r, v.z);
-            r = __fadd_rn(r, v.w);
-        }
+        float r = ordered_tile_sum(c.tile, trow);
         const int full = ix.full;
         const float* row = static_cast<const float*>(ix.vectors) + (size_t)id * ix.row_stride + full * 32;
         const float* qt = c.qs + full * 32;
@@ -505,9 +557,7 @@ struct DistF32Generic {
 // registers (8 dp4a), and the exact integer sums are reduced inside the group with log2(L) xor-shuffles — integer
 // addition is order independent.  A 100-byte row costs a quarter of a pass instead of a full-warp pass + 2 REDUX.
 struct DistI8 {
-    static constexpr bool kStaged = true;
-    static constexpr bool kMbar = false;
-    int4 qv;       // the 16 query bytes of this lane's chunk
+    int4 qv;      // the 16 query bytes of this lane's chunk
     uint32_t lg;   // log2(L)
     uint32_t C;    // chunks per row (0: rows wider than 512 bytes, generic path)
 
@@ -623,8 +673,6 @@ struct DistI8 {
 // EMBEDDINGS: element = ordered sum of embedding rows, normalised, then the f32 angular distance
 // (src/elements/embeddings/mod.rs:124-143,164-174; src/math.rs:92-150).  Natural row layout, runtime dim.
 struct DistSum {
-    static constexpr bool kStaged = false;
-    static constexpr bool kMbar = false;
     __device__ __forceinline__ void load_query(const DeviceIndex&, const WarpCtx&) {}
 
     // materialises ElementContainer::get(id) into c.xs (all lanes participate)
@@ -643,38 +691,13 @@ struct DistSum {
             c.xs[i] = x;
         }
         __syncwarp();
-        // normalize_f32: norm = sqrt(dot(x,x)); if norm > 0 { x[i] /= norm }
-        const int full = ix.full;
-        float p = 0.0f;
-        for (int ch = 0; ch < full; ++ch) {
-            const float v = c.xs[ch * 32 + c.lane];
-            p = __fmaf_rn(v, v, p);
-        }
-        float r = ordered_lane_sum_bcast(p);
-        for (int t = full * 32; t < dim; ++t) {
-            const float v = c.xs[t];
-            r = __fmaf_rn(v, v, r);
-        }
-        const float norm = __fsqrt_rn(r);
-        __syncwarp();  // every lane has finished reading the un-normalised tail before anyone overwrites it
-        if (norm > 0.0f)
-            for (int i = c.lane; i < dim; i += 32) c.xs[i] = __fdiv_rn(c.xs[i], norm);
-        __syncwarp();
+        normalize_f32(c.xs, dim, (int)ix.full, c.lane);
     }
 
     // Ordered 32-lane sum of tile row `trow` (math.rs:27-30) followed by the FMA tail over x[t]*y[t] (:32-39).
     static __device__ __forceinline__ float ordered_dot(const WarpCtx& c, int trow, const float* x, const float* y,
                                                         int full, int dim) {
-        float r = 0.0f;
-        const float4* t = reinterpret_cast<const float4*>(c.tile + trow * kTileStride);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-            const float4 v = t[i];
-            r = __fadd_rn(r, v.x);
-            r = __fadd_rn(r, v.y);
-            r = __fadd_rn(r, v.z);
-            r = __fadd_rn(r, v.w);
-        }
+        float r = ordered_tile_sum(c.tile, trow);
         for (int e = full * 32; e < dim; ++e) r = __fmaf_rn(x[e], y[e], r);
         return r;
     }
@@ -1410,10 +1433,7 @@ __device__ __forceinline__ void load_element_to_qs(const DeviceIndex& ix, WarpCt
         const uint32_t V = ix.vec_group;
         for (uint32_t e = lane; e < dim; e += 32) {
             uint32_t o = e;
-            if (e < ix.full * 32) {
-                const uint32_t ch = e / 32, i = e % 32, g = ch / V, vv = ch % V;
-                o = g * 32 * V + i * V + vv;
-            }
+            if (e < ix.full * 32) o = permuted_offset(e, V);
             c.qs[e] = __ldg(row + o);
         }
     } else {
@@ -1443,31 +1463,8 @@ __device__ __forceinline__ void prepare_query(const DeviceIndex& ix, const Searc
             const int8_t* src = static_cast<const int8_t*>(a.queries) + qi * dim;
             for (int i = lane; i < dim; i += 32) qb[i] = src[i];
         } else {
-            // angular_int.rs:28-45: max |x| (NotNan max; NaN input is an error), vi = x*127/max, `as i8`
-            const float* src = static_cast<const float*>(a.queries) + qi * dim;
-            float mx = 0.0f;
-            bool bad = false;
-            for (int i = lane; i < dim; i += 32) {
-                const float v = src[i];
-                if (v != v) bad = true;
-                mx = fmaxf(mx, fabsf(v));
-            }
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(kFullMask, mx, o));
-            if (__any_sync(kFullMask, bad)) c.status |= kStatusNotFinite;
-            for (int i = lane; i < dim; i += 32) {
-                const float vi = __fdiv_rn(__fmul_rn(src[i], 127.0f), mx);
-                int q;
-                if (vi != vi)
-                    q = 0;
-                else if (vi >= 127.0f)
-                    q = 127;
-                else if (vi <= -128.0f)
-                    q = -128;
-                else
-                    q = (int)vi;  // truncation toward zero
-                qb[i] = (int8_t)q;
-            }
+            // Vector::from(Vec<f32>) -> quantize; NaN input is an error (NotNan max)
+            quantize_i8(static_cast<const float*>(a.queries) + qi * dim, qb, dim, lane, &c.status);
         }
         __syncwarp();
         int dy = 0;
@@ -1479,25 +1476,8 @@ __device__ __forceinline__ void prepare_query(const DeviceIndex& ix, const Searc
         const float* src = static_cast<const float*>(a.queries) + qi * dim;
         for (int i = lane; i < dim; i += 32) c.qs[i] = src[i];
         __syncwarp();
-        if (a.query_format == kQueryRawF32) {
-            // Vector::from(Vec<f32>) -> normalize_f32 (angular.rs:55-61, math.rs:124-150)
-            const int full = ix.full;
-            float p = 0.0f;
-            for (int ch = 0; ch < full; ++ch) {
-                const float v = c.qs[ch * 32 + lane];
-                p = __fmaf_rn(v, v, p);
-            }
-            float r = ordered_lane_sum_bcast(p);
-            for (int t = full * 32; t < dim; ++t) {
-                const float v = c.qs[t];
-                r = __fmaf_rn(v, v, r);
-            }
-            const float norm = __fsqrt_rn(r);
-            __syncwarp();
-            if (norm > 0.0f)
-                for (int i = lane; i < dim; i += 32) c.qs[i] = __fdiv_rn(c.qs[i], norm);
-            __syncwarp();
-        }
+        if (a.query_format == kQueryRawF32)
+            normalize_f32(c.qs, dim, (int)ix.full, lane);  // Vector::from(Vec<f32>) (angular.rs:55-61)
     }
 }
 
@@ -1543,17 +1523,16 @@ __global__ void __launch_bounds__(32, R > 0 ? GB_MIN_BLOCKS : 1) search_kernel(c
     extern __shared__ __align__(16) unsigned char smem_raw[];
     WarpCtx c;
     c.lane = threadIdx.x;
-    // shared layout: tile + id scratch | mbarrier | qs | xs | staging | list      (fast pass: visited set in global)
-    //                                                          ... | list | visited (generic pass, slow_pass == 0)
+    // shared layout: SmemLayout | list            (fast pass: visited set in global)
+    //                SmemLayout | list | visited  (generic pass, slow_pass == 0)
+    // The SmemLayout walk is spelled out here rather than called through place_warp_smem: the call compiles to a
+    // differently scheduled prologue, and this kernel runs at its register cap.
     unsigned char* sp = smem_raw;
     c.tile = reinterpret_cast<float*>(sp);
     c.ids = reinterpret_cast<uint32_t*>(sp + tile_bytes_for_rows(a.tile_rows) - kIdScratchBytes);
     sp += tile_bytes_for_rows(a.tile_rows);
-    c.bar = smem_u32(sp);
-    c.phase = 0;
-    c.pol_stream = make_policy_evict_first();
     c.pol_keep = make_policy_evict_last();
-    sp += 16;
+    sp += SmemLayout<unsigned char*>::kReservedBytes;
     const uint32_t qbytes = (ix.kind == kAngularI8) ? ix.row_stride : ((ix.dim + 3u) & ~3u) * 4u;
     c.qs = reinterpret_cast<float*>(sp);
     sp += (qbytes + 15u) & ~15u;
@@ -1562,14 +1541,10 @@ __global__ void __launch_bounds__(32, R > 0 ? GB_MIN_BLOCKS : 1) search_kernel(c
     c.stg = nullptr;
     c.stg_rows = a.stg_rows;
     c.stg_row_bytes = a.stg_row_bytes;
-    if (a.stg_rows) {  // staging tile: bulk-copied candidate rows (f32 / i8) or summed candidate vectors (embeddings)
+    if (a.stg_rows) {  // staging tile: gathered candidate rows (f32 / i8) or summed candidate vectors (embeddings)
         sp = smem_raw + (((size_t)(sp - smem_raw) + 127u) & ~(size_t)127u);
         c.stg = sp;
         sp += (size_t)a.stg_rows * a.stg_row_bytes;
-    }
-    if (Dist::kMbar) {
-        if (c.lane == 0) mbar_init(c.bar, 1);
-        __syncwarp();
     }
     // the fast list always lives in this CTA's shared window (derived from smem_raw only, so that the compiler keeps
     // its accesses in the shared address space: LDS/STS with 32-bit addresses)
@@ -1766,15 +1741,8 @@ __global__ void __launch_bounds__(32) get_element_kernel(const DeviceIndex ix, u
         for (uint32_t i = lane; i < dim; i += 32) static_cast<int8_t*>(out)[i] = row[i];
     } else if (ix.kind == kAngularF32) {
         const float* row = static_cast<const float*>(ix.vectors) + idx * ix.row_stride;
-        const uint32_t V = ix.vec_group;
-        for (uint32_t e = lane; e < dim; e += 32) {
-            uint32_t o = e;
-            if (e < ix.full * 32) {
-                const uint32_t ch = e / 32, i = e % 32, g = ch / V, vv = ch % V;
-                o = g * 32 * V + i * V + vv;
-            }
-            static_cast<float*>(out)[e] = row[o];
-        }
+        for (uint32_t e = lane; e < dim; e += 32)
+            static_cast<float*>(out)[e] = row[e < ix.full * 32 ? permuted_offset(e, ix.vec_group) : e];
     } else {
         WarpCtx c;
         c.lane = lane;
