@@ -37,6 +37,17 @@ int fail(int code, const std::string& msg) {
     return code;
 }
 
+// The exception boundary of the C ABI: every entry point that can allocate or throw runs its body through this, so
+// that no C++ exception (std::bad_alloc from a container, ...) escapes into a C, C++ or Rust caller.
+template <class F>
+int guarded(F&& body) {
+    try {
+        return body();
+    } catch (const std::exception& e) {
+        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, std::string("exception: ") + e.what());
+    }
+}
+
 #define GB_CUDA(expr)                                                                                   \
     do {                                                                                                \
         cudaError_t _e = (expr);                                                                        \
@@ -46,13 +57,16 @@ int fail(int code, const std::string& msg) {
     } while (0)
 
 // Every entry point runs on its handle's device and leaves the caller's current device as it found it (a host
-// application — e.g. one torch process per GPU — must not see its default device change under it).
+// application — e.g. one torch process per GPU — must not see its default device change under it).  A guard is
+// declared before anything that owns device memory, so that the memory is also freed on that device.
 struct DeviceGuard {
     int prev = -1;
     cudaError_t err = cudaSuccess;
-    explicit DeviceGuard(int device) {
+    DeviceGuard() = default;
+    explicit DeviceGuard(int device) : err(enter(device)) {}
+    cudaError_t enter(int device) {
         if (cudaGetDevice(&prev) != cudaSuccess) prev = -1;
-        err = cudaSetDevice(device);
+        return cudaSetDevice(device);
     }
     ~DeviceGuard() {
         if (prev >= 0) cudaSetDevice(prev);
@@ -64,38 +78,69 @@ struct DeviceGuard {
     DeviceGuard _device_guard(device); \
     GB_CUDA(_device_guard.err)
 
+// The owners of the host layer's CUDA resources; nothing else frees them.
+struct DeviceFree {
+    void operator()(void* p) const { cudaFree(p); }
+};
+struct HostFree {
+    void operator()(void* p) const { cudaFreeHost(p); }
+};
+struct StreamDestroy {
+    void operator()(cudaStream_t s) const { cudaStreamDestroy(s); }
+};
+using Stream = std::unique_ptr<CUstream_st, StreamDestroy>;
+
+// `cap` elements of T in device memory (PINNED: pinned host memory).
+template <class T, bool PINNED = false>
+struct Buffer {
+    std::unique_ptr<T, std::conditional_t<PINNED, HostFree, DeviceFree>> p;
+    size_t cap = 0;
+    T* get() const { return p.get(); }
+    // Makes room for `count` elements.  Reallocates only when `count` exceeds the capacity; the old buffer may still
+    // be in use by work queued on `stream`, so the stream is synchronised before it is freed.
+    int grow(size_t count, cudaStream_t stream) {
+        if (count <= cap) return GRANNE_B200_OK;
+        if (p) GB_CUDA(cudaStreamSynchronize(stream));
+        p.reset();
+        cap = 0;
+        void* q = nullptr;
+        if constexpr (PINNED)
+            GB_CUDA(cudaMallocHost(&q, count * sizeof(T)));
+        else
+            GB_CUDA(cudaMalloc(&q, count * sizeof(T)));
+        p.reset(static_cast<T*>(q));
+        cap = count;
+        return GRANNE_B200_OK;
+    }
+};
+template <class T>
+using Pinned = Buffer<T, true>;
+
 // Per-call scratch: device copies of queries/results, status words, stream.  Pooled per handle so that several host
 // threads can search concurrently (the reference's `search` is `&self` and reentrant).
 struct Workspace {
-    cudaStream_t stream = nullptr;
-    void* d_queries = nullptr;
-    size_t queries_cap = 0;
-    uint32_t* d_ids = nullptr;
-    float* d_dists = nullptr;
+    Stream stream;  // declared first: destroyed after the buffers
+    Buffer<uint8_t> d_queries;
+    Buffer<uint32_t> d_ids;  // one block: ids | dists | counts, so that one copy brings a whole result back
+    float* d_dists = nullptr;    // inside d_ids, packed for the current call's nq x k
     uint32_t* d_counts = nullptr;
-    unsigned long long* d_stats = nullptr;
-    size_t out_cap_q = 0, out_cap_k = 0;
-    int* d_status = nullptr;  // nq ints
-    size_t status_cap = 0;
+    Buffer<unsigned long long> d_stats;
+    Buffer<int> d_status;  // nq ints
     // one 64-byte block, zeroed once per call: [0..2] work counters of the three passes, [3] fast pass flagged
     // something, [4] retry pass flagged something, [5] done counter (fused gather); d_error = words [8..11]
-    unsigned int* d_counters = nullptr;
+    Buffer<unsigned int> d_counters;
     int* d_error = nullptr;              // [0]=sticky error bits of this call (inside the counters block)
-    unsigned long long* d_retried = nullptr;  // cumulative: queries that needed more than the fast pass
-    unsigned long long* h_retried = nullptr;  // pinned mirror (copied at the end of every call, read without a sync)
+    Buffer<unsigned long long> d_retried;  // cumulative: queries that needed more than the fast pass
+    Pinned<unsigned long long> h_retried;  // pinned mirror (copied at the end of every call, read without a sync)
     unsigned long long seen_retried = 0, seen_total = 0, total_queries = 0;
-    void* h_pinned = nullptr;            // staging for host<->device copies
-    size_t pinned_cap = 0;
+    Pinned<uint8_t> h_pinned;            // staging for host<->device copies
     // slow path
-    unsigned long long* d_slow_list = nullptr;
-    uint32_t* d_slow_vis = nullptr;
-    size_t slow_vis_cap = 0;  // u32 entries allocated for d_slow_vis
+    Buffer<unsigned long long> d_slow_list;
+    Buffer<uint32_t> d_slow_vis;
     // fast pass: per-CTA visited tables in global memory
-    uint32_t* d_vis = nullptr;
-    size_t vis_cap = 0;  // u32 entries
+    Buffer<uint32_t> d_vis;
     // retry pass: fewer CTAs, larger tables
-    uint32_t* d_vis_retry = nullptr;
-    size_t vis_retry_cap = 0;
+    Buffer<uint32_t> d_vis_retry;
 };
 
 }  // namespace
@@ -145,15 +190,30 @@ int check_device(int device, int* num_sms, size_t* smem_optin) {
     return GRANNE_B200_OK;
 }
 
+// Device memory for staged data (elements, layers): `count` T, at least 16 bytes so that every buffer has an address
+// of its own.
 template <class T>
-int dev_alloc(Handle* h, T** out, size_t count) {
-    void* p = nullptr;
-    const size_t bytes = std::max<size_t>(count * sizeof(T), 16);
-    GB_CUDA(cudaMalloc(&p, bytes));
-    h->allocations.emplace_back(p, [](void* q) { cudaFree(q); });
-    h->device_bytes += bytes;
-    *out = static_cast<T*>(p);
-    return GRANNE_B200_OK;
+int dev_alloc(Buffer<T>* mem, size_t count) {
+    return mem->grow(std::max<size_t>(count, 16 / sizeof(T)), nullptr);
+}
+
+// Hands the filled buffer `mem` to the handle, which counts it in device_bytes, and returns its address.  `old`: the
+// staged buffer (`old_bytes` long) that `mem` replaces.  The handle drops its reference to it; get_index snapshots
+// keep theirs.
+template <class T>
+T* stage(Handle* h, Buffer<T> mem, const void* old = nullptr, size_t old_bytes = 0) {
+    T* p = mem.get();
+    h->device_bytes += mem.cap * sizeof(T);
+    std::shared_ptr<void> owner(std::move(mem.p));
+    auto it = std::find_if(h->allocations.begin(), h->allocations.end(),
+                           [&](const std::shared_ptr<void>& a) { return old && a.get() == old; });
+    if (it == h->allocations.end()) {
+        h->allocations.push_back(std::move(owner));
+    } else {
+        h->device_bytes -= std::max<size_t>(old_bytes, 16);
+        *it = std::move(owner);
+    }
+    return p;
 }
 
 // Which distance engine serves an index: calls f.template run<Dist>() for the engine of `d`'s element kind and chunk
@@ -193,66 +253,63 @@ struct FixedChunksProbe {
 };
 int fixed_f32_chunks(const gb::DeviceIndex& d) { return DistDispatch::call(d, FixedChunksProbe{}); }
 
-// Uploads `nrows` dense rows in slabs through a temporary device buffer and re-lays them out on the device.
-int stage_dense(Handle* h, const uint8_t* host_rows, uint64_t nrows, uint32_t dim, bool is_i8,
-                bool device_src = false) {
+// Writes `nrows` dense rows of the handle's kind and width from `src` (host memory, or device memory if
+// `device_src`) to the staged rows at `dst`: in 64 MB slabs through a temporary device buffer, re-laid out on the
+// device by pad_rows_i8_kernel / permute_rows_f32_kernel.
+int upload_rows(Handle* h, const uint8_t* src, uint64_t nrows, bool device_src, uint8_t* dst) {
+    const gb::DeviceIndex& d = h->dev;
+    const bool i8 = d.kind == gb::kAngularI8;
+    const size_t esz = i8 ? 1 : 4, src_row = (size_t)d.dim * esz;
+    const uint64_t slab = std::max<uint64_t>(1, (64ull << 20) / src_row);
+    Buffer<uint8_t> tmp;
+    int rc;
+    if (!device_src && (rc = tmp.grow((size_t)std::min(slab, std::max<uint64_t>(nrows, 1)) * src_row, nullptr)))
+        return rc;
+    for (uint64_t r0 = 0; r0 < nrows; r0 += slab) {
+        const uint64_t nr = std::min(slab, nrows - r0);
+        const uint8_t* from = src + r0 * src_row;
+        if (!device_src) {
+            GB_CUDA(cudaMemcpy(tmp.get(), from, (size_t)nr * src_row, cudaMemcpyHostToDevice));
+            from = tmp.get();
+        }
+        uint8_t* to = dst + r0 * d.row_stride * esz;
+        if (i8)
+            gb::pad_rows_i8_kernel<<<h->num_sms * 8, 256>>>(reinterpret_cast<const int8_t*>(from),
+                                                            reinterpret_cast<int8_t*>(to), nr, d.dim, d.row_stride);
+        else
+            gb::permute_rows_f32_kernel<<<h->num_sms * 8, 256>>>(reinterpret_cast<const float*>(from),
+                                                                 reinterpret_cast<float*>(to), nr, d.dim, d.full,
+                                                                 d.vec_group, d.row_stride);
+        h->launches++;
+        GB_CUDA(cudaGetLastError());
+    }
+    GB_CUDA(cudaDeviceSynchronize());
+    return GRANNE_B200_OK;
+}
+
+// Stages `nrows` dense rows of the handle's kind (host memory, or device memory if `device_src`).
+int stage_dense(Handle* h, const uint8_t* rows, uint64_t nrows, uint32_t dim, bool device_src = false) {
     gb::DeviceIndex& d = h->dev;
     d.dim = dim;
     d.full = dim / 32;
     d.tail = dim % 32;
     d.num_vectors = nrows;
-    if (is_i8) {
+    const bool i8 = d.kind == gb::kAngularI8;
+    if (i8) {
         d.vec_group = 1;
         d.row_stride = (dim + 31u) & ~31u;  // rows start on 32-byte sector boundaries (DistI8)
-        int8_t* dst = nullptr;
-        int rc = dev_alloc(h, &dst, (size_t)nrows * d.row_stride);
-        if (rc) return rc;
-        d.vectors = dst;
-        const uint64_t slab = std::max<uint64_t>(1, (64ull << 20) / dim);
-        int8_t* tmp = nullptr;
-        if (!device_src) GB_CUDA(cudaMalloc(&tmp, (size_t)std::min(slab, std::max<uint64_t>(nrows, 1)) * dim));
-        for (uint64_t r0 = 0; r0 < nrows; r0 += slab) {
-            const uint64_t nr = std::min(slab, nrows - r0);
-            const int8_t* src = reinterpret_cast<const int8_t*>(host_rows) + r0 * dim;  // device memory if device_src
-            if (!device_src) {
-                GB_CUDA(cudaMemcpy(tmp, src, (size_t)nr * dim, cudaMemcpyHostToDevice));
-                src = tmp;
-            }
-            gb::pad_rows_i8_kernel<<<h->num_sms * 8, 256>>>(src, dst + r0 * d.row_stride, nr, dim, d.row_stride);
-            h->launches++;
-            GB_CUDA(cudaGetLastError());
-        }
-        GB_CUDA(cudaDeviceSynchronize());
-        if (tmp) GB_CUDA(cudaFree(tmp));
     } else {
         const uint32_t full = d.full;
         // DistF32<full> reads rows lane-permuted in groups of V = DistF32<full>::V chunks; the other engines read the
         // natural layout (V = 1 permutes nothing)
         d.vec_group = fixed_f32_chunks(d) > 0 ? (full % 4 == 0 ? 4 : (full % 2 == 0 ? 2 : 1)) : 1;
         d.row_stride = (dim + 3u) & ~3u;
-        float* dst = nullptr;
-        int rc = dev_alloc(h, &dst, (size_t)nrows * d.row_stride);
-        if (rc) return rc;
-        d.vectors = dst;
-        const uint64_t slab = std::max<uint64_t>(1, (64ull << 20) / (dim * 4ull));
-        float* tmp = nullptr;
-        if (!device_src) GB_CUDA(cudaMalloc(&tmp, (size_t)std::min(slab, std::max<uint64_t>(nrows, 1)) * dim * 4));
-        const float* src = reinterpret_cast<const float*>(host_rows);  // device memory if device_src
-        for (uint64_t r0 = 0; r0 < nrows; r0 += slab) {
-            const uint64_t nr = std::min(slab, nrows - r0);
-            const float* from = src + r0 * dim;
-            if (!device_src) {
-                GB_CUDA(cudaMemcpy(tmp, from, (size_t)nr * dim * 4, cudaMemcpyHostToDevice));
-                from = tmp;
-            }
-            gb::permute_rows_f32_kernel<<<h->num_sms * 8, 256>>>(from, dst + r0 * d.row_stride, nr, dim, full,
-                                                                 d.vec_group, d.row_stride);
-            h->launches++;
-            GB_CUDA(cudaGetLastError());
-        }
-        GB_CUDA(cudaDeviceSynchronize());
-        if (tmp) GB_CUDA(cudaFree(tmp));
     }
+    Buffer<uint8_t> dst;
+    int rc;
+    if ((rc = dev_alloc(&dst, (size_t)nrows * d.row_stride * (i8 ? 1 : 4)))) return rc;
+    if ((rc = upload_rows(h, rows, nrows, device_src, dst.get()))) return rc;
+    d.vectors = stage(h, std::move(dst));
     return GRANNE_B200_OK;
 }
 
@@ -270,24 +327,23 @@ int stage_elements(Handle* h, int kind, const uint8_t* el, size_t el_len, const 
         for (uint32_t t : se.terms)
             if (t >= ev.num) return fail(GRANNE_B200_ERR_FORMAT, "element refers to a missing embedding id");
         if (ev.dim > 4096) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "embeddings wider than 4096 are unsupported");
-        rc = stage_dense(h, ev.data, ev.num, (uint32_t)ev.dim, false);
+        rc = stage_dense(h, ev.data, ev.num, (uint32_t)ev.dim);
         if (rc) return rc;
         d.num_elements = se.offsets.size() - 1;
-        unsigned long long* doff = nullptr;
-        uint32_t* dterms = nullptr;
-        if ((rc = dev_alloc(h, &doff, se.offsets.size()))) return rc;
-        if ((rc = dev_alloc(h, &dterms, se.terms.size()))) return rc;
-        GB_CUDA(cudaMemcpy(doff, se.offsets.data(), se.offsets.size() * 8, cudaMemcpyHostToDevice));
+        Buffer<unsigned long long> doff;
+        Buffer<uint32_t> dterms;
+        if ((rc = dev_alloc(&doff, se.offsets.size())) || (rc = dev_alloc(&dterms, se.terms.size()))) return rc;
+        GB_CUDA(cudaMemcpy(doff.get(), se.offsets.data(), se.offsets.size() * 8, cudaMemcpyHostToDevice));
         if (!se.terms.empty())
-            GB_CUDA(cudaMemcpy(dterms, se.terms.data(), se.terms.size() * 4, cudaMemcpyHostToDevice));
-        d.sum_offsets = doff;
-        d.sum_terms = dterms;
+            GB_CUDA(cudaMemcpy(dterms.get(), se.terms.data(), se.terms.size() * 4, cudaMemcpyHostToDevice));
+        d.sum_offsets = stage(h, std::move(doff));
+        d.sum_terms = stage(h, std::move(dterms));
     } else {
         gb::DenseView dv;
         const bool i8 = kind == GRANNE_B200_ANGULAR_INT;
         if (!gb::parse_dense(el, el_len, i8 ? 1 : 4, &dv, &err)) return fail(GRANNE_B200_ERR_FORMAT, err);
         if (dv.dim > 16384) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "vectors wider than 16384 are unsupported");
-        rc = stage_dense(h, dv.data, dv.num, (uint32_t)dv.dim, i8);
+        rc = stage_dense(h, dv.data, dv.num, (uint32_t)dv.dim);
         if (rc) return rc;
         d.num_elements = dv.num;
     }
@@ -307,7 +363,7 @@ int stage_device_elements(Handle* h, int kind, const void* d_rows, uint64_t n, u
         return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "elements pointer is not device memory of the requested device");
     }
     h->dev.kind = kind;
-    int rc = stage_dense(h, static_cast<const uint8_t*>(d_rows), n, dim, kind == GRANNE_B200_ANGULAR_INT, true);
+    int rc = stage_dense(h, static_cast<const uint8_t*>(d_rows), n, dim, true);
     if (rc) return rc;
     h->dev.num_elements = n;
     return GRANNE_B200_OK;
@@ -329,6 +385,27 @@ void finish_handle(Handle* h) {
     h->slow_vis_slots = (uint32_t)std::min<uint64_t>(want, 16ull << 20);
 }
 
+// Makes a handle on `device` with its elements staged: from a file image (el, emb) or, when `dev_rows` is given, from
+// n_dev x dim_dev rows already in that device's memory.  `guard` is the caller's, declared before whatever will own
+// the handle: it makes the device current here and keeps it current while the caller finishes the handle, so that
+// every error path frees the handle's memory on its device.
+int new_handle(DeviceGuard* guard, int device, int kind, const uint8_t* el, size_t el_len, const uint8_t* emb,
+               size_t emb_len, const void* dev_rows, uint64_t n_dev, uint32_t dim_dev, std::unique_ptr<Handle>* out) {
+    int rc = dev_rows ? GRANNE_B200_OK : check_open_args(el, kind, emb);
+    if (rc) return rc;
+    int num_sms = 0;
+    size_t smem_optin = 0;
+    if ((rc = check_device(device, &num_sms, &smem_optin))) return rc;
+    GB_CUDA(guard->enter(device));
+    out->reset(new Handle());
+    Handle* h = out->get();
+    h->device = device;
+    h->num_sms = num_sms;
+    h->smem_optin = smem_optin;
+    if (dev_rows) return stage_device_elements(h, kind, dev_rows, n_dev, dim_dev);
+    return stage_elements(h, kind, el, el_len, emb, emb_len);
+}
+
 // `dev_rows` != nullptr: the element container is given as device-resident rows (n_dev x dim_dev) instead of a file image
 int open_impl(const uint8_t* index_bytes, size_t index_len, int kind, const uint8_t* el, size_t el_len,
               const uint8_t* emb, size_t emb_len, int device, Handle** out, const void* dev_rows = nullptr,
@@ -336,35 +413,25 @@ int open_impl(const uint8_t* index_bytes, size_t index_len, int kind, const uint
     if (!out) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "out handle pointer is null");
     *out = nullptr;
     if (!index_bytes) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "index buffer is null");
-    int rc = dev_rows ? GRANNE_B200_OK : check_open_args(el, kind, emb);
+    DeviceGuard guard;
+    std::unique_ptr<Handle> h;
+    int rc = new_handle(&guard, device, kind, el, el_len, emb, emb_len, dev_rows, n_dev, dim_dev, &h);
     if (rc) return rc;
-
-    std::unique_ptr<Handle> h(new Handle());
-    rc = check_device(device, &h->num_sms, &h->smem_optin);
-    if (rc) return rc;
-    h->device = device;
-    GB_DEVICE(device);
 
     std::string err;
     gb::HostGraph graph;
     if (!gb::parse_index(index_bytes, index_len, &graph, &err)) return fail(GRANNE_B200_ERR_FORMAT, err);
     if (graph.layers.size() > (size_t)gb::kMaxLayers) return fail(GRANNE_B200_ERR_FORMAT, "too many layers");
-    if (dev_rows)
-        rc = stage_device_elements(h.get(), kind, dev_rows, n_dev, dim_dev);
-    else
-        rc = stage_elements(h.get(), kind, el, el_len, emb, emb_len);
-    if (rc) return rc;
-
     gb::DeviceIndex& d = h->dev;
     d.num_layers = (int)graph.layers.size();
     for (int l = 0; l < d.num_layers; ++l) {
         const gb::HostLayer& L = graph.layers[l];
         if (L.num_nodes > d.num_elements)
             return fail(GRANNE_B200_ERR_FORMAT, "index refers to more elements than the container holds");
-        uint32_t* rows = nullptr;
-        if ((rc = dev_alloc(h.get(), &rows, L.rows.size()))) return rc;
-        if (!L.rows.empty()) GB_CUDA(cudaMemcpy(rows, L.rows.data(), L.rows.size() * 4, cudaMemcpyHostToDevice));
-        d.layer_rows[l] = rows;
+        Buffer<uint32_t> rows;
+        if ((rc = dev_alloc(&rows, L.rows.size()))) return rc;
+        if (!L.rows.empty()) GB_CUDA(cudaMemcpy(rows.get(), L.rows.data(), L.rows.size() * 4, cudaMemcpyHostToDevice));
+        d.layer_rows[l] = stage(h.get(), std::move(rows));
         d.layer_width[l] = L.width;
         d.layer_len[l] = L.num_nodes;
         h->layer_max_degree.push_back(L.max_degree);
@@ -518,23 +585,15 @@ int launch_kernels(Handle* h, Workspace* w, gb::SearchArgs a, const LaunchPlan& 
     const unsigned grid = (unsigned)std::min<unsigned long long>(a.nq, slots);
     if (R > 0) {
         // per-CTA visited tables (global memory, L2 resident); sized for a full wave so later calls reuse it
-        const size_t need = (size_t)slots * plan.vis_slots;
-        if (need > w->vis_cap) {
-            GB_CUDA(cudaStreamSynchronize(stream));
-            cudaFree(w->d_vis);
-            w->d_vis = nullptr;
-            w->vis_cap = 0;
-            GB_CUDA(cudaMalloc(&w->d_vis, need * sizeof(uint32_t)));
-            w->vis_cap = need;
-        }
-        a.vis_global = w->d_vis;
+        if ((rc = w->d_vis.grow((size_t)slots * plan.vis_slots, stream))) return rc;
+        a.vis_global = w->d_vis.get();
     }
     const bool have_retry = R > 0 && RR > 0;
     a.pass = 0;
     a.slow_pass = 0;
     a.final_pass = 0;
     a.gate_in = nullptr;
-    a.gate_out = w->d_counters + 3;
+    a.gate_out = w->d_counters.get() + 3;
     kern<<<grid, 32, plan.smem, stream>>>(dv, a);
     h->launches++;
     GB_CUDA(cudaGetLastError());
@@ -544,22 +603,14 @@ int launch_kernels(Handle* h, Workspace* w, gb::SearchArgs a, const LaunchPlan& 
         // uniform test distribution before the table scale has adapted) never funnels through the 4-CTA slow pass
         gb::SearchArgs r = a;
         r.pass = 1;
-        r.work_counter = w->d_counters + 1;
-        r.gate_in = w->d_counters + 3;
-        r.gate_out = w->d_counters + 4;
+        r.work_counter = w->d_counters.get() + 1;
+        r.gate_in = w->d_counters.get() + 3;
+        r.gate_out = w->d_counters.get() + 4;
         r.vis_slots = std::max(plan.vis_slots, plan.vis_retry);
         r.vis_slots_upper = plan.vis_upper;
         const unsigned rgrid = (unsigned)std::min<unsigned long long>(a.nq, (unsigned long long)h->num_sms * 4);
-        const size_t need = (size_t)h->num_sms * 4 * r.vis_slots;
-        if (need > w->vis_retry_cap) {
-            GB_CUDA(cudaStreamSynchronize(stream));
-            cudaFree(w->d_vis_retry);
-            w->d_vis_retry = nullptr;
-            w->vis_retry_cap = 0;
-            GB_CUDA(cudaMalloc(&w->d_vis_retry, need * sizeof(uint32_t)));
-            w->vis_retry_cap = need;
-        }
-        r.vis_global = w->d_vis_retry;
+        if ((rc = w->d_vis_retry.grow((size_t)h->num_sms * 4 * r.vis_slots, stream))) return rc;
+        r.vis_global = w->d_vis_retry.get();
         const size_t rsmem = plan.base_smem + gb::fast_list_bytes(RR > 0 ? RR : 1);
         retry<<<rgrid, 32, rsmem, stream>>>(dv, r);
         h->launches++;
@@ -570,8 +621,8 @@ int launch_kernels(Handle* h, Workspace* w, gb::SearchArgs a, const LaunchPlan& 
     s.pass = 2;
     s.slow_pass = 1;
     s.final_pass = 1;
-    s.work_counter = w->d_counters + 2;
-    s.gate_in = w->d_counters + (have_retry ? 4 : 3);
+    s.work_counter = w->d_counters.get() + 2;
+    s.gate_in = w->d_counters.get() + (have_retry ? 4 : 3);
     s.gate_out = nullptr;
     slow<<<h->slow_ctas, 32, plan.base_smem, stream>>>(dv, s);
     h->launches++;
@@ -601,90 +652,45 @@ struct SearchLaunch {
 };
 
 // ---- workspace pool -----------------------------------------------------------------------------------------------
-int ws_acquire(Handle* h, Workspace** out) {
+int ws_acquire(Handle* h, std::unique_ptr<Workspace>* out) {
     {
         std::lock_guard<std::mutex> g(h->pool_mu);
         if (!h->pool.empty()) {
-            *out = h->pool.back().release();
+            *out = std::move(h->pool.back());
             h->pool.pop_back();
             return GRANNE_B200_OK;
         }
     }
     std::unique_ptr<Workspace> w(new Workspace());
-    GB_CUDA(cudaStreamCreateWithFlags(&w->stream, cudaStreamNonBlocking));
-    GB_CUDA(cudaMalloc(&w->d_counters, 64));
-    w->d_error = reinterpret_cast<int*>(w->d_counters + 8);
-    GB_CUDA(cudaMalloc(&w->d_retried, 8));
-    GB_CUDA(cudaMemset(w->d_retried, 0, 8));
-    GB_CUDA(cudaMallocHost(&w->h_retried, 8));
-    *w->h_retried = 0;
-    GB_CUDA(cudaMalloc(&w->d_slow_list, (size_t)h->slow_ctas * h->slow_list_cap * 8));
-    w->slow_vis_cap = (size_t)h->slow_ctas * h->slow_vis_slots;
-    GB_CUDA(cudaMalloc(&w->d_slow_vis, w->slow_vis_cap * 4));
-    *out = w.release();
+    cudaStream_t s = nullptr;
+    GB_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+    w->stream.reset(s);
+    int rc;
+    if ((rc = w->d_counters.grow(16, s))) return rc;
+    w->d_error = reinterpret_cast<int*>(w->d_counters.get() + 8);
+    if ((rc = w->d_retried.grow(1, s))) return rc;
+    GB_CUDA(cudaMemset(w->d_retried.get(), 0, 8));
+    if ((rc = w->h_retried.grow(1, s))) return rc;
+    *w->h_retried.get() = 0;
+    if ((rc = w->d_slow_list.grow((size_t)h->slow_ctas * h->slow_list_cap, s))) return rc;
+    if ((rc = w->d_slow_vis.grow((size_t)h->slow_ctas * h->slow_vis_slots, s))) return rc;
+    *out = std::move(w);
     return GRANNE_B200_OK;
 }
-void ws_release(Handle* h, Workspace* w) {
+void ws_release(Handle* h, std::unique_ptr<Workspace> w) {
     std::lock_guard<std::mutex> g(h->pool_mu);
-    h->pool.emplace_back(w);
-}
-void ws_destroy(Workspace* w) {
-    if (!w) return;
-    cudaFree(w->d_queries);
-    cudaFree(w->d_ids);  // ids | dists | counts are one block
-    cudaFree(w->d_stats);
-    cudaFree(w->d_status);
-    cudaFree(w->d_counters);  // d_error lives inside this block
-    cudaFree(w->d_retried);
-    if (w->h_retried) cudaFreeHost(w->h_retried);
-    cudaFree(w->d_vis_retry);
-    cudaFree(w->d_slow_list);
-    cudaFree(w->d_slow_vis);
-    cudaFree(w->d_vis);
-    if (w->h_pinned) cudaFreeHost(w->h_pinned);
-    if (w->stream) cudaStreamDestroy(w->stream);
+    h->pool.push_back(std::move(w));
 }
 
 int ws_reserve(Workspace* w, size_t query_bytes, size_t nq, size_t k) {
-    if (query_bytes > w->queries_cap) {
-        cudaFree(w->d_queries);
-        w->d_queries = nullptr;
-        w->queries_cap = 0;
-        GB_CUDA(cudaMalloc(&w->d_queries, query_bytes));
-        w->queries_cap = query_bytes;
-    }
-    if (nq * k > w->out_cap_q * w->out_cap_k || nq > w->out_cap_q) {
-        cudaFree(w->d_ids);  // one block: ids | dists | counts, so that one copy brings a whole result back
-        cudaFree(w->d_stats);
-        w->d_ids = nullptr, w->d_dists = nullptr, w->d_counts = nullptr, w->d_stats = nullptr;
-        w->out_cap_q = w->out_cap_k = 0;
-        GB_CUDA(cudaMalloc(&w->d_ids, (2 * std::max<size_t>(nq * k, 1) + std::max<size_t>(nq, 1)) * 4));
-        GB_CUDA(cudaMalloc(&w->d_stats, std::max<size_t>(nq, 1) * 4 * 8));
-        w->out_cap_q = nq;
-        w->out_cap_k = k;
-    }
-    w->d_dists = reinterpret_cast<float*>(w->d_ids + nq * k);  // packed for THIS call's nq x k
-    w->d_counts = w->d_ids + 2 * nq * k;
-    const size_t pinned = query_bytes + nq * k * 8 + nq * 4 + nq * 32 + 128;
-    if (pinned > w->pinned_cap) {
-        if (w->h_pinned) cudaFreeHost(w->h_pinned);
-        w->h_pinned = nullptr;
-        w->pinned_cap = 0;
-        GB_CUDA(cudaMallocHost(&w->h_pinned, pinned));
-        w->pinned_cap = pinned;
-    }
-    return GRANNE_B200_OK;
-}
-
-int ws_reserve_status(Workspace* w, size_t nq) {
-    if (nq > w->status_cap) {
-        cudaFree(w->d_status);
-        w->d_status = nullptr;
-        w->status_cap = 0;
-        GB_CUDA(cudaMalloc(&w->d_status, std::max<size_t>(nq, 1) * sizeof(int)));
-        w->status_cap = nq;
-    }
-    return GRANNE_B200_OK;
+    cudaStream_t s = w->stream.get();
+    int rc;
+    if ((rc = w->d_queries.grow(query_bytes, s)) || (rc = w->d_ids.grow(2 * nq * k + nq, s)) ||
+        (rc = w->d_stats.grow(nq * 4, s)))
+        return rc;
+    w->d_dists = reinterpret_cast<float*>(w->d_ids.get() + nq * k);
+    w->d_counts = w->d_ids.get() + 2 * nq * k;
+    return w->h_pinned.grow(query_bytes + nq * k * 8 + nq * 4 + nq * 32 + 128, s);
 }
 
 int validate_search(const Handle* h, const void* q, size_t nq, int fmt, uint32_t max_search, uint32_t k,
@@ -708,22 +714,15 @@ int enqueue_search(Handle* h, Workspace* w, const void* d_queries, size_t nq, in
     const LaunchPlan plan = make_plan(h, max_search);
     if (plan.smem == 0 || max_search + 64 > h->slow_list_cap)
         return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "max_search exceeds the supported maximum (about 27000)");
-    int rc = ws_reserve_status(w, nq);
+    int rc = w->d_status.grow(nq, stream);
     if (rc) return rc;
     // the slow-path visited tables follow the index size (a builder's index grows after its workspace was made)
-    if ((size_t)h->slow_ctas * h->slow_vis_slots > w->slow_vis_cap) {
-        GB_CUDA(cudaStreamSynchronize(stream));
-        cudaFree(w->d_slow_vis);
-        w->d_slow_vis = nullptr;
-        w->slow_vis_cap = 0;
-        GB_CUDA(cudaMalloc(&w->d_slow_vis, (size_t)h->slow_ctas * h->slow_vis_slots * 4));
-        w->slow_vis_cap = (size_t)h->slow_ctas * h->slow_vis_slots;
-    }
+    if ((rc = w->d_slow_vis.grow((size_t)h->slow_ctas * h->slow_vis_slots, stream))) return rc;
     // Adapt the visited-table scale to the data: more than 1% of the recent queries needed the retry pass -> double
     // it (read from the pinned mirror of the device counter, i.e. without synchronising; it lags by a call or two).
     w->total_queries += nq;
     {
-        const unsigned long long retried = *reinterpret_cast<volatile unsigned long long*>(w->h_retried);
+        const unsigned long long retried = *reinterpret_cast<volatile unsigned long long*>(w->h_retried.get());
         const unsigned long long dq = w->total_queries - w->seen_total, dr = retried - w->seen_retried;
         if (dq >= 2048) {
             if (dr * 100 > dq) {
@@ -738,7 +737,7 @@ int enqueue_search(Handle* h, Workspace* w, const void* d_queries, size_t nq, in
     }
     // one memset per call: the work counters / gates of the three passes (and the error word of a host-API call);
     // the per-query status words need no reset: the fast pass writes every one of them
-    GB_CUDA(cudaMemsetAsync(w->d_counters, 0, reset_error ? 64 : 32, stream));
+    GB_CUDA(cudaMemsetAsync(w->d_counters.get(), 0, reset_error ? 64 : 32, stream));
     gb::SearchArgs a{};
     a.queries = d_queries;
     a.query_format = fmt;
@@ -752,12 +751,12 @@ int enqueue_search(Handle* h, Workspace* w, const void* d_queries, size_t nq, in
     a.out_dists = d_dists;
     a.out_counts = d_counts;
     a.out_stats = d_stats;
-    a.query_status = w->d_status;
-    a.work_counter = w->d_counters;
-    a.retried = w->d_retried;
+    a.query_status = w->d_status.get();
+    a.work_counter = w->d_counters.get();
+    a.retried = w->d_retried.get();
     a.error_flag = w->d_error;
-    a.slow_list = w->d_slow_list;
-    a.slow_visited = w->d_slow_vis;
+    a.slow_list = w->d_slow_list.get();
+    a.slow_visited = w->d_slow_vis.get();
     a.slow_list_cap = h->slow_list_cap;
     a.slow_vis_slots = h->slow_vis_slots;
     a.pass = a.slow_pass = a.final_pass = 0;
@@ -767,7 +766,7 @@ int enqueue_search(Handle* h, Workspace* w, const void* d_queries, size_t nq, in
         a.pg.my_rank = pg->my_rank;
         a.pg.row_offset = pg->row_offset;
         a.pg.seq = pg->seq;
-        a.pg.done_counter = w->d_counters + 5;
+        a.pg.done_counter = w->d_counters.get() + 5;
         for (uint32_t p = 0; p < pg->n_peers; ++p) {
             a.pg.ids[p] = static_cast<uint32_t*>(pg->ids[p]);
             a.pg.dists[p] = static_cast<float*>(pg->dists[p]);
@@ -781,7 +780,7 @@ int enqueue_search(Handle* h, Workspace* w, const void* d_queries, size_t nq, in
     const gb::DeviceIndex& dv = view ? *view : h->dev;
     rc = DistDispatch::call(dv, SearchLaunch{h, w, a, plan, stream, dv});
     if (rc) return rc;
-    GB_CUDA(cudaMemcpyAsync(w->h_retried, w->d_retried, 8, cudaMemcpyDeviceToHost, stream));
+    GB_CUDA(cudaMemcpyAsync(w->h_retried.get(), w->d_retried.get(), 8, cudaMemcpyDeviceToHost, stream));
     return GRANNE_B200_OK;
 }
 
@@ -842,44 +841,19 @@ struct granne_b200_builder {
     granne_b200_build_config cfg{};
     uint32_t stride = 0;  // physical row stride (node_width rounded up to 8)
     std::vector<std::shared_ptr<void>> layer_mem;
-    Workspace* ws = nullptr;
+    std::unique_ptr<Workspace> ws;
     // batch scratch
-    uint32_t* d_ids = nullptr;
-    uint32_t* d_cand_ids = nullptr;
-    float* d_cand_d = nullptr;
-    uint32_t* d_cand_cnt = nullptr;
-    int* d_locks = nullptr;
-    unsigned int* d_counter = nullptr;
-    size_t batch_cap = 0, cand_cap = 0, locks_cap = 0;
+    Buffer<uint32_t> d_ids;
+    Buffer<uint32_t> d_cand_ids;
+    Buffer<float> d_cand_d;
+    Buffer<uint32_t> d_cand_cnt;
+    Buffer<int> d_locks;
+    Buffer<unsigned int> d_counter;
 };
 
 namespace {
 
 using Builder = granne_b200_builder;
-
-int builder_reserve(Builder* b, size_t batch, size_t ef, size_t nodes) {
-    if (batch > b->batch_cap || ef > b->cand_cap) {
-        cudaFree(b->d_ids);
-        cudaFree(b->d_cand_ids);
-        cudaFree(b->d_cand_d);
-        cudaFree(b->d_cand_cnt);
-        b->d_ids = nullptr, b->d_cand_ids = nullptr, b->d_cand_d = nullptr, b->d_cand_cnt = nullptr;
-        b->batch_cap = std::max(batch, b->batch_cap);
-        b->cand_cap = std::max(ef, b->cand_cap);
-        GB_CUDA(cudaMalloc(&b->d_ids, b->batch_cap * 4));
-        GB_CUDA(cudaMalloc(&b->d_cand_ids, b->batch_cap * b->cand_cap * 4));
-        GB_CUDA(cudaMalloc(&b->d_cand_d, b->batch_cap * b->cand_cap * 4));
-        GB_CUDA(cudaMalloc(&b->d_cand_cnt, b->batch_cap * 4));
-    }
-    if (nodes > b->locks_cap) {
-        cudaFree(b->d_locks);
-        b->d_locks = nullptr;
-        GB_CUDA(cudaMalloc(&b->d_locks, nodes * sizeof(int)));
-        b->locks_cap = nodes;
-    }
-    if (!b->d_counter) GB_CUDA(cudaMalloc(&b->d_counter, 16));
-    return GRANNE_B200_OK;
-}
 
 // index_elements (:716-802) for the layer at dev.layer_rows[num_layers-1]
 int builder_index_elements(Builder* b, uint32_t layer_m, uint32_t ef, uint64_t already, uint64_t num, bool reinsert) {
@@ -887,7 +861,7 @@ int builder_index_elements(Builder* b, uint32_t layer_m, uint32_t ef, uint64_t a
     gb::DeviceIndex& d = h->dev;
     const int cur = d.num_layers - 1;
     uint32_t* rows = const_cast<uint32_t*>(d.layer_rows[cur]);
-    cudaStream_t stream = b->ws->stream;
+    cudaStream_t stream = b->ws->stream.get();
     const LaunchPlan plan = make_plan(h, ef);
     if (plan.smem == 0) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "max_search too large");
     const uint64_t first = reinsert ? 0 : already;
@@ -902,9 +876,12 @@ int builder_index_elements(Builder* b, uint32_t layer_m, uint32_t ef, uint64_t a
     uint64_t link_warps = (uint64_t)h->num_sms * 8;
     if (const char* e = std::getenv("GRANNE_B200_BUILD_LINK_WARPS"))
         link_warps = std::min<uint64_t>(link_warps, (uint64_t)std::max(1, std::atoi(e)));
-    int rc = builder_reserve(b, max_batch, ef, num);
-    if (rc) return rc;
-    GB_CUDA(cudaMemsetAsync(b->d_locks, 0, num * sizeof(int), stream));
+    int rc;
+    if ((rc = b->d_ids.grow(max_batch, stream)) || (rc = b->d_cand_ids.grow(max_batch * ef, stream)) ||
+        (rc = b->d_cand_d.grow(max_batch * ef, stream)) || (rc = b->d_cand_cnt.grow(max_batch, stream)) ||
+        (rc = b->d_locks.grow(num, stream)) || (rc = b->d_counter.grow(4, stream)))
+        return rc;
+    GB_CUDA(cudaMemsetAsync(b->d_locks.get(), 0, num * sizeof(int), stream));
     const size_t link_smem = plan.base_smem + gb::link_scratch_bytes(gb::link_cand_cap(ef, b->cfg.num_neighbors),
                                                                       b->cfg.num_neighbors);
     uint64_t pos = 0;
@@ -913,36 +890,37 @@ int builder_index_elements(Builder* b, uint32_t layer_m, uint32_t ef, uint64_t a
         const uint64_t present = reinsert ? num : first + pos;
         const uint64_t bsz = std::min<uint64_t>(std::min<uint64_t>(max_batch, std::max<uint64_t>(1, present / 16)), total - pos);
         const uint32_t start = reinsert ? (uint32_t)(num - 1 - pos) : (uint32_t)(first + pos);
-        gb::iota_kernel<<<(unsigned)((bsz + 255) / 256), 256, 0, stream>>>(b->d_ids, (uint32_t)bsz, start, reinsert ? -1 : 1);
+        gb::iota_kernel<<<(unsigned)((bsz + 255) / 256), 256, 0, stream>>>(b->d_ids.get(), (uint32_t)bsz, start,
+                                                                            reinsert ? -1 : 1);
         h->launches++;
         // candidates = search_for_neighbors(layer, prev_layers.search(e,1,1), e, max_search) (:819-820)
-        rc = enqueue_search(h, b->ws, b->d_ids, bsz, gb::kQueryById, ef, ef, b->d_cand_ids, b->d_cand_d, b->d_cand_cnt,
-                            nullptr, stream, false);
+        rc = enqueue_search(h, b->ws.get(), b->d_ids.get(), bsz, gb::kQueryById, ef, ef, b->d_cand_ids.get(),
+                            b->d_cand_d.get(), b->d_cand_cnt.get(), nullptr, stream, false);
         if (rc) return rc;
-        GB_CUDA(cudaMemsetAsync(b->d_counter, 0, 16, stream));
+        GB_CUDA(cudaMemsetAsync(b->d_counter.get(), 0, 16, stream));
         LinkLaunch L{h, {}, link_smem, 0, stream, false};
-        L.a.ids = b->d_ids;
+        L.a.ids = b->d_ids.get();
         L.a.n_batch = (uint32_t)bsz;
-        L.a.cand_ids = b->d_cand_ids;
-        L.a.cand_dists = b->d_cand_d;
-        L.a.cand_counts = b->d_cand_cnt;
+        L.a.cand_ids = b->d_cand_ids.get();
+        L.a.cand_dists = b->d_cand_d.get();
+        L.a.cand_counts = b->d_cand_cnt.get();
         L.a.cand_stride = ef;
         L.a.rows = rows;
         L.a.stride = b->stride;
         L.a.node_width = b->cfg.num_neighbors;
         L.a.max_neighbors = layer_m;
-        L.a.locks = b->d_locks;
+        L.a.locks = b->d_locks.get();
         L.a.stg_rows = plan.stg_rows;
         L.a.stg_row_bytes = plan.stg_row_bytes;
         L.a.tile_rows = plan.tile_rows;
-        L.a.work_counter = b->d_counter;
+        L.a.work_counter = b->d_counter.get();
         L.a.num_nodes = (uint32_t)num;
         L.grid = (unsigned)std::min<uint64_t>(bsz, link_warps);
         if ((rc = DistDispatch::call(d, L))) return rc;
         pos += bsz;
     }
     // limit number of neighbors (:794-797)
-    GB_CUDA(cudaMemsetAsync(b->d_counter, 0, 16, stream));
+    GB_CUDA(cudaMemsetAsync(b->d_counter.get(), 0, 16, stream));
     LinkLaunch P{h, {}, plan.base_smem + gb::link_scratch_bytes(gb::link_cand_cap(0, b->cfg.num_neighbors),
                                                                b->cfg.num_neighbors), 0, stream, true};
     P.a.rows = rows;
@@ -952,7 +930,7 @@ int builder_index_elements(Builder* b, uint32_t layer_m, uint32_t ef, uint64_t a
     P.a.stg_rows = plan.stg_rows;
     P.a.stg_row_bytes = plan.stg_row_bytes;
     P.a.tile_rows = plan.tile_rows;
-    P.a.work_counter = b->d_counter;
+    P.a.work_counter = b->d_counter.get();
     P.a.num_nodes = (uint32_t)num;
     P.grid = (unsigned)std::min<uint64_t>(num, (uint64_t)h->num_sms * 8);
     if ((rc = DistDispatch::call(d, P))) return rc;
@@ -979,8 +957,8 @@ int builder_index_last_layer(Builder* b, uint64_t max_num_elements) {
     // the layer grows: fresh allocation (snapshots handed out by get_index keep the old one alive)
     uint32_t* grown = nullptr;
     GB_CUDA(cudaMalloc(&grown, std::max<size_t>((size_t)num * b->stride * 4, 16)));
-    std::shared_ptr<void> mem(grown, [](void* q) { cudaFree(q); });
-    cudaStream_t stream = b->ws->stream;
+    std::shared_ptr<void> mem(grown, DeviceFree{});
+    cudaStream_t stream = b->ws->stream.get();
     gb::fill_u32_kernel<<<h->num_sms * 4, 256, 0, stream>>>(grown, (unsigned long long)num * b->stride, gb::kUnusedId);
     h->launches++;
     if (have) GB_CUDA(cudaMemcpyAsync(grown, d.layer_rows[cur], (size_t)have * b->stride * 4, cudaMemcpyDeviceToDevice, stream));
@@ -1041,30 +1019,26 @@ const char* granne_b200_last_error(void) { return g_last_error.c_str(); }
 int granne_b200_open(const void* index_bytes, size_t index_len, int element_kind, const void* elements_bytes,
                      size_t elements_len, const void* embeddings_bytes, size_t embeddings_len, int device,
                      granne_b200_index** out) {
-    try {
+    return guarded([&] {
         return open_impl(static_cast<const uint8_t*>(index_bytes), index_len, element_kind,
                          static_cast<const uint8_t*>(elements_bytes), elements_len,
                          static_cast<const uint8_t*>(embeddings_bytes), embeddings_len, device, out);
-    } catch (const std::exception& e) {
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, std::string("exception: ") + e.what());
-    }
+    });
 }
 
 int granne_b200_open_device_elements(const void* index_bytes, size_t index_len, int element_kind,
                                      const void* d_element_rows, uint64_t num_elements, uint32_t dim, int device,
                                      granne_b200_index** out) {
-    try {
+    return guarded([&] {
         if (!d_element_rows) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "elements pointer is null");
         return open_impl(static_cast<const uint8_t*>(index_bytes), index_len, element_kind, nullptr, 0, nullptr, 0,
                          device, out, d_element_rows, num_elements, dim);
-    } catch (const std::exception& e) {
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, std::string("exception: ") + e.what());
-    }
+    });
 }
 
 int granne_b200_open_files(const char* index_path, int element_kind, const char* elements_path,
                            const char* embeddings_path, int device, granne_b200_index** out) {
-    try {
+    return guarded([&] {
         std::vector<uint8_t> ib, eb, mb;
         int rc;
         if ((rc = read_file(index_path, &ib))) return rc;
@@ -1076,20 +1050,13 @@ int granne_b200_open_files(const char* index_path, int element_kind, const char*
         }
         return open_impl(ib.data(), ib.size(), element_kind, eb.data(), eb.size(), mb.empty() ? nullptr : mb.data(),
                          mb.size(), device, out);
-    } catch (const std::exception& e) {
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, std::string("exception: ") + e.what());
-    }
+    });
 }
 
 void granne_b200_close(granne_b200_index* h) {
     if (!h) return;
     DeviceGuard guard(h->device);
     cudaDeviceSynchronize();
-    for (auto& w : h->pool) ws_destroy(w.get());
-    h->pool.clear();
-    for (auto& kv : h->stream_ws) ws_destroy(kv.second.get());
-    h->stream_ws.clear();
-    h->allocations.clear();
     delete h;
 }
 
@@ -1110,31 +1077,34 @@ int granne_b200_get_neighbors(const granne_b200_index* h, uint64_t idx, uint64_t
     if (!h || !out_n) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
     if (layer >= (uint64_t)h->dev.num_layers || idx >= h->dev.layer_len[layer])
         return fail(GRANNE_B200_ERR_OUT_OF_RANGE, "node or layer out of range");
-    GB_DEVICE(h->device);
-    const uint32_t w = h->dev.layer_width[layer];
-    std::vector<uint32_t> row(w);
-    GB_CUDA(cudaMemcpy(row.data(), h->dev.layer_rows[layer] + idx * w, w * 4, cudaMemcpyDeviceToHost));
-    size_t n = 0;
-    while (n < w && row[n] != gb::kUnusedId) ++n;
-    *out_n = n;
-    for (size_t i = 0; i < n && i < cap && out; ++i) out[i] = row[i];
-    return GRANNE_B200_OK;
+    return guarded([&] {
+        GB_DEVICE(h->device);
+        const uint32_t w = h->dev.layer_width[layer];
+        std::vector<uint32_t> row(w);
+        GB_CUDA(cudaMemcpy(row.data(), h->dev.layer_rows[layer] + idx * w, w * 4, cudaMemcpyDeviceToHost));
+        size_t n = 0;
+        while (n < w && row[n] != gb::kUnusedId) ++n;
+        *out_n = n;
+        for (size_t i = 0; i < n && i < cap && out; ++i) out[i] = row[i];
+        return GRANNE_B200_OK;
+    });
 }
 
 int granne_b200_get_element(const granne_b200_index* hc, uint64_t idx, void* out) {
     granne_b200_index* h = const_cast<granne_b200_index*>(hc);
     if (!h || !out) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
     if (idx >= h->dev.num_elements) return fail(GRANNE_B200_ERR_OUT_OF_RANGE, "element index out of range");
-    GB_DEVICE(h->device);
-    const size_t bytes = h->dev.kind == gb::kAngularI8 ? h->dev.dim : (size_t)h->dev.dim * 4;
-    void* d = nullptr;
-    GB_CUDA(cudaMalloc(&d, bytes));
-    gb::get_element_kernel<<<1, 32>>>(h->dev, idx, d);
-    h->launches++;
-    cudaError_t e = cudaMemcpy(out, d, bytes, cudaMemcpyDeviceToHost);
-    cudaFree(d);
-    GB_CUDA(e);
-    return GRANNE_B200_OK;
+    return guarded([&] {
+        GB_DEVICE(h->device);
+        const size_t bytes = h->dev.kind == gb::kAngularI8 ? h->dev.dim : (size_t)h->dev.dim * 4;
+        Buffer<uint8_t> d;
+        int rc = d.grow(bytes, nullptr);
+        if (rc) return rc;
+        gb::get_element_kernel<<<1, 32>>>(h->dev, idx, d.get());
+        h->launches++;
+        GB_CUDA(cudaMemcpy(out, d.get(), bytes, cudaMemcpyDeviceToHost));
+        return GRANNE_B200_OK;
+    });
 }
 
 static int search_device_impl(granne_b200_index* h, const void* d_queries, size_t nq, int query_format,
@@ -1152,37 +1122,34 @@ static int search_device_impl(granne_b200_index* h, const void* d_queries, size_
                 return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "peer gather: null peer pointer");
     }
     if (nq == 0) return GRANNE_B200_OK;
-    GB_DEVICE(h->device);
-    cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
-    // One workspace per caller stream: calls on the same stream are serialised by the stream itself, so the status
-    // words / slow-path buffers can be reused; the error word stays sticky until granne_b200_stream_status().
-    Workspace* w = nullptr;
-    {
-        std::lock_guard<std::mutex> g(h->pool_mu);
-        auto it = h->stream_ws.find(stream);
-        if (it != h->stream_ws.end()) w = it->second.get();
-    }
-    if (!w) {
-        Workspace* fresh = nullptr;
-        if ((rc = ws_acquire(h, &fresh))) return rc;
-        cudaError_t e = cudaMemset(fresh->d_error, 0, 4 * sizeof(int));
-        bool lost_race = false;
+    return guarded([&] {
+        GB_DEVICE(h->device);
+        cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+        // One workspace per caller stream: calls on the same stream are serialised by the stream itself, so the
+        // status words / slow-path buffers can be reused; the error word stays sticky until
+        // granne_b200_stream_status().
+        Workspace* w = nullptr;
         {
             std::lock_guard<std::mutex> g(h->pool_mu);
-            auto it = h->stream_ws.find(stream);  // two threads may meet here on the first use of a stream
-            if (it != h->stream_ws.end()) {
-                w = it->second.get();
-                lost_race = true;
-            } else {
-                h->stream_ws[stream] = std::unique_ptr<Workspace>(fresh);
-                w = fresh;
-            }
+            auto it = h->stream_ws.find(stream);
+            if (it != h->stream_ws.end()) w = it->second.get();
         }
-        if (lost_race) ws_release(h, fresh);  // back to the pool, nothing is leaked
-        GB_CUDA(e);
-    }
-    return enqueue_search(h, w, d_queries, nq, query_format, max_search, num_neighbors, d_out_ids, d_out_dists,
-                          d_out_counts, reinterpret_cast<unsigned long long*>(d_out_stats), stream, false, pg);
+        if (!w) {
+            std::unique_ptr<Workspace> fresh;
+            if ((rc = ws_acquire(h, &fresh))) return rc;
+            cudaError_t e = cudaMemset(fresh->d_error, 0, 4 * sizeof(int));
+            {
+                std::lock_guard<std::mutex> g(h->pool_mu);
+                auto it = h->stream_ws.find(stream);  // two threads may meet here on the first use of a stream
+                if (it == h->stream_ws.end()) it = h->stream_ws.emplace(stream, std::move(fresh)).first;
+                w = it->second.get();
+            }
+            if (fresh) ws_release(h, std::move(fresh));  // lost that race: back to the pool
+            GB_CUDA(e);
+        }
+        return enqueue_search(h, w, d_queries, nq, query_format, max_search, num_neighbors, d_out_ids, d_out_dists,
+                              d_out_counts, reinterpret_cast<unsigned long long*>(d_out_stats), stream, false, pg);
+    });
 }
 
 int granne_b200_search_batch_device(granne_b200_index* h, const void* d_queries, size_t nq, int query_format,
@@ -1207,37 +1174,40 @@ int granne_b200_search_batch_device_gather(granne_b200_index* h, const void* d_q
 // the stream first); granne_b200_close releases everything anyway.
 int granne_b200_release_stream(granne_b200_index* h, void* cuda_stream) {
     if (!h) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "index handle is null");
-    GB_DEVICE(h->device);
-    cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
-    std::unique_ptr<Workspace> w;
-    {
-        std::lock_guard<std::mutex> g(h->pool_mu);
-        auto it = h->stream_ws.find(stream);
-        if (it == h->stream_ws.end()) return GRANNE_B200_OK;
-        w = std::move(it->second);
-        h->stream_ws.erase(it);
-    }
-    GB_CUDA(cudaStreamSynchronize(stream));
-    int e[4] = {0, 0, 0, 0};
-    GB_CUDA(cudaMemcpy(e, w->d_error, sizeof(e), cudaMemcpyDeviceToHost));
-    h->sticky_error.fetch_or(e[0]);  // reported by the next granne_b200_stream_status
-    ws_destroy(w.get());
-    return GRANNE_B200_OK;
+    return guarded([&] {
+        GB_DEVICE(h->device);
+        cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+        std::unique_ptr<Workspace> w;
+        {
+            std::lock_guard<std::mutex> g(h->pool_mu);
+            auto it = h->stream_ws.find(stream);
+            if (it == h->stream_ws.end()) return GRANNE_B200_OK;
+            w = std::move(it->second);
+            h->stream_ws.erase(it);
+        }
+        GB_CUDA(cudaStreamSynchronize(stream));
+        int e[4] = {0, 0, 0, 0};
+        GB_CUDA(cudaMemcpy(e, w->d_error, sizeof(e), cudaMemcpyDeviceToHost));
+        h->sticky_error.fetch_or(e[0]);  // reported by the next granne_b200_stream_status
+        return GRANNE_B200_OK;
+    });
 }
 
 int granne_b200_stream_status(granne_b200_index* h) {
     if (!h) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "index handle is null");
-    GB_DEVICE(h->device);
-    GB_CUDA(cudaDeviceSynchronize());
-    int bits = h->sticky_error.exchange(0);
-    std::lock_guard<std::mutex> g(h->pool_mu);
-    for (auto& kv : h->stream_ws) {
-        int e[4] = {0, 0, 0, 0};
-        GB_CUDA(cudaMemcpy(e, kv.second->d_error, sizeof(e), cudaMemcpyDeviceToHost));
-        bits |= e[0];
-        GB_CUDA(cudaMemset(kv.second->d_error, 0, sizeof(e)));
-    }
-    return error_from_bits(bits);
+    return guarded([&] {
+        GB_DEVICE(h->device);
+        GB_CUDA(cudaDeviceSynchronize());
+        int bits = h->sticky_error.exchange(0);
+        std::lock_guard<std::mutex> g(h->pool_mu);
+        for (auto& kv : h->stream_ws) {
+            int e[4] = {0, 0, 0, 0};
+            GB_CUDA(cudaMemcpy(e, kv.second->d_error, sizeof(e), cudaMemcpyDeviceToHost));
+            bits |= e[0];
+            GB_CUDA(cudaMemset(kv.second->d_error, 0, sizeof(e)));
+        }
+        return error_from_bits(bits);
+    });
 }
 
 int granne_b200_search_batch(granne_b200_index* h, const void* queries, size_t nq, int query_format,
@@ -1246,51 +1216,54 @@ int granne_b200_search_batch(granne_b200_index* h, const void* queries, size_t n
     int rc = validate_search(h, queries, nq, query_format, max_search, num_neighbors, out_ids, out_dists);
     if (rc) return rc;
     if (nq == 0) return GRANNE_B200_OK;
-    GB_DEVICE(h->device);
-    const size_t k = num_neighbors;
-    const bool i8q = h->dev.kind == gb::kAngularI8 && query_format == GRANNE_B200_QUERY_ELEMENT;
-    const size_t qbytes = nq * h->dev.dim * (i8q ? 1 : 4);
-    Workspace* w = nullptr;
-    if ((rc = ws_acquire(h, &w))) return rc;
-    struct Releaser {
-        Handle* h;
-        Workspace* w;
-        ~Releaser() { ws_release(h, w); }
-    } rel{h, w};
-    if ((rc = ws_reserve(w, qbytes, nq, k))) return rc;
-    // pinned staging layout: queries | ids | dists | counts | stats | error
-    uint8_t* hp = static_cast<uint8_t*>(w->h_pinned);
-    uint8_t* hq = hp;
-    uint32_t* hids = reinterpret_cast<uint32_t*>(hp + ((qbytes + 15) & ~size_t(15)));
-    float* hd = reinterpret_cast<float*>(hids + nq * k);
-    uint32_t* hc = reinterpret_cast<uint32_t*>(hd + nq * k);
-    int* herr = reinterpret_cast<int*>(hc + nq);
-    unsigned long long* hstats = reinterpret_cast<unsigned long long*>(
-        reinterpret_cast<uint8_t*>(hp) + ((reinterpret_cast<uint8_t*>(herr + 4) - hp + 15) & ~size_t(15)));
-    // (pinned_cap was sized with slack for the alignment above)
-    std::memcpy(hq, queries, qbytes);
-    GB_CUDA(cudaMemcpyAsync(w->d_queries, hq, qbytes, cudaMemcpyHostToDevice, w->stream));
-    rc = enqueue_search(h, w, w->d_queries, nq, query_format, max_search, num_neighbors, w->d_ids, w->d_dists,
-                        w->d_counts, out_stats ? w->d_stats : nullptr, w->stream, true);
-    if (rc) return rc;
-    // one packed copy: ids | dists | counts (device and pinned layouts match), then the 16-byte error word
-    GB_CUDA(cudaMemcpyAsync(hids, w->d_ids, (2 * nq * k + nq) * 4, cudaMemcpyDeviceToHost, w->stream));
-    GB_CUDA(cudaMemcpyAsync(herr, w->d_error, 4 * sizeof(int), cudaMemcpyDeviceToHost, w->stream));
-    if (out_stats) GB_CUDA(cudaMemcpyAsync(hstats, w->d_stats, nq * 32, cudaMemcpyDeviceToHost, w->stream));
-    GB_CUDA(cudaStreamSynchronize(w->stream));
-    if (out_stats) std::memcpy(out_stats, hstats, nq * 32);
-    if (k) {
-        std::memcpy(out_ids, hids, nq * k * 4);
-        std::memcpy(out_dists, hd, nq * k * 4);
-    }
-    if (out_counts) std::memcpy(out_counts, hc, nq * 4);
-    return error_from_bits(herr[0]);
+    return guarded([&] {
+        GB_DEVICE(h->device);
+        const size_t k = num_neighbors;
+        const bool i8q = h->dev.kind == gb::kAngularI8 && query_format == GRANNE_B200_QUERY_ELEMENT;
+        const size_t qbytes = nq * h->dev.dim * (i8q ? 1 : 4);
+        std::unique_ptr<Workspace> ws;
+        if ((rc = ws_acquire(h, &ws))) return rc;
+        Workspace* w = ws.get();
+        const int status = [&] {
+            if ((rc = ws_reserve(w, qbytes, nq, k))) return rc;
+            cudaStream_t stream = w->stream.get();
+            // pinned staging layout: queries | ids | dists | counts | stats | error
+            uint8_t* hp = w->h_pinned.get();
+            uint8_t* hq = hp;
+            uint32_t* hids = reinterpret_cast<uint32_t*>(hp + ((qbytes + 15) & ~size_t(15)));
+            float* hd = reinterpret_cast<float*>(hids + nq * k);
+            uint32_t* hc = reinterpret_cast<uint32_t*>(hd + nq * k);
+            int* herr = reinterpret_cast<int*>(hc + nq);
+            unsigned long long* hstats = reinterpret_cast<unsigned long long*>(
+                reinterpret_cast<uint8_t*>(hp) + ((reinterpret_cast<uint8_t*>(herr + 4) - hp + 15) & ~size_t(15)));
+            // (the pinned buffer was sized with slack for the alignment above)
+            std::memcpy(hq, queries, qbytes);
+            GB_CUDA(cudaMemcpyAsync(w->d_queries.get(), hq, qbytes, cudaMemcpyHostToDevice, stream));
+            rc = enqueue_search(h, w, w->d_queries.get(), nq, query_format, max_search, num_neighbors, w->d_ids.get(),
+                                w->d_dists, w->d_counts, out_stats ? w->d_stats.get() : nullptr, stream, true);
+            if (rc) return rc;
+            // one packed copy: ids | dists | counts (device and pinned layouts match), then the 16-byte error word
+            GB_CUDA(cudaMemcpyAsync(hids, w->d_ids.get(), (2 * nq * k + nq) * 4, cudaMemcpyDeviceToHost, stream));
+            GB_CUDA(cudaMemcpyAsync(herr, w->d_error, 4 * sizeof(int), cudaMemcpyDeviceToHost, stream));
+            if (out_stats) GB_CUDA(cudaMemcpyAsync(hstats, w->d_stats.get(), nq * 32, cudaMemcpyDeviceToHost, stream));
+            GB_CUDA(cudaStreamSynchronize(stream));
+            if (out_stats) std::memcpy(out_stats, hstats, nq * 32);
+            if (k) {
+                std::memcpy(out_ids, hids, nq * k * 4);
+                std::memcpy(out_dists, hd, nq * k * 4);
+            }
+            if (out_counts) std::memcpy(out_counts, hc, nq * 4);
+            return error_from_bits(herr[0]);
+        }();
+        ws_release(h, std::move(ws));  // back to the pool on every path
+        return status;
+    });
 }
 
 int granne_b200_inspect_index(const void* index_bytes, size_t index_len, uint64_t* out_num_layers,
                               uint64_t* out_layer_len, uint32_t* out_max_degree, uint32_t* out_row_width, size_t cap) {
     if (!index_bytes || !out_num_layers) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
-    try {
+    return guarded([&] {
         gb::HostGraph graph;
         std::string err;
         if (!gb::parse_index(static_cast<const uint8_t*>(index_bytes), index_len, &graph, &err))
@@ -1302,15 +1275,13 @@ int granne_b200_inspect_index(const void* index_bytes, size_t index_len, uint64_
             if (out_row_width) out_row_width[l] = graph.layers[l].width;
         }
         return GRANNE_B200_OK;
-    } catch (const std::exception& e) {
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, std::string("exception: ") + e.what());
-    }
+    });
 }
 
 int granne_b200_decode_layer(const void* index_bytes, size_t index_len, uint64_t layer, uint32_t* rows,
                              size_t rows_cap_u32) {
     if (!index_bytes || !rows) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
-    try {
+    return guarded([&] {
         gb::HostGraph graph;
         std::string err;
         if (!gb::parse_index(static_cast<const uint8_t*>(index_bytes), index_len, &graph, &err))
@@ -1320,9 +1291,7 @@ int granne_b200_decode_layer(const void* index_bytes, size_t index_len, uint64_t
         if (L.rows.size() > rows_cap_u32) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "rows buffer too small");
         std::memcpy(rows, L.rows.data(), L.rows.size() * 4);
         return GRANNE_B200_OK;
-    } catch (const std::exception& e) {
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, std::string("exception: ") + e.what());
-    }
+    });
 }
 
 // ---- GranneBuilder ------------------------------------------------------------------------------------------------
@@ -1339,32 +1308,23 @@ void granne_b200_build_config_default(granne_b200_build_config* cfg) {
 static int builder_new_impl(const granne_b200_build_config* cfg, int element_kind, const void* elements_bytes,
                             size_t elements_len, const void* embeddings_bytes, size_t embeddings_len, int device,
                             granne_b200_builder** out, const void* dev_rows, uint64_t n_dev, uint32_t dim_dev) {
-    try {
-        if (!out || !cfg) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
-        *out = nullptr;
-        int rc = dev_rows ? GRANNE_B200_OK : check_open_args(elements_bytes, element_kind, embeddings_bytes);
-        if (rc) return rc;
-        // the on-disk format counts a list's entries in one byte (set_vector.rs:91-99): 255 is the format's limit
-        if (cfg->num_neighbors < 1 || cfg->num_neighbors > 255)
-            return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "num_neighbors must be in 1..255");
-        if (cfg->max_search < 1) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "max_search must be >= 1");
-        if (!(cfg->layer_multiplier > 1.0f))
-            return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "layer_multiplier must be > 1");
+    if (!out || !cfg) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
+    *out = nullptr;
+    // the on-disk format counts a list's entries in one byte (set_vector.rs:91-99): 255 is the format's limit
+    if (cfg->num_neighbors < 1 || cfg->num_neighbors > 255)
+        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "num_neighbors must be in 1..255");
+    if (cfg->max_search < 1) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "max_search must be >= 1");
+    if (!(cfg->layer_multiplier > 1.0f)) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "layer_multiplier must be > 1");
+    return guarded([&] {
+        DeviceGuard guard;
         std::unique_ptr<granne_b200_builder> b(new granne_b200_builder());
         b->cfg = *cfg;
         b->stride = (cfg->num_neighbors + 7u) & ~7u;
-        b->h.reset(new Handle());
+        int rc = new_handle(&guard, device, element_kind, static_cast<const uint8_t*>(elements_bytes), elements_len,
+                            static_cast<const uint8_t*>(embeddings_bytes), embeddings_len, dev_rows, n_dev, dim_dev,
+                            &b->h);
+        if (rc) return rc;
         Handle* h = b->h.get();
-        rc = check_device(device, &h->num_sms, &h->smem_optin);
-        if (rc) return rc;
-        h->device = device;
-        GB_DEVICE(device);
-        if (dev_rows)
-            rc = stage_device_elements(h, element_kind, dev_rows, n_dev, dim_dev);
-        else
-            rc = stage_elements(h, element_kind, static_cast<const uint8_t*>(elements_bytes), elements_len,
-                                static_cast<const uint8_t*>(embeddings_bytes), embeddings_len);
-        if (rc) return rc;
         if (h->dev.num_elements >= 0xFFFFFFFFull)  // assert!(elements.len() < UNUSED) (:420)
             return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "too many elements");
         h->dev.num_layers = 0;
@@ -1373,9 +1333,7 @@ static int builder_new_impl(const granne_b200_build_config* cfg, int element_kin
         GB_CUDA(cudaMemset(b->ws->d_error, 0, 4 * sizeof(int)));
         *out = b.release();
         return GRANNE_B200_OK;
-    } catch (const std::exception& e) {
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, std::string("exception: ") + e.what());
-    }
+    });
 }
 
 int granne_b200_builder_new(const granne_b200_build_config* cfg, int element_kind, const void* elements_bytes,
@@ -1397,7 +1355,7 @@ int granne_b200_builder_new_device_elements(const granne_b200_build_config* cfg,
 // appended to the staged container.  The appended elements are indexed by the next build() / build_partial().
 int granne_b200_builder_append(granne_b200_builder* b, const void* elements_bytes, size_t elements_len) {
     if (!b || !elements_bytes) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
-    try {
+    return guarded([&] {
         Handle* h = b->h.get();
         gb::DeviceIndex& d = h->dev;
         if (d.kind == gb::kSumEmbeddings) {
@@ -1415,27 +1373,28 @@ int granne_b200_builder_append(granne_b200_builder* b, const void* elements_byte
             const uint64_t old_n = d.num_elements, new_n = old_n + add;
             if (new_n >= 0xFFFFFFFFull) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "too many elements");  // :420
             GB_DEVICE(h->device);
-            GB_CUDA(cudaStreamSynchronize(b->ws->stream));
+            GB_CUDA(cudaStreamSynchronize(b->ws->stream.get()));
             unsigned long long old_terms = 0;
             if (old_n)
                 GB_CUDA(cudaMemcpy(&old_terms, d.sum_offsets + old_n, 8, cudaMemcpyDeviceToHost));
             std::vector<unsigned long long> off(add + 1);
             for (uint64_t i = 0; i <= add; ++i) off[i] = old_terms + se.offsets[i];
-            unsigned long long* doff = nullptr;
-            uint32_t* dterms = nullptr;
+            Buffer<unsigned long long> doff;
+            Buffer<uint32_t> dterms;
             int rc;
-            if ((rc = dev_alloc(h, &doff, new_n + 1))) return rc;
-            if ((rc = dev_alloc(h, &dterms, (size_t)old_terms + se.terms.size()))) return rc;
+            if ((rc = dev_alloc(&doff, new_n + 1)) || (rc = dev_alloc(&dterms, (size_t)old_terms + se.terms.size())))
+                return rc;
             if (old_n) {
-                GB_CUDA(cudaMemcpy(doff, d.sum_offsets, (size_t)old_n * 8, cudaMemcpyDeviceToDevice));
-                if (old_terms) GB_CUDA(cudaMemcpy(dterms, d.sum_terms, (size_t)old_terms * 4, cudaMemcpyDeviceToDevice));
+                GB_CUDA(cudaMemcpy(doff.get(), d.sum_offsets, (size_t)old_n * 8, cudaMemcpyDeviceToDevice));
+                if (old_terms)
+                    GB_CUDA(cudaMemcpy(dterms.get(), d.sum_terms, (size_t)old_terms * 4, cudaMemcpyDeviceToDevice));
             }
-            GB_CUDA(cudaMemcpy(doff + old_n, off.data(), (add + 1) * 8, cudaMemcpyHostToDevice));
+            GB_CUDA(cudaMemcpy(doff.get() + old_n, off.data(), (add + 1) * 8, cudaMemcpyHostToDevice));
             if (!se.terms.empty())
-                GB_CUDA(cudaMemcpy(dterms + old_terms, se.terms.data(), se.terms.size() * 4, cudaMemcpyHostToDevice));
-            // (the old arrays stay alive in h->allocations: snapshots handed out by get_index may still read them)
-            d.sum_offsets = doff;
-            d.sum_terms = dterms;
+                GB_CUDA(cudaMemcpy(dterms.get() + old_terms, se.terms.data(), se.terms.size() * 4,
+                                   cudaMemcpyHostToDevice));
+            d.sum_offsets = stage(h, std::move(doff), d.sum_offsets, (size_t)(old_n + 1) * 8);
+            d.sum_terms = stage(h, std::move(dterms), d.sum_terms, (size_t)old_terms * 4);
             d.num_elements = new_n;
             return GRANNE_B200_OK;
         }
@@ -1452,58 +1411,23 @@ int granne_b200_builder_append(granne_b200_builder* b, const void* elements_byte
         const uint64_t old_n = d.num_vectors, new_n = old_n + dv.num;
         if (new_n >= 0xFFFFFFFFull) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "too many elements");  // :420
         GB_DEVICE(h->device);
-        GB_CUDA(cudaStreamSynchronize(b->ws->stream));
+        GB_CUDA(cudaStreamSynchronize(b->ws->stream.get()));
         const size_t row_bytes = (size_t)d.row_stride * esz;
-        uint8_t* dst = nullptr;
-        GB_CUDA(cudaMalloc(&dst, std::max<size_t>((size_t)new_n * row_bytes, 16)));
-        std::shared_ptr<void> owner(dst, [](void* q) { cudaFree(q); });
-        if (old_n) GB_CUDA(cudaMemcpy(dst, d.vectors, (size_t)old_n * row_bytes, cudaMemcpyDeviceToDevice));
-        // new rows: upload in slabs, then the same re-layout kernels as the loader
-        const uint64_t slab = std::max<uint64_t>(1, (64ull << 20) / ((size_t)d.dim * esz));
-        uint8_t* tmp = nullptr;
-        GB_CUDA(cudaMalloc(&tmp, (size_t)std::min<uint64_t>(slab, dv.num) * d.dim * esz));
-        std::shared_ptr<void> tmp_owner(tmp, [](void* q) { cudaFree(q); });
-        for (uint64_t r0 = 0; r0 < dv.num; r0 += slab) {
-            const uint64_t nr = std::min<uint64_t>(slab, dv.num - r0);
-            GB_CUDA(cudaMemcpy(tmp, dv.data + r0 * d.dim * esz, (size_t)nr * d.dim * esz, cudaMemcpyHostToDevice));
-            uint8_t* out_rows = dst + (size_t)(old_n + r0) * row_bytes;
-            if (i8)
-                gb::pad_rows_i8_kernel<<<h->num_sms * 8, 256>>>(reinterpret_cast<const int8_t*>(tmp),
-                                                                reinterpret_cast<int8_t*>(out_rows), nr, d.dim,
-                                                                d.row_stride);
-            else
-                gb::permute_rows_f32_kernel<<<h->num_sms * 8, 256>>>(reinterpret_cast<const float*>(tmp),
-                                                                     reinterpret_cast<float*>(out_rows), nr, d.dim,
-                                                                     d.full, d.vec_group, d.row_stride);
-            h->launches++;
-            GB_CUDA(cudaGetLastError());
-        }
-        GB_CUDA(cudaDeviceSynchronize());
-        // swap the container; snapshots handed out by get_index keep the old buffer alive through their own reference
-        for (auto it = h->allocations.begin(); it != h->allocations.end(); ++it)
-            if (it->get() == d.vectors) {
-                h->device_bytes -= std::min<uint64_t>(h->device_bytes, std::max<size_t>((size_t)old_n * row_bytes, 16));
-                h->allocations.erase(it);
-                break;
-            }
-        h->allocations.push_back(owner);
-        h->device_bytes += std::max<size_t>((size_t)new_n * row_bytes, 16);
-        d.vectors = dst;
+        Buffer<uint8_t> rows;
+        int rc;
+        if ((rc = dev_alloc(&rows, (size_t)new_n * row_bytes))) return rc;
+        if (old_n) GB_CUDA(cudaMemcpy(rows.get(), d.vectors, (size_t)old_n * row_bytes, cudaMemcpyDeviceToDevice));
+        if ((rc = upload_rows(h, dv.data, dv.num, false, rows.get() + (size_t)old_n * row_bytes))) return rc;
+        d.vectors = stage(h, std::move(rows), d.vectors, (size_t)old_n * row_bytes);
         d.num_vectors = new_n;
         d.num_elements = new_n;
         return GRANNE_B200_OK;
-    } catch (const std::exception& e) {
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, std::string("exception: ") + e.what());
-    }
+    });
 }
 
 int granne_b200_builder_build(granne_b200_builder* b, uint64_t num_elements) {
     if (!b) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "builder is null");
-    try {
-        return builder_build_partial(b, num_elements ? num_elements : b->h->dev.num_elements);
-    } catch (const std::exception& e) {
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, std::string("exception: ") + e.what());
-    }
+    return guarded([&] { return builder_build_partial(b, num_elements ? num_elements : b->h->dev.num_elements); });
 }
 
 uint64_t granne_b200_builder_len(const granne_b200_builder* b) { return b ? b->h->index_len : 0; }
@@ -1522,7 +1446,7 @@ int granne_b200_builder_get_neighbors(const granne_b200_builder* b, uint64_t idx
 // Index::write_index (src/index/io.rs:11-70) from the staged fixed-width rows of any handle.
 int granne_b200_write_index(const granne_b200_index* h, void* out, size_t cap, size_t* out_len) {
     if (!h || !out_len) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
-    try {
+    return guarded([&] {
         GB_DEVICE(h->device);
         std::vector<std::vector<uint32_t>> host(h->dev.num_layers);
         std::vector<gb::LayerView> views;
@@ -1541,9 +1465,7 @@ int granne_b200_write_index(const granne_b200_index* h, void* out, size_t cap, s
         if (cap < image.size()) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "output buffer too small");
         std::memcpy(out, image.data(), image.size());
         return GRANNE_B200_OK;
-    } catch (const std::exception& e) {
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, std::string("exception: ") + e.what());
-    }
+    });
 }
 
 int granne_b200_builder_write_index(granne_b200_builder* b, void* out, size_t cap, size_t* out_len) {
@@ -1553,7 +1475,7 @@ int granne_b200_builder_write_index(granne_b200_builder* b, void* out, size_t ca
 
 int granne_b200_builder_get_index(granne_b200_builder* b, granne_b200_index** out) {
     if (!b || !out) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
-    try {
+    return guarded([&] {
         const Handle* src = b->h.get();
         std::unique_ptr<Handle> h(new Handle());
         h->device = src->device;
@@ -1568,25 +1490,13 @@ int granne_b200_builder_get_index(granne_b200_builder* b, granne_b200_index** ou
         finish_handle(h.get());
         *out = h.release();
         return GRANNE_B200_OK;
-    } catch (const std::exception& e) {
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, std::string("exception: ") + e.what());
-    }
+    });
 }
 
 void granne_b200_builder_free(granne_b200_builder* b) {
     if (!b) return;
     DeviceGuard guard(b->h->device);
     cudaDeviceSynchronize();
-    cudaFree(b->d_ids);
-    cudaFree(b->d_cand_ids);
-    cudaFree(b->d_cand_d);
-    cudaFree(b->d_cand_cnt);
-    cudaFree(b->d_locks);
-    cudaFree(b->d_counter);
-    if (b->ws) {
-        ws_destroy(b->ws);
-        delete b->ws;
-    }
     delete b;
 }
 
@@ -1610,30 +1520,20 @@ int granne_b200_elements_from_raw(int element_kind, const float* raw, uint64_t n
     uint8_t* o = static_cast<uint8_t*>(out);
     for (int b8 = 0; b8 < 8; ++b8) o[b8] = (uint8_t)((uint64_t)dim >> (8 * b8));
     const uint64_t slab = std::max<uint64_t>(1, (256ull << 20) / ((size_t)dim * 4));
-    float* d_raw = nullptr;
-    void* d_out = nullptr;
     const uint64_t rows_alloc = std::min<uint64_t>(slab, std::max<uint64_t>(n, 1));
-    GB_CUDA(cudaMalloc(&d_raw, rows_alloc * dim * 4));
-    cudaError_t e = cudaMalloc(&d_out, rows_alloc * dim * esz);
-    if (e != cudaSuccess) {
-        cudaFree(d_raw);
-        GB_CUDA(e);
-    }
-    for (uint64_t r0 = 0; r0 < n && rc == GRANNE_B200_OK; r0 += slab) {
+    Buffer<float> d_raw;
+    Buffer<uint8_t> d_out;
+    if ((rc = d_raw.grow(rows_alloc * dim, nullptr)) || (rc = d_out.grow(rows_alloc * dim * esz, nullptr))) return rc;
+    for (uint64_t r0 = 0; r0 < n; r0 += slab) {
         const uint64_t nr = std::min(slab, n - r0);
-        e = cudaMemcpy(d_raw, raw + r0 * dim, (size_t)nr * dim * 4, cudaMemcpyHostToDevice);
-        if (e == cudaSuccess) {
-            gb::make_elements_kernel<<<(unsigned)std::min<uint64_t>(nr, (uint64_t)sms * 32), 32, (size_t)dim * 4>>>(
-                d_raw, nr, dim, element_kind, d_out);
-            e = cudaGetLastError();
-        }
-        if (e == cudaSuccess)
-            e = cudaMemcpy(o + 8 + (size_t)r0 * dim * esz, d_out, (size_t)nr * dim * esz, cudaMemcpyDeviceToHost);
-        if (e != cudaSuccess) rc = fail(GRANNE_B200_ERR_CUDA, cudaGetErrorString(e));
+        GB_CUDA(cudaMemcpy(d_raw.get(), raw + r0 * dim, (size_t)nr * dim * 4, cudaMemcpyHostToDevice));
+        gb::make_elements_kernel<<<(unsigned)std::min<uint64_t>(nr, (uint64_t)sms * 32), 32, (size_t)dim * 4>>>(
+            d_raw.get(), nr, dim, element_kind, d_out.get());
+        GB_CUDA(cudaGetLastError());
+        GB_CUDA(cudaMemcpy(o + 8 + (size_t)r0 * dim * esz, d_out.get(), (size_t)nr * dim * esz,
+                           cudaMemcpyDeviceToHost));
     }
-    cudaFree(d_raw);
-    cudaFree(d_out);
-    return rc;
+    return GRANNE_B200_OK;
 }
 
 // Vector::from per row (angular.rs:55-61 / angular_int.rs:28-45), device to device: d_raw = n x dim f32 rows in HBM,
@@ -1662,7 +1562,7 @@ int granne_b200_compute_distances(int element_kind, const float* a, const float*
     if (n == 0) return GRANNE_B200_OK;
     if (!a || !b || !out) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
     if (n > 0xFFFFFFFFull) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "too many pairs for one call");
-    try {
+    return guarded([&] {
         // the b vectors become an element container (Vector::from per row, on the device) ...
         size_t need = 0;
         int rc = granne_b200_elements_from_raw(element_kind, nullptr, n, dim, device, nullptr, 0, &need);
@@ -1679,27 +1579,18 @@ int granne_b200_compute_distances(int element_kind, const float* a, const float*
             return rc;
         std::unique_ptr<Handle, void (*)(Handle*)> h(raw_h, [](Handle* p) { granne_b200_close(p); });
         const LaunchPlan plan = make_plan(h.get(), 1);
-        float *d_a = nullptr, *d_out = nullptr;
-        int* d_err = nullptr;
-        struct Free {
-            float **a, **o;
-            int** e;
-            ~Free() {
-                cudaFree(*a);
-                cudaFree(*o);
-                cudaFree(*e);
-            }
-        } guard{&d_a, &d_out, &d_err};
-        GB_CUDA(cudaMalloc(&d_a, (size_t)n * dim * 4));
-        GB_CUDA(cudaMalloc(&d_out, (size_t)n * 4));
-        GB_CUDA(cudaMalloc(&d_err, 4));
-        GB_CUDA(cudaMemcpy(d_a, a, (size_t)n * dim * 4, cudaMemcpyHostToDevice));
-        GB_CUDA(cudaMemset(d_err, 0, 4));
+        GB_DEVICE(device);
+        Buffer<float> d_a, d_out;
+        Buffer<int> d_err;
+        if ((rc = d_a.grow((size_t)n * dim, nullptr)) || (rc = d_out.grow(n, nullptr)) || (rc = d_err.grow(1, nullptr)))
+            return rc;
+        GB_CUDA(cudaMemcpy(d_a.get(), a, (size_t)n * dim * 4, cudaMemcpyHostToDevice));
+        GB_CUDA(cudaMemset(d_err.get(), 0, 4));
         PairLaunch L{h.get(), {}, plan.base_smem + gb::link_scratch_bytes(8, 32), 0, nullptr};
-        L.a.queries = d_a;
+        L.a.queries = d_a.get();
         L.a.n = (uint32_t)n;
-        L.a.out = d_out;
-        L.a.error_flag = d_err;
+        L.a.out = d_out.get();
+        L.a.error_flag = d_err.get();
         L.a.stg_rows = plan.stg_rows;
         L.a.stg_row_bytes = plan.stg_row_bytes;
         L.a.tile_rows = plan.tile_rows;
@@ -1707,17 +1598,15 @@ int granne_b200_compute_distances(int element_kind, const float* a, const float*
         if ((rc = DistDispatch::call(h->dev, L))) return rc;
         GB_CUDA(cudaDeviceSynchronize());
         int herr = 0;
-        GB_CUDA(cudaMemcpy(&herr, d_err, 4, cudaMemcpyDeviceToHost));
-        GB_CUDA(cudaMemcpy(out, d_out, (size_t)n * 4, cudaMemcpyDeviceToHost));
+        GB_CUDA(cudaMemcpy(&herr, d_err.get(), 4, cudaMemcpyDeviceToHost));
+        GB_CUDA(cudaMemcpy(out, d_out.get(), (size_t)n * 4, cudaMemcpyDeviceToHost));
         return error_from_bits(herr);
-    } catch (const std::exception& e) {
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, std::string("exception: ") + e.what());
-    }
+    });
 }
 
 int granne_b200_reencode_index(const void* index_bytes, size_t index_len, void* out, size_t cap, size_t* out_len) {
     if (!index_bytes || !out_len) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
-    try {
+    return guarded([&] {
         gb::HostGraph graph;
         std::string err;
         if (!gb::parse_index(static_cast<const uint8_t*>(index_bytes), index_len, &graph, &err))
@@ -1731,9 +1620,7 @@ int granne_b200_reencode_index(const void* index_bytes, size_t index_len, void* 
         if (cap < image.size()) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "output buffer too small");
         std::memcpy(out, image.data(), image.size());
         return GRANNE_B200_OK;
-    } catch (const std::exception& e) {
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, std::string("exception: ") + e.what());
-    }
+    });
 }
 
 // ---- reorder (src/index/reorder.rs) -----------------------------------------------------------------------------------
@@ -1747,70 +1634,62 @@ int granne_b200_compute_order(granne_b200_index* h, uint64_t* order_out, uint64_
     if (cap < n) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "order buffer shorter than Index::len");
     const int nl = h->dev.num_layers;
     if (nl == 0) return GRANNE_B200_OK;
-    try {
+    return guarded([&] {
         GB_DEVICE(h->device);
         std::vector<uint64_t> layer_lens(nl);
         for (int l = 0; l < nl; ++l) layer_lens[l] = h->dev.layer_len[l];
         const size_t trail_layers = std::min<size_t>(gb::kTrailLayers, (size_t)nl - 1);
         std::vector<std::vector<uint32_t>> eps(trail_layers);
-        Workspace* w = nullptr;
-        int rc = ws_acquire(h, &w);
+        std::unique_ptr<Workspace> ws;
+        int rc = ws_acquire(h, &ws);
         if (rc) return rc;
-        const size_t batch = (size_t)std::min<uint64_t>(std::max<uint64_t>(n, 1), 1u << 20);
-        uint32_t *d_q = nullptr, *d_ids = nullptr, *d_cnt = nullptr;
-        float* d_d = nullptr;
-        // the trail searches run over a PRIVATE single-layer view of the staged index: the shared handle is never
-        // modified, so concurrent searches on it stay correct
-        gb::DeviceIndex view = h->dev;
-        struct Cleanup {
-            Handle* h;
-            Workspace* w;
-            uint32_t **q, **ids, **cnt;
-            float** d;
-            ~Cleanup() {
-                cudaFree(*q);
-                cudaFree(*ids);
-                cudaFree(*cnt);
-                cudaFree(*d);
-                ws_release(h, w);
+        Workspace* w = ws.get();
+        const int status = [&] {
+            const size_t batch = (size_t)std::min<uint64_t>(std::max<uint64_t>(n, 1), 1u << 20);
+            cudaStream_t stream = w->stream.get();
+            Buffer<uint32_t> d_q, d_ids, d_cnt;
+            Buffer<float> d_d;
+            if ((rc = d_q.grow(batch, stream)) || (rc = d_ids.grow(batch, stream)) || (rc = d_cnt.grow(batch, stream)) ||
+                (rc = d_d.grow(batch, stream)))
+                return rc;
+            // the trail searches run over a PRIVATE single-layer view of the staged index: the shared handle is never
+            // modified, so concurrent searches on it stay correct
+            gb::DeviceIndex view = h->dev;
+            for (size_t j = 0; j < trail_layers; ++j) {
+                eps[j].resize(n - layer_lens[j]);
+                view.num_layers = 1;
+                view.layer_rows[0] = h->dev.layer_rows[j];
+                view.layer_width[0] = h->dev.layer_width[j];
+                view.layer_len[0] = h->dev.layer_len[j];
+                for (uint64_t base = layer_lens[j]; base < n; base += batch) {
+                    const uint64_t bsz = std::min<uint64_t>(batch, n - base);
+                    gb::iota_kernel<<<(unsigned)((bsz + 255) / 256), 256, 0, stream>>>(d_q.get(), (uint32_t)bsz,
+                                                                                        (uint32_t)base, 1);
+                    h->launches++;
+                    rc = enqueue_search(h, w, d_q.get(), bsz, gb::kQueryById, 1, 1, d_ids.get(), d_d.get(), d_cnt.get(),
+                                        nullptr, stream, true, nullptr, &view);
+                    if (rc) return rc;
+                    GB_CUDA(cudaMemcpyAsync(eps[j].data() + (base - layer_lens[j]), d_ids.get(), bsz * 4,
+                                            cudaMemcpyDeviceToHost, stream));
+                    int herr[4] = {0, 0, 0, 0};
+                    GB_CUDA(cudaMemcpyAsync(herr, w->d_error, sizeof(herr), cudaMemcpyDeviceToHost, stream));
+                    GB_CUDA(cudaStreamSynchronize(stream));
+                    if ((rc = error_from_bits(herr[0]))) return rc;
+                }
             }
-        } cleanup{h, w, &d_q, &d_ids, &d_cnt, &d_d};
-        GB_CUDA(cudaMalloc(&d_q, batch * 4));
-        GB_CUDA(cudaMalloc(&d_ids, batch * 4));
-        GB_CUDA(cudaMalloc(&d_cnt, batch * 4));
-        GB_CUDA(cudaMalloc(&d_d, batch * 4));
-        for (size_t j = 0; j < trail_layers; ++j) {
-            eps[j].resize(n - layer_lens[j]);
-            view.num_layers = 1;
-            view.layer_rows[0] = h->dev.layer_rows[j];
-            view.layer_width[0] = h->dev.layer_width[j];
-            view.layer_len[0] = h->dev.layer_len[j];
-            for (uint64_t base = layer_lens[j]; base < n; base += batch) {
-                const uint64_t bsz = std::min<uint64_t>(batch, n - base);
-                gb::iota_kernel<<<(unsigned)((bsz + 255) / 256), 256, 0, w->stream>>>(d_q, (uint32_t)bsz, (uint32_t)base, 1);
-                h->launches++;
-                rc = enqueue_search(h, w, d_q, bsz, gb::kQueryById, 1, 1, d_ids, d_d, d_cnt, nullptr, w->stream, true,
-                                    nullptr, &view);
-                if (rc) return rc;
-                GB_CUDA(cudaMemcpyAsync(eps[j].data() + (base - layer_lens[j]), d_ids, bsz * 4, cudaMemcpyDeviceToHost,
-                                        w->stream));
-                int herr[4] = {0, 0, 0, 0};
-                GB_CUDA(cudaMemcpyAsync(herr, w->d_error, sizeof(herr), cudaMemcpyDeviceToHost, w->stream));
-                GB_CUDA(cudaStreamSynchronize(w->stream));
-                if ((rc = error_from_bits(herr[0]))) return rc;
-            }
-        }
+            return GRANNE_B200_OK;
+        }();
+        ws_release(h, std::move(ws));  // back to the pool on every path
+        if (status) return status;
         gb::order_from_trails(layer_lens, eps, order_out);
         return GRANNE_B200_OK;
-    } catch (const std::exception& e) {
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, std::string("exception: ") + e.what());
-    }
+    });
 }
 
 int granne_b200_order_from_trails(const uint64_t* layer_lens, uint32_t num_layers, const uint32_t* trails, uint64_t n,
                                   uint64_t* order_out) {
     if (!layer_lens || !trails || !order_out) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
-    try {
+    return guarded([&] {
         std::vector<uint64_t> lens(layer_lens, layer_lens + num_layers);
         if (num_layers == 0 || lens.back() != n) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "n must equal the last layer's length");
         for (uint32_t l = 1; l < num_layers; ++l)
@@ -1827,16 +1706,14 @@ int granne_b200_order_from_trails(const uint64_t* layer_lens, uint32_t num_layer
         }
         gb::order_from_trails(lens, eps, order_out);
         return GRANNE_B200_OK;
-    } catch (const std::exception& e) {
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, std::string("exception: ") + e.what());
-    }
+    });
 }
 
 int granne_b200_order_by_keys(const void* index_bytes, size_t index_len, const uint64_t* keys, uint64_t num_keys,
                               uint32_t key_width, uint64_t* order_out) {
     if (!index_bytes || !keys || !order_out || key_width == 0)
         return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
-    try {
+    return guarded([&] {
         gb::HostGraph graph;
         std::string err;
         if (!gb::parse_index(static_cast<const uint8_t*>(index_bytes), index_len, &graph, &err))
@@ -1847,23 +1724,19 @@ int granne_b200_order_by_keys(const void* index_bytes, size_t index_len, const u
             return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "number of keys must equal Index::len");
         gb::order_by_keys(layer_lens, keys, key_width, order_out);
         return GRANNE_B200_OK;
-    } catch (const std::exception& e) {
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, std::string("exception: ") + e.what());
-    }
+    });
 }
 
 int granne_b200_embedding_reorder_keys(const void* elements_bytes, size_t elements_len, const void* embeddings_bytes,
                                        size_t embeddings_len, uint64_t* keys_out) {
     if (!elements_bytes || !embeddings_bytes || !keys_out) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
-    try {
+    return guarded([&] {
         std::string err;
         if (!gb::embedding_reorder_keys(static_cast<const uint8_t*>(elements_bytes), elements_len,
                                         static_cast<const uint8_t*>(embeddings_bytes), embeddings_len, keys_out, &err))
             return fail(GRANNE_B200_ERR_FORMAT, err);
         return GRANNE_B200_OK;
-    } catch (const std::exception& e) {
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, std::string("exception: ") + e.what());
-    }
+    });
 }
 
 int granne_b200_apply_order(const void* index_bytes, size_t index_len, int element_kind, const void* elements_bytes,
@@ -1871,7 +1744,7 @@ int granne_b200_apply_order(const void* index_bytes, size_t index_len, int eleme
                             size_t* index_out_len, void* out_elements, size_t elements_cap, size_t* elements_out_len) {
     if (!index_bytes || !elements_bytes || !order || !index_out_len || !elements_out_len)
         return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
-    try {
+    return guarded([&] {
         gb::HostGraph graph;
         std::string err;
         if (!gb::parse_index(static_cast<const uint8_t*>(index_bytes), index_len, &graph, &err))
@@ -1895,9 +1768,7 @@ int granne_b200_apply_order(const void* index_bytes, size_t index_len, int eleme
         std::memcpy(out_index, image.data(), image.size());
         std::memcpy(out_elements, elements.data(), elements.size());
         return GRANNE_B200_OK;
-    } catch (const std::exception& e) {
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, std::string("exception: ") + e.what());
-    }
+    });
 }
 
 int granne_b200_merge_topk_device(int device, const uint32_t* d_part_ids, const float* d_part_dists,
@@ -1972,7 +1843,7 @@ int granne_b200_multi_open(int mode, const int* devices, size_t num_devices, int
         return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
     if (mode == GRANNE_B200_MODE_REPLICATED && num_shards != 1)
         return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "replicated mode takes exactly one index image");
-    try {
+    return guarded([&] {
         std::unique_ptr<granne_b200_multi> m(new granne_b200_multi());
         m->mode = mode;
         m->kind = element_kind;
@@ -2008,9 +1879,7 @@ int granne_b200_multi_open(int mode, const int* devices, size_t num_devices, int
             for (auto* p : m->parts) m->total_len += p->index_len;
         *out = m.release();
         return GRANNE_B200_OK;
-    } catch (const std::exception& e) {
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, std::string("exception: ") + e.what());
-    }
+    });
 }
 
 void granne_b200_multi_close(granne_b200_multi* m) {
@@ -2032,7 +1901,7 @@ int granne_b200_multi_search_batch(granne_b200_multi* m, const void* queries, si
     if (nq == 0) return GRANNE_B200_OK;
     if (!queries || (num_neighbors && (!out_ids || !out_dists)))
         return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null buffer");
-    try {
+    return guarded([&] {
         const size_t n = m->parts.size(), k = num_neighbors;
         const bool i8q = m->kind == GRANNE_B200_ANGULAR_INT && query_format == GRANNE_B200_QUERY_ELEMENT;
         const size_t qrow = (size_t)m->dim * (i8q ? 1 : 4);
@@ -2093,9 +1962,7 @@ int granne_b200_multi_search_batch(granne_b200_multi* m, const void* queries, si
             if (out_counts) out_counts[qi] = found;
         }
         return GRANNE_B200_OK;
-    } catch (const std::exception& e) {
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, std::string("exception: ") + e.what());
-    }
+    });
 }
 
 }  // extern "C"
