@@ -373,9 +373,7 @@ class Granne:
                         or not t.is_contiguous()):
                     raise ValueError("out tensors must be contiguous (ids int32 [nq,k], dists float32 [nq,k], counts "
                                      "int32 [nq]) on the queries' device")
-        if stats is not None and (not stats.is_cuda or stats.device != q.device or stats.dtype != torch.int64
-                                  or tuple(stats.shape) != (nq, STATS_PER_QUERY) or not stats.is_contiguous()):
-            raise ValueError("stats must be a contiguous int64 [nq, %d] tensor on the queries' device" % STATS_PER_QUERY)
+        _check_stats(stats, q)
         if out is None:
             dev = q.device
             out = (torch.empty((nq, k), dtype=torch.int32, device=dev),
@@ -390,17 +388,20 @@ class Granne:
         return ids, dists, counts
 
     def search_batch_device_gather(self, queries, gather, max_search=DEFAULT_MAX_SEARCH,
-                                   num_elements=DEFAULT_NUM_ELEMENTS, already_element=False, counts=None, stream=None):
+                                   num_elements=DEFAULT_NUM_ELEMENTS, already_element=False, counts=None, stats=None,
+                                   stream=None):
         """Like search_batch_device, but the result rows are stored by the kernels straight into every peer's
         gathered buffer described by `gather` (a PeerGather)."""
         import torch
 
         q = self._check_device_queries(queries)
         fmt = QUERY_ELEMENT if already_element or q.dtype == torch.int8 else QUERY_RAW_F32
+        _check_stats(stats, q)
         s = stream if stream is not None else torch.cuda.current_stream(q.device).cuda_stream
         _check(load_library().granne_b200_search_batch_device_gather(
             self._h, C.c_void_p(q.data_ptr()), q.shape[0], fmt, int(max_search), int(num_elements), C.byref(gather),
-            C.c_void_p(counts.data_ptr()) if counts is not None else None, None, C.c_void_p(s)))
+            C.c_void_p(counts.data_ptr()) if counts is not None else None,
+            C.c_void_p(stats.data_ptr()) if stats is not None else None, C.c_void_p(s)))
 
     def _check_device_queries(self, q):
         """Same checks as the host path (search_batch): a wrong dtype, width, device or a strided view would make the
@@ -555,6 +556,15 @@ def _write_index(fn, handle, layer_lens):
         rc = fn(handle, _ptr(out), out.size, C.byref(need))
     _check(rc)
     return out[:need.value]
+
+
+def _check_stats(stats, q):
+    import torch
+
+    if stats is not None and (not isinstance(stats, torch.Tensor) or not stats.is_cuda or stats.device != q.device
+                              or stats.dtype != torch.int64 or tuple(stats.shape) != (q.shape[0], STATS_PER_QUERY)
+                              or not stats.is_contiguous()):
+        raise ValueError("stats must be a contiguous int64 [nq, %d] tensor on the queries' device" % STATS_PER_QUERY)
 
 
 def _check_device_rows(kind, t):
@@ -857,10 +867,26 @@ def merge_topk_device(device, part_ids, part_dists, part_base, out_ids=None, out
     float32 [P, nq, k], part_base list of P global id offsets.  Returns (int64 [nq,k] global ids, float32 dists)."""
     import torch
 
+    # the library takes raw pointers and indexes them as [P][nq][k]: anything else would be read out of bounds
+    def tensor_ok(t, dtype, shape):
+        return (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == dtype and t.is_contiguous()
+                and tuple(t.shape) == shape and t.device == torch.device("cuda", device))
+
+    if not isinstance(part_ids, torch.Tensor) or part_ids.dim() != 3:
+        raise ValueError("part_ids must be a CUDA int32 tensor [P, nq, k]")
     P, nq, k = part_ids.shape
+    if not tensor_ok(part_ids, torch.int32, (P, nq, k)) or not tensor_ok(part_dists, torch.float32, (P, nq, k)):
+        raise ValueError("part_ids (int32) and part_dists (float32) must be contiguous [P, nq, k] tensors on cuda:%d"
+                         % device)
+    if len(part_base) != P:
+        raise ValueError("part_base must hold one global id offset per part (%d), not %d" % (P, len(part_base)))
+    if (out_ids is None) != (out_dists is None):
+        raise ValueError("pass both out_ids and out_dists, or neither")
     if out_ids is None:
         out_ids = torch.empty((nq, k), dtype=torch.int64, device=part_ids.device)
         out_dists = torch.empty((nq, k), dtype=torch.float32, device=part_ids.device)
+    if not tensor_ok(out_ids, torch.int64, (nq, k)) or not tensor_ok(out_dists, torch.float32, (nq, k)):
+        raise ValueError("out_ids (int64) and out_dists (float32) must be contiguous [nq, k] tensors on cuda:%d" % device)
     base = np.ascontiguousarray(part_base, dtype=np.uint64)
     s = stream if stream is not None else torch.cuda.current_stream(part_ids.device).cuda_stream
     _check(load_library().granne_b200_merge_topk_device(

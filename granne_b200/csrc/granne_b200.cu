@@ -706,6 +706,21 @@ int validate_search(const Handle* h, const void* q, size_t nq, int fmt, uint32_t
     return GRANNE_B200_OK;
 }
 
+gb::PeerGather device_gather(const granne_b200_peer_gather& pg, unsigned int* done_counter) {
+    gb::PeerGather d{};
+    d.n_peers = pg.n_peers;
+    d.my_rank = pg.my_rank;
+    d.row_offset = pg.row_offset;
+    d.seq = pg.seq;
+    d.done_counter = done_counter;
+    for (uint32_t p = 0; p < pg.n_peers; ++p) {
+        d.ids[p] = static_cast<uint32_t*>(pg.ids[p]);
+        d.dists[p] = static_cast<float*>(pg.dists[p]);
+        d.flags[p] = static_cast<unsigned int*>(pg.flags[p]);
+    }
+    return d;
+}
+
 // Enqueues one batch on `stream` with device pointers.  Needs a workspace for status words / slow path.
 int enqueue_search(Handle* h, Workspace* w, const void* d_queries, size_t nq, int fmt, uint32_t max_search,
                    uint32_t k, uint32_t* d_ids, float* d_dists, uint32_t* d_counts, unsigned long long* d_stats,
@@ -760,19 +775,7 @@ int enqueue_search(Handle* h, Workspace* w, const void* d_queries, size_t nq, in
     a.slow_list_cap = h->slow_list_cap;
     a.slow_vis_slots = h->slow_vis_slots;
     a.pass = a.slow_pass = a.final_pass = 0;
-    a.pg = gb::PeerGather{};
-    if (pg) {
-        a.pg.n_peers = pg->n_peers;
-        a.pg.my_rank = pg->my_rank;
-        a.pg.row_offset = pg->row_offset;
-        a.pg.seq = pg->seq;
-        a.pg.done_counter = w->d_counters.get() + 5;
-        for (uint32_t p = 0; p < pg->n_peers; ++p) {
-            a.pg.ids[p] = static_cast<uint32_t*>(pg->ids[p]);
-            a.pg.dists[p] = static_cast<float*>(pg->dists[p]);
-            a.pg.flags[p] = static_cast<unsigned int*>(pg->flags[p]);
-        }
-    }
+    a.pg = pg ? device_gather(*pg, w->d_counters.get() + 5) : gb::PeerGather{};
     a.stg_rows = plan.stg_rows;
     a.stg_row_bytes = plan.stg_row_bytes;
     a.tile_rows = plan.tile_rows;
@@ -1121,10 +1124,16 @@ static int search_device_impl(granne_b200_index* h, const void* d_queries, size_
             if (!pg->ids[p] || !pg->dists[p] || !pg->flags[p])
                 return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "peer gather: null peer pointer");
     }
-    if (nq == 0) return GRANNE_B200_OK;
+    if (nq == 0 && !pg) return GRANNE_B200_OK;
     return guarded([&] {
         GB_DEVICE(h->device);
         cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+        if (nq == 0) {  // nothing to store, but the peers wait for this call's sequence number all the same
+            gb::publish_seq_kernel<<<1, 1, 0, stream>>>(device_gather(*pg, nullptr));
+            h->launches++;
+            GB_CUDA(cudaGetLastError());
+            return GRANNE_B200_OK;
+        }
         // One workspace per caller stream: calls on the same stream are serialised by the stream itself, so the
         // status words / slow-path buffers can be reused; the error word stays sticky until
         // granne_b200_stream_status().

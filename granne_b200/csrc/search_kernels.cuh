@@ -1499,6 +1499,12 @@ __device__ __forceinline__ void store_result(const SearchArgs& a, unsigned long 
     }
 }
 
+// flags[p][my_rank] = seq for every peer, released system-wide
+__device__ __forceinline__ void publish_seq(const PeerGather& pg) {
+    for (uint32_t p = 0; p < pg.n_peers; ++p)
+        asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(pg.flags[p] + pg.my_rank), "r"(pg.seq) : "memory");
+}
+
 // Called by every CTA of the LAST kernel of a search (the slow pass) before it exits: once all CTAs are through,
 // publish the sequence number to every peer.
 __device__ __forceinline__ void signal_peers(const SearchArgs& a, int lane) {
@@ -1509,11 +1515,15 @@ __device__ __forceinline__ void signal_peers(const SearchArgs& a, int lane) {
         const unsigned int old = atomicAdd(a.pg.done_counter, 1u);
         if (old == gridDim.x - 1) {
             __threadfence_system();
-            for (uint32_t p = 0; p < a.pg.n_peers; ++p)
-                asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(a.pg.flags[p] + a.pg.my_rank), "r"(a.pg.seq)
-                             : "memory");
+            publish_seq(a.pg);
         }
     }
+}
+
+// A gather call without queries has no stores to wait for, but its peers still wait for its sequence number.
+__global__ void publish_seq_kernel(const PeerGather pg) {
+    __threadfence_system();
+    publish_seq(pg);
 }
 
 // R == 0: generic list (64-bit keys, any capacity, shared or global memory) — the slow pass and very large max_search.

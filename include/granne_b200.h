@@ -144,7 +144,8 @@ int granne_b200_search_batch_device(granne_b200_index* h, const void* d_queries,
  * (peer-mapped memory, e.g. torch symmetric memory or cudaIpc/cuMem mappings; entry `my_rank` is this GPU's own
  * buffer), each [total_queries][num_neighbors].  The kernels store the rows of this call at row `row_offset + i` of
  * every peer buffer over NVLink — no collective, no rendezvous — and, when every store is done, release
- * `flags[p][my_rank] = seq` system-wide. */
+ * `flags[p][my_rank] = seq` system-wide.  Every successful call publishes `seq`, including one with nq == 0 (no row is
+ * stored) or num_neighbors == 0 (no column is stored); a call rejected for its arguments touches no buffer or flag. */
 #define GRANNE_B200_MAX_PEERS 8
 typedef struct granne_b200_peer_gather {
     uint32_t n_peers; /* 1..8 */

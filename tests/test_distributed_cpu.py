@@ -15,6 +15,7 @@ import torch.multiprocessing as mp
 
 from granne_b200.distributed import PartitionedGranne, ReplicatedGranne, merge_topk_host, shard_bounds
 from helpers.data import random_vectors
+from helpers.topk_tiles import make_tiles, reference_merge, tie_bases
 
 
 def test_shard_bounds_cover_everything():
@@ -33,6 +34,17 @@ def test_merge_topk_host_orders_by_distance_then_global_id():
     gi, gd = merge_topk_host(ids, d, [10, 0], 3)
     assert gi.tolist() == [[1, 10, 12]]  # equal distances: the smaller global id first (tuple order)
     assert gd.tolist() == [[0.5, 0.5, np.float32(0.7)]]
+
+
+@pytest.mark.parametrize("P,k,nq", [(1, 200, 3), (2, 1, 129), (3, 10, 5000), (3, 33, 128), (64, 10, 127), (64, 200, 1)])
+def test_merge_topk_host_on_tied_short_tiles(P, k, nq):
+    # the numpy merge against the plain sort the GPU merge is held to (tests/test_merge_topk_gpu.py)
+    ids, d = make_tiles(P, nq, k, seed=P * 1000 + k + nq)
+    base = tie_bases(P)
+    want_ids, want_d = reference_merge(ids, d, base, k)
+    gi, gd = merge_topk_host(ids, d, base, k)
+    assert np.array_equal(gi.view(np.uint64), want_ids)
+    assert np.array_equal(gd.view(np.uint32), want_d.view(np.uint32))
 
 
 def _free_port():
