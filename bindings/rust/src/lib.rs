@@ -62,6 +62,15 @@ extern "C" {
         cfg: *const RawBuildConfig, element_kind: c_int, elements: *const c_void, elements_len: usize,
         embeddings: *const c_void, embeddings_len: usize, device: c_int, out: *mut *mut RawBuilder,
     ) -> c_int;
+    fn granne_b200_builder_from_index(
+        cfg: *const RawBuildConfig, index: *const c_void, index_len: usize, element_kind: c_int,
+        elements: *const c_void, elements_len: usize, embeddings: *const c_void, embeddings_len: usize, device: c_int,
+        out: *mut *mut RawBuilder,
+    ) -> c_int;
+    fn granne_b200_builder_from_index_device_elements(
+        cfg: *const RawBuildConfig, index: *const c_void, index_len: usize, element_kind: c_int,
+        d_element_rows: *const c_void, num_elements: u64, dim: u32, device: c_int, out: *mut *mut RawBuilder,
+    ) -> c_int;
     fn granne_b200_builder_free(b: *mut RawBuilder);
     fn granne_b200_builder_append(b: *mut RawBuilder, elements: *const c_void, elements_len: usize) -> c_int;
     fn granne_b200_builder_build(b: *mut RawBuilder, num_elements: u64) -> c_int;
@@ -253,6 +262,35 @@ impl GpuGranneBuilder {
                 &config.0, element_kind, elements.as_ptr() as *const c_void, elements.len(), emb, emb_len, device, &mut b,
             )
         });
+        Self { b }
+    }
+    /// `GranneBuilder::from_bytes(config, index, elements)` (`:428-461`): continues from an index file image; every
+    /// neighbour list is truncated or padded to the config's `num_neighbors`, like the reference.
+    pub fn from_bytes(
+        config: GpuBuildConfig, index: &[u8], element_kind: c_int, elements: &[u8], embeddings: Option<&[u8]>,
+        device: i32,
+    ) -> Self {
+        let mut b = std::ptr::null_mut();
+        let (emb, emb_len) = ptr_or_null(embeddings);
+        check(unsafe {
+            granne_b200_builder_from_index(
+                &config.0, index.as_ptr() as *const c_void, index.len(), element_kind,
+                elements.as_ptr() as *const c_void, elements.len(), emb, emb_len, device, &mut b,
+            )
+        });
+        Self { b }
+    }
+    /// `from_bytes` over a device-resident container: `d_element_rows` is `num_elements x dim` elements in the
+    /// memory of `device` (see `granne_b200_builder_new_device_elements`).
+    pub unsafe fn from_bytes_device_elements(
+        config: GpuBuildConfig, index: &[u8], element_kind: c_int, d_element_rows: *const c_void, num_elements: usize,
+        dim: usize, device: i32,
+    ) -> Self {
+        let mut b = std::ptr::null_mut();
+        check(granne_b200_builder_from_index_device_elements(
+            &config.0, index.as_ptr() as *const c_void, index.len(), element_kind, d_element_rows,
+            num_elements as u64, dim as u32, device, &mut b,
+        ));
         Self { b }
     }
     /// `Builder::build` (`:366-368`)

@@ -73,6 +73,8 @@ def load_library():
         "granne_b200_apply_order": (i32, [vp, sz, i32, vp, sz, vp, u64, vp, sz, C.POINTER(sz), vp, sz, C.POINTER(sz)]),
         "granne_b200_build_config_default": (None, [vp]),
         "granne_b200_builder_new": (i32, [vp, i32, vp, sz, vp, sz, i32, C.POINTER(vp)]),
+        "granne_b200_builder_from_index": (i32, [vp, vp, sz, i32, vp, sz, vp, sz, i32, C.POINTER(vp)]),
+        "granne_b200_builder_from_index_device_elements": (i32, [vp, vp, sz, i32, vp, u64, u32, i32, C.POINTER(vp)]),
         "granne_b200_builder_append": (i32, [vp, vp, sz]),
         "granne_b200_builder_build": (i32, [vp, u64]),
         "granne_b200_builder_len": (u64, [vp]),
@@ -530,6 +532,19 @@ class BuildConfig(C.Structure):
                 ("show_progress", C.c_int32)]
 
 
+def _build_config(num_neighbors, max_search, layer_multiplier, reinsert_elements, expected_num_elements,
+                  show_progress=False):
+    cfg = BuildConfig()
+    load_library().granne_b200_build_config_default(C.byref(cfg))
+    cfg.num_neighbors = num_neighbors
+    cfg.max_search = max_search
+    cfg.layer_multiplier = layer_multiplier
+    cfg.reinsert_elements = int(bool(reinsert_elements))
+    cfg.expected_num_elements = -1 if expected_num_elements is None else int(expected_num_elements)
+    cfg.show_progress = int(bool(show_progress))
+    return cfg
+
+
 def elements_from_raw(element_type, raw, device=0):
     """Builds an elements file image from raw f32 rows on the GPU exactly like `Vector::from(Vec<f32>)` per row
     (normalise for "angular", quantise for "angular_int")."""
@@ -602,28 +617,31 @@ class GranneBuilder:
     """granne.GranneBuilder (py/src/lib.rs:346-579; src/index/mod.rs:295-531) on the GPU.
 
     GranneBuilder(element_type, elements_bytes, embeddings_bytes=None, num_neighbors=30, max_search=200,
-                  layer_multiplier=15.0, reinsert_elements=True, expected_num_elements=None, device=0)
+                  layer_multiplier=15.0, reinsert_elements=True, expected_num_elements=None, device=0,
+                  index_bytes=None)
     `elements_bytes` is an elements file image (see elements_from_raw / Granne.save_elements).  num_neighbors may be
-    anything the file format can hold (1..255: a list's length is one byte); show_progress is accepted and ignored."""
+    anything the file format can hold (1..255: a list's length is one byte); show_progress is accepted and ignored.
+    With `index_bytes` (an index file image built over these elements, or over a prefix of them) the builder continues
+    from that index (GranneBuilder::from_bytes, src/index/mod.rs:428-461): the next build() indexes only the elements
+    beyond it.  Every loaded neighbour list is cut to its first `num_neighbors` ids (the lowest, as in the reference)."""
 
     def __init__(self, element_type, elements_bytes, embeddings_bytes=None, num_neighbors=30, max_search=200,
                  layer_multiplier=15.0, reinsert_elements=True, expected_num_elements=None, show_progress=False,
-                 device=0):
+                 device=0, index_bytes=None):
         L = load_library()
-        cfg = BuildConfig()
-        L.granne_b200_build_config_default(C.byref(cfg))
-        cfg.num_neighbors = num_neighbors
-        cfg.max_search = max_search
-        cfg.layer_multiplier = layer_multiplier
-        cfg.reinsert_elements = int(bool(reinsert_elements))
-        cfg.expected_num_elements = -1 if expected_num_elements is None else int(expected_num_elements)
-        cfg.show_progress = int(bool(show_progress))
+        cfg = _build_config(num_neighbors, max_search, layer_multiplier, reinsert_elements, expected_num_elements,
+                            show_progress)
         eb = np.frombuffer(elements_bytes, dtype=np.uint8)
         mb = np.frombuffer(embeddings_bytes, dtype=np.uint8) if embeddings_bytes is not None else None
         h = C.c_void_p()
-        _check(L.granne_b200_builder_new(C.byref(cfg), _kind(element_type), _ptr(eb), eb.size,
-                                         _ptr(mb) if mb is not None else None, mb.size if mb is not None else 0,
-                                         device, C.byref(h)))
+        mb_args = (_ptr(mb) if mb is not None else None, mb.size if mb is not None else 0)
+        if index_bytes is None:
+            _check(L.granne_b200_builder_new(C.byref(cfg), _kind(element_type), _ptr(eb), eb.size, *mb_args, device,
+                                             C.byref(h)))
+        else:
+            ib = np.frombuffer(index_bytes, dtype=np.uint8)
+            _check(L.granne_b200_builder_from_index(C.byref(cfg), _ptr(ib), ib.size, _kind(element_type), _ptr(eb),
+                                                    eb.size, *mb_args, device, C.byref(h)))
         self._h = h
         self.device = device
         self._element_type = element_type
@@ -632,24 +650,42 @@ class GranneBuilder:
         self._pending = []
 
     @classmethod
+    def from_files(cls, element_type, elements_path, index_path=None, embeddings_path=None, **config):
+        """The reference's keyword form GranneBuilder(element_type, elements_path=..., index_path=...,
+        embeddings_path=...) (py/src/lib.rs:384-442): reads the files and builds from them; with `index_path` the
+        builder continues from that index.  `config`: the keyword arguments of GranneBuilder (num_neighbors, ...,
+        device).  An "embeddings" builder takes term lists, not a words file."""
+        kind = _kind(element_type)
+        if elements_path is None:
+            raise ValueError("elements_path is required%s" % (" together with index_path" if index_path else ""))
+        if kind == EMBEDDINGS and embeddings_path is None:
+            raise ValueError("embeddings_path required for this element type!")
+
+        def read(path):
+            with open(path, "rb") as f:
+                return f.read()
+
+        return cls(element_type, read(elements_path), read(embeddings_path) if kind == EMBEDDINGS else None,
+                   index_bytes=read(index_path) if index_path is not None else None, **config)
+
+    @classmethod
     def from_device_elements(cls, element_type, elements, num_neighbors=30, max_search=200, layer_multiplier=15.0,
-                             reinsert_elements=True, expected_num_elements=None, device=None):
-        """GranneBuilder::new(config, elements) over a device-resident container (see Granne.from_device_elements)."""
+                             reinsert_elements=True, expected_num_elements=None, device=None, index_bytes=None):
+        """GranneBuilder::new(config, elements) over a device-resident container (see Granne.from_device_elements);
+        with `index_bytes`, GranneBuilder::from_bytes over it (see GranneBuilder)."""
         L = load_library()
         kind = _kind(element_type)
         _check_device_rows(kind, elements)
         device = elements.device.index if device is None else device
-        cfg = BuildConfig()
-        L.granne_b200_build_config_default(C.byref(cfg))
-        cfg.num_neighbors = num_neighbors
-        cfg.max_search = max_search
-        cfg.layer_multiplier = layer_multiplier
-        cfg.reinsert_elements = int(bool(reinsert_elements))
-        cfg.expected_num_elements = -1 if expected_num_elements is None else int(expected_num_elements)
+        cfg = _build_config(num_neighbors, max_search, layer_multiplier, reinsert_elements, expected_num_elements)
         self = cls.__new__(cls)
         h = C.c_void_p()
-        _check(L.granne_b200_builder_new_device_elements(C.byref(cfg), kind, C.c_void_p(elements.data_ptr()),
-                                                         elements.shape[0], elements.shape[1], device, C.byref(h)))
+        rows = (kind, C.c_void_p(elements.data_ptr()), elements.shape[0], elements.shape[1], device, C.byref(h))
+        if index_bytes is None:
+            _check(L.granne_b200_builder_new_device_elements(C.byref(cfg), *rows))
+        else:
+            ib = np.frombuffer(index_bytes, dtype=np.uint8)
+            _check(L.granne_b200_builder_from_index_device_elements(C.byref(cfg), _ptr(ib), ib.size, *rows))
         self._h = h
         self.device = device
         self._element_type = element_type

@@ -1008,6 +1008,37 @@ int builder_build_partial(Builder* b, uint64_t num_elements) {
     return GRANNE_B200_OK;
 }
 
+// GranneBuilder::from_bytes (:440-451): every layer of `graph` becomes a layer of the builder, in its own allocation
+// at the builder's row stride.  Row i keeps node i's ids in stored (ascending) order, truncated to the first
+// num_neighbors (the lowest ids, not the nearest) or padded with UNUSED, like `neighbors.resize(num_neighbors,
+// UNUSED)`.  The link and prune kernels compute the distances of whatever a row holds, so they need no other order.
+int builder_load_layers(Builder* b, const gb::HostGraph& graph) {
+    Handle* h = b->h.get();
+    gb::DeviceIndex& d = h->dev;
+    const uint32_t m = b->cfg.num_neighbors;
+    std::vector<uint32_t> rows;
+    for (size_t l = 0; l < graph.layers.size(); ++l) {
+        const gb::HostLayer& L = graph.layers[l];
+        if (L.num_nodes > d.num_elements)
+            return fail(GRANNE_B200_ERR_FORMAT, "index refers to more elements than the container holds");
+        const uint32_t keep = std::min(m, L.width);  // decoded rows are padded with UNUSED up to L.width
+        rows.assign((size_t)L.num_nodes * b->stride, gb::kUnusedId);
+        for (uint64_t i = 0; i < L.num_nodes; ++i)
+            std::copy_n(L.rows.data() + i * L.width, keep, rows.data() + i * b->stride);
+        Buffer<uint32_t> mem;
+        int rc;
+        if ((rc = dev_alloc(&mem, rows.size()))) return rc;
+        if (!rows.empty()) GB_CUDA(cudaMemcpy(mem.get(), rows.data(), rows.size() * 4, cudaMemcpyHostToDevice));
+        d.layer_rows[l] = mem.get();
+        d.layer_len[l] = L.num_nodes;
+        d.layer_width[l] = b->stride;
+        b->layer_mem.push_back(std::shared_ptr<void>(std::move(mem.p)));
+        h->layer_max_degree.push_back(m);
+    }
+    d.num_layers = (int)graph.layers.size();
+    return GRANNE_B200_OK;
+}
+
 }  // namespace
 
 // =================================================================================================================
@@ -1314,9 +1345,11 @@ void granne_b200_build_config_default(granne_b200_build_config* cfg) {
     cfg->show_progress = 0;
 }
 
+// `index_bytes` != nullptr: GranneBuilder::from_bytes, the builder continues from that index image
 static int builder_new_impl(const granne_b200_build_config* cfg, int element_kind, const void* elements_bytes,
                             size_t elements_len, const void* embeddings_bytes, size_t embeddings_len, int device,
-                            granne_b200_builder** out, const void* dev_rows, uint64_t n_dev, uint32_t dim_dev) {
+                            granne_b200_builder** out, const void* dev_rows, uint64_t n_dev, uint32_t dim_dev,
+                            const void* index_bytes = nullptr, size_t index_len = 0) {
     if (!out || !cfg) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
     *out = nullptr;
     // the on-disk format counts a list's entries in one byte (set_vector.rs:91-99): 255 is the format's limit
@@ -1325,6 +1358,14 @@ static int builder_new_impl(const granne_b200_build_config* cfg, int element_kin
     if (cfg->max_search < 1) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "max_search must be >= 1");
     if (!(cfg->layer_multiplier > 1.0f)) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "layer_multiplier must be > 1");
     return guarded([&] {
+        // the image is decoded and checked on the host first, so that a malformed one is reported without a device
+        gb::HostGraph graph;
+        if (index_bytes) {
+            std::string err;
+            if (!gb::parse_index(static_cast<const uint8_t*>(index_bytes), index_len, &graph, &err))
+                return fail(GRANNE_B200_ERR_FORMAT, err);
+            if (graph.layers.size() > (size_t)gb::kMaxLayers) return fail(GRANNE_B200_ERR_FORMAT, "too many layers");
+        }
         DeviceGuard guard;
         std::unique_ptr<granne_b200_builder> b(new granne_b200_builder());
         b->cfg = *cfg;
@@ -1337,6 +1378,7 @@ static int builder_new_impl(const granne_b200_build_config* cfg, int element_kin
         if (h->dev.num_elements >= 0xFFFFFFFFull)  // assert!(elements.len() < UNUSED) (:420)
             return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "too many elements");
         h->dev.num_layers = 0;
+        if ((rc = builder_load_layers(b.get(), graph))) return rc;
         finish_handle(h);
         if ((rc = ws_acquire(h, &b->ws))) return rc;
         GB_CUDA(cudaMemset(b->ws->d_error, 0, 4 * sizeof(int)));
@@ -1357,6 +1399,25 @@ int granne_b200_builder_new_device_elements(const granne_b200_build_config* cfg,
                                             int device, granne_b200_builder** out) {
     if (!d_element_rows) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "elements pointer is null");
     return builder_new_impl(cfg, element_kind, nullptr, 0, nullptr, 0, device, out, d_element_rows, num_elements, dim);
+}
+
+int granne_b200_builder_from_index(const granne_b200_build_config* cfg, const void* index_bytes, size_t index_len,
+                                   int element_kind, const void* elements_bytes, size_t elements_len,
+                                   const void* embeddings_bytes, size_t embeddings_len, int device,
+                                   granne_b200_builder** out) {
+    if (!index_bytes) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "index buffer is null");
+    return builder_new_impl(cfg, element_kind, elements_bytes, elements_len, embeddings_bytes, embeddings_len, device,
+                            out, nullptr, 0, 0, index_bytes, index_len);
+}
+
+int granne_b200_builder_from_index_device_elements(const granne_b200_build_config* cfg, const void* index_bytes,
+                                                   size_t index_len, int element_kind, const void* d_element_rows,
+                                                   uint64_t num_elements, uint32_t dim, int device,
+                                                   granne_b200_builder** out) {
+    if (!index_bytes) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "index buffer is null");
+    if (!d_element_rows) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "elements pointer is null");
+    return builder_new_impl(cfg, element_kind, nullptr, 0, nullptr, 0, device, out, d_element_rows, num_elements, dim,
+                            index_bytes, index_len);
 }
 
 // GranneBuilder::push for the dense containers (ExtendableElementContainer::push, src/index/mod.rs:512-531;

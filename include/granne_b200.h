@@ -261,6 +261,24 @@ int granne_b200_builder_new(const granne_b200_build_config* cfg, int element_kin
 int granne_b200_builder_new_device_elements(const granne_b200_build_config* cfg, int element_kind,
                                             const void* d_element_rows, uint64_t num_elements, uint32_t dim,
                                             int device, granne_b200_builder** out);
+/* GranneBuilder::from_bytes(config, index, elements) (src/index/mod.rs:428-461): a builder that continues from an
+ * index file image over the elements it was built from (or more of them).  Every loaded neighbour list keeps its ids
+ * in stored (ascending) order and is truncated to the first cfg->num_neighbors ids or padded, exactly as the reference
+ * does; the next build indexes only the elements beyond the loaded last layer.  The config is checked as in
+ * granne_b200_builder_new, then the image is decoded and checked before any device call: a malformed image or one with
+ * more than 24 layers gives GRANNE_B200_ERR_FORMAT even without a device.  An image whose last layer holds more nodes
+ * than the container holds elements gives GRANNE_B200_ERR_FORMAT too (checked once the elements are staged).  An
+ * image without layers gives the same builder as granne_b200_builder_new.  Element buffers as in granne_b200_open. */
+int granne_b200_builder_from_index(const granne_b200_build_config* cfg, const void* index_bytes, size_t index_len,
+                                   int element_kind, const void* elements_bytes, size_t elements_len,
+                                   const void* embeddings_bytes, size_t embeddings_len, int device,
+                                   granne_b200_builder** out);
+/* granne_b200_builder_from_index with the element container given as device rows (as in
+ * granne_b200_builder_new_device_elements). */
+int granne_b200_builder_from_index_device_elements(const granne_b200_build_config* cfg, const void* index_bytes,
+                                                   size_t index_len, int element_kind, const void* d_element_rows,
+                                                   uint64_t num_elements, uint32_t dim, int device,
+                                                   granne_b200_builder** out);
 /* GranneBuilder::push (src/index/mod.rs:512-531; py GranneBuilder.append, py/src/lib.rs:474-476): appends the
  * elements of an elements file image of the builder's own kind to its container; they are indexed by the next build.
  * angular / angular_int: rows of the same width (ExtendableElementContainer for Vectors, dense_vector.rs:120-136);

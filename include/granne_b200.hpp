@@ -7,8 +7,8 @@
 //   granne::Granne::from_bytes / from_file, search, Index::{len, num_layers, layer_len, get_neighbors}, get_element
 //                                                      (src/index/mod.rs:38-160)        -> granne_b200::Granne
 //   granne::BuildConfig (fluent setters, src/index/mod.rs:198-291)                      -> granne_b200::BuildConfig
-//   granne::GranneBuilder::{new, build, build_partial, push, get_index, write_index,
-//                           num_elements} (src/index/mod.rs:295-531)                    -> granne_b200::GranneBuilder
+//   granne::GranneBuilder::{new, from_bytes, from_file, build, build_partial, push, get_index,
+//                           write_index, num_elements} (src/index/mod.rs:295-531)       -> granne_b200::GranneBuilder
 //   angular::Vectors / angular_int::Vectors / embeddings::SumEmbeddings file images     -> granne_b200::Elements
 //   Granne::reorder / reorder_by_keys (src/index/reorder.rs:59-124)                     -> Granne::reorder*
 //
@@ -342,6 +342,28 @@ public:
                                       elements.bytes.size(), elements.embeddings.empty() ? nullptr : elements.embeddings.data(),
                                       elements.embeddings.size(), device, &b_));
     }
+    // GranneBuilder::from_bytes(config, index, elements) (:428-461): continues from an index built over `elements`
+    // (or over a prefix of them); every neighbour list is truncated or padded to config's num_neighbors
+    static GranneBuilder from_bytes(const BuildConfig& config, const void* index, size_t index_len,
+                                    const Elements& elements, int device = 0) {
+        GranneBuilder g;
+        check(granne_b200_builder_from_index(&config.raw(), index, index_len, static_cast<int>(elements.kind),
+                                             elements.bytes.data(), elements.bytes.size(),
+                                             elements.embeddings.empty() ? nullptr : elements.embeddings.data(),
+                                             elements.embeddings.size(), device, &g.b_));
+        g.elements_ = elements;
+        g.device_ = device;
+        return g;
+    }
+    static GranneBuilder from_bytes(const BuildConfig& config, const std::vector<uint8_t>& index,
+                                    const Elements& elements, int device = 0) {
+        return from_bytes(config, index.data(), index.size(), elements, device);
+    }
+    // GranneBuilder::from_file(config, &file, elements) (:463-469)
+    static GranneBuilder from_file(const BuildConfig& config, const std::string& index_path, const Elements& elements,
+                                   int device = 0) {
+        return from_bytes(config, read_file(index_path), elements, device);
+    }
     GranneBuilder(const GranneBuilder&) = delete;
     GranneBuilder& operator=(const GranneBuilder&) = delete;
     GranneBuilder(GranneBuilder&& o) noexcept : b_(o.b_), elements_(std::move(o.elements_)), device_(o.device_) { o.b_ = nullptr; }
@@ -387,6 +409,7 @@ public:
     }
 
 private:
+    GranneBuilder() = default;
     granne_b200_builder* b_ = nullptr;
     Elements elements_;
     int device_ = 0;
