@@ -81,6 +81,11 @@ extern "C" {
     fn granne_b200_builder_write_index(b: *mut RawBuilder, out: *mut c_void, cap: usize, out_len: *mut usize) -> c_int;
     fn granne_b200_builder_get_index(b: *mut RawBuilder, out: *mut *mut RawIndex) -> c_int;
 
+    fn granne_b200_compute_embeddings(
+        element_kind: c_int, elements: *const c_void, elements_len: usize, embeddings: *const c_void,
+        embeddings_len: usize, device: c_int, out: *mut c_void, cap: usize, out_len: *mut usize,
+    ) -> c_int;
+
     fn granne_b200_multi_open(
         mode: c_int, devices: *const c_int, num_devices: usize, element_kind: c_int, index: *const *const c_void,
         index_len: *const usize, elements: *const *const c_void, elements_len: *const usize, num_shards: usize,
@@ -116,6 +121,28 @@ fn ptr_or_null(bytes: Option<&[u8]>) -> (*const c_void, usize) {
         Some(b) => (b.as_ptr() as *const c_void, b.len()),
         None => (std::ptr::null(), 0),
     }
+}
+
+/// `granne::embeddings::parsing::compute_embeddings_and_save_to_disk` (`src/elements/embeddings/parsing.rs:102-152`)
+/// in memory: the elements file image of the sum of embeddings of every element of a SumEmbeddings container
+/// (`elements`, `embeddings`: its two file images), as `ANGULAR_INT` vectors (the quantised raw sum, what the reference
+/// writes) or `ANGULAR` vectors (the normalised sum, `SumEmbeddings::get`).  Write the returned image to a file to get
+/// the reference's output file.  Panics where the reference does (malformed images, a NaN in a sum).
+pub fn compute_embeddings(element_kind: c_int, elements: &[u8], embeddings: &[u8], device: i32) -> Vec<u8> {
+    let (el, el_len) = ptr_or_null(Some(elements));
+    let (emb, emb_len) = ptr_or_null(Some(embeddings));
+    let mut need = 0usize;
+    check(unsafe {
+        granne_b200_compute_embeddings(element_kind, el, el_len, emb, emb_len, device, std::ptr::null_mut(), 0, &mut need)
+    });
+    let mut out = vec![0u8; need];
+    check(unsafe {
+        granne_b200_compute_embeddings(
+            element_kind, el, el_len, emb, emb_len, device, out.as_mut_ptr() as *mut c_void, out.len(), &mut need,
+        )
+    });
+    out.truncate(need);
+    out
 }
 
 /// Drop-in for `Granne<'_, Elements>` on the search path.

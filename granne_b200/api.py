@@ -46,6 +46,9 @@ def load_library():
         "granne_b200_open_device_elements": (i32, [vp, sz, i32, vp, u64, u32, i32, C.POINTER(vp)]),
         "granne_b200_builder_new_device_elements": (i32, [vp, i32, vp, u64, u32, i32, C.POINTER(vp)]),
         "granne_b200_elements_from_raw_device": (i32, [i32, vp, u64, u32, i32, vp, vp]),
+        "granne_b200_compute_embeddings": (i32, [i32, vp, sz, vp, sz, i32, vp, sz, C.POINTER(sz)]),
+        "granne_b200_compute_embeddings_device": (i32, [i32, vp, sz, vp, sz, i32, vp, C.POINTER(u64), C.POINTER(u32),
+                                                        vp]),
         "granne_b200_close": (None, [vp]),
         "granne_b200_len": (u64, [vp]),
         "granne_b200_num_layers": (u64, [vp]),
@@ -611,6 +614,88 @@ def elements_from_raw_device(element_type, raw, out=None, stream=None):
                                                                raw.device.index, C.c_void_p(out.data_ptr()),
                                                                C.c_void_p(s)))
     return out
+
+
+def _embeddings_kind(element_type):
+    kind = _kind(element_type)
+    if kind not in (ANGULAR, ANGULAR_INT):
+        raise ValueError("compute_embeddings writes \"angular\" or \"angular_int\" vectors")
+    return kind
+
+
+def compute_embeddings(element_type, elements_bytes, embeddings_bytes, out=None, device=0):
+    """compute_embeddings_and_save_to_disk (src/elements/embeddings/parsing.rs:102-152) in memory: the elements file
+    image of the sum of embeddings of every element of a SumEmbeddings container, made into "angular_int" vectors (the
+    quantised raw sum; what the reference writes) or "angular" vectors (the normalised sum: SumEmbeddings::get, so that
+    searching the rows searches the container).  Returns the image as a uint8 array, or fills `out` (a writable
+    uint8 buffer of at least the image's size, e.g. an np.memmap) and returns the image's part of it."""
+    L = load_library()
+    kind = _embeddings_kind(element_type)
+    eb = np.frombuffer(elements_bytes, dtype=np.uint8)
+    mb = np.frombuffer(embeddings_bytes, dtype=np.uint8)
+    need = C.c_size_t()
+    _check(L.granne_b200_compute_embeddings(kind, _ptr(eb), eb.size, _ptr(mb), mb.size, device, None, 0,
+                                            C.byref(need)))
+    if out is None:
+        out = np.empty(need.value, dtype=np.uint8)
+    elif (not isinstance(out, np.ndarray) or out.dtype != np.uint8 or out.ndim != 1 or not out.flags.c_contiguous
+          or not out.flags.writeable):
+        raise ValueError("out must be a writable contiguous 1-d uint8 array")
+    elif out.size < need.value:
+        raise ValueError("out holds %d bytes; the image needs %d" % (out.size, need.value))
+    _check(L.granne_b200_compute_embeddings(kind, _ptr(eb), eb.size, _ptr(mb), mb.size, device, _ptr(out), out.size,
+                                            C.byref(need)))
+    return out[:need.value]
+
+
+def compute_embeddings_device(element_type, elements_bytes, embeddings_bytes, out=None, device=None, stream=None):
+    """The rows of compute_embeddings as a CUDA tensor [n, dim] (float32 for "angular", int8 for "angular_int"), or
+    written into `out`; for Granne.from_device_elements / GranneBuilder.from_device_elements.  device: out's device,
+    else the current one.  Returns when the rows are written."""
+    import torch
+
+    L = load_library()
+    kind = _embeddings_kind(element_type)
+    eb = np.frombuffer(elements_bytes, dtype=np.uint8)
+    mb = np.frombuffer(embeddings_bytes, dtype=np.uint8)
+    n, dim = C.c_uint64(), C.c_uint32()
+    _check(L.granne_b200_compute_embeddings_device(kind, _ptr(eb), eb.size, _ptr(mb), mb.size, 0, None, C.byref(n),
+                                                   C.byref(dim), None))
+    if device is None:
+        device = out.device.index if isinstance(out, torch.Tensor) and out.is_cuda else torch.cuda.current_device()
+    if out is None:
+        out = torch.empty((n.value, dim.value), dtype=torch.int8 if kind == ANGULAR_INT else torch.float32,
+                          device=torch.device("cuda", device))
+    _check_device_rows(kind, out)
+    if tuple(out.shape) != (n.value, dim.value) or out.device != torch.device("cuda", device):
+        raise ValueError("out must be a [%d, %d] tensor on cuda:%d" % (n.value, dim.value, device))
+    s = stream if stream is not None else torch.cuda.current_stream(out.device).cuda_stream
+    _check(L.granne_b200_compute_embeddings_device(kind, _ptr(eb), eb.size, _ptr(mb), mb.size, device,
+                                                   C.c_void_p(out.data_ptr()), C.byref(n), C.byref(dim),
+                                                   C.c_void_p(s)))
+    return out
+
+
+def compute_embeddings_and_save_to_disk(elements_path, embeddings_path, output_path, show_progress=True,
+                                        element_type="angular_int", device=0):
+    """granne.compute_embeddings_and_save_to_disk (py/src/lib.rs:132-147; parsing.rs:102-152) on the GPU, same
+    argument order.  The image is written through a memory map of the output file.  show_progress is accepted and
+    ignored."""
+    L = load_library()
+    kind = _embeddings_kind(element_type)
+    eb = np.memmap(elements_path, dtype=np.uint8, mode="r") if os.path.getsize(elements_path) else np.zeros(0, np.uint8)
+    mb = (np.memmap(embeddings_path, dtype=np.uint8, mode="r") if os.path.getsize(embeddings_path)
+          else np.zeros(0, np.uint8))
+    need = C.c_size_t()
+    _check(L.granne_b200_compute_embeddings(kind, _ptr(eb), eb.size, _ptr(mb), mb.size, device, None, 0,
+                                            C.byref(need)))
+    out = np.memmap(output_path, dtype=np.uint8, mode="w+", shape=(need.value,))
+    try:
+        _check(L.granne_b200_compute_embeddings(kind, _ptr(eb), eb.size, _ptr(mb), mb.size, device, _ptr(out),
+                                                out.size, C.byref(need)))
+        out.flush()
+    finally:
+        del out
 
 
 class GranneBuilder:

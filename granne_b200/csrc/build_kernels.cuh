@@ -414,4 +414,73 @@ __global__ void __launch_bounds__(32) make_elements_kernel(const float* __restri
     }
 }
 
+// compute_embeddings_and_save_to_disk (embeddings/parsing.rs:102-152), its first step: raw_i =
+// SumEmbeddings::get_embedding(i) (embeddings/mod.rs:112-143) for a window of elements, written as raw f32 rows.
+// make_elements_kernel then turns them into elements (the second step, `.into()`).
+struct SumRowsArgs {
+    const float* table;                 // embedding rows, dim f32 each (no padding)
+    const unsigned long long* offsets;  // n + 1 term offsets of the window's elements
+    unsigned long long term_base;       // the full term list's position of terms[0]: element r's terms are
+                                        // terms[offsets[r] - term_base .. offsets[r + 1] - term_base)
+    const uint32_t* terms;
+    unsigned long long n;
+    uint32_t dim;
+    int kind;     // output kind: kAngularI8 flags a NaN row, kAngularF32 any non-finite row
+    float* out;   // n x dim raw rows
+    int* status;  // kStatusNotFinite is or-ed in when a row is flagged
+};
+
+// Persistent warps, one element per warp at a time.  The term loop is the one of DistSum::dists: lane t holds the id
+// of term t, and four 32-float chunks of the row are accumulated per pass, so that four independent 128-byte loads
+// per term are in flight.  The first term's row is copied (-0.0 stays -0.0), the others are added in term order
+// (sum_into_f32); an element without terms is a row of zeros.  Four blocks of 8 warps per SM (62 registers: at the
+// default bound of one block, ptxas caps the kernel at 48 and spills).
+__global__ void __launch_bounds__(256, 4) sum_embeddings_kernel(const SumRowsArgs a) {
+    const int lane = threadIdx.x & 31;
+    const unsigned long long warps = (unsigned long long)gridDim.x * (blockDim.x / 32);
+    const int dim = (int)a.dim;
+    bool bad = false;
+    for (unsigned long long r = (unsigned long long)blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32; r < a.n;
+         r += warps) {
+        const unsigned long long tb = a.offsets[r] - a.term_base, te = a.offsets[r + 1] - a.term_base;
+        const uint32_t m = (uint32_t)(te - tb);
+        float* xb = a.out + r * dim;
+        for (int i0 = 0; i0 < dim; i0 += 128) {
+            const int i = i0 + lane;
+            const bool in0 = i < dim, in1 = i + 32 < dim, in2 = i + 64 < dim, in3 = i + 96 < dim;
+            float a0 = 0.0f, a1 = 0.0f, a2 = 0.0f, a3 = 0.0f;
+            for (uint32_t g = 0; g < m; g += 32) {
+                const uint32_t gm = (m - g) < 32u ? (m - g) : 32u;
+                const uint32_t my_term = ((uint32_t)lane < gm) ? __ldg(a.terms + tb + g + lane) : 0u;
+                for (uint32_t t = 0; t < gm; ++t) {
+                    const uint32_t term = __shfl_sync(kFullMask, my_term, t);
+                    const float* row = a.table + (size_t)term * dim + i;
+                    const float v0 = in0 ? __ldg(row) : 0.0f;
+                    const float v1 = in1 ? __ldg(row + 32) : 0.0f;
+                    const float v2 = in2 ? __ldg(row + 64) : 0.0f;
+                    const float v3 = in3 ? __ldg(row + 96) : 0.0f;
+                    if (g + t == 0) {  // x = row_0, then x += row_t in order
+                        a0 = v0, a1 = v1, a2 = v2, a3 = v3;
+                    } else {
+                        a0 = __fadd_rn(a0, v0);
+                        a1 = __fadd_rn(a1, v1);
+                        a2 = __fadd_rn(a2, v2);
+                        a3 = __fadd_rn(a3, v3);
+                    }
+                }
+            }
+            // angular_int: quantize's NotNan::new(|x|).unwrap() panics on NaN (angular_int.rs:31); angular: a
+            // non-finite sum normalises to a row holding NaN, and every distance to it panics (angular.rs:70)
+            const float lim = a.kind == kAngularI8 ? __int_as_float(0x7f800000) : __int_as_float(0x7f7fffff);
+            bad |= (in0 && !(fabsf(a0) <= lim)) || (in1 && !(fabsf(a1) <= lim)) || (in2 && !(fabsf(a2) <= lim)) ||
+                   (in3 && !(fabsf(a3) <= lim));
+            if (in0) xb[i] = a0;
+            if (in1) xb[i + 32] = a1;
+            if (in2) xb[i + 64] = a2;
+            if (in3) xb[i + 96] = a3;
+        }
+    }
+    if (__any_sync(kFullMask, bad) && lane == 0) atomicOr(a.status, kStatusNotFinite);
+}
+
 }  // namespace granne_b200

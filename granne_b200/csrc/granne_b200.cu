@@ -313,6 +313,19 @@ int stage_dense(Handle* h, const uint8_t* rows, uint64_t nrows, uint32_t dim, bo
     return GRANNE_B200_OK;
 }
 
+// SumEmbeddings::from_bytes (embeddings/mod.rs:56-61) on the host: the embedding table and the element term lists,
+// every term id checked against the table.
+int parse_sum_container(const uint8_t* el, size_t el_len, const uint8_t* emb, size_t emb_len, gb::DenseView* ev,
+                        gb::SumElements* se) {
+    std::string err;
+    if (!gb::parse_dense(emb, emb_len, 4, ev, &err)) return fail(GRANNE_B200_ERR_FORMAT, "embeddings: " + err);
+    if (!gb::parse_sum_elements(el, el_len, se, &err)) return fail(GRANNE_B200_ERR_FORMAT, err);
+    for (uint32_t t : se->terms)
+        if (t >= ev->num) return fail(GRANNE_B200_ERR_FORMAT, "element refers to a missing embedding id");
+    if (ev->dim > 4096) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "embeddings wider than 4096 are unsupported");
+    return GRANNE_B200_OK;
+}
+
 // Stages the element container (vectors / embedding table + element term lists) in HBM.
 int stage_elements(Handle* h, int kind, const uint8_t* el, size_t el_len, const uint8_t* emb, size_t emb_len) {
     std::string err;
@@ -321,12 +334,8 @@ int stage_elements(Handle* h, int kind, const uint8_t* el, size_t el_len, const 
     d.kind = kind;
     if (kind == GRANNE_B200_EMBEDDINGS) {
         gb::DenseView ev;
-        if (!gb::parse_dense(emb, emb_len, 4, &ev, &err)) return fail(GRANNE_B200_ERR_FORMAT, "embeddings: " + err);
         gb::SumElements se;
-        if (!gb::parse_sum_elements(el, el_len, &se, &err)) return fail(GRANNE_B200_ERR_FORMAT, err);
-        for (uint32_t t : se.terms)
-            if (t >= ev.num) return fail(GRANNE_B200_ERR_FORMAT, "element refers to a missing embedding id");
-        if (ev.dim > 4096) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "embeddings wider than 4096 are unsupported");
+        if ((rc = parse_sum_container(el, el_len, emb, emb_len, &ev, &se))) return rc;
         rc = stage_dense(h, ev.data, ev.num, (uint32_t)ev.dim);
         if (rc) return rc;
         d.num_elements = se.offsets.size() - 1;
@@ -347,6 +356,73 @@ int stage_elements(Handle* h, int kind, const uint8_t* el, size_t el_len, const 
         if (rc) return rc;
         d.num_elements = dv.num;
     }
+    return GRANNE_B200_OK;
+}
+
+// ---- compute_embeddings_and_save_to_disk (embeddings/parsing.rs:102-152) -------------------------------------------
+// The rows are made in windows of elements, so that the device holds the embedding table plus a constant window
+// (the reference makes them in 100 chunks for the same reason): at most kEmbWindowBytes of raw f32 rows and
+// kEmbWindowMaxRows rows, and at most kEmbWindowTerms term ids unless a single element holds more.
+constexpr uint64_t kEmbWindowBytes = 64ull << 20;
+constexpr uint64_t kEmbWindowMaxRows = 1ull << 20;
+constexpr uint64_t kEmbWindowTerms = 1ull << 24;
+
+struct EmbeddingsInput {
+    gb::DenseView table;
+    gb::SumElements el;
+    uint64_t n = 0;
+    uint32_t dim = 0;  // width of the output rows; 0 when there is no row to write (n == 0, or a table without rows)
+};
+
+// Every argument and image check of the compute_embeddings calls; runs on the host, before any device call.
+int check_embeddings_input(int kind, const void* el, size_t el_len, const void* emb, size_t emb_len,
+                           EmbeddingsInput* in) {
+    if (!el || !emb) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
+    if (kind != GRANNE_B200_ANGULAR && kind != GRANNE_B200_ANGULAR_INT)
+        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "compute_embeddings writes angular or angular_int vectors");
+    const int rc = parse_sum_container(static_cast<const uint8_t*>(el), el_len, static_cast<const uint8_t*>(emb),
+                                       emb_len, &in->table, &in->el);
+    if (rc) return rc;
+    in->n = in->el.offsets.size() - 1;
+    // an element without terms over a table without rows is the empty vector (embeddings/mod.rs:127-132), and a
+    // FixedWidthSliceVector of empty vectors keeps width 0
+    in->dim = in->n > 0 && in->table.num > 0 ? (uint32_t)in->table.dim : 0;
+    return GRANNE_B200_OK;
+}
+
+uint64_t emb_window_rows(uint32_t dim) {
+    return std::min(kEmbWindowMaxRows, std::max<uint64_t>(1, kEmbWindowBytes / ((uint64_t)dim * 4)));
+}
+
+// End of the window that starts at element r0.
+uint64_t emb_window_end(const EmbeddingsInput& in, uint64_t r0) {
+    const uint64_t* off = in.el.offsets.data();
+    uint64_t r1 = std::min(in.n, r0 + emb_window_rows(in.dim));
+    if (off[r1] - off[r0] > kEmbWindowTerms)
+        r1 = std::max<uint64_t>(r0 + 1, std::upper_bound(off + r0 + 1, off + r1 + 1, off[r0] + kEmbWindowTerms) - off - 1);
+    return r1;
+}
+
+// The two kernels for `nr` elements on `stream`: raw rows into d_raw, then Vector::from per row into d_out.  d_out may
+// be d_raw (ANGULAR): make_elements_kernel holds a row in shared memory before it writes the row back.
+int launch_embeddings(const EmbeddingsInput& in, int kind, int num_sms, const float* d_table,
+                      const unsigned long long* d_off, uint64_t term_base, const uint32_t* d_terms, uint64_t nr,
+                      float* d_raw, void* d_out, int* d_status, cudaStream_t stream) {
+    const gb::SumRowsArgs a{d_table, d_off, term_base, d_terms, nr, in.dim, kind, d_raw, d_status};
+    gb::sum_embeddings_kernel<<<(unsigned)std::min<uint64_t>((nr + 7) / 8, (uint64_t)num_sms * 4), 256, 0, stream>>>(a);
+    GB_CUDA(cudaGetLastError());
+    gb::make_elements_kernel<<<(unsigned)std::min<uint64_t>(nr, (uint64_t)num_sms * 32), 32, (size_t)in.dim * 4,
+                               stream>>>(d_raw, nr, in.dim, kind, d_out);
+    GB_CUDA(cudaGetLastError());
+    return GRANNE_B200_OK;
+}
+
+int embeddings_status(int* d_status) {
+    int bits = 0;
+    GB_CUDA(cudaMemcpy(&bits, d_status, 4, cudaMemcpyDeviceToHost));
+    if (bits & gb::kStatusNotFinite)
+        return fail(GRANNE_B200_ERR_NOT_FINITE,
+                    "an element's sum of embeddings is not finite (angular) or holds NaN (angular_int)");
     return GRANNE_B200_OK;
 }
 
@@ -1624,6 +1700,148 @@ int granne_b200_elements_from_raw_device(int element_kind, const float* d_raw, u
                                static_cast<cudaStream_t>(cuda_stream)>>>(d_raw, n, dim, element_kind, d_out);
     GB_CUDA(cudaGetLastError());
     return GRANNE_B200_OK;
+}
+
+// compute_embeddings_and_save_to_disk (embeddings/parsing.rs:102-152) into a caller buffer.  Two windows are in
+// flight on two streams: while one window's kernels run, the other's rows come back through pinned memory and the
+// next window's term lists go out.
+int granne_b200_compute_embeddings(int element_kind, const void* elements_bytes, size_t elements_len,
+                                   const void* embeddings_bytes, size_t embeddings_len, int device, void* out,
+                                   size_t cap, size_t* out_len) {
+    if (!out_len) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
+    return guarded([&] {
+        EmbeddingsInput in;
+        int rc = check_embeddings_input(element_kind, elements_bytes, elements_len, embeddings_bytes, embeddings_len,
+                                        &in);
+        if (rc) return rc;
+        const size_t row_bytes = (size_t)in.dim * (element_kind == GRANNE_B200_ANGULAR ? 4 : 1);
+        const size_t need = 8 + (size_t)in.n * row_bytes;
+        *out_len = need;
+        if (!out) return GRANNE_B200_OK;
+        if (cap < need) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "output buffer too small");
+        int sms = 0;
+        size_t optin = 0;
+        if ((rc = check_device(device, &sms, &optin))) return rc;
+        GB_DEVICE(device);
+        uint8_t* o = static_cast<uint8_t*>(out);
+        for (int b = 0; b < 8; ++b) o[b] = (uint8_t)((uint64_t)in.dim >> (8 * b));  // FixedWidthSliceVector::write
+        if (in.dim == 0) return GRANNE_B200_OK;
+
+        const uint64_t* off = in.el.offsets.data();
+        const uint64_t rows = std::min(in.n, emb_window_rows(in.dim));
+        Buffer<float> d_table;
+        Buffer<int> d_status;
+        if ((rc = dev_alloc(&d_table, in.table.num * in.dim)) || (rc = dev_alloc(&d_status, 1))) return rc;
+        GB_CUDA(cudaMemcpy(d_table.get(), in.table.data, in.table.num * in.dim * 4, cudaMemcpyHostToDevice));
+        GB_CUDA(cudaMemset(d_status.get(), 0, 4));
+        GB_CUDA(cudaStreamSynchronize(nullptr));  // the windows' streams do not wait for the legacy stream
+        struct Window {
+            Stream stream;  // declared first: destroyed after the buffers
+            Buffer<unsigned long long> d_off;
+            Buffer<uint32_t> d_terms;
+            Buffer<float> d_raw;
+            Buffer<int8_t> d_i8;
+            Pinned<unsigned long long> h_off;
+            Pinned<uint32_t> h_terms;
+            Pinned<uint8_t> h_out;
+            uint64_t r0 = 0, nr = 0;  // the elements in flight
+        } win[2];
+        for (Window& w : win) {
+            cudaStream_t s = nullptr;
+            GB_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+            w.stream.reset(s);
+            if ((rc = w.d_off.grow(rows + 1, s)) || (rc = w.d_raw.grow(rows * in.dim, s)) ||
+                (rc = w.h_off.grow(rows + 1, s)) || (rc = w.h_out.grow(rows * row_bytes, s)) ||
+                (element_kind == GRANNE_B200_ANGULAR_INT && (rc = w.d_i8.grow(rows * in.dim, s))))
+                return rc;
+        }
+        // waits for a window's rows and moves them into the image
+        auto land = [&](Window& w) {
+            if (!w.nr) return GRANNE_B200_OK;
+            GB_CUDA(cudaStreamSynchronize(w.stream.get()));
+            std::memcpy(o + 8 + w.r0 * row_bytes, w.h_out.get(), w.nr * row_bytes);
+            w.nr = 0;
+            return GRANNE_B200_OK;
+        };
+        uint64_t k = 0;
+        for (uint64_t r0 = 0; r0 < in.n; ++k) {
+            Window& w = win[k & 1];
+            cudaStream_t s = w.stream.get();
+            if ((rc = land(w))) return rc;
+            const uint64_t r1 = emb_window_end(in, r0), nr = r1 - r0, t0 = off[r0], nt = off[r1] - t0;
+            if ((rc = w.d_terms.grow(std::max<uint64_t>(nt, 1), s)) || (rc = w.h_terms.grow(std::max<uint64_t>(nt, 1), s)))
+                return rc;
+            std::memcpy(w.h_off.get(), off + r0, (nr + 1) * 8);
+            if (nt) std::memcpy(w.h_terms.get(), in.el.terms.data() + t0, nt * 4);
+            GB_CUDA(cudaMemcpyAsync(w.d_off.get(), w.h_off.get(), (nr + 1) * 8, cudaMemcpyHostToDevice, s));
+            if (nt) GB_CUDA(cudaMemcpyAsync(w.d_terms.get(), w.h_terms.get(), nt * 4, cudaMemcpyHostToDevice, s));
+            void* rows_out = element_kind == GRANNE_B200_ANGULAR ? static_cast<void*>(w.d_raw.get()) : w.d_i8.get();
+            if ((rc = launch_embeddings(in, element_kind, sms, d_table.get(), w.d_off.get(), t0, w.d_terms.get(), nr,
+                                        w.d_raw.get(), rows_out, d_status.get(), s)))
+                return rc;
+            GB_CUDA(cudaMemcpyAsync(w.h_out.get(), rows_out, nr * row_bytes, cudaMemcpyDeviceToHost, s));
+            w.r0 = r0;
+            w.nr = nr;
+            r0 = r1;
+        }
+        if ((rc = land(win[k & 1])) || (rc = land(win[(k + 1) & 1]))) return rc;
+        return embeddings_status(d_status.get());
+    });
+}
+
+// The rows of granne_b200_compute_embeddings, written to device memory on the caller's stream.
+int granne_b200_compute_embeddings_device(int element_kind, const void* elements_bytes, size_t elements_len,
+                                          const void* embeddings_bytes, size_t embeddings_len, int device,
+                                          void* d_out, uint64_t* out_n, uint32_t* out_dim, void* cuda_stream) {
+    if (!out_n || !out_dim) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
+    return guarded([&] {
+        EmbeddingsInput in;
+        int rc = check_embeddings_input(element_kind, elements_bytes, elements_len, embeddings_bytes, embeddings_len,
+                                        &in);
+        if (rc) return rc;
+        *out_n = in.n;
+        *out_dim = in.dim;
+        if (!d_out) return GRANNE_B200_OK;
+        int sms = 0;
+        size_t optin = 0;
+        if ((rc = check_device(device, &sms, &optin))) return rc;
+        GB_DEVICE(device);
+        if (in.dim == 0) return GRANNE_B200_OK;
+        cudaPointerAttributes at{};
+        if (cudaPointerGetAttributes(&at, d_out) != cudaSuccess || at.type != cudaMemoryTypeDevice ||
+            at.device != device) {
+            cudaGetLastError();
+            return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "d_out is not device memory of the requested device");
+        }
+        const cudaStream_t s = static_cast<cudaStream_t>(cuda_stream);
+        const uint64_t rows = std::min(in.n, emb_window_rows(in.dim));
+        Buffer<float> d_table, d_raw;
+        Buffer<unsigned long long> d_off;
+        Buffer<uint32_t> d_terms;
+        Buffer<int> d_status;
+        if ((rc = dev_alloc(&d_table, in.table.num * in.dim)) || (rc = dev_alloc(&d_off, in.n + 1)) ||
+            (rc = dev_alloc(&d_terms, in.el.terms.size())) || (rc = dev_alloc(&d_status, 1)) ||
+            (element_kind == GRANNE_B200_ANGULAR_INT && (rc = d_raw.grow(rows * in.dim, nullptr))))
+            return rc;
+        GB_CUDA(cudaMemcpy(d_table.get(), in.table.data, in.table.num * in.dim * 4, cudaMemcpyHostToDevice));
+        GB_CUDA(cudaMemcpy(d_off.get(), in.el.offsets.data(), (in.n + 1) * 8, cudaMemcpyHostToDevice));
+        if (!in.el.terms.empty())
+            GB_CUDA(cudaMemcpy(d_terms.get(), in.el.terms.data(), in.el.terms.size() * 4, cudaMemcpyHostToDevice));
+        GB_CUDA(cudaMemset(d_status.get(), 0, 4));
+        GB_CUDA(cudaStreamSynchronize(nullptr));  // the caller's stream may not wait for the legacy stream
+        for (uint64_t r0 = 0; r0 < in.n;) {
+            const uint64_t r1 = emb_window_end(in, r0), nr = r1 - r0;
+            float* raw = element_kind == GRANNE_B200_ANGULAR ? static_cast<float*>(d_out) + r0 * in.dim : d_raw.get();
+            void* rows_out = element_kind == GRANNE_B200_ANGULAR ? static_cast<void*>(raw)
+                                                                  : static_cast<int8_t*>(d_out) + r0 * in.dim;
+            if ((rc = launch_embeddings(in, element_kind, sms, d_table.get(), d_off.get() + r0, 0, d_terms.get(), nr,
+                                        raw, rows_out, d_status.get(), s)))
+                return rc;
+            r0 = r1;
+        }
+        GB_CUDA(cudaStreamSynchronize(s));
+        return embeddings_status(d_status.get());
+    });
 }
 
 // ---- compute_distance (py/src/lib.rs:71-89) -----------------------------------------------------------------------

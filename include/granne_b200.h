@@ -322,6 +322,27 @@ int granne_b200_elements_from_raw(int element_kind, const float* raw, uint64_t n
 int granne_b200_elements_from_raw_device(int element_kind, const float* d_raw, uint64_t n, uint32_t dim, int device,
                                          void* d_out, void* cuda_stream);
 
+/* compute_embeddings_and_save_to_disk (src/elements/embeddings/parsing.rs:102-152) as an elements file image: for every
+ * element of a SumEmbeddings container (elements_bytes, embeddings_bytes as in granne_b200_open), its raw sum of
+ * embeddings (embeddings/mod.rs:112-143) made into a vector.  kind ANGULAR_INT is the reference function:
+ * angular_int::Vector::from(sum), the quantised raw sum (angular_int.rs:19-45).  kind ANGULAR is SumEmbeddings::get
+ * per element (embeddings/mod.rs:164-166): the normalised sum, so searching these rows searches the SumEmbeddings
+ * container.  The image is FixedWidthSliceVector::write (u64 width | rows); with no element, or a table without rows,
+ * it is the 8-byte header of width 0.  Every argument and image check runs on the host before any device call
+ * (ERR_FORMAT as in granne_b200_open; ERR_INVALID_ARGUMENT for a bad kind, a null pointer, a table wider than 4096 or
+ * too small a `cap`).  A sum holding NaN (ANGULAR_INT; the reference panics) or any non-finite value (ANGULAR)
+ * returns ERR_NOT_FINITE.  The device holds the table and a fixed window of elements, whatever their number.
+ * out == NULL queries the size (no device needed). */
+int granne_b200_compute_embeddings(int element_kind, const void* elements_bytes, size_t elements_len,
+                                   const void* embeddings_bytes, size_t embeddings_len, int device, void* out,
+                                   size_t cap, size_t* out_len);
+/* The same rows, device-resident (n x dim, f32 or i8, memory of `device`) for granne_b200_open_device_elements /
+ * granne_b200_builder_new_device_elements.  d_out == NULL writes n and dim only.  Synchronises cuda_stream (NULL = the
+ * default stream) before returning, so that ERR_NOT_FINITE can be reported. */
+int granne_b200_compute_embeddings_device(int element_kind, const void* elements_bytes, size_t elements_len,
+                                          const void* embeddings_bytes, size_t embeddings_len, int device,
+                                          void* d_out, uint64_t* out_n, uint32_t* out_dim, void* cuda_stream);
+
 /* Granne::from_bytes (src/index/mod.rs:108-113) with the element container given as device rows. */
 int granne_b200_open_device_elements(const void* index_bytes, size_t index_len, int element_kind,
                                      const void* d_element_rows, uint64_t num_elements, uint32_t dim, int device,

@@ -71,6 +71,21 @@ struct Elements {
         check(granne_b200_elements_from_raw(static_cast<int>(kind), rows, n, dim, device, e.bytes.data(), need, &need));
         return e;
     }
+    // compute_embeddings_and_save_to_disk (src/elements/embeddings/parsing.rs:102-152): the sum of embeddings of every
+    // element of a SumEmbeddings container as an AngularInt (quantised raw sum, what the reference writes) or Angular
+    // (normalised sum: SumEmbeddings::get) container
+    static Elements compute_embeddings(ElementKind kind, const Elements& sum, int device = 0) {
+        Elements e;
+        e.kind = kind;
+        size_t need = 0;
+        check(granne_b200_compute_embeddings(static_cast<int>(kind), sum.bytes.data(), sum.bytes.size(),
+                                             sum.embeddings.data(), sum.embeddings.size(), device, nullptr, 0, &need));
+        e.bytes.resize(need);
+        check(granne_b200_compute_embeddings(static_cast<int>(kind), sum.bytes.data(), sum.bytes.size(),
+                                             sum.embeddings.data(), sum.embeddings.size(), device, e.bytes.data(),
+                                             need, &need));
+        return e;
+    }
     // Vectors::from_file / SumEmbeddings::from_files
     static Elements from_files(ElementKind kind, const std::string& elements_path,
                                const std::string& embeddings_path = std::string()) {
