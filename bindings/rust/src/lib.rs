@@ -98,6 +98,14 @@ extern "C" {
         m: *mut RawMulti, queries: *const c_void, nq: usize, query_format: c_int, max_search: u32, num_neighbors: u32,
         out_ids: *mut u64, out_dists: *mut f32, out_counts: *mut u32,
     ) -> c_int;
+    fn granne_b200_exact_search_batch(
+        h: *mut RawIndex, queries: *const c_void, nq: usize, query_format: c_int, num_neighbors: u32,
+        out_ids: *mut u32, out_dists: *mut f32, out_counts: *mut u32,
+    ) -> c_int;
+    fn granne_b200_multi_exact_search_batch(
+        m: *mut RawMulti, queries: *const c_void, nq: usize, query_format: c_int, num_neighbors: u32,
+        out_ids: *mut u64, out_dists: *mut f32, out_counts: *mut u32,
+    ) -> c_int;
 }
 
 pub const ANGULAR: c_int = 0; // angular::Vectors
@@ -222,6 +230,29 @@ impl GpuGranne {
             granne_b200_search_batch(
                 self.h, queries.as_ptr() as *const c_void, nq, query_format, max_search as u32, num_neighbors as u32,
                 ids.as_mut_ptr(), dists.as_mut_ptr(), counts.as_mut_ptr(), std::ptr::null_mut(),
+            )
+        });
+        (0..nq)
+            .map(|q| {
+                (0..counts[q] as usize)
+                    .map(|j| (ids[q * num_neighbors + j] as usize, dists[q * num_neighbors + j]))
+                    .collect()
+            })
+            .collect()
+    }
+    /// Exact k nearest neighbours (not a reference function): the first `min(k, len())` elements by
+    /// `(dist_to_element, id)`, the reference's distance bit for bit; `k <= 1024`.  The ground truth of recall.
+    pub fn exact_search_batch(
+        &self, queries: &[f32], nq: usize, query_format: c_int, num_neighbors: usize,
+    ) -> Vec<Vec<(usize, f32)>> {
+        assert_eq!(queries.len(), nq * self.dim);
+        let mut ids = vec![0u32; nq * num_neighbors];
+        let mut dists = vec![0f32; nq * num_neighbors];
+        let mut counts = vec![0u32; nq];
+        check(unsafe {
+            granne_b200_exact_search_batch(
+                self.h, queries.as_ptr() as *const c_void, nq, query_format, num_neighbors as u32, ids.as_mut_ptr(),
+                dists.as_mut_ptr(), counts.as_mut_ptr(),
             )
         });
         (0..nq)
@@ -412,6 +443,19 @@ impl GpuMultiGranne {
             granne_b200_multi_search_batch(self.m, elements.as_ptr() as *const c_void, nq, QUERY_ELEMENT,
                                            max_search as u32, num_neighbors as u32, ids.as_mut_ptr(), d.as_mut_ptr(),
                                            c.as_mut_ptr())
+        });
+        (0..nq)
+            .map(|i| (0..c[i] as usize).map(|j| (ids[i * num_neighbors + j] as usize, d[i * num_neighbors + j])).collect())
+            .collect()
+    }
+    /// Exact k nearest neighbours over every shard for a batch of normalised vectors; ids are global.
+    pub fn exact_search_batch(&self, elements: &[f32], num_neighbors: usize) -> Vec<Vec<(usize, f32)>> {
+        let nq = elements.len() / self.dim;
+        let (mut ids, mut d, mut c) = (vec![0u64; nq * num_neighbors], vec![0f32; nq * num_neighbors], vec![0u32; nq]);
+        check(unsafe {
+            granne_b200_multi_exact_search_batch(self.m, elements.as_ptr() as *const c_void, nq, QUERY_ELEMENT,
+                                                 num_neighbors as u32, ids.as_mut_ptr(), d.as_mut_ptr(),
+                                                 c.as_mut_ptr())
         });
         (0..nq)
             .map(|i| (0..c[i] as usize).map(|j| (ids[i * num_neighbors + j] as usize, d[i * num_neighbors + j])).collect())

@@ -11,6 +11,7 @@ ANGULAR, ANGULAR_INT, EMBEDDINGS = 0, 1, 2
 QUERY_RAW_F32, QUERY_ELEMENT = 0, 1
 _ELEMENT_TYPES = {"angular": ANGULAR, "angular_int": ANGULAR_INT, "embeddings": EMBEDDINGS}
 STATS_PER_QUERY = 4
+EXACT_MAX_K = 1024  # GRANNE_B200_EXACT_MAX_K
 DEFAULT_MAX_SEARCH = 200   # py/src/lib.rs:14
 DEFAULT_NUM_ELEMENTS = 10  # py/src/lib.rs:15
 
@@ -96,6 +97,9 @@ def load_library():
         "granne_b200_multi_num_parts": (sz, [vp]),
         "granne_b200_multi_shard_base": (u64, [vp, sz]),
         "granne_b200_multi_search_batch": (i32, [vp, vp, sz, i32, u32, u32, vp, vp, vp]),
+        "granne_b200_exact_search_batch": (i32, [vp, vp, sz, i32, u32, vp, vp, vp]),
+        "granne_b200_exact_search_batch_device": (i32, [vp, vp, sz, i32, u32, vp, vp, vp, vp]),
+        "granne_b200_multi_exact_search_batch": (i32, [vp, vp, sz, i32, u32, vp, vp, vp]),
         "granne_b200_device_bytes": (u64, [vp]),
     }
     for name, (res, args) in sig.items():
@@ -333,6 +337,65 @@ class Granne:
             return ids, dists, counts, stats
         return ids, dists, counts
 
+    def _host_queries(self, queries, already_element):
+        """(contiguous queries, query format) with search_batch's checks."""
+        q = np.asarray(queries)
+        fmt = QUERY_ELEMENT if already_element else QUERY_RAW_F32
+        if q.dtype == np.int8:
+            if self.element_kind != ANGULAR_INT:
+                raise ValueError("int8 queries need an angular_int index")
+            fmt = QUERY_ELEMENT
+            q = np.ascontiguousarray(q)
+        else:
+            q = np.ascontiguousarray(q, dtype=np.float32)
+            if fmt == QUERY_ELEMENT and self.element_kind == ANGULAR_INT:
+                raise ValueError("angular_int elements are int8")
+        if q.ndim != 2 or q.shape[1] != self.dim:
+            raise ValueError("queries must have shape (nq, %d)" % self.dim)
+        return q, fmt
+
+    def exact_search_batch(self, queries, num_elements=DEFAULT_NUM_ELEMENTS, already_element=False):
+        """Exact k nearest neighbours: the first min(k, len(self)) of all elements i < len(self) by (distance, id),
+        with the reference's distance bit for bit (granne_b200_exact_search_batch) — the ground truth of recall.
+        Not a reference function.  Queries as in search_batch; k <= EXACT_MAX_K.  Returns (ids, dists, counts) in
+        search_batch's layout."""
+        q, fmt = self._host_queries(queries, already_element)
+        nq, k = q.shape[0], int(num_elements)
+        ids = np.empty((nq, k), dtype=np.uint32)
+        dists = np.empty((nq, k), dtype=np.float32)
+        counts = np.empty(nq, dtype=np.uint32)
+        _check(load_library().granne_b200_exact_search_batch(self._h, _ptr(q), nq, fmt, k, _ptr(ids), _ptr(dists),
+                                                             _ptr(counts)))
+        return ids, dists, counts
+
+    def exact_search_batch_device(self, queries, num_elements=DEFAULT_NUM_ELEMENTS, already_element=False, out=None,
+                                  stream=None):
+        """Device-resident exact_search_batch: CUDA tensors in and out, asynchronous on `stream` (default: the current
+        torch stream); a NaN distance is reported by stream_status()."""
+        import torch
+
+        q = self._check_device_queries(queries)
+        fmt = QUERY_ELEMENT if already_element or q.dtype == torch.int8 else QUERY_RAW_F32
+        nq, k = q.shape[0], int(num_elements)
+        if out is not None:
+            for t, dt, shape in zip(out, (torch.int32, torch.float32, torch.int32), ((nq, k), (nq, k), (nq,))):
+                if (not t.is_cuda or t.device != q.device or t.dtype != dt or tuple(t.shape) != shape
+                        or not t.is_contiguous()):
+                    raise ValueError("out tensors must be contiguous (ids int32 [nq,k], dists float32 [nq,k], counts "
+                                     "int32 [nq]) on the queries' device")
+        else:
+            dev = q.device
+            out = (torch.empty((nq, k), dtype=torch.int32, device=dev),
+                   torch.empty((nq, k), dtype=torch.float32, device=dev),
+                   torch.empty((nq,), dtype=torch.int32, device=dev))
+        ids, dists, counts = out
+        s = stream if stream is not None else torch.cuda.current_stream(q.device).cuda_stream
+        s = getattr(s, "cuda_stream", s)
+        _check(load_library().granne_b200_exact_search_batch_device(
+            self._h, C.c_void_p(q.data_ptr()), nq, fmt, k, C.c_void_p(ids.data_ptr()), C.c_void_p(dists.data_ptr()),
+            C.c_void_p(counts.data_ptr()), C.c_void_p(s)))
+        return ids, dists, counts
+
     def _word_tables(self):
         """(WordDict, embeddings table, per-element id lists) for an "embeddings" index opened with words_path."""
         if getattr(self, "_words", None) is None:
@@ -507,6 +570,25 @@ class MultiGranne:
         counts = np.empty(nq, dtype=np.uint32)
         _check(load_library().granne_b200_multi_search_batch(self._h, _ptr(q), nq, fmt, int(max_search), k, _ptr(ids),
                                                              _ptr(dists), _ptr(counts)))
+        return ids, dists, counts
+
+    def exact_search_batch(self, queries, num_elements=DEFAULT_NUM_ELEMENTS, already_element=False):
+        """Exact k nearest neighbours over all shards (granne_b200_multi_exact_search_batch): GLOBAL uint64 ids."""
+        q = np.asarray(queries)
+        fmt = QUERY_ELEMENT if already_element else QUERY_RAW_F32
+        if q.dtype == np.int8:
+            fmt = QUERY_ELEMENT
+            q = np.ascontiguousarray(q)
+        else:
+            q = np.ascontiguousarray(q, dtype=np.float32)
+        if q.ndim != 2:
+            raise ValueError("queries must have shape (nq, dim)")
+        nq, k = q.shape[0], int(num_elements)
+        ids = np.empty((nq, k), dtype=np.uint64)
+        dists = np.empty((nq, k), dtype=np.float32)
+        counts = np.empty(nq, dtype=np.uint32)
+        _check(load_library().granne_b200_multi_exact_search_batch(self._h, _ptr(q), nq, fmt, k, _ptr(ids),
+                                                                   _ptr(dists), _ptr(counts)))
         return ids, dists, counts
 
     def close(self):

@@ -25,6 +25,7 @@
 #include "reorder.hpp"
 #include "build_kernels.cuh"
 #include "search_kernels.cuh"
+#include "exact_kernels.cuh"
 
 namespace gb = granne_b200;
 
@@ -141,6 +142,14 @@ struct Workspace {
     Buffer<uint32_t> d_vis;
     // retry pass: fewer CTAs, larger tables
     Buffer<uint32_t> d_vis_retry;
+    // exact search: prepared queries of a chunk, their dy (i8), a slab's distances, the running top-k lists, and for
+    // EMBEDDINGS a window of materialised rows (and a dense copy of the table when its staged rows are padded)
+    Buffer<uint8_t> d_exact_q;
+    Buffer<int> d_exact_qnorm;
+    Buffer<float> d_exact_dists;
+    Buffer<unsigned long long> d_exact_lists;
+    Buffer<float> d_exact_rows;
+    Buffer<float> d_exact_table;
 };
 
 }  // namespace
@@ -871,6 +880,139 @@ int error_from_bits(int bits) {
     return GRANNE_B200_OK;
 }
 
+// ---- exact k-NN (exact_kernels.cuh) -------------------------------------------------------------------------------
+// The slab buffer holds at most kExactSlabFloats distances (256 MB) and a slab at most kExactMaxSlabRows rows, so the
+// workspace of a call is bounded whatever nq and n are.
+constexpr uint64_t kExactSlabFloats = 64ull << 20;
+constexpr uint64_t kExactMaxSlabRows = 1ull << 20;
+
+// validate_search's rules without max_search, plus the bound on k.
+int validate_exact(const Handle* h, const void* q, size_t nq, int fmt, uint32_t k, const void* ids,
+                   const void* dists) {
+    if (!h) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "index handle is null");
+    if (fmt != GRANNE_B200_QUERY_RAW_F32 && fmt != GRANNE_B200_QUERY_ELEMENT)
+        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "unknown query format");
+    if (k > GRANNE_B200_EXACT_MAX_K)
+        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "num_neighbors exceeds GRANNE_B200_EXACT_MAX_K (1024)");
+    if (nq > 0xFFFFFFF0ull) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "too many queries in one batch");
+    if (nq && (!q || (k && (!ids || !dists)))) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null buffer");
+    return GRANNE_B200_OK;
+}
+
+// Distances of the prepared query chunk (qc queries in w->d_exact_q) to `nrows` rows, slab by slab, each slab's keys
+// merged into the running lists.  Row r has id base + r.
+int exact_scan_rows(Handle* h, Workspace* w, uint32_t qc, uint32_t k, const void* rows, uint64_t nrows,
+                    uint32_t row_stride, uint32_t vec_group, uint64_t base, uint64_t slab, cudaStream_t stream) {
+    const gb::DeviceIndex& d = h->dev;
+    for (uint64_t s0 = 0; s0 < nrows; s0 += slab) {
+        const uint64_t ns = std::min(slab, nrows - s0);
+        gb::ExactScanArgs a{};
+        a.row_stride = row_stride;
+        a.vec_group = vec_group;
+        a.nrows = ns;
+        a.dim = d.dim;
+        a.full = d.full;
+        a.tail = d.tail;
+        a.queries = w->d_exact_q.get();
+        a.qnorm = w->d_exact_qnorm.get();
+        a.nq = qc;
+        a.dists = w->d_exact_dists.get();
+        a.ld = slab;
+        a.error = w->d_error;
+        const dim3 grid((unsigned)((ns + gb::kExactRB - 1) / gb::kExactRB), (qc + gb::kExactQB - 1) / gb::kExactQB);
+        if (d.kind == gb::kAngularI8) {
+            a.rows = static_cast<const int8_t*>(rows) + s0 * row_stride;
+            gb::exact_scan_i8_kernel<<<grid, 256, 0, stream>>>(a);
+        } else {
+            a.rows = static_cast<const float*>(rows) + s0 * row_stride;
+            gb::exact_scan_f32_kernel<<<grid, 256, 0, stream>>>(a);
+        }
+        h->launches++;
+        GB_CUDA(cudaGetLastError());
+        gb::exact_select_kernel<<<qc, gb::kExactSelThreads, 0, stream>>>(w->d_exact_dists.get(), slab, ns,
+                                                                         (uint32_t)(base + s0), k,
+                                                                         w->d_exact_lists.get());
+        h->launches++;
+        GB_CUDA(cudaGetLastError());
+    }
+    return GRANNE_B200_OK;
+}
+
+// Enqueues one exact search on `stream`: nq queries (device memory, the caller's format) against [0, Index::len),
+// results in search_batch's layout.  A NaN distance or query sets kStatusNotFinite in w->d_error.
+int enqueue_exact(Handle* h, Workspace* w, const void* d_queries, size_t nq, int fmt, uint32_t k, uint32_t* d_ids,
+                  float* d_dists, uint32_t* d_counts, cudaStream_t stream) {
+    const gb::DeviceIndex& d = h->dev;
+    const uint64_t n = h->index_len;
+    const uint32_t count = (uint32_t)std::min<uint64_t>(k, n);
+    const bool i8 = d.kind == gb::kAngularI8, emb = d.kind == gb::kSumEmbeddings;
+    const bool scan = k > 0 && n > 0;
+    const size_t in_row = (i8 && fmt == GRANNE_B200_QUERY_ELEMENT) ? d.dim : (size_t)d.dim * 4;
+    const size_t qc_max = std::min<size_t>(nq, gb::kExactMaxChunk);
+    uint64_t slab = 0;
+    const float* table = static_cast<const float*>(d.vectors);
+    uint64_t wrows = 0;
+    int rc;
+    if (scan) {
+        slab = std::min<uint64_t>(kExactMaxSlabRows, kExactSlabFloats / qc_max) / gb::kExactRB * gb::kExactRB;
+        slab = std::min<uint64_t>(slab, (n + gb::kExactRB - 1) / gb::kExactRB * gb::kExactRB);
+        const size_t qrow = i8 ? d.row_stride : (size_t)d.dim * 4;
+        if ((rc = w->d_exact_q.grow(std::max<size_t>(qc_max * qrow, 16), stream)) ||
+            (rc = w->d_exact_qnorm.grow(qc_max, stream)) || (rc = w->d_exact_dists.grow(qc_max * slab, stream)) ||
+            (rc = w->d_exact_lists.grow(qc_max * gb::kExactMaxK, stream)))
+            return rc;
+        if (emb) {
+            // SumEmbeddings::get rows, window by window (compute_embeddings' ANGULAR rows, which search exactly like
+            // the container); the staged table's rows are padded to a multiple of 4 floats, the sum kernel reads
+            // dense rows
+            wrows = std::min<uint64_t>(n, emb_window_rows(std::max<uint32_t>(d.dim, 1)));
+            if ((rc = w->d_exact_rows.grow(std::max<size_t>(wrows * d.dim, 16), stream))) return rc;
+            if (d.row_stride != d.dim && d.num_vectors) {
+                if ((rc = w->d_exact_table.grow((size_t)d.num_vectors * d.dim, stream))) return rc;
+                GB_CUDA(cudaMemcpy2DAsync(w->d_exact_table.get(), (size_t)d.dim * 4, d.vectors,
+                                          (size_t)d.row_stride * 4, (size_t)d.dim * 4, d.num_vectors,
+                                          cudaMemcpyDeviceToDevice, stream));
+                table = w->d_exact_table.get();
+            }
+        }
+    }
+    for (size_t c0 = 0; c0 < nq; c0 += gb::kExactMaxChunk) {
+        const uint32_t qc = (uint32_t)std::min<size_t>(gb::kExactMaxChunk, nq - c0);
+        if (scan) {
+            GB_CUDA(cudaMemsetAsync(w->d_exact_lists.get(), 0xFF, (size_t)qc * gb::kExactMaxK * 8, stream));
+            gb::exact_prepare_kernel<<<(unsigned)std::min<uint64_t>(qc, (uint64_t)h->num_sms * 32), 32, 0, stream>>>(
+                d, static_cast<const uint8_t*>(d_queries) + c0 * in_row, fmt, qc, w->d_exact_q.get(),
+                w->d_exact_qnorm.get(), w->d_error);
+            h->launches++;
+            GB_CUDA(cudaGetLastError());
+            if (emb) {
+                EmbeddingsInput in;
+                in.dim = d.dim;
+                for (uint64_t r0 = 0; r0 < n; r0 += wrows) {
+                    const uint64_t nr = std::min(wrows, n - r0);
+                    if ((rc = launch_embeddings(in, gb::kAngularF32, h->num_sms, table, d.sum_offsets + r0, 0,
+                                                d.sum_terms, nr, w->d_exact_rows.get(), w->d_exact_rows.get(),
+                                                w->d_error, stream)))
+                        return rc;
+                    h->launches += 2;
+                    if ((rc = exact_scan_rows(h, w, qc, k, w->d_exact_rows.get(), nr, d.dim, 1, r0, slab, stream)))
+                        return rc;
+                }
+            } else if ((rc = exact_scan_rows(h, w, qc, k, d.vectors, n, d.row_stride, d.vec_group, 0, slab, stream))) {
+                return rc;
+            }
+        }
+        const uint64_t outs = std::max<uint64_t>((uint64_t)qc * k, d_counts ? qc : 0);
+        if (outs == 0) continue;
+        gb::exact_write_kernel<<<(unsigned)((outs + 255) / 256), 256, 0, stream>>>(
+            w->d_exact_lists.get(), qc, k, count, d_ids ? d_ids + c0 * k : nullptr, d_dists ? d_dists + c0 * k : nullptr,
+            d_counts ? d_counts + c0 : nullptr);
+        h->launches++;
+        GB_CUDA(cudaGetLastError());
+    }
+    return GRANNE_B200_OK;
+}
+
 // ---- GranneBuilder (src/index/mod.rs:295-531, 645-960) on the device ---------------------------------------------
 struct PairLaunch {
     Handle* h;
@@ -1217,6 +1359,33 @@ int granne_b200_get_element(const granne_b200_index* hc, uint64_t idx, void* out
     });
 }
 
+// One workspace per caller stream: calls on the same stream are serialised by the stream itself, so the status words /
+// slow-path buffers can be reused; the error word stays sticky until granne_b200_stream_status().
+static int stream_workspace(granne_b200_index* h, cudaStream_t stream, Workspace** out) {
+    Workspace* w = nullptr;
+    {
+        std::lock_guard<std::mutex> g(h->pool_mu);
+        auto it = h->stream_ws.find(stream);
+        if (it != h->stream_ws.end()) w = it->second.get();
+    }
+    if (!w) {
+        std::unique_ptr<Workspace> fresh;
+        int rc;
+        if ((rc = ws_acquire(h, &fresh))) return rc;
+        cudaError_t e = cudaMemset(fresh->d_error, 0, 4 * sizeof(int));
+        {
+            std::lock_guard<std::mutex> g(h->pool_mu);
+            auto it = h->stream_ws.find(stream);  // two threads may meet here on the first use of a stream
+            if (it == h->stream_ws.end()) it = h->stream_ws.emplace(stream, std::move(fresh)).first;
+            w = it->second.get();
+        }
+        if (fresh) ws_release(h, std::move(fresh));  // lost that race: back to the pool
+        GB_CUDA(e);
+    }
+    *out = w;
+    return GRANNE_B200_OK;
+}
+
 static int search_device_impl(granne_b200_index* h, const void* d_queries, size_t nq, int query_format,
                               uint32_t max_search, uint32_t num_neighbors, uint32_t* d_out_ids, float* d_out_dists,
                               uint32_t* d_out_counts, uint64_t* d_out_stats, void* cuda_stream,
@@ -1241,28 +1410,8 @@ static int search_device_impl(granne_b200_index* h, const void* d_queries, size_
             GB_CUDA(cudaGetLastError());
             return GRANNE_B200_OK;
         }
-        // One workspace per caller stream: calls on the same stream are serialised by the stream itself, so the
-        // status words / slow-path buffers can be reused; the error word stays sticky until
-        // granne_b200_stream_status().
         Workspace* w = nullptr;
-        {
-            std::lock_guard<std::mutex> g(h->pool_mu);
-            auto it = h->stream_ws.find(stream);
-            if (it != h->stream_ws.end()) w = it->second.get();
-        }
-        if (!w) {
-            std::unique_ptr<Workspace> fresh;
-            if ((rc = ws_acquire(h, &fresh))) return rc;
-            cudaError_t e = cudaMemset(fresh->d_error, 0, 4 * sizeof(int));
-            {
-                std::lock_guard<std::mutex> g(h->pool_mu);
-                auto it = h->stream_ws.find(stream);  // two threads may meet here on the first use of a stream
-                if (it == h->stream_ws.end()) it = h->stream_ws.emplace(stream, std::move(fresh)).first;
-                w = it->second.get();
-            }
-            if (fresh) ws_release(h, std::move(fresh));  // lost that race: back to the pool
-            GB_CUDA(e);
-        }
+        if ((rc = stream_workspace(h, stream, &w))) return rc;
         return enqueue_search(h, w, d_queries, nq, query_format, max_search, num_neighbors, d_out_ids, d_out_dists,
                               d_out_counts, reinterpret_cast<unsigned long long*>(d_out_stats), stream, false, pg);
     });
@@ -1373,6 +1522,65 @@ int granne_b200_search_batch(granne_b200_index* h, const void* queries, size_t n
         }();
         ws_release(h, std::move(ws));  // back to the pool on every path
         return status;
+    });
+}
+
+int granne_b200_exact_search_batch(granne_b200_index* h, const void* queries, size_t nq, int query_format,
+                                   uint32_t num_neighbors, uint32_t* out_ids, float* out_dists, uint32_t* out_counts) {
+    int rc = validate_exact(h, queries, nq, query_format, num_neighbors, out_ids, out_dists);
+    if (rc) return rc;
+    if (nq == 0) return GRANNE_B200_OK;
+    return guarded([&] {
+        GB_DEVICE(h->device);
+        const size_t k = num_neighbors;
+        const bool i8q = h->dev.kind == gb::kAngularI8 && query_format == GRANNE_B200_QUERY_ELEMENT;
+        const size_t qbytes = nq * h->dev.dim * (i8q ? 1 : 4);
+        std::unique_ptr<Workspace> ws;
+        if ((rc = ws_acquire(h, &ws))) return rc;
+        Workspace* w = ws.get();
+        const int status = [&] {
+            if ((rc = ws_reserve(w, qbytes, nq, k))) return rc;
+            cudaStream_t stream = w->stream.get();
+            // pinned staging layout: queries | ids | dists | counts | error
+            uint8_t* hp = w->h_pinned.get();
+            uint32_t* hids = reinterpret_cast<uint32_t*>(hp + ((qbytes + 15) & ~size_t(15)));
+            float* hd = reinterpret_cast<float*>(hids + nq * k);
+            uint32_t* hc = reinterpret_cast<uint32_t*>(hd + nq * k);
+            int* herr = reinterpret_cast<int*>(hc + nq);
+            std::memcpy(hp, queries, qbytes);
+            GB_CUDA(cudaMemcpyAsync(w->d_queries.get(), hp, qbytes, cudaMemcpyHostToDevice, stream));
+            GB_CUDA(cudaMemsetAsync(w->d_error, 0, 4 * sizeof(int), stream));
+            rc = enqueue_exact(h, w, w->d_queries.get(), nq, query_format, num_neighbors, w->d_ids.get(), w->d_dists,
+                               w->d_counts, stream);
+            if (rc) return rc;
+            GB_CUDA(cudaMemcpyAsync(hids, w->d_ids.get(), (2 * nq * k + nq) * 4, cudaMemcpyDeviceToHost, stream));
+            GB_CUDA(cudaMemcpyAsync(herr, w->d_error, 4 * sizeof(int), cudaMemcpyDeviceToHost, stream));
+            GB_CUDA(cudaStreamSynchronize(stream));
+            if (k) {
+                std::memcpy(out_ids, hids, nq * k * 4);
+                std::memcpy(out_dists, hd, nq * k * 4);
+            }
+            if (out_counts) std::memcpy(out_counts, hc, nq * 4);
+            return error_from_bits(herr[0]);
+        }();
+        ws_release(h, std::move(ws));  // back to the pool on every path
+        return status;
+    });
+}
+
+int granne_b200_exact_search_batch_device(granne_b200_index* h, const void* d_queries, size_t nq, int query_format,
+                                          uint32_t num_neighbors, uint32_t* d_out_ids, float* d_out_dists,
+                                          uint32_t* d_out_counts, void* cuda_stream) {
+    int rc = validate_exact(h, d_queries, nq, query_format, num_neighbors, d_out_ids, d_out_dists);
+    if (rc) return rc;
+    if (nq == 0) return GRANNE_B200_OK;
+    return guarded([&] {
+        GB_DEVICE(h->device);
+        cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+        Workspace* w = nullptr;
+        if ((rc = stream_workspace(h, stream, &w))) return rc;
+        return enqueue_exact(h, w, d_queries, nq, query_format, num_neighbors, d_out_ids, d_out_dists, d_out_counts,
+                             stream);
     });
 }
 
@@ -2182,13 +2390,15 @@ uint64_t granne_b200_multi_shard_base(const granne_b200_multi* m, size_t s) {
     return (m && s < m->base.size()) ? m->base[s] : 0;
 }
 
-int granne_b200_multi_search_batch(granne_b200_multi* m, const void* queries, size_t nq, int query_format,
-                                   uint32_t max_search, uint32_t num_neighbors, uint64_t* out_ids, float* out_dists,
-                                   uint32_t* out_counts) {
-    if (!m) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "multi handle is null");
-    if (nq == 0) return GRANNE_B200_OK;
-    if (!queries || (num_neighbors && (!out_ids || !out_dists)))
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null buffer");
+}  // extern "C"
+
+namespace {
+
+// A batch on a multi handle: `part(handle, queries, nq, ids, dists, counts)` runs the single-device call.  REPLICATED
+// slices the queries over the devices; RANGE_PARTITIONED runs every query on every shard and merges the shard lists.
+template <class Part>
+int multi_batch(granne_b200_multi* m, const void* queries, size_t nq, int query_format, uint32_t num_neighbors,
+                uint64_t* out_ids, float* out_dists, uint32_t* out_counts, Part&& part) {
     return guarded([&] {
         const size_t n = m->parts.size(), k = num_neighbors;
         const bool i8q = m->kind == GRANNE_B200_ANGULAR_INT && query_format == GRANNE_B200_QUERY_ELEMENT;
@@ -2202,8 +2412,7 @@ int granne_b200_multi_search_batch(granne_b200_multi* m, const void* queries, si
             int rc = for_each_part(n, [&](size_t i) {
                 const size_t b = i * per + std::min(i, extra), cntq = per + (i < extra ? 1 : 0);
                 if (cntq == 0) return (int)GRANNE_B200_OK;
-                return granne_b200_search_batch(m->parts[i], q + b * qrow, cntq, query_format, max_search, num_neighbors,
-                                                ids.data() + b * k, out_dists + b * k, cnt.data() + b, nullptr);
+                return part(m->parts[i], q + b * qrow, cntq, ids.data() + b * k, out_dists + b * k, cnt.data() + b);
             });
             if (rc) return rc;
             for (size_t i = 0; i < nq * k; ++i) out_ids[i] = ids[i] == gb::kUnusedId ? ~0ull : (uint64_t)ids[i];
@@ -2214,8 +2423,7 @@ int granne_b200_multi_search_batch(granne_b200_multi* m, const void* queries, si
         std::vector<uint32_t> ids(n * nq * k);
         std::vector<float> ds(n * nq * k);
         int rc = for_each_part(n, [&](size_t i) {
-            return granne_b200_search_batch(m->parts[i], q, nq, query_format, max_search, num_neighbors,
-                                            ids.data() + i * nq * k, ds.data() + i * nq * k, nullptr, nullptr);
+            return part(m->parts[i], q, nq, ids.data() + i * nq * k, ds.data() + i * nq * k, nullptr);
         });
         if (rc) return rc;
         std::vector<size_t> cur(n);
@@ -2251,6 +2459,39 @@ int granne_b200_multi_search_batch(granne_b200_multi* m, const void* queries, si
         }
         return GRANNE_B200_OK;
     });
+}
+
+}  // namespace
+
+extern "C" {
+
+int granne_b200_multi_search_batch(granne_b200_multi* m, const void* queries, size_t nq, int query_format,
+                                   uint32_t max_search, uint32_t num_neighbors, uint64_t* out_ids, float* out_dists,
+                                   uint32_t* out_counts) {
+    if (!m) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "multi handle is null");
+    if (nq == 0) return GRANNE_B200_OK;
+    if (!queries || (num_neighbors && (!out_ids || !out_dists)))
+        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null buffer");
+    return multi_batch(m, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts,
+                       [&](granne_b200_index* h, const void* q, size_t cnt, uint32_t* ids, float* ds, uint32_t* c) {
+                           return granne_b200_search_batch(h, q, cnt, query_format, max_search, num_neighbors, ids,
+                                                           ds, c, nullptr);
+                       });
+}
+
+// Each shard's exact answer is exact, and a shard's ids are monotone in the global ids, so merging the shard lists by
+// (distance, global id) gives the exact answer over the union of the shards.
+int granne_b200_multi_exact_search_batch(granne_b200_multi* m, const void* queries, size_t nq, int query_format,
+                                         uint32_t num_neighbors, uint64_t* out_ids, float* out_dists,
+                                         uint32_t* out_counts) {
+    if (!m) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "multi handle is null");
+    int rc = validate_exact(m->parts[0], queries, nq, query_format, num_neighbors, out_ids, out_dists);
+    if (rc) return rc;
+    if (nq == 0) return GRANNE_B200_OK;
+    return multi_batch(m, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts,
+                       [&](granne_b200_index* h, const void* q, size_t cnt, uint32_t* ids, float* ds, uint32_t* c) {
+                           return granne_b200_exact_search_batch(h, q, cnt, query_format, num_neighbors, ids, ds, c);
+                       });
 }
 
 }  // extern "C"

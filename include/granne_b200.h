@@ -163,6 +163,34 @@ int granne_b200_search_batch_device_gather(granne_b200_index* h, const void* d_q
                                            const granne_b200_peer_gather* gather, uint32_t* d_out_counts,
                                            uint64_t* d_out_stats, void* cuda_stream);
 
+/* ---- exact k-nearest neighbours -------------------------------------------------------------------------------------
+ * NOT a reference function: the reference's distance and result order applied to every element, the ground truth the
+ * approximate search is measured against (recall).  For n = granne_b200_len(h) (Index::len) and a query q the result is
+ * the first min(k, n) entries of
+ *     sort ascending { (dist_to_element(q, i), i) : 0 <= i < n }
+ * with dist_to_element the reference's distance of the handle's element kind (src/index/mod.rs:1012; angular.rs:63-74,
+ * math.rs:16-42; angular_int.rs:47-59; embeddings/mod.rs:164-174), bit for bit, and the (NotNan<f32>, usize) order of
+ * into_sorted_vec (src/index/mod.rs:1036).  Elements past Index::len (a container larger than the index) are never
+ * returned: this is the set granne_b200_search_batch can return.  If max_search >= n and every bottom-layer node is
+ * reachable from the entry point, the reference's search expands every node and returns exactly this answer.
+ *   queries        as granne_b200_search_batch (RAW_F32 normalised / quantised, or ELEMENT); there is no max_search
+ *   num_neighbors  k, 0..GRANNE_B200_EXACT_MAX_K; more is ERR_INVALID_ARGUMENT
+ *   out_ids        nq x k u32, padded with 0xFFFFFFFF; out_dists nq x k f32, padded with +inf
+ *   out_counts     nq u32 (may be NULL): min(k, n), so 0 when k == 0 or n == 0
+ * nq == 0, k == 0 and n == 0 are valid; no element is read when k == 0 or n == 0.  A NaN distance returns
+ * GRANNE_B200_ERR_NOT_FINITE, as in search; the exact scan meets every element, so a single NaN element makes every call
+ * with nq > 0, k > 0 fail (search may step around it).  Argument checks run on the host before any device call.  Safe
+ * concurrently with the search calls on the same handle. */
+#define GRANNE_B200_EXACT_MAX_K 1024
+int granne_b200_exact_search_batch(granne_b200_index* h, const void* queries, size_t nq, int query_format,
+                                   uint32_t num_neighbors, uint32_t* out_ids, float* out_dists, uint32_t* out_counts);
+/* Same with DEVICE pointers and an optional cudaStream_t (NULL = the default stream), asynchronous like
+ * granne_b200_search_batch_device: it uses that stream's workspace, and ERR_NOT_FINITE is reported by
+ * granne_b200_stream_status after the stream is synchronised. */
+int granne_b200_exact_search_batch_device(granne_b200_index* h, const void* d_queries, size_t nq, int query_format,
+                                          uint32_t num_neighbors, uint32_t* d_out_ids, float* d_out_dists,
+                                          uint32_t* d_out_counts, void* cuda_stream);
+
 /* The device-pointer calls keep one workspace per distinct caller stream (status words, per-warp visited tables) until
  * granne_b200_close.  A caller that retires a stream returns its workspace with this call (it synchronises the stream;
  * an error raised by its last batches is reported by the next granne_b200_stream_status). */
@@ -213,6 +241,12 @@ uint64_t granne_b200_multi_shard_base(const granne_b200_multi* m, size_t s);
 int granne_b200_multi_search_batch(granne_b200_multi* m, const void* queries, size_t nq, int query_format,
                                    uint32_t max_search, uint32_t num_neighbors, uint64_t* out_ids, float* out_dists,
                                    uint32_t* out_counts);
+/* granne_b200_exact_search_batch over a multi handle, with u64 GLOBAL ids like granne_b200_multi_search_batch.
+ * REPLICATED slices the queries over the devices; RANGE_PARTITIONED runs the exact scan on every shard and merges by
+ * (distance, global id): the exact answer over the union of the shards' Index::len ranges. */
+int granne_b200_multi_exact_search_batch(granne_b200_multi* m, const void* queries, size_t nq, int query_format,
+                                         uint32_t num_neighbors, uint64_t* out_ids, float* out_dists,
+                                         uint32_t* out_counts);
 
 /* Host-only helpers (no device needed): the loader's view of an index image.
  * granne_b200_inspect_index replaces io::read_layer_sizes + Index::num_layers/layer_len on raw bytes

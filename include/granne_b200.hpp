@@ -206,6 +206,20 @@ public:
                 out[q].emplace_back(ids[q * num_neighbors + j], dists[q * num_neighbors + j]);
         return out;
     }
+    // Exact k nearest neighbours (granne_b200_exact_search_batch): the first min(k, len()) elements by (distance, id),
+    // the reference's distance bit for bit.  Not a reference function: the ground truth of recall.
+    std::vector<SearchResult> exact_search_batch(const void* queries, size_t nq, int query_format,
+                                                 size_t num_neighbors) const {
+        std::vector<uint32_t> ids(nq * num_neighbors), counts(nq);
+        std::vector<float> dists(nq * num_neighbors);
+        check(granne_b200_exact_search_batch(h_, queries, nq, query_format, static_cast<uint32_t>(num_neighbors),
+                                             ids.data(), dists.data(), counts.data()));
+        std::vector<SearchResult> out(nq);
+        for (size_t q = 0; q < nq; ++q)
+            for (uint32_t j = 0; j < counts[q]; ++j)
+                out[q].emplace_back(ids[q * num_neighbors + j], dists[q * num_neighbors + j]);
+        return out;
+    }
 
     // Granne::reorder (reorder.rs:59-82) / reorder_by_keys (:89-124): reorders index and elements, returns the order
     // (`order[i] == j`: element j moved to i).
@@ -320,6 +334,20 @@ public:
         check(granne_b200_multi_search_batch(h_, queries.data(), nq, GRANNE_B200_QUERY_RAW_F32,
                                              static_cast<uint32_t>(max_search), static_cast<uint32_t>(num_neighbors),
                                              ids.data(), d.data(), c.data()));
+        std::vector<Result> out(nq);
+        for (size_t i = 0; i < nq; ++i)
+            for (uint32_t j = 0; j < c[i]; ++j) out[i].emplace_back(ids[i * num_neighbors + j], d[i * num_neighbors + j]);
+        return out;
+    }
+    // exact k nearest neighbours over every shard for nq raw f32 queries (granne_b200_multi_exact_search_batch)
+    std::vector<Result> exact_search_batch_raw(const std::vector<float>& queries, size_t num_neighbors) const {
+        const size_t nq = dim_ ? queries.size() / dim_ : 0;
+        std::vector<uint64_t> ids(nq * num_neighbors);
+        std::vector<float> d(nq * num_neighbors);
+        std::vector<uint32_t> c(nq);
+        check(granne_b200_multi_exact_search_batch(h_, queries.data(), nq, GRANNE_B200_QUERY_RAW_F32,
+                                                   static_cast<uint32_t>(num_neighbors), ids.data(), d.data(),
+                                                   c.data()));
         std::vector<Result> out(nq);
         for (size_t i = 0; i < nq; ++i)
             for (uint32_t j = 0; j < c[i]; ++j) out[i].emplace_back(ids[i * num_neighbors + j], d[i * num_neighbors + j]);
