@@ -106,6 +106,18 @@ extern "C" {
         m: *mut RawMulti, queries: *const c_void, nq: usize, query_format: c_int, num_neighbors: u32,
         out_ids: *mut u64, out_dists: *mut f32, out_counts: *mut u32,
     ) -> c_int;
+    fn granne_b200_set_rerank_elements(h: *mut RawIndex, elements: *const c_void, elements_len: usize) -> c_int;
+    fn granne_b200_search_rerank_batch(
+        h: *mut RawIndex, queries: *const f32, nq: usize, query_format: c_int, max_search: u32, num_candidates: u32,
+        num_neighbors: u32, out_ids: *mut u32, out_dists: *mut f32, out_counts: *mut u32, out_stats: *mut u64,
+    ) -> c_int;
+    fn granne_b200_multi_set_rerank_elements(
+        m: *mut RawMulti, elements: *const *const c_void, elements_len: *const usize,
+    ) -> c_int;
+    fn granne_b200_multi_search_rerank_batch(
+        m: *mut RawMulti, queries: *const f32, nq: usize, query_format: c_int, max_search: u32, num_candidates: u32,
+        num_neighbors: u32, out_ids: *mut u64, out_dists: *mut f32, out_counts: *mut u32,
+    ) -> c_int;
 }
 
 pub const ANGULAR: c_int = 0; // angular::Vectors

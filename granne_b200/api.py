@@ -12,6 +12,7 @@ QUERY_RAW_F32, QUERY_ELEMENT = 0, 1
 _ELEMENT_TYPES = {"angular": ANGULAR, "angular_int": ANGULAR_INT, "embeddings": EMBEDDINGS}
 STATS_PER_QUERY = 4
 EXACT_MAX_K = 1024  # GRANNE_B200_EXACT_MAX_K
+RERANK_MAX_CANDIDATES = 1024  # GRANNE_B200_RERANK_MAX_CANDIDATES
 DEFAULT_MAX_SEARCH = 200   # py/src/lib.rs:14
 DEFAULT_NUM_ELEMENTS = 10  # py/src/lib.rs:15
 
@@ -100,6 +101,12 @@ def load_library():
         "granne_b200_exact_search_batch": (i32, [vp, vp, sz, i32, u32, vp, vp, vp]),
         "granne_b200_exact_search_batch_device": (i32, [vp, vp, sz, i32, u32, vp, vp, vp, vp]),
         "granne_b200_multi_exact_search_batch": (i32, [vp, vp, sz, i32, u32, vp, vp, vp]),
+        "granne_b200_set_rerank_elements": (i32, [vp, vp, sz]),
+        "granne_b200_set_rerank_elements_device": (i32, [vp, vp, u64, u32]),
+        "granne_b200_search_rerank_batch": (i32, [vp, vp, sz, i32, u32, u32, u32, vp, vp, vp, vp]),
+        "granne_b200_search_rerank_batch_device": (i32, [vp, vp, sz, i32, u32, u32, u32, vp, vp, vp, vp, vp]),
+        "granne_b200_multi_set_rerank_elements": (i32, [vp, vp, vp]),
+        "granne_b200_multi_search_rerank_batch": (i32, [vp, vp, sz, i32, u32, u32, u32, vp, vp, vp]),
         "granne_b200_device_bytes": (u64, [vp]),
     }
     for name, (res, args) in sig.items():
@@ -396,6 +403,78 @@ class Granne:
             C.c_void_p(counts.data_ptr()), C.c_void_p(s)))
         return ids, dists, counts
 
+    # ---- two-stage search (granne_b200_search_rerank_batch*) ----
+    def set_rerank_elements(self, elements):
+        """Attaches the angular f32 rows (an angular elements file image, `bytes`) that re-rank the candidates of
+        this angular_int index: at least len(self) rows of its width.  Once, before searching."""
+        eb = np.frombuffer(elements, dtype=np.uint8)
+        _check(load_library().granne_b200_set_rerank_elements(self._h, _ptr(eb), eb.size))
+
+    def set_rerank_elements_device(self, elements):
+        """set_rerank_elements from a contiguous CUDA float32 tensor [n, dim] of normalised rows on this index's
+        device (e.g. elements_from_raw_device("angular", raw)); the rows are copied."""
+        _check_device_rows(ANGULAR, elements)
+        if elements.device.index != self.device:
+            raise ValueError("elements tensor lives on cuda:%d, not cuda:%d" % (elements.device.index, self.device))
+        _check(load_library().granne_b200_set_rerank_elements_device(self._h, C.c_void_p(elements.data_ptr()),
+                                                                     elements.shape[0], elements.shape[1]))
+
+    def search_batch_rerank(self, queries, num_candidates, max_search=DEFAULT_MAX_SEARCH,
+                            num_elements=DEFAULT_NUM_ELEMENTS, with_stats=False):
+        """Two-stage search: the first num_candidates results of search_batch on this angular_int index, re-ranked
+        by their exact f32 angular distance to the query over the attached rows; the first num_elements by
+        (distance, id).  Not a reference function.  queries: raw float32 (nq, dim).  Returns (ids, dists, counts)
+        in search_batch's layout; with_stats adds stage 1's counters."""
+        q = np.asarray(queries)
+        if q.dtype == np.int8:
+            raise ValueError("the two-stage search takes raw float32 queries")
+        q = np.ascontiguousarray(q, dtype=np.float32)
+        if q.ndim != 2 or q.shape[1] != self.dim:
+            raise ValueError("queries must have shape (nq, %d)" % self.dim)
+        nq, k = q.shape[0], int(num_elements)
+        ids = np.empty((nq, k), dtype=np.uint32)
+        dists = np.empty((nq, k), dtype=np.float32)
+        counts = np.empty(nq, dtype=np.uint32)
+        stats = np.zeros((nq, STATS_PER_QUERY), dtype=np.uint64) if with_stats else None
+        _check(load_library().granne_b200_search_rerank_batch(
+            self._h, _ptr(q), nq, QUERY_RAW_F32, int(max_search), int(num_candidates), k, _ptr(ids), _ptr(dists),
+            _ptr(counts), _ptr(stats) if with_stats else None))
+        if with_stats:
+            return ids, dists, counts, stats
+        return ids, dists, counts
+
+    def search_batch_rerank_device(self, queries, num_candidates, max_search=DEFAULT_MAX_SEARCH,
+                                   num_elements=DEFAULT_NUM_ELEMENTS, out=None, stats=None, stream=None):
+        """Device-resident search_batch_rerank: a CUDA float32 tensor in, CUDA tensors out (ids int32 view of u32
+        bits, dists float32, counts int32), asynchronous on `stream` (default: the current torch stream); a NaN
+        distance is reported by stream_status()."""
+        import torch
+
+        q = self._check_device_queries(queries)
+        if q.dtype != torch.float32:
+            raise ValueError("the two-stage search takes raw float32 queries")
+        nq, k = q.shape[0], int(num_elements)
+        if out is not None:
+            for t, dt, shape in zip(out, (torch.int32, torch.float32, torch.int32), ((nq, k), (nq, k), (nq,))):
+                if (not t.is_cuda or t.device != q.device or t.dtype != dt or tuple(t.shape) != shape
+                        or not t.is_contiguous()):
+                    raise ValueError("out tensors must be contiguous (ids int32 [nq,k], dists float32 [nq,k], counts "
+                                     "int32 [nq]) on the queries' device")
+        else:
+            dev = q.device
+            out = (torch.empty((nq, k), dtype=torch.int32, device=dev),
+                   torch.empty((nq, k), dtype=torch.float32, device=dev),
+                   torch.empty((nq,), dtype=torch.int32, device=dev))
+        _check_stats(stats, q)
+        ids, dists, counts = out
+        s = stream if stream is not None else torch.cuda.current_stream(q.device).cuda_stream
+        s = getattr(s, "cuda_stream", s)
+        _check(load_library().granne_b200_search_rerank_batch_device(
+            self._h, C.c_void_p(q.data_ptr()), nq, QUERY_RAW_F32, int(max_search), int(num_candidates), k,
+            C.c_void_p(ids.data_ptr()), C.c_void_p(dists.data_ptr()), C.c_void_p(counts.data_ptr()),
+            C.c_void_p(stats.data_ptr()) if stats is not None else None, C.c_void_p(s)))
+        return ids, dists, counts
+
     def _word_tables(self):
         """(WordDict, embeddings table, per-element id lists) for an "embeddings" index opened with words_path."""
         if getattr(self, "_words", None) is None:
@@ -589,6 +668,35 @@ class MultiGranne:
         counts = np.empty(nq, dtype=np.uint32)
         _check(load_library().granne_b200_multi_exact_search_batch(self._h, _ptr(q), nq, fmt, k, _ptr(ids),
                                                                    _ptr(dists), _ptr(counts)))
+        return ids, dists, counts
+
+    def set_rerank_elements(self, elements):
+        """Granne.set_rerank_elements on every part: one angular elements image (`bytes`) for a replicated handle,
+        a list with one image per shard for a partitioned one."""
+        images = [elements] if isinstance(elements, (bytes, bytearray, memoryview)) else list(elements)
+        keep = [np.frombuffer(e, dtype=np.uint8) for e in images]
+        ptrs = (C.c_void_p * len(keep))(*[a.ctypes.data for a in keep])
+        lens = (C.c_size_t * len(keep))(*[a.size for a in keep])
+        if len(keep) != (1 if self.mode == MODE_REPLICATED else self.num_parts()):
+            raise ValueError("one image for a replicated handle, one per shard for a partitioned one")
+        _check(load_library().granne_b200_multi_set_rerank_elements(self._h, ptrs, lens))
+
+    def search_batch_rerank(self, queries, num_candidates, max_search=DEFAULT_MAX_SEARCH,
+                            num_elements=DEFAULT_NUM_ELEMENTS):
+        """Two-stage search over all parts (granne_b200_multi_search_rerank_batch): GLOBAL uint64 ids."""
+        q = np.asarray(queries)
+        if q.dtype == np.int8:
+            raise ValueError("the two-stage search takes raw float32 queries")
+        q = np.ascontiguousarray(q, dtype=np.float32)
+        if q.ndim != 2:
+            raise ValueError("queries must have shape (nq, dim)")
+        nq, k = q.shape[0], int(num_elements)
+        ids = np.empty((nq, k), dtype=np.uint64)
+        dists = np.empty((nq, k), dtype=np.float32)
+        counts = np.empty(nq, dtype=np.uint32)
+        _check(load_library().granne_b200_multi_search_rerank_batch(self._h, _ptr(q), nq, QUERY_RAW_F32,
+                                                                    int(max_search), int(num_candidates), k,
+                                                                    _ptr(ids), _ptr(dists), _ptr(counts)))
         return ids, dists, counts
 
     def close(self):

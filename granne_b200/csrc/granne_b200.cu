@@ -16,6 +16,7 @@
 #include <limits>
 #include <map>
 #include <thread>
+#include <type_traits>
 #include <memory>
 #include <mutex>
 #include <string>
@@ -26,6 +27,7 @@
 #include "build_kernels.cuh"
 #include "search_kernels.cuh"
 #include "exact_kernels.cuh"
+#include "rerank_kernels.cuh"
 
 namespace gb = granne_b200;
 
@@ -128,7 +130,8 @@ struct Workspace {
     Buffer<unsigned long long> d_stats;
     Buffer<int> d_status;  // nq ints
     // one 64-byte block, zeroed once per call: [0..2] work counters of the three passes, [3] fast pass flagged
-    // something, [4] retry pass flagged something, [5] done counter (fused gather); d_error = words [8..11]
+    // something, [4] retry pass flagged something, [5] done counter (fused gather), [6] work counter of the re-rank
+    // kernel; d_error = words [8..11]
     Buffer<unsigned int> d_counters;
     int* d_error = nullptr;              // [0]=sticky error bits of this call (inside the counters block)
     Buffer<unsigned long long> d_retried;  // cumulative: queries that needed more than the fast pass
@@ -150,6 +153,8 @@ struct Workspace {
     Buffer<unsigned long long> d_exact_lists;
     Buffer<float> d_exact_rows;
     Buffer<float> d_exact_table;
+    // two-stage search: stage 1's candidates, one block ids | dists | counts for the current call's nq x C
+    Buffer<uint32_t> d_rerank;
 };
 
 }  // namespace
@@ -159,6 +164,9 @@ struct granne_b200_index {
     int num_sms = 0;
     size_t smem_optin = 0;
     gb::DeviceIndex dev{};
+    // angular f32 rows that re-rank the candidates of an angular_int index (granne_b200_set_rerank_elements*);
+    // vectors == nullptr until they are attached
+    gb::DeviceIndex rerank{};
     std::vector<std::shared_ptr<void>> allocations;  // device memory (shared with builder snapshots)
     uint64_t device_bytes = 0;
     uint64_t index_len = 0;  // Index::len
@@ -166,6 +174,7 @@ struct granne_b200_index {
     std::atomic<uint64_t> launches{0};
     std::atomic<int> sticky_error{0};
     std::mutex pool_mu;
+    std::mutex rerank_mu;  // serialises the attaches of re-rank rows (granne_b200_set_rerank_elements*)
     std::vector<std::unique_ptr<Workspace>> pool;                     // host-pointer API: one per concurrent call
     std::map<cudaStream_t, std::unique_ptr<Workspace>> stream_ws;     // device-pointer API: one per caller stream
     // fast-pass visited tables are sized max_search x degree x vis_scale; the scale doubles (up to 8) when more than
@@ -262,11 +271,11 @@ struct FixedChunksProbe {
 };
 int fixed_f32_chunks(const gb::DeviceIndex& d) { return DistDispatch::call(d, FixedChunksProbe{}); }
 
-// Writes `nrows` dense rows of the handle's kind and width from `src` (host memory, or device memory if
-// `device_src`) to the staged rows at `dst`: in 64 MB slabs through a temporary device buffer, re-laid out on the
-// device by pad_rows_i8_kernel / permute_rows_f32_kernel.
-int upload_rows(Handle* h, const uint8_t* src, uint64_t nrows, bool device_src, uint8_t* dst) {
-    const gb::DeviceIndex& d = h->dev;
+// Writes `nrows` dense rows of d's kind and width from `src` (host memory, or device memory if `device_src`) to the
+// staged rows at `dst`: in 64 MB slabs through a temporary device buffer, re-laid out on the device by
+// pad_rows_i8_kernel / permute_rows_f32_kernel.
+int upload_rows(Handle* h, const gb::DeviceIndex& d, const uint8_t* src, uint64_t nrows, bool device_src,
+                uint8_t* dst) {
     const bool i8 = d.kind == gb::kAngularI8;
     const size_t esz = i8 ? 1 : 4, src_row = (size_t)d.dim * esz;
     const uint64_t slab = std::max<uint64_t>(1, (64ull << 20) / src_row);
@@ -296,9 +305,10 @@ int upload_rows(Handle* h, const uint8_t* src, uint64_t nrows, bool device_src, 
     return GRANNE_B200_OK;
 }
 
-// Stages `nrows` dense rows of the handle's kind (host memory, or device memory if `device_src`).
-int stage_dense(Handle* h, const uint8_t* rows, uint64_t nrows, uint32_t dim, bool device_src = false) {
-    gb::DeviceIndex& d = h->dev;
+// Stages `nrows` dense rows of d's kind (host memory, or device memory if `device_src`) as d's vectors: the handle's
+// own container (h->dev) or the re-rank rows (h->rerank).  The handle owns the memory and counts it.
+int stage_dense(Handle* h, gb::DeviceIndex& d, const uint8_t* rows, uint64_t nrows, uint32_t dim,
+                bool device_src = false) {
     d.dim = dim;
     d.full = dim / 32;
     d.tail = dim % 32;
@@ -317,7 +327,7 @@ int stage_dense(Handle* h, const uint8_t* rows, uint64_t nrows, uint32_t dim, bo
     Buffer<uint8_t> dst;
     int rc;
     if ((rc = dev_alloc(&dst, (size_t)nrows * d.row_stride * (i8 ? 1 : 4)))) return rc;
-    if ((rc = upload_rows(h, rows, nrows, device_src, dst.get()))) return rc;
+    if ((rc = upload_rows(h, d, rows, nrows, device_src, dst.get()))) return rc;
     d.vectors = stage(h, std::move(dst));
     return GRANNE_B200_OK;
 }
@@ -345,7 +355,7 @@ int stage_elements(Handle* h, int kind, const uint8_t* el, size_t el_len, const 
         gb::DenseView ev;
         gb::SumElements se;
         if ((rc = parse_sum_container(el, el_len, emb, emb_len, &ev, &se))) return rc;
-        rc = stage_dense(h, ev.data, ev.num, (uint32_t)ev.dim);
+        rc = stage_dense(h, d, ev.data, ev.num, (uint32_t)ev.dim);
         if (rc) return rc;
         d.num_elements = se.offsets.size() - 1;
         Buffer<unsigned long long> doff;
@@ -361,7 +371,7 @@ int stage_elements(Handle* h, int kind, const uint8_t* el, size_t el_len, const 
         const bool i8 = kind == GRANNE_B200_ANGULAR_INT;
         if (!gb::parse_dense(el, el_len, i8 ? 1 : 4, &dv, &err)) return fail(GRANNE_B200_ERR_FORMAT, err);
         if (dv.dim > 16384) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "vectors wider than 16384 are unsupported");
-        rc = stage_dense(h, dv.data, dv.num, (uint32_t)dv.dim);
+        rc = stage_dense(h, d, dv.data, dv.num, (uint32_t)dv.dim);
         if (rc) return rc;
         d.num_elements = dv.num;
     }
@@ -448,7 +458,7 @@ int stage_device_elements(Handle* h, int kind, const void* d_rows, uint64_t n, u
         return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "elements pointer is not device memory of the requested device");
     }
     h->dev.kind = kind;
-    int rc = stage_dense(h, static_cast<const uint8_t*>(d_rows), n, dim, true);
+    int rc = stage_dense(h, h->dev, static_cast<const uint8_t*>(d_rows), n, dim, true);
     if (rc) return rc;
     h->dev.num_elements = n;
     return GRANNE_B200_OK;
@@ -550,8 +560,9 @@ struct LaunchPlan {
     size_t smem;        // fast pass total
 };
 
-LaunchPlan make_plan(const Handle* h, uint32_t max_search) {
-    const gb::DeviceIndex& d = h->dev;
+// `view`: the staged rows the kernels read, when they are not the handle's own (the re-rank rows)
+LaunchPlan make_plan(const Handle* h, uint32_t max_search, const gb::DeviceIndex* view = nullptr) {
+    const gb::DeviceIndex& d = view ? *view : h->dev;
     LaunchPlan p{};
     // fast list: capacity 32*R with R odd (conflict-free lane-major access); slack >= 16 entries over max_search
     p.rows = 0;
@@ -1011,6 +1022,132 @@ int enqueue_exact(Handle* h, Workspace* w, const void* d_queries, size_t nq, int
         GB_CUDA(cudaGetLastError());
     }
     return GRANNE_B200_OK;
+}
+
+// ---- two-stage search: angular_int traversal, f32 re-rank (rerank_kernels.cuh) -----------------------------------
+// The checks on the handle before any rows are read: an angular_int index without re-rank rows.
+int check_rerank_target(const Handle* h) {
+    if (!h) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "index handle is null");
+    if (h->dev.kind != gb::kAngularI8)
+        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "re-rank rows are attached to an angular_int index only");
+    if (h->rerank.vectors)
+        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "re-rank rows are already attached to this index");
+    return GRANNE_B200_OK;
+}
+
+// The checks on the rows: the index's width, and a row for every element of [0, Index::len).
+int check_rerank_shape(const Handle* h, uint64_t n, uint64_t dim) {
+    if (dim != h->dev.dim) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "re-rank rows must have the index's width");
+    if (n < h->index_len)
+        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "re-rank rows must cover every element of the index");
+    return GRANNE_B200_OK;
+}
+
+// Stages n angular f32 element rows as h's re-rank rows, laid out for the engine DistDispatch picks for their width.
+// They become visible to searches only once fully staged.  The target check is repeated under the handle's attach
+// lock, so that of two concurrent attaches one stages its rows and the other fails.
+int stage_rerank(Handle* h, const uint8_t* rows, uint64_t n, uint32_t dim, bool device_src) {
+    std::lock_guard<std::mutex> g(h->rerank_mu);
+    int rc = check_rerank_target(h);
+    if (rc) return rc;
+    gb::DeviceIndex r{};
+    r.kind = gb::kAngularF32;
+    if ((rc = stage_dense(h, r, rows, n, dim, device_src))) return rc;
+    r.num_elements = n;
+    h->rerank = r;
+    return GRANNE_B200_OK;
+}
+
+// Drops h's re-rank rows and their memory (the multi handle's attach undoes a partial attach with it).  The caller
+// makes h's device current.
+void release_rerank(Handle* h) {
+    std::lock_guard<std::mutex> g(h->rerank_mu);
+    const gb::DeviceIndex& r = h->rerank;
+    if (!r.vectors) return;
+    auto it = std::find_if(h->allocations.begin(), h->allocations.end(),
+                           [&](const std::shared_ptr<void>& a) { return a.get() == r.vectors; });
+    if (it != h->allocations.end()) {
+        h->allocations.erase(it);
+        // stage_dense's allocation: the rows, at least 16 bytes (dev_alloc)
+        h->device_bytes -= std::max<uint64_t>(r.num_vectors * r.row_stride * 4ull, 16);
+    }
+    h->rerank = gb::DeviceIndex{};
+}
+
+// validate_search's rules plus the two-stage ones.
+int validate_rerank(const Handle* h, const void* q, size_t nq, int fmt, uint32_t max_search, uint32_t c,
+                    uint32_t k, const void* ids, const void* dists) {
+    int rc = validate_search(h, q, nq, fmt, max_search, k, ids, dists);
+    if (rc) return rc;
+    if (fmt != GRANNE_B200_QUERY_RAW_F32)
+        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "the two-stage search takes raw f32 queries");
+    if (!h->rerank.vectors)
+        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "no re-rank rows are attached to this index");
+    if (c == 0 || c > GRANNE_B200_RERANK_MAX_CANDIDATES)
+        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "num_candidates must be in 1..1024");
+    if (k > c) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "num_neighbors exceeds num_candidates");
+    return GRANNE_B200_OK;
+}
+
+// rerank_kernel for the f32 engine DistDispatch picks for the re-rank rows (never an i8 or embeddings engine: the
+// rows are staged as angular f32).
+struct RerankLaunch {
+    Handle* h;
+    const gb::RerankArgs& a;
+    size_t smem;
+    cudaStream_t stream;
+    template <class Dist>
+    int run() {
+        if constexpr (std::is_same<Dist, gb::DistI8>::value || std::is_same<Dist, gb::DistSum>::value) {
+            return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "re-rank rows must be angular f32 rows");
+        } else {
+            auto kern = gb::rerank_kernel<Dist>;
+            static std::atomic<bool> attr_set[64];  // function attributes are per device
+            int rc = set_smem_attr(kern, h, &attr_set[h->device & 63]);
+            if (rc) return rc;
+            int occ = 0;
+            GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, 32, smem));
+            if (occ < 1) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "re-rank workspace exceeds shared memory");
+            const unsigned grid = (unsigned)std::min<unsigned long long>(a.nq, (unsigned long long)occ * h->num_sms);
+            kern<<<grid, 32, smem, stream>>>(h->rerank, a);
+            h->launches++;
+            GB_CUDA(cudaGetLastError());
+            return GRANNE_B200_OK;
+        }
+    }
+};
+
+// Enqueues one two-stage search on `stream`: stage 1 is enqueue_search with k = C into the workspace's candidate
+// block, stage 2 is rerank_kernel over h->rerank into the caller's outputs.  Stage 1 writes `d_stats` as search does.
+int enqueue_rerank(Handle* h, Workspace* w, const void* d_queries, size_t nq, uint32_t max_search, uint32_t c,
+                   uint32_t k, uint32_t* d_ids, float* d_dists, uint32_t* d_counts, unsigned long long* d_stats,
+                   cudaStream_t stream, bool reset_error) {
+    int rc = w->d_rerank.grow(2 * nq * c + nq, stream);
+    if (rc) return rc;
+    uint32_t* cand_ids = w->d_rerank.get();
+    uint32_t* cand_counts = cand_ids + 2 * nq * c;
+    if ((rc = enqueue_search(h, w, d_queries, nq, GRANNE_B200_QUERY_RAW_F32, max_search, c, cand_ids,
+                             reinterpret_cast<float*>(cand_ids + nq * c), cand_counts, d_stats, stream, reset_error)))
+        return rc;
+    const LaunchPlan plan = make_plan(h, 1, &h->rerank);
+    gb::RerankArgs a{};
+    a.queries = static_cast<const float*>(d_queries);
+    a.nq = nq;
+    a.cand_ids = cand_ids;
+    a.cand_counts = cand_counts;
+    a.cand_stride = c;
+    a.num_neighbors = k;
+    a.out_ids = d_ids;
+    a.out_dists = d_dists;
+    a.out_counts = d_counts;
+    a.work_counter = w->d_counters.get() + 6;  // zeroed by enqueue_search's memset on this stream
+    a.error_flag = w->d_error;
+    a.stg_rows = plan.stg_rows;
+    a.stg_row_bytes = plan.stg_row_bytes;
+    a.tile_rows = plan.tile_rows;
+    // the keys start on the first 16-byte boundary behind the engine's SmemLayout (rerank_kernel)
+    const size_t smem = ((plan.base_smem + 15) & ~size_t(15)) + (size_t)gb::rerank_key_slots(c) * 8;
+    return DistDispatch::call(h->rerank, RerankLaunch{h, a, smem, stream});
 }
 
 // ---- GranneBuilder (src/index/mod.rs:295-531, 645-960) on the device ---------------------------------------------
@@ -1584,6 +1721,104 @@ int granne_b200_exact_search_batch_device(granne_b200_index* h, const void* d_qu
     });
 }
 
+int granne_b200_set_rerank_elements(granne_b200_index* h, const void* elements_bytes, size_t elements_len) {
+    int rc = check_rerank_target(h);
+    if (rc) return rc;
+    if (!elements_bytes) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "elements buffer is null");
+    return guarded([&] {
+        gb::DenseView dv;
+        std::string err;
+        if (!gb::parse_dense(static_cast<const uint8_t*>(elements_bytes), elements_len, 4, &dv, &err))
+            return fail(GRANNE_B200_ERR_FORMAT, err);
+        if ((rc = check_rerank_shape(h, dv.num, dv.dim))) return rc;
+        GB_DEVICE(h->device);
+        return stage_rerank(h, dv.data, dv.num, (uint32_t)dv.dim, false);
+    });
+}
+
+int granne_b200_set_rerank_elements_device(granne_b200_index* h, const float* d_rows, uint64_t n, uint32_t dim) {
+    int rc = check_rerank_target(h);
+    if (rc) return rc;
+    if (!d_rows && n) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "elements pointer is null");
+    if ((rc = check_rerank_shape(h, n, dim))) return rc;
+    return guarded([&] {
+        GB_DEVICE(h->device);
+        cudaPointerAttributes at{};
+        if (n && (cudaPointerGetAttributes(&at, d_rows) != cudaSuccess || at.type != cudaMemoryTypeDevice ||
+                  at.device != h->device)) {
+            cudaGetLastError();
+            return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "elements pointer is not device memory of the index's device");
+        }
+        return stage_rerank(h, reinterpret_cast<const uint8_t*>(d_rows), n, dim, true);
+    });
+}
+
+int granne_b200_search_rerank_batch(granne_b200_index* h, const float* queries, size_t nq, int query_format,
+                                    uint32_t max_search, uint32_t num_candidates, uint32_t num_neighbors,
+                                    uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint64_t* out_stats) {
+    int rc = validate_rerank(h, queries, nq, query_format, max_search, num_candidates, num_neighbors, out_ids,
+                             out_dists);
+    if (rc) return rc;
+    if (nq == 0) return GRANNE_B200_OK;
+    return guarded([&] {
+        GB_DEVICE(h->device);
+        const size_t k = num_neighbors;
+        const size_t qbytes = nq * h->dev.dim * 4;
+        std::unique_ptr<Workspace> ws;
+        if ((rc = ws_acquire(h, &ws))) return rc;
+        Workspace* w = ws.get();
+        const int status = [&] {
+            if ((rc = ws_reserve(w, qbytes, nq, k))) return rc;
+            cudaStream_t stream = w->stream.get();
+            // pinned staging layout as in granne_b200_search_batch: queries | ids | dists | counts | error | stats
+            uint8_t* hp = w->h_pinned.get();
+            uint32_t* hids = reinterpret_cast<uint32_t*>(hp + ((qbytes + 15) & ~size_t(15)));
+            float* hd = reinterpret_cast<float*>(hids + nq * k);
+            uint32_t* hc = reinterpret_cast<uint32_t*>(hd + nq * k);
+            int* herr = reinterpret_cast<int*>(hc + nq);
+            unsigned long long* hstats = reinterpret_cast<unsigned long long*>(
+                hp + ((reinterpret_cast<uint8_t*>(herr + 4) - hp + 15) & ~size_t(15)));
+            std::memcpy(hp, queries, qbytes);
+            GB_CUDA(cudaMemcpyAsync(w->d_queries.get(), hp, qbytes, cudaMemcpyHostToDevice, stream));
+            rc = enqueue_rerank(h, w, w->d_queries.get(), nq, max_search, num_candidates, num_neighbors,
+                                w->d_ids.get(), w->d_dists, w->d_counts, out_stats ? w->d_stats.get() : nullptr,
+                                stream, true);
+            if (rc) return rc;
+            GB_CUDA(cudaMemcpyAsync(hids, w->d_ids.get(), (2 * nq * k + nq) * 4, cudaMemcpyDeviceToHost, stream));
+            GB_CUDA(cudaMemcpyAsync(herr, w->d_error, 4 * sizeof(int), cudaMemcpyDeviceToHost, stream));
+            if (out_stats) GB_CUDA(cudaMemcpyAsync(hstats, w->d_stats.get(), nq * 32, cudaMemcpyDeviceToHost, stream));
+            GB_CUDA(cudaStreamSynchronize(stream));
+            if (out_stats) std::memcpy(out_stats, hstats, nq * 32);
+            if (k) {
+                std::memcpy(out_ids, hids, nq * k * 4);
+                std::memcpy(out_dists, hd, nq * k * 4);
+            }
+            if (out_counts) std::memcpy(out_counts, hc, nq * 4);
+            return error_from_bits(herr[0]);
+        }();
+        ws_release(h, std::move(ws));  // back to the pool on every path
+        return status;
+    });
+}
+
+int granne_b200_search_rerank_batch_device(granne_b200_index* h, const float* d_queries, size_t nq, int query_format,
+                                           uint32_t max_search, uint32_t num_candidates, uint32_t num_neighbors,
+                                           uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts,
+                                           uint64_t* d_out_stats, void* cuda_stream) {
+    int rc = validate_rerank(h, d_queries, nq, query_format, max_search, num_candidates, num_neighbors, d_out_ids,
+                             d_out_dists);
+    if (rc) return rc;
+    if (nq == 0) return GRANNE_B200_OK;
+    return guarded([&] {
+        GB_DEVICE(h->device);
+        cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+        Workspace* w = nullptr;
+        if ((rc = stream_workspace(h, stream, &w))) return rc;
+        return enqueue_rerank(h, w, d_queries, nq, max_search, num_candidates, num_neighbors, d_out_ids, d_out_dists,
+                              d_out_counts, reinterpret_cast<unsigned long long*>(d_out_stats), stream, false);
+    });
+}
+
 int granne_b200_inspect_index(const void* index_bytes, size_t index_len, uint64_t* out_num_layers,
                               uint64_t* out_layer_len, uint32_t* out_max_degree, uint32_t* out_row_width, size_t cap) {
     if (!index_bytes || !out_num_layers) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
@@ -1771,7 +2006,7 @@ int granne_b200_builder_append(granne_b200_builder* b, const void* elements_byte
         int rc;
         if ((rc = dev_alloc(&rows, (size_t)new_n * row_bytes))) return rc;
         if (old_n) GB_CUDA(cudaMemcpy(rows.get(), d.vectors, (size_t)old_n * row_bytes, cudaMemcpyDeviceToDevice));
-        if ((rc = upload_rows(h, dv.data, dv.num, false, rows.get() + (size_t)old_n * row_bytes))) return rc;
+        if ((rc = upload_rows(h, d, dv.data, dv.num, false, rows.get() + (size_t)old_n * row_bytes))) return rc;
         d.vectors = stage(h, std::move(rows), d.vectors, (size_t)old_n * row_bytes);
         d.num_vectors = new_n;
         d.num_elements = new_n;
@@ -2491,6 +2726,61 @@ int granne_b200_multi_exact_search_batch(granne_b200_multi* m, const void* queri
     return multi_batch(m, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts,
                        [&](granne_b200_index* h, const void* q, size_t cnt, uint32_t* ids, float* ds, uint32_t* c) {
                            return granne_b200_exact_search_batch(h, q, cnt, query_format, num_neighbors, ids, ds, c);
+                       });
+}
+
+// Every image is checked on the host against its part before any part stages rows; if a part then fails to stage
+// (a device error), the parts this call attached drop their rows again, so that the call can be repeated.
+int granne_b200_multi_set_rerank_elements(granne_b200_multi* m, const void* const* elements_bytes,
+                                          const size_t* elements_len) {
+    if (!m || !elements_bytes || !elements_len) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
+    return guarded([&] {
+        const size_t n = m->parts.size();
+        auto image = [&](size_t i) { return m->mode == GRANNE_B200_MODE_REPLICATED ? 0 : i; };
+        for (size_t i = 0; i < n; ++i) {
+            int rc = check_rerank_target(m->parts[i]);
+            if (rc) return rc;
+            if (!elements_bytes[image(i)]) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "elements buffer is null");
+            gb::DenseView dv;
+            std::string err;
+            if (!gb::parse_dense(static_cast<const uint8_t*>(elements_bytes[image(i)]), elements_len[image(i)], 4, &dv,
+                                 &err))
+                return fail(GRANNE_B200_ERR_FORMAT, err);
+            if ((rc = check_rerank_shape(m->parts[i], dv.num, dv.dim))) return rc;
+        }
+        std::vector<char> attached(n, 0);
+        const int rc = for_each_part(n, [&](size_t i) {
+            const int r = granne_b200_set_rerank_elements(m->parts[i], elements_bytes[image(i)], elements_len[image(i)]);
+            attached[i] = r == GRANNE_B200_OK;
+            return r;
+        });
+        if (rc) {
+            for (size_t i = 0; i < n; ++i) {
+                if (!attached[i]) continue;
+                DeviceGuard guard(m->parts[i]->device);
+                release_rerank(m->parts[i]);
+            }
+        }
+        return rc;
+    });
+}
+
+// RANGE_PARTITIONED: every shard re-ranks its own candidates; the shard lists are sorted by (distance, local id) and
+// a shard's local ids are monotone in the global ids, so the (distance, global id) merge of multi_batch equals the
+// re-rank of the union of the shards' candidate sets.
+int granne_b200_multi_search_rerank_batch(granne_b200_multi* m, const float* queries, size_t nq, int query_format,
+                                          uint32_t max_search, uint32_t num_candidates, uint32_t num_neighbors,
+                                          uint64_t* out_ids, float* out_dists, uint32_t* out_counts) {
+    if (!m) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "multi handle is null");
+    int rc = validate_rerank(m->parts[0], queries, nq, query_format, max_search, num_candidates, num_neighbors,
+                             out_ids, out_dists);
+    if (rc) return rc;
+    if (nq == 0) return GRANNE_B200_OK;
+    return multi_batch(m, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts,
+                       [&](granne_b200_index* h, const void* q, size_t cnt, uint32_t* ids, float* ds, uint32_t* c) {
+                           return granne_b200_search_rerank_batch(h, static_cast<const float*>(q), cnt, query_format,
+                                                                  max_search, num_candidates, num_neighbors, ids, ds,
+                                                                  c, nullptr);
                        });
 }
 

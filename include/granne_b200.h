@@ -191,6 +191,42 @@ int granne_b200_exact_search_batch_device(granne_b200_index* h, const void* d_qu
                                           uint32_t num_neighbors, uint32_t* d_out_ids, float* d_out_dists,
                                           uint32_t* d_out_counts, void* cuda_stream);
 
+/* ---- two-stage search: traverse angular_int rows, re-rank by exact f32 angular distance ----------------------------
+ * NOT a reference function: what a user of granne assembles by hand from two containers over one index.  For an
+ * angular_int handle h with attached angular f32 rows F and a raw f32 query q:
+ *   1. S = Granne<angular_int::Vectors>::search(&angular_int::Vector::from(q), max_search, C), i.e. exactly
+ *      granne_b200_search_batch(h, q, RAW_F32, max_search, C): at most min(C, max_search) ids;
+ *   2. d_i = F.dist_to_element(i, &angular::Vector::from(q)) for i in S, the reference's f32 angular distance bit for
+ *      bit (angular.rs:63-74, math.rs:16-42);
+ *   3. the first min(k, |S|) entries of sort ascending { (d_i, i) }, the order of into_sorted_vec (src/index/mod.rs:1036).
+ * The result depends only on the set S.  Per query, its intersection with the exact f32 top-k equals S's, so its
+ * recall is the candidate set's and never below the i8 search's.  Output layout as granne_b200_search_batch.
+ *
+ * Attach F once, before searching; there is no replacement while searches may be in flight, and an attach concurrent
+ * with a search on h is not supported.  Concurrent attaches on h are serialised: one attaches its rows, the others
+ * return ERR_INVALID_ARGUMENT.  The rows are copied into HBM (counted by granne_b200_device_bytes) in the layout the
+ * search path's f32 engine for their width reads.
+ * ERR_INVALID_ARGUMENT: h is not ANGULAR_INT, rows are already attached, their width differs from the index's, or
+ * there are fewer than granne_b200_len(h) rows.  ERR_FORMAT: a malformed image.
+ *   elements_bytes   an angular elements file image (u64 dim | normalised f32 rows)
+ *   d_rows           n x dim normalised f32 rows in device memory of h's device */
+#define GRANNE_B200_RERANK_MAX_CANDIDATES 1024
+int granne_b200_set_rerank_elements(granne_b200_index* h, const void* elements_bytes, size_t elements_len);
+int granne_b200_set_rerank_elements_device(granne_b200_index* h, const float* d_rows, uint64_t n, uint32_t dim);
+/* The two-stage search for nq raw f32 queries (host buffers).  ERR_INVALID_ARGUMENT, before any device call, when
+ * query_format is not RAW_F32, no rows are attached, num_candidates is 0 or above GRANNE_B200_RERANK_MAX_CANDIDATES,
+ * num_neighbors > num_candidates, or a rule of granne_b200_search_batch is broken.  out_stats (may be NULL) holds stage
+ * 1's counters as granne_b200_search_batch writes them.  A NaN distance in either stage returns ERR_NOT_FINITE. */
+int granne_b200_search_rerank_batch(granne_b200_index* h, const float* queries, size_t nq, int query_format,
+                                    uint32_t max_search, uint32_t num_candidates, uint32_t num_neighbors,
+                                    uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint64_t* out_stats);
+/* Same with DEVICE pointers on cuda_stream (NULL = the default stream), asynchronous like
+ * granne_b200_search_batch_device; ERR_NOT_FINITE is reported by granne_b200_stream_status. */
+int granne_b200_search_rerank_batch_device(granne_b200_index* h, const float* d_queries, size_t nq, int query_format,
+                                           uint32_t max_search, uint32_t num_candidates, uint32_t num_neighbors,
+                                           uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts,
+                                           uint64_t* d_out_stats, void* cuda_stream);
+
 /* The device-pointer calls keep one workspace per distinct caller stream (status words, per-warp visited tables) until
  * granne_b200_close.  A caller that retires a stream returns its workspace with this call (it synchronises the stream;
  * an error raised by its last batches is reported by the next granne_b200_stream_status). */
@@ -247,6 +283,17 @@ int granne_b200_multi_search_batch(granne_b200_multi* m, const void* queries, si
 int granne_b200_multi_exact_search_batch(granne_b200_multi* m, const void* queries, size_t nq, int query_format,
                                          uint32_t num_neighbors, uint64_t* out_ids, float* out_dists,
                                          uint32_t* out_counts);
+/* granne_b200_set_rerank_elements on every part: REPLICATED takes one image (elements_bytes[0]) and stages it on every
+ * device; RANGE_PARTITIONED takes one image per shard.  Every image is checked before any is staged; if a part then fails to
+ * stage its rows (a device error), the parts this call attached release theirs again, so the call can be repeated. */
+int granne_b200_multi_set_rerank_elements(granne_b200_multi* m, const void* const* elements_bytes,
+                                          const size_t* elements_len);
+/* granne_b200_search_rerank_batch over a multi handle, with u64 GLOBAL ids like granne_b200_multi_search_batch.
+ * RANGE_PARTITIONED: every shard re-ranks its own candidates and the lists are merged by (distance, global id), which
+ * equals re-ranking the union of the shards' candidate sets. */
+int granne_b200_multi_search_rerank_batch(granne_b200_multi* m, const float* queries, size_t nq, int query_format,
+                                          uint32_t max_search, uint32_t num_candidates, uint32_t num_neighbors,
+                                          uint64_t* out_ids, float* out_dists, uint32_t* out_counts);
 
 /* Host-only helpers (no device needed): the loader's view of an index image.
  * granne_b200_inspect_index replaces io::read_layer_sizes + Index::num_layers/layer_len on raw bytes

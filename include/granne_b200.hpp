@@ -221,6 +221,29 @@ public:
         return out;
     }
 
+    // Two-stage search (granne_b200_search_rerank_batch): attach the angular f32 rows of this angular_int index's
+    // elements once, then search_rerank returns, for nq raw f32 queries, the first num_candidates results of the i8
+    // search re-ranked by their exact f32 angular distance.  Not a reference function.
+    void set_rerank_elements(const Elements& angular_rows) {
+        if (angular_rows.kind != ElementKind::Angular)
+            throw Error(GRANNE_B200_ERR_INVALID_ARGUMENT, "re-rank rows are angular elements");
+        check(granne_b200_set_rerank_elements(h_, angular_rows.bytes.data(), angular_rows.bytes.size()));
+    }
+    std::vector<SearchResult> search_rerank(const float* queries, size_t nq, size_t max_search, size_t num_candidates,
+                                            size_t num_neighbors) const {
+        std::vector<uint32_t> ids(nq * num_neighbors), counts(nq);
+        std::vector<float> dists(nq * num_neighbors);
+        check(granne_b200_search_rerank_batch(h_, queries, nq, GRANNE_B200_QUERY_RAW_F32,
+                                              static_cast<uint32_t>(max_search), static_cast<uint32_t>(num_candidates),
+                                              static_cast<uint32_t>(num_neighbors), ids.data(), dists.data(),
+                                              counts.data(), nullptr));
+        std::vector<SearchResult> out(nq);
+        for (size_t q = 0; q < nq; ++q)
+            for (uint32_t j = 0; j < counts[q]; ++j)
+                out[q].emplace_back(ids[q * num_neighbors + j], dists[q * num_neighbors + j]);
+        return out;
+    }
+
     // Granne::reorder (reorder.rs:59-82) / reorder_by_keys (:89-124): reorders index and elements, returns the order
     // (`order[i] == j`: element j moved to i).
     std::vector<size_t> reorder(bool /*show_progress*/ = false) {
