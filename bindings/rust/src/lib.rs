@@ -114,6 +114,14 @@ extern "C" {
     fn granne_b200_multi_set_rerank_elements(
         m: *mut RawMulti, elements: *const *const c_void, elements_len: *const usize,
     ) -> c_int;
+    fn granne_b200_set_rerank_embeddings(
+        h: *mut RawIndex, elements: *const c_void, elements_len: usize, embeddings: *const c_void,
+        embeddings_len: usize,
+    ) -> c_int;
+    fn granne_b200_multi_set_rerank_embeddings(
+        m: *mut RawMulti, elements: *const *const c_void, elements_len: *const usize, embeddings: *const c_void,
+        embeddings_len: usize,
+    ) -> c_int;
     fn granne_b200_multi_search_rerank_batch(
         m: *mut RawMulti, queries: *const f32, nq: usize, query_format: c_int, max_search: u32, num_candidates: u32,
         num_neighbors: u32, out_ids: *mut u64, out_dists: *mut f32, out_counts: *mut u32,

@@ -106,6 +106,8 @@ def load_library():
         "granne_b200_search_rerank_batch": (i32, [vp, vp, sz, i32, u32, u32, u32, vp, vp, vp, vp]),
         "granne_b200_search_rerank_batch_device": (i32, [vp, vp, sz, i32, u32, u32, u32, vp, vp, vp, vp, vp]),
         "granne_b200_multi_set_rerank_elements": (i32, [vp, vp, vp]),
+        "granne_b200_set_rerank_embeddings": (i32, [vp, vp, sz, vp, sz]),
+        "granne_b200_multi_set_rerank_embeddings": (i32, [vp, vp, vp, vp, sz]),
         "granne_b200_multi_search_rerank_batch": (i32, [vp, vp, sz, i32, u32, u32, u32, vp, vp, vp]),
         "granne_b200_device_bytes": (u64, [vp]),
     }
@@ -419,6 +421,21 @@ class Granne:
         _check(load_library().granne_b200_set_rerank_elements_device(self._h, C.c_void_p(elements.data_ptr()),
                                                                      elements.shape[0], elements.shape[1]))
 
+    def set_rerank_embeddings(self, elements, embeddings, words_path=None):
+        """Attaches the SumEmbeddings container (`bytes` images of its term lists and of its embedding table, as
+        from_bytes takes them for an "embeddings" index) whose angular_int rows this index was built over
+        (compute_embeddings): the candidates are re-ranked by their exact sum-of-embeddings distance.  At least
+        len(self) elements, a table of the index's width (at most 4096).  Once, before searching; no other re-rank
+        container may be attached.  With `words_path` (a words file of the table's rows), search_rerank also takes
+        string queries."""
+        eb = np.frombuffer(elements, dtype=np.uint8)
+        mb = np.frombuffer(embeddings, dtype=np.uint8)
+        _check(load_library().granne_b200_set_rerank_embeddings(self._h, _ptr(eb), eb.size, _ptr(mb), mb.size))
+        if words_path is not None:
+            from . import words as W
+
+            self._rerank_words = (W.WordDict(words_path), W.read_dense_f32(embeddings))
+
     def search_batch_rerank(self, queries, num_candidates, max_search=DEFAULT_MAX_SEARCH,
                             num_elements=DEFAULT_NUM_ELEMENTS, with_stats=False):
         """Two-stage search: the first num_candidates results of search_batch on this angular_int index, re-ranked
@@ -442,6 +459,21 @@ class Granne:
         if with_stats:
             return ids, dists, counts, stats
         return ids, dists, counts
+
+    def search_rerank(self, element, num_candidates, max_search=DEFAULT_MAX_SEARCH, num_elements=DEFAULT_NUM_ELEMENTS):
+        """search_batch_rerank for one raw float32 query -> [(id, distance)], like search.  A str query, after
+        set_rerank_embeddings(..., words_path=...), is the sum of its words' embeddings (create_embedding), as
+        search builds it for an "embeddings" index (py/src/variants/index.rs:98-105)."""
+        if isinstance(element, str):
+            from . import words as W
+
+            if getattr(self, "_rerank_words", None) is None:
+                raise ValueError("string queries need set_rerank_embeddings(..., words_path=...)")
+            words, table = self._rerank_words
+            element = W.create_embedding(table, words.get_word_ids(element))
+        ids, dists, counts = self.search_batch_rerank(np.asarray(element)[None, :], num_candidates, max_search,
+                                                      num_elements)
+        return [(int(ids[0, i]), float(dists[0, i])) for i in range(int(counts[0]))]
 
     def search_batch_rerank_device(self, queries, num_candidates, max_search=DEFAULT_MAX_SEARCH,
                                    num_elements=DEFAULT_NUM_ELEMENTS, out=None, stats=None, stream=None):
@@ -680,6 +712,19 @@ class MultiGranne:
         if len(keep) != (1 if self.mode == MODE_REPLICATED else self.num_parts()):
             raise ValueError("one image for a replicated handle, one per shard for a partitioned one")
         _check(load_library().granne_b200_multi_set_rerank_elements(self._h, ptrs, lens))
+
+    def set_rerank_embeddings(self, elements_list, embeddings):
+        """Granne.set_rerank_embeddings on every part: one term-list image (`bytes`) for a replicated handle, a list
+        with one per shard for a partitioned one, and one embedding table image shared by all parts."""
+        images = ([elements_list] if isinstance(elements_list, (bytes, bytearray, memoryview))
+                  else list(elements_list))
+        keep = [np.frombuffer(e, dtype=np.uint8) for e in images]
+        ptrs = (C.c_void_p * len(keep))(*[a.ctypes.data for a in keep])
+        lens = (C.c_size_t * len(keep))(*[a.size for a in keep])
+        if len(keep) != (1 if self.mode == MODE_REPLICATED else self.num_parts()):
+            raise ValueError("one image for a replicated handle, one per shard for a partitioned one")
+        mb = np.frombuffer(embeddings, dtype=np.uint8)
+        _check(load_library().granne_b200_multi_set_rerank_embeddings(self._h, ptrs, lens, _ptr(mb), mb.size))
 
     def search_batch_rerank(self, queries, num_candidates, max_search=DEFAULT_MAX_SEARCH,
                             num_elements=DEFAULT_NUM_ELEMENTS):

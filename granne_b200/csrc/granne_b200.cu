@@ -164,9 +164,11 @@ struct granne_b200_index {
     int num_sms = 0;
     size_t smem_optin = 0;
     gb::DeviceIndex dev{};
-    // angular f32 rows that re-rank the candidates of an angular_int index (granne_b200_set_rerank_elements*);
-    // vectors == nullptr until they are attached
+    // the container that re-ranks the candidates of an angular_int index: angular f32 rows
+    // (granne_b200_set_rerank_elements*) or a SumEmbeddings container (granne_b200_set_rerank_embeddings);
+    // vectors == nullptr until one is attached.  rerank_bytes: its share of device_bytes.
     gb::DeviceIndex rerank{};
+    uint64_t rerank_bytes = 0;
     std::vector<std::shared_ptr<void>> allocations;  // device memory (shared with builder snapshots)
     uint64_t device_bytes = 0;
     uint64_t index_len = 0;  // Index::len
@@ -174,7 +176,7 @@ struct granne_b200_index {
     std::atomic<uint64_t> launches{0};
     std::atomic<int> sticky_error{0};
     std::mutex pool_mu;
-    std::mutex rerank_mu;  // serialises the attaches of re-rank rows (granne_b200_set_rerank_elements*)
+    std::mutex rerank_mu;  // serialises the attaches of re-rank containers (granne_b200_set_rerank_*)
     std::vector<std::unique_ptr<Workspace>> pool;                     // host-pointer API: one per concurrent call
     std::map<cudaStream_t, std::unique_ptr<Workspace>> stream_ws;     // device-pointer API: one per caller stream
     // fast-pass visited tables are sized max_search x degree x vis_scale; the scale doubles (up to 8) when more than
@@ -345,6 +347,24 @@ int parse_sum_container(const uint8_t* el, size_t el_len, const uint8_t* emb, si
     return GRANNE_B200_OK;
 }
 
+// Stages a parsed SumEmbeddings container (parse_sum_container) as d's embedding table, element offsets and term ids:
+// the handle's own container (h->dev) or its re-rank container (h->rerank).  The handle owns the memory and counts it.
+int stage_sum(Handle* h, gb::DeviceIndex& d, const gb::DenseView& ev, const gb::SumElements& se) {
+    d.kind = gb::kSumEmbeddings;
+    int rc = stage_dense(h, d, ev.data, ev.num, (uint32_t)ev.dim);
+    if (rc) return rc;
+    d.num_elements = se.offsets.size() - 1;
+    Buffer<unsigned long long> doff;
+    Buffer<uint32_t> dterms;
+    if ((rc = dev_alloc(&doff, se.offsets.size())) || (rc = dev_alloc(&dterms, se.terms.size()))) return rc;
+    GB_CUDA(cudaMemcpy(doff.get(), se.offsets.data(), se.offsets.size() * 8, cudaMemcpyHostToDevice));
+    if (!se.terms.empty())
+        GB_CUDA(cudaMemcpy(dterms.get(), se.terms.data(), se.terms.size() * 4, cudaMemcpyHostToDevice));
+    d.sum_offsets = stage(h, std::move(doff));
+    d.sum_terms = stage(h, std::move(dterms));
+    return GRANNE_B200_OK;
+}
+
 // Stages the element container (vectors / embedding table + element term lists) in HBM.
 int stage_elements(Handle* h, int kind, const uint8_t* el, size_t el_len, const uint8_t* emb, size_t emb_len) {
     std::string err;
@@ -355,17 +375,7 @@ int stage_elements(Handle* h, int kind, const uint8_t* el, size_t el_len, const 
         gb::DenseView ev;
         gb::SumElements se;
         if ((rc = parse_sum_container(el, el_len, emb, emb_len, &ev, &se))) return rc;
-        rc = stage_dense(h, d, ev.data, ev.num, (uint32_t)ev.dim);
-        if (rc) return rc;
-        d.num_elements = se.offsets.size() - 1;
-        Buffer<unsigned long long> doff;
-        Buffer<uint32_t> dterms;
-        if ((rc = dev_alloc(&doff, se.offsets.size())) || (rc = dev_alloc(&dterms, se.terms.size()))) return rc;
-        GB_CUDA(cudaMemcpy(doff.get(), se.offsets.data(), se.offsets.size() * 8, cudaMemcpyHostToDevice));
-        if (!se.terms.empty())
-            GB_CUDA(cudaMemcpy(dterms.get(), se.terms.data(), se.terms.size() * 4, cudaMemcpyHostToDevice));
-        d.sum_offsets = stage(h, std::move(doff));
-        d.sum_terms = stage(h, std::move(dterms));
+        if ((rc = stage_sum(h, d, ev, se))) return rc;
     } else {
         gb::DenseView dv;
         const bool i8 = kind == GRANNE_B200_ANGULAR_INT;
@@ -560,7 +570,7 @@ struct LaunchPlan {
     size_t smem;        // fast pass total
 };
 
-// `view`: the staged rows the kernels read, when they are not the handle's own (the re-rank rows)
+// `view`: the staged container the kernels read, when it is not the handle's own (the re-rank container)
 LaunchPlan make_plan(const Handle* h, uint32_t max_search, const gb::DeviceIndex* view = nullptr) {
     const gb::DeviceIndex& d = view ? *view : h->dev;
     LaunchPlan p{};
@@ -1024,54 +1034,89 @@ int enqueue_exact(Handle* h, Workspace* w, const void* d_queries, size_t nq, int
     return GRANNE_B200_OK;
 }
 
-// ---- two-stage search: angular_int traversal, f32 re-rank (rerank_kernels.cuh) -----------------------------------
-// The checks on the handle before any rows are read: an angular_int index without re-rank rows.
+// ---- two-stage search: angular_int traversal, exact re-rank (rerank_kernels.cuh) ---------------------------------
+// The re-rank container is angular f32 rows (DistF32 engines) or a SumEmbeddings container (DistSum); one per handle.
+// The checks on the handle before any container is read: an angular_int index without a re-rank container.
 int check_rerank_target(const Handle* h) {
     if (!h) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "index handle is null");
     if (h->dev.kind != gb::kAngularI8)
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "re-rank rows are attached to an angular_int index only");
+        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "a re-rank container is attached to an angular_int index only");
     if (h->rerank.vectors)
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "re-rank rows are already attached to this index");
+        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "a re-rank container is already attached to this index");
     return GRANNE_B200_OK;
 }
 
-// The checks on the rows: the index's width, and a row for every element of [0, Index::len).
+// The checks on the container: the index's width, and an element for every element of [0, Index::len).
 int check_rerank_shape(const Handle* h, uint64_t n, uint64_t dim) {
-    if (dim != h->dev.dim) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "re-rank rows must have the index's width");
+    if (dim != h->dev.dim)
+        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "the re-rank container must have the index's width");
     if (n < h->index_len)
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "re-rank rows must cover every element of the index");
+        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "the re-rank container must cover every element of the index");
     return GRANNE_B200_OK;
 }
 
-// Stages n angular f32 element rows as h's re-rank rows, laid out for the engine DistDispatch picks for their width.
-// They become visible to searches only once fully staged.  The target check is repeated under the handle's attach
-// lock, so that of two concurrent attaches one stages its rows and the other fails.
-int stage_rerank(Handle* h, const uint8_t* rows, uint64_t n, uint32_t dim, bool device_src) {
+// Drops the device allocations of the view r (its rows or table, and a sum view's offsets and terms), which hold
+// `bytes` of h->device_bytes.
+void drop_rerank_view(Handle* h, const gb::DeviceIndex& r, uint64_t bytes) {
+    for (const void* p : {r.vectors, static_cast<const void*>(r.sum_offsets), static_cast<const void*>(r.sum_terms)}) {
+        if (!p) continue;
+        auto it = std::find_if(h->allocations.begin(), h->allocations.end(),
+                               [&](const std::shared_ptr<void>& a) { return a.get() == p; });
+        if (it != h->allocations.end()) h->allocations.erase(it);
+    }
+    h->device_bytes -= bytes;
+}
+
+// Stages h's re-rank container with stage_into(r) (stage_dense or stage_sum into an empty view r).  It becomes visible
+// to searches only once fully staged; a container that fails part-way gives its memory back.  The target check is
+// repeated under the handle's attach lock, so that of two concurrent attaches one stages its container and the other
+// fails.
+template <class StageInto>
+int stage_rerank(Handle* h, StageInto&& stage_into) {
     std::lock_guard<std::mutex> g(h->rerank_mu);
     int rc = check_rerank_target(h);
     if (rc) return rc;
     gb::DeviceIndex r{};
-    r.kind = gb::kAngularF32;
-    if ((rc = stage_dense(h, r, rows, n, dim, device_src))) return rc;
-    r.num_elements = n;
+    const uint64_t before = h->device_bytes;
+    if ((rc = stage_into(r))) {
+        drop_rerank_view(h, r, h->device_bytes - before);
+        return rc;
+    }
     h->rerank = r;
+    h->rerank_bytes = h->device_bytes - before;
     return GRANNE_B200_OK;
 }
 
-// Drops h's re-rank rows and their memory (the multi handle's attach undoes a partial attach with it).  The caller
+// Stages n angular f32 element rows as h's re-rank rows, laid out for the engine DistDispatch picks for their width.
+int stage_rerank_rows(Handle* h, const uint8_t* rows, uint64_t n, uint32_t dim, bool device_src) {
+    return stage_rerank(h, [&](gb::DeviceIndex& r) {
+        r.kind = gb::kAngularF32;
+        const int rc = stage_dense(h, r, rows, n, dim, device_src);
+        r.num_elements = n;
+        return rc;
+    });
+}
+
+// Every host check of a SumEmbeddings re-rank container against h (h itself passed check_rerank_target): the images
+// parse, every term id is a row of the table, the table is at most 4096 wide (parse_sum_container), it has the index's
+// width, and there is an element for every element of the index.
+int check_rerank_sum(const Handle* h, const void* el, size_t el_len, const void* emb, size_t emb_len,
+                     gb::DenseView* ev, gb::SumElements* se) {
+    if (!el || !emb) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "elements or embeddings buffer is null");
+    const int rc = parse_sum_container(static_cast<const uint8_t*>(el), el_len, static_cast<const uint8_t*>(emb),
+                                       emb_len, ev, se);
+    if (rc) return rc;
+    return check_rerank_shape(h, se->offsets.size() - 1, ev->dim);
+}
+
+// Drops h's re-rank container and its memory (the multi handle's attach undoes a partial attach with it).  The caller
 // makes h's device current.
 void release_rerank(Handle* h) {
     std::lock_guard<std::mutex> g(h->rerank_mu);
-    const gb::DeviceIndex& r = h->rerank;
-    if (!r.vectors) return;
-    auto it = std::find_if(h->allocations.begin(), h->allocations.end(),
-                           [&](const std::shared_ptr<void>& a) { return a.get() == r.vectors; });
-    if (it != h->allocations.end()) {
-        h->allocations.erase(it);
-        // stage_dense's allocation: the rows, at least 16 bytes (dev_alloc)
-        h->device_bytes -= std::max<uint64_t>(r.num_vectors * r.row_stride * 4ull, 16);
-    }
+    if (!h->rerank.vectors) return;
+    drop_rerank_view(h, h->rerank, h->rerank_bytes);
     h->rerank = gb::DeviceIndex{};
+    h->rerank_bytes = 0;
 }
 
 // validate_search's rules plus the two-stage ones.
@@ -1082,15 +1127,15 @@ int validate_rerank(const Handle* h, const void* q, size_t nq, int fmt, uint32_t
     if (fmt != GRANNE_B200_QUERY_RAW_F32)
         return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "the two-stage search takes raw f32 queries");
     if (!h->rerank.vectors)
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "no re-rank rows are attached to this index");
+        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "no re-rank container is attached to this index");
     if (c == 0 || c > GRANNE_B200_RERANK_MAX_CANDIDATES)
         return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "num_candidates must be in 1..1024");
     if (k > c) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "num_neighbors exceeds num_candidates");
     return GRANNE_B200_OK;
 }
 
-// rerank_kernel for the f32 engine DistDispatch picks for the re-rank rows (never an i8 or embeddings engine: the
-// rows are staged as angular f32).
+// rerank_kernel for the engine DistDispatch picks for the re-rank container: the f32 engine for the width of angular
+// rows, DistSum for a SumEmbeddings container (never the i8 engine: no container is staged as angular_int).
 struct RerankLaunch {
     Handle* h;
     const gb::RerankArgs& a;
@@ -1098,8 +1143,8 @@ struct RerankLaunch {
     cudaStream_t stream;
     template <class Dist>
     int run() {
-        if constexpr (std::is_same<Dist, gb::DistI8>::value || std::is_same<Dist, gb::DistSum>::value) {
-            return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "re-rank rows must be angular f32 rows");
+        if constexpr (std::is_same<Dist, gb::DistI8>::value) {
+            return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "re-rank container must be angular f32 rows or SumEmbeddings");
         } else {
             auto kern = gb::rerank_kernel<Dist>;
             static std::atomic<bool> attr_set[64];  // function attributes are per device
@@ -1732,7 +1777,7 @@ int granne_b200_set_rerank_elements(granne_b200_index* h, const void* elements_b
             return fail(GRANNE_B200_ERR_FORMAT, err);
         if ((rc = check_rerank_shape(h, dv.num, dv.dim))) return rc;
         GB_DEVICE(h->device);
-        return stage_rerank(h, dv.data, dv.num, (uint32_t)dv.dim, false);
+        return stage_rerank_rows(h, dv.data, dv.num, (uint32_t)dv.dim, false);
     });
 }
 
@@ -1749,7 +1794,21 @@ int granne_b200_set_rerank_elements_device(granne_b200_index* h, const float* d_
             cudaGetLastError();
             return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "elements pointer is not device memory of the index's device");
         }
-        return stage_rerank(h, reinterpret_cast<const uint8_t*>(d_rows), n, dim, true);
+        return stage_rerank_rows(h, reinterpret_cast<const uint8_t*>(d_rows), n, dim, true);
+    });
+}
+
+int granne_b200_set_rerank_embeddings(granne_b200_index* h, const void* elements_bytes, size_t elements_len,
+                                      const void* embeddings_bytes, size_t embeddings_len) {
+    int rc = check_rerank_target(h);
+    if (rc) return rc;
+    return guarded([&] {
+        gb::DenseView ev;
+        gb::SumElements se;
+        if ((rc = check_rerank_sum(h, elements_bytes, elements_len, embeddings_bytes, embeddings_len, &ev, &se)))
+            return rc;
+        GB_DEVICE(h->device);
+        return stage_rerank(h, [&](gb::DeviceIndex& r) { return stage_sum(h, r, ev, se); });
     });
 }
 
@@ -2696,6 +2755,35 @@ int multi_batch(granne_b200_multi* m, const void* queries, size_t nq, int query_
     });
 }
 
+// Attaches a re-rank container to every part: check(i) runs every host check of part i's images (i: the part, whose
+// image is 0 for a replicated handle), for every part, before attach(i) stages any.  If a part then fails to stage (a
+// device error), the parts this call attached drop their containers again, so that the call can be repeated.
+template <class Check, class Attach>
+int multi_attach_rerank(granne_b200_multi* m, Check&& check, Attach&& attach) {
+    return guarded([&] {
+        const size_t n = m->parts.size();
+        for (size_t i = 0; i < n; ++i) {
+            int rc = check_rerank_target(m->parts[i]);
+            if (rc) return rc;
+            if ((rc = check(i))) return rc;
+        }
+        std::vector<char> attached(n, 0);
+        const int rc = for_each_part(n, [&](size_t i) {
+            const int r = attach(i);
+            attached[i] = r == GRANNE_B200_OK;
+            return r;
+        });
+        if (rc) {
+            for (size_t i = 0; i < n; ++i) {
+                if (!attached[i]) continue;
+                DeviceGuard guard(m->parts[i]->device);
+                release_rerank(m->parts[i]);
+            }
+        }
+        return rc;
+    });
+}
+
 }  // namespace
 
 extern "C" {
@@ -2729,40 +2817,47 @@ int granne_b200_multi_exact_search_batch(granne_b200_multi* m, const void* queri
                        });
 }
 
-// Every image is checked on the host against its part before any part stages rows; if a part then fails to stage
-// (a device error), the parts this call attached drop their rows again, so that the call can be repeated.
+// Every image is checked on the host against its part before any part stages rows (multi_attach_rerank).
 int granne_b200_multi_set_rerank_elements(granne_b200_multi* m, const void* const* elements_bytes,
                                           const size_t* elements_len) {
     if (!m || !elements_bytes || !elements_len) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
-    return guarded([&] {
-        const size_t n = m->parts.size();
-        auto image = [&](size_t i) { return m->mode == GRANNE_B200_MODE_REPLICATED ? 0 : i; };
-        for (size_t i = 0; i < n; ++i) {
-            int rc = check_rerank_target(m->parts[i]);
-            if (rc) return rc;
+    auto image = [&](size_t i) { return m->mode == GRANNE_B200_MODE_REPLICATED ? 0 : i; };
+    return multi_attach_rerank(
+        m,
+        [&](size_t i) {
             if (!elements_bytes[image(i)]) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "elements buffer is null");
             gb::DenseView dv;
             std::string err;
             if (!gb::parse_dense(static_cast<const uint8_t*>(elements_bytes[image(i)]), elements_len[image(i)], 4, &dv,
                                  &err))
                 return fail(GRANNE_B200_ERR_FORMAT, err);
-            if ((rc = check_rerank_shape(m->parts[i], dv.num, dv.dim))) return rc;
-        }
-        std::vector<char> attached(n, 0);
-        const int rc = for_each_part(n, [&](size_t i) {
-            const int r = granne_b200_set_rerank_elements(m->parts[i], elements_bytes[image(i)], elements_len[image(i)]);
-            attached[i] = r == GRANNE_B200_OK;
-            return r;
+            return check_rerank_shape(m->parts[i], dv.num, dv.dim);
+        },
+        [&](size_t i) {
+            return granne_b200_set_rerank_elements(m->parts[i], elements_bytes[image(i)], elements_len[image(i)]);
         });
-        if (rc) {
-            for (size_t i = 0; i < n; ++i) {
-                if (!attached[i]) continue;
-                DeviceGuard guard(m->parts[i]->device);
-                release_rerank(m->parts[i]);
-            }
-        }
-        return rc;
-    });
+}
+
+// One term-list image per part's shard (one for a replicated handle), one embedding table for all parts, as
+// granne_b200_multi_open takes them; every image is checked on the host before any part stages (multi_attach_rerank).
+int granne_b200_multi_set_rerank_embeddings(granne_b200_multi* m, const void* const* elements_bytes,
+                                            const size_t* elements_len, const void* embeddings_bytes,
+                                            size_t embeddings_len) {
+    if (!m || !elements_bytes || !elements_len || !embeddings_bytes)
+        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
+    auto image = [&](size_t i) { return m->mode == GRANNE_B200_MODE_REPLICATED ? 0 : i; };
+    return multi_attach_rerank(
+        m,
+        [&](size_t i) {
+            gb::DenseView ev;
+            gb::SumElements se;
+            return check_rerank_sum(m->parts[i], elements_bytes[image(i)], elements_len[image(i)], embeddings_bytes,
+                                    embeddings_len, &ev, &se);
+        },
+        [&](size_t i) {
+            return granne_b200_set_rerank_embeddings(m->parts[i], elements_bytes[image(i)], elements_len[image(i)],
+                                                     embeddings_bytes, embeddings_len);
+        });
 }
 
 // RANGE_PARTITIONED: every shard re-ranks its own candidates; the shard lists are sorted by (distance, local id) and

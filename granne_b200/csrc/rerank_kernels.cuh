@@ -1,11 +1,14 @@
 // rerank_kernels.cuh — stage 2 of the two-stage search (granne_b200_search_rerank_batch*).
 //
 // Stage 1 is Granne::search over an angular_int index with k = C candidates (search_kernel, unchanged).  Stage 2, here,
-// gives each candidate i its f32 angular distance to the query, angular::Vectors::dist_to_element(i,
-// &angular::Vector::from(q)) (angular.rs:63-74, math.rs:16-42), and keeps the first k by (distance, id), the order of
-// into_sorted_vec (src/index/mod.rs:1036).  The distances come from the search path's own f32 engines (DistF32<FULL>,
-// DistF32Generic) run over a DeviceIndex view of the attached f32 rows, so they are the reference's bit for bit; the
-// result depends only on the set of candidates, not on the order stage 1 wrote them in.
+// gives each candidate i its f32 angular distance to the query over the attached container F,
+// F.dist_to_element(i, &angular::Vector::from(q)), and keeps the first k by (distance, id), the order of
+// into_sorted_vec (src/index/mod.rs:1036).  The distances come from the search path's own engines run over a
+// DeviceIndex view of F, so they are the reference's bit for bit:
+//   - angular f32 rows: DistF32<FULL> / DistF32Generic (angular.rs:63-74, math.rs:16-42);
+//   - a SumEmbeddings container: DistSum, which materialises each candidate (ordered term sum, normalize_f32) in the
+//     staging tile, stg_rows at a time, before the f32 angular distance (embeddings/mod.rs:124-143,164-174).
+// The result depends only on the set of candidates, not on the order stage 1 wrote them in.
 //
 // One warp per query, persistent over a work counter: normalise the query (prepare_query), distances of the candidates
 // 32 at a time through Dist::dists, their make_key(d, id) keys into shared memory padded with ~0 to a power of two, a
@@ -36,7 +39,7 @@ struct RerankArgs {
     uint32_t* out_counts;        // nq (or null)
     unsigned int* work_counter;  // zeroed before the launch
     int* error_flag;             // kStatusNotFinite is or-ed in on a NaN distance
-    uint32_t stg_rows, stg_row_bytes, tile_rows;  // the f32 engine's staging and ordered-sum tiles (make_plan)
+    uint32_t stg_rows, stg_row_bytes, tile_rows;  // the engine's staging and ordered-sum tiles (make_plan)
 };
 
 // Ascending sort of keys[0, p) (p a power of two) by the warp.  The pairs (i, i ^ j) of one step are disjoint, so a

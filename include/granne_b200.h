@@ -193,26 +193,34 @@ int granne_b200_exact_search_batch_device(granne_b200_index* h, const void* d_qu
 
 /* ---- two-stage search: traverse angular_int rows, re-rank by exact f32 angular distance ----------------------------
  * NOT a reference function: what a user of granne assembles by hand from two containers over one index.  For an
- * angular_int handle h with attached angular f32 rows F and a raw f32 query q:
+ * angular_int handle h with an attached container F (angular rows or SumEmbeddings) and a raw f32 query q:
  *   1. S = Granne<angular_int::Vectors>::search(&angular_int::Vector::from(q), max_search, C), i.e. exactly
  *      granne_b200_search_batch(h, q, RAW_F32, max_search, C): at most min(C, max_search) ids;
- *   2. d_i = F.dist_to_element(i, &angular::Vector::from(q)) for i in S, the reference's f32 angular distance bit for
- *      bit (angular.rs:63-74, math.rs:16-42);
+ *   2. d_i = F.dist_to_element(i, &angular::Vector::from(q)) for i in S, over the attached container (angular rows or
+ *      SumEmbeddings), the reference's f32 angular distance bit for bit (angular.rs:63-74, math.rs:16-42; for
+ *      SumEmbeddings the ordered term sum and normalize_f32 first, embeddings/mod.rs:124-143,164-174, math.rs:92-150);
  *   3. the first min(k, |S|) entries of sort ascending { (d_i, i) }, the order of into_sorted_vec (src/index/mod.rs:1036).
  * The result depends only on the set S.  Per query, its intersection with the exact f32 top-k equals S's, so its
  * recall is the candidate set's and never below the i8 search's.  Output layout as granne_b200_search_batch.
  *
- * Attach F once, before searching; there is no replacement while searches may be in flight, and an attach concurrent
- * with a search on h is not supported.  Concurrent attaches on h are serialised: one attaches its rows, the others
- * return ERR_INVALID_ARGUMENT.  The rows are copied into HBM (counted by granne_b200_device_bytes) in the layout the
- * search path's f32 engine for their width reads.
- * ERR_INVALID_ARGUMENT: h is not ANGULAR_INT, rows are already attached, their width differs from the index's, or
- * there are fewer than granne_b200_len(h) rows.  ERR_FORMAT: a malformed image.
+ * Attach F once, before searching; one container per handle, of either kind, with no replacement while searches may
+ * be in flight, and an attach concurrent with a search on h is not supported.  Concurrent attaches on h are
+ * serialised: one attaches its container, the others return ERR_INVALID_ARGUMENT.  The container is copied into HBM
+ * (counted by granne_b200_device_bytes): angular rows in the layout the search path's f32 engine for their width
+ * reads, a SumEmbeddings container as an EMBEDDINGS index stages it (table, offsets, term ids).
+ * ERR_INVALID_ARGUMENT: h is not ANGULAR_INT, a container is already attached, its width differs from the index's, or
+ * it holds fewer than granne_b200_len(h) elements.  ERR_FORMAT: a malformed image.  Every image check runs on the host
+ * before any device call.
  *   elements_bytes   an angular elements file image (u64 dim | normalised f32 rows)
  *   d_rows           n x dim normalised f32 rows in device memory of h's device */
 #define GRANNE_B200_RERANK_MAX_CANDIDATES 1024
 int granne_b200_set_rerank_elements(granne_b200_index* h, const void* elements_bytes, size_t elements_len);
 int granne_b200_set_rerank_elements_device(granne_b200_index* h, const float* d_rows, uint64_t n, uint32_t dim);
+/* Attaches a SumEmbeddings container: the two images granne_b200_open takes for GRANNE_B200_EMBEDDINGS (the element
+ * term lists, the embedding table).  Besides the rules above, ERR_INVALID_ARGUMENT for a table wider than 4096, and
+ * ERR_FORMAT for a term id past the table.  A NaN distance in stage 2 returns ERR_NOT_FINITE from the search. */
+int granne_b200_set_rerank_embeddings(granne_b200_index* h, const void* elements_bytes, size_t elements_len,
+                                      const void* embeddings_bytes, size_t embeddings_len);
 /* The two-stage search for nq raw f32 queries (host buffers).  ERR_INVALID_ARGUMENT, before any device call, when
  * query_format is not RAW_F32, no rows are attached, num_candidates is 0 or above GRANNE_B200_RERANK_MAX_CANDIDATES,
  * num_neighbors > num_candidates, or a rule of granne_b200_search_batch is broken.  out_stats (may be NULL) holds stage
@@ -288,6 +296,12 @@ int granne_b200_multi_exact_search_batch(granne_b200_multi* m, const void* queri
  * stage its rows (a device error), the parts this call attached release theirs again, so the call can be repeated. */
 int granne_b200_multi_set_rerank_elements(granne_b200_multi* m, const void* const* elements_bytes,
                                           const size_t* elements_len);
+/* granne_b200_set_rerank_embeddings on every part: REPLICATED takes one term-list image (elements_bytes[0]),
+ * RANGE_PARTITIONED one per shard; the one embedding table is shared by all parts, as granne_b200_multi_open shares
+ * it.  Images are checked and a failed attach is undone as in granne_b200_multi_set_rerank_elements. */
+int granne_b200_multi_set_rerank_embeddings(granne_b200_multi* m, const void* const* elements_bytes,
+                                            const size_t* elements_len, const void* embeddings_bytes,
+                                            size_t embeddings_len);
 /* granne_b200_search_rerank_batch over a multi handle, with u64 GLOBAL ids like granne_b200_multi_search_batch.
  * RANGE_PARTITIONED: every shard re-ranks its own candidates and the lists are merged by (distance, global id), which
  * equals re-ranking the union of the shards' candidate sets. */

@@ -221,13 +221,19 @@ public:
         return out;
     }
 
-    // Two-stage search (granne_b200_search_rerank_batch): attach the angular f32 rows of this angular_int index's
-    // elements once, then search_rerank returns, for nq raw f32 queries, the first num_candidates results of the i8
-    // search re-ranked by their exact f32 angular distance.  Not a reference function.
-    void set_rerank_elements(const Elements& angular_rows) {
-        if (angular_rows.kind != ElementKind::Angular)
-            throw Error(GRANNE_B200_ERR_INVALID_ARGUMENT, "re-rank rows are angular elements");
-        check(granne_b200_set_rerank_elements(h_, angular_rows.bytes.data(), angular_rows.bytes.size()));
+    // Two-stage search (granne_b200_search_rerank_batch): attach the container of this angular_int index's elements
+    // once (angular f32 rows, or the SumEmbeddings container the rows were computed from), then search_rerank
+    // returns, for nq raw f32 queries, the first num_candidates results of the i8 search re-ranked by their exact f32
+    // angular distance over that container.  Not a reference function.
+    void set_rerank_elements(const Elements& container) {
+        if (container.kind == ElementKind::Angular) {
+            check(granne_b200_set_rerank_elements(h_, container.bytes.data(), container.bytes.size()));
+        } else if (container.kind == ElementKind::Embeddings) {
+            check(granne_b200_set_rerank_embeddings(h_, container.bytes.data(), container.bytes.size(),
+                                                    container.embeddings.data(), container.embeddings.size()));
+        } else {
+            throw Error(GRANNE_B200_ERR_INVALID_ARGUMENT, "re-rank containers are angular or SumEmbeddings elements");
+        }
     }
     std::vector<SearchResult> search_rerank(const float* queries, size_t nq, size_t max_search, size_t num_candidates,
                                             size_t num_neighbors) const {
