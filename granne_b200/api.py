@@ -137,6 +137,58 @@ def _kind(element_type):
     return int(element_type)
 
 
+def _host_queries(queries, already_element, dim=None):
+    """(contiguous queries, query format) of a host call: int8 rows are elements, everything else becomes float32.
+    dim: the index's width, where the handle tells it."""
+    q = np.asarray(queries)
+    fmt = QUERY_ELEMENT if already_element or q.dtype == np.int8 else QUERY_RAW_F32
+    q = np.ascontiguousarray(q, dtype=None if q.dtype == np.int8 else np.float32)
+    if q.ndim != 2 or (dim is not None and q.shape[1] != dim):
+        raise ValueError("queries must have shape (nq, %s)" % ("dim" if dim is None else dim))
+    return q, fmt
+
+
+def _raw_f32_queries(queries, dim=None):
+    """The queries of a two-stage call: raw float32 only."""
+    if np.asarray(queries).dtype == np.int8:
+        raise ValueError("the two-stage search takes raw float32 queries")
+    return _host_queries(queries, False, dim)[0]
+
+
+def _host_outputs(nq, k, id_dtype, with_stats=False):
+    """(ids, dists, counts, stats) for the results of nq queries; stats is None unless with_stats."""
+    shape = (nq, k)
+    return (np.empty(shape, dtype=id_dtype), np.empty(shape, dtype=np.float32), np.empty(nq, dtype=np.uint32),
+            np.zeros((nq, STATS_PER_QUERY), dtype=np.uint64) if with_stats else None)
+
+
+def _device_outputs(q, k, out):
+    """The (ids, dists, counts) tensors of a device call for the queries q: `out` checked, or fresh ones."""
+    import torch
+
+    nq = q.shape[0]
+    if out is None:
+        return (torch.empty((nq, k), dtype=torch.int32, device=q.device),
+                torch.empty((nq, k), dtype=torch.float32, device=q.device),
+                torch.empty((nq,), dtype=torch.int32, device=q.device))
+    for t, dt, shape in zip(out, (torch.int32, torch.float32, torch.int32), ((nq, k), (nq, k), (nq,))):
+        if (not t.is_cuda or t.device != q.device or t.dtype != dt or tuple(t.shape) != shape
+                or not t.is_contiguous()):
+            raise ValueError("out tensors must be contiguous (ids int32 [nq,k], dists float32 [nq,k], counts "
+                             "int32 [nq]) on the queries' device")
+    return out
+
+
+def _raw_stream(stream, device):
+    """The raw cudaStream_t of `stream`, a torch.cuda.Stream or a raw pointer; None: torch's current stream on
+    `device`."""
+    if stream is None:
+        import torch
+
+        stream = torch.cuda.current_stream(device)
+    return getattr(stream, "cuda_stream", stream)
+
+
 class Granne:
     """granne.Granne (py/src/lib.rs:149-344) on the GPU.
 
@@ -321,24 +373,9 @@ class Granne:
         queries: (nq, dim) float32 raw vectors (normalised / quantised by the library like the reference's Python
         binding), or with already_element=True rows that already are elements (normalised f32; int8 for
         angular_int).  Returns (ids uint32 [nq,k] padded 0xFFFFFFFF, dists float32 [nq,k] padded +inf, counts)."""
-        q = np.asarray(queries)
-        fmt = QUERY_ELEMENT if already_element else QUERY_RAW_F32
-        if q.dtype == np.int8:
-            if self.element_kind != ANGULAR_INT:
-                raise ValueError("int8 queries need an angular_int index")
-            fmt = QUERY_ELEMENT
-            q = np.ascontiguousarray(q)
-        else:
-            q = np.ascontiguousarray(q, dtype=np.float32)
-            if fmt == QUERY_ELEMENT and self.element_kind == ANGULAR_INT:
-                raise ValueError("angular_int elements are int8")
-        if q.ndim != 2 or q.shape[1] != self.dim:
-            raise ValueError("queries must have shape (nq, %d)" % self.dim)
+        q, fmt = self._host_queries(queries, already_element)
         nq, k = q.shape[0], int(num_elements)
-        ids = np.empty((nq, k), dtype=np.uint32)
-        dists = np.empty((nq, k), dtype=np.float32)
-        counts = np.empty(nq, dtype=np.uint32)
-        stats = np.zeros((nq, STATS_PER_QUERY), dtype=np.uint64) if with_stats else None
+        ids, dists, counts, stats = _host_outputs(nq, k, np.uint32, with_stats)
         _check(load_library().granne_b200_search_batch(self._h, _ptr(q), nq, fmt, int(max_search), k, _ptr(ids),
                                                        _ptr(dists), _ptr(counts),
                                                        _ptr(stats) if with_stats else None))
@@ -347,21 +384,14 @@ class Granne:
         return ids, dists, counts
 
     def _host_queries(self, queries, already_element):
-        """(contiguous queries, query format) with search_batch's checks."""
+        """_host_queries for this index: its width, and its rules on int8 rows."""
         q = np.asarray(queries)
-        fmt = QUERY_ELEMENT if already_element else QUERY_RAW_F32
         if q.dtype == np.int8:
             if self.element_kind != ANGULAR_INT:
                 raise ValueError("int8 queries need an angular_int index")
-            fmt = QUERY_ELEMENT
-            q = np.ascontiguousarray(q)
-        else:
-            q = np.ascontiguousarray(q, dtype=np.float32)
-            if fmt == QUERY_ELEMENT and self.element_kind == ANGULAR_INT:
-                raise ValueError("angular_int elements are int8")
-        if q.ndim != 2 or q.shape[1] != self.dim:
-            raise ValueError("queries must have shape (nq, %d)" % self.dim)
-        return q, fmt
+        elif already_element and self.element_kind == ANGULAR_INT:
+            raise ValueError("angular_int elements are int8")
+        return _host_queries(q, already_element, self.dim)
 
     def exact_search_batch(self, queries, num_elements=DEFAULT_NUM_ELEMENTS, already_element=False):
         """Exact k nearest neighbours: the first min(k, len(self)) of all elements i < len(self) by (distance, id),
@@ -370,39 +400,24 @@ class Granne:
         search_batch's layout."""
         q, fmt = self._host_queries(queries, already_element)
         nq, k = q.shape[0], int(num_elements)
-        ids = np.empty((nq, k), dtype=np.uint32)
-        dists = np.empty((nq, k), dtype=np.float32)
-        counts = np.empty(nq, dtype=np.uint32)
+        ids, dists, counts, _ = _host_outputs(nq, k, np.uint32)
         _check(load_library().granne_b200_exact_search_batch(self._h, _ptr(q), nq, fmt, k, _ptr(ids), _ptr(dists),
                                                              _ptr(counts)))
         return ids, dists, counts
 
     def exact_search_batch_device(self, queries, num_elements=DEFAULT_NUM_ELEMENTS, already_element=False, out=None,
                                   stream=None):
-        """Device-resident exact_search_batch: CUDA tensors in and out, asynchronous on `stream` (default: the current
-        torch stream); a NaN distance is reported by stream_status()."""
+        """Device-resident exact_search_batch: CUDA tensors in and out, asynchronous on `stream` (a torch.cuda.Stream
+        or a raw cudaStream_t; default: the current torch stream); a NaN distance is reported by stream_status()."""
         import torch
 
         q = self._check_device_queries(queries)
         fmt = QUERY_ELEMENT if already_element or q.dtype == torch.int8 else QUERY_RAW_F32
         nq, k = q.shape[0], int(num_elements)
-        if out is not None:
-            for t, dt, shape in zip(out, (torch.int32, torch.float32, torch.int32), ((nq, k), (nq, k), (nq,))):
-                if (not t.is_cuda or t.device != q.device or t.dtype != dt or tuple(t.shape) != shape
-                        or not t.is_contiguous()):
-                    raise ValueError("out tensors must be contiguous (ids int32 [nq,k], dists float32 [nq,k], counts "
-                                     "int32 [nq]) on the queries' device")
-        else:
-            dev = q.device
-            out = (torch.empty((nq, k), dtype=torch.int32, device=dev),
-                   torch.empty((nq, k), dtype=torch.float32, device=dev),
-                   torch.empty((nq,), dtype=torch.int32, device=dev))
-        ids, dists, counts = out
-        s = stream if stream is not None else torch.cuda.current_stream(q.device).cuda_stream
-        s = getattr(s, "cuda_stream", s)
+        ids, dists, counts = _device_outputs(q, k, out)
         _check(load_library().granne_b200_exact_search_batch_device(
             self._h, C.c_void_p(q.data_ptr()), nq, fmt, k, C.c_void_p(ids.data_ptr()), C.c_void_p(dists.data_ptr()),
-            C.c_void_p(counts.data_ptr()), C.c_void_p(s)))
+            C.c_void_p(counts.data_ptr()), C.c_void_p(_raw_stream(stream, q.device))))
         return ids, dists, counts
 
     # ---- two-stage search (granne_b200_search_rerank_batch*) ----
@@ -442,17 +457,9 @@ class Granne:
         by their exact f32 angular distance to the query over the attached rows; the first num_elements by
         (distance, id).  Not a reference function.  queries: raw float32 (nq, dim).  Returns (ids, dists, counts)
         in search_batch's layout; with_stats adds stage 1's counters."""
-        q = np.asarray(queries)
-        if q.dtype == np.int8:
-            raise ValueError("the two-stage search takes raw float32 queries")
-        q = np.ascontiguousarray(q, dtype=np.float32)
-        if q.ndim != 2 or q.shape[1] != self.dim:
-            raise ValueError("queries must have shape (nq, %d)" % self.dim)
+        q = _raw_f32_queries(queries, self.dim)
         nq, k = q.shape[0], int(num_elements)
-        ids = np.empty((nq, k), dtype=np.uint32)
-        dists = np.empty((nq, k), dtype=np.float32)
-        counts = np.empty(nq, dtype=np.uint32)
-        stats = np.zeros((nq, STATS_PER_QUERY), dtype=np.uint64) if with_stats else None
+        ids, dists, counts, stats = _host_outputs(nq, k, np.uint32, with_stats)
         _check(load_library().granne_b200_search_rerank_batch(
             self._h, _ptr(q), nq, QUERY_RAW_F32, int(max_search), int(num_candidates), k, _ptr(ids), _ptr(dists),
             _ptr(counts), _ptr(stats) if with_stats else None))
@@ -478,33 +485,20 @@ class Granne:
     def search_batch_rerank_device(self, queries, num_candidates, max_search=DEFAULT_MAX_SEARCH,
                                    num_elements=DEFAULT_NUM_ELEMENTS, out=None, stats=None, stream=None):
         """Device-resident search_batch_rerank: a CUDA float32 tensor in, CUDA tensors out (ids int32 view of u32
-        bits, dists float32, counts int32), asynchronous on `stream` (default: the current torch stream); a NaN
-        distance is reported by stream_status()."""
+        bits, dists float32, counts int32), asynchronous on `stream` (a torch.cuda.Stream or a raw cudaStream_t;
+        default: the current torch stream); a NaN distance is reported by stream_status()."""
         import torch
 
         q = self._check_device_queries(queries)
         if q.dtype != torch.float32:
             raise ValueError("the two-stage search takes raw float32 queries")
         nq, k = q.shape[0], int(num_elements)
-        if out is not None:
-            for t, dt, shape in zip(out, (torch.int32, torch.float32, torch.int32), ((nq, k), (nq, k), (nq,))):
-                if (not t.is_cuda or t.device != q.device or t.dtype != dt or tuple(t.shape) != shape
-                        or not t.is_contiguous()):
-                    raise ValueError("out tensors must be contiguous (ids int32 [nq,k], dists float32 [nq,k], counts "
-                                     "int32 [nq]) on the queries' device")
-        else:
-            dev = q.device
-            out = (torch.empty((nq, k), dtype=torch.int32, device=dev),
-                   torch.empty((nq, k), dtype=torch.float32, device=dev),
-                   torch.empty((nq,), dtype=torch.int32, device=dev))
+        ids, dists, counts = _device_outputs(q, k, out)
         _check_stats(stats, q)
-        ids, dists, counts = out
-        s = stream if stream is not None else torch.cuda.current_stream(q.device).cuda_stream
-        s = getattr(s, "cuda_stream", s)
         _check(load_library().granne_b200_search_rerank_batch_device(
             self._h, C.c_void_p(q.data_ptr()), nq, QUERY_RAW_F32, int(max_search), int(num_candidates), k,
             C.c_void_p(ids.data_ptr()), C.c_void_p(dists.data_ptr()), C.c_void_p(counts.data_ptr()),
-            C.c_void_p(stats.data_ptr()) if stats is not None else None, C.c_void_p(s)))
+            C.c_void_p(stats.data_ptr()) if stats is not None else None, C.c_void_p(_raw_stream(stream, q.device))))
         return ids, dists, counts
 
     def _word_tables(self):
@@ -540,47 +534,35 @@ class Granne:
     def search_batch_device(self, queries, max_search=DEFAULT_MAX_SEARCH, num_elements=DEFAULT_NUM_ELEMENTS,
                             already_element=False, out=None, stats=None, stream=None):
         """Device-resident variant: `queries` is a CUDA torch tensor on this index's device; returns CUDA tensors
-        (ids int32 view of u32 bits, dists float32, counts int32).  Asynchronous on the current torch stream."""
+        (ids int32 view of u32 bits, dists float32, counts int32).  Asynchronous on `stream` (a torch.cuda.Stream or a
+        raw cudaStream_t; default: the current torch stream)."""
         import torch
 
         q = self._check_device_queries(queries)
         fmt = QUERY_ELEMENT if already_element or q.dtype == torch.int8 else QUERY_RAW_F32
         nq, k = q.shape[0], int(num_elements)
-        if out is not None:
-            for t, dt, shape in zip(out, (torch.int32, torch.float32, torch.int32), ((nq, k), (nq, k), (nq,))):
-                if (not t.is_cuda or t.device != q.device or t.dtype != dt or tuple(t.shape) != shape
-                        or not t.is_contiguous()):
-                    raise ValueError("out tensors must be contiguous (ids int32 [nq,k], dists float32 [nq,k], counts "
-                                     "int32 [nq]) on the queries' device")
+        ids, dists, counts = _device_outputs(q, k, out)
         _check_stats(stats, q)
-        if out is None:
-            dev = q.device
-            out = (torch.empty((nq, k), dtype=torch.int32, device=dev),
-                   torch.empty((nq, k), dtype=torch.float32, device=dev),
-                   torch.empty((nq,), dtype=torch.int32, device=dev))
-        ids, dists, counts = out
-        s = stream if stream is not None else torch.cuda.current_stream(q.device).cuda_stream
         _check(load_library().granne_b200_search_batch_device(
             self._h, C.c_void_p(q.data_ptr()), nq, fmt, int(max_search), k, C.c_void_p(ids.data_ptr()),
             C.c_void_p(dists.data_ptr()), C.c_void_p(counts.data_ptr()),
-            C.c_void_p(stats.data_ptr()) if stats is not None else None, C.c_void_p(s)))
+            C.c_void_p(stats.data_ptr()) if stats is not None else None, C.c_void_p(_raw_stream(stream, q.device))))
         return ids, dists, counts
 
     def search_batch_device_gather(self, queries, gather, max_search=DEFAULT_MAX_SEARCH,
                                    num_elements=DEFAULT_NUM_ELEMENTS, already_element=False, counts=None, stats=None,
                                    stream=None):
         """Like search_batch_device, but the result rows are stored by the kernels straight into every peer's
-        gathered buffer described by `gather` (a PeerGather)."""
+        gathered buffer described by `gather` (a PeerGather).  stream: as for search_batch_device."""
         import torch
 
         q = self._check_device_queries(queries)
         fmt = QUERY_ELEMENT if already_element or q.dtype == torch.int8 else QUERY_RAW_F32
         _check_stats(stats, q)
-        s = stream if stream is not None else torch.cuda.current_stream(q.device).cuda_stream
         _check(load_library().granne_b200_search_batch_device_gather(
             self._h, C.c_void_p(q.data_ptr()), q.shape[0], fmt, int(max_search), int(num_elements), C.byref(gather),
             C.c_void_p(counts.data_ptr()) if counts is not None else None,
-            C.c_void_p(stats.data_ptr()) if stats is not None else None, C.c_void_p(s)))
+            C.c_void_p(stats.data_ptr()) if stats is not None else None, C.c_void_p(_raw_stream(stream, q.device))))
 
     def _check_device_queries(self, q):
         """Same checks as the host path (search_batch): a wrong dtype, width, device or a strided view would make the
@@ -666,38 +648,18 @@ class MultiGranne:
 
     def search_batch(self, queries, max_search=DEFAULT_MAX_SEARCH, num_elements=DEFAULT_NUM_ELEMENTS,
                      already_element=False):
-        q = np.asarray(queries)
-        fmt = QUERY_ELEMENT if already_element else QUERY_RAW_F32
-        if q.dtype == np.int8:
-            fmt = QUERY_ELEMENT
-            q = np.ascontiguousarray(q)
-        else:
-            q = np.ascontiguousarray(q, dtype=np.float32)
-        if q.ndim != 2:
-            raise ValueError("queries must have shape (nq, dim)")
+        q, fmt = _host_queries(queries, already_element)
         nq, k = q.shape[0], int(num_elements)
-        ids = np.empty((nq, k), dtype=np.uint64)
-        dists = np.empty((nq, k), dtype=np.float32)
-        counts = np.empty(nq, dtype=np.uint32)
+        ids, dists, counts, _ = _host_outputs(nq, k, np.uint64)
         _check(load_library().granne_b200_multi_search_batch(self._h, _ptr(q), nq, fmt, int(max_search), k, _ptr(ids),
                                                              _ptr(dists), _ptr(counts)))
         return ids, dists, counts
 
     def exact_search_batch(self, queries, num_elements=DEFAULT_NUM_ELEMENTS, already_element=False):
         """Exact k nearest neighbours over all shards (granne_b200_multi_exact_search_batch): GLOBAL uint64 ids."""
-        q = np.asarray(queries)
-        fmt = QUERY_ELEMENT if already_element else QUERY_RAW_F32
-        if q.dtype == np.int8:
-            fmt = QUERY_ELEMENT
-            q = np.ascontiguousarray(q)
-        else:
-            q = np.ascontiguousarray(q, dtype=np.float32)
-        if q.ndim != 2:
-            raise ValueError("queries must have shape (nq, dim)")
+        q, fmt = _host_queries(queries, already_element)
         nq, k = q.shape[0], int(num_elements)
-        ids = np.empty((nq, k), dtype=np.uint64)
-        dists = np.empty((nq, k), dtype=np.float32)
-        counts = np.empty(nq, dtype=np.uint32)
+        ids, dists, counts, _ = _host_outputs(nq, k, np.uint64)
         _check(load_library().granne_b200_multi_exact_search_batch(self._h, _ptr(q), nq, fmt, k, _ptr(ids),
                                                                    _ptr(dists), _ptr(counts)))
         return ids, dists, counts
@@ -705,40 +667,32 @@ class MultiGranne:
     def set_rerank_elements(self, elements):
         """Granne.set_rerank_elements on every part: one angular elements image (`bytes`) for a replicated handle,
         a list with one image per shard for a partitioned one."""
-        images = [elements] if isinstance(elements, (bytes, bytearray, memoryview)) else list(elements)
-        keep = [np.frombuffer(e, dtype=np.uint8) for e in images]
-        ptrs = (C.c_void_p * len(keep))(*[a.ctypes.data for a in keep])
-        lens = (C.c_size_t * len(keep))(*[a.size for a in keep])
-        if len(keep) != (1 if self.mode == MODE_REPLICATED else self.num_parts()):
-            raise ValueError("one image for a replicated handle, one per shard for a partitioned one")
+        keep, ptrs, lens = self._part_images(elements)
         _check(load_library().granne_b200_multi_set_rerank_elements(self._h, ptrs, lens))
 
     def set_rerank_embeddings(self, elements_list, embeddings):
         """Granne.set_rerank_embeddings on every part: one term-list image (`bytes`) for a replicated handle, a list
         with one per shard for a partitioned one, and one embedding table image shared by all parts."""
-        images = ([elements_list] if isinstance(elements_list, (bytes, bytearray, memoryview))
-                  else list(elements_list))
-        keep = [np.frombuffer(e, dtype=np.uint8) for e in images]
-        ptrs = (C.c_void_p * len(keep))(*[a.ctypes.data for a in keep])
-        lens = (C.c_size_t * len(keep))(*[a.size for a in keep])
-        if len(keep) != (1 if self.mode == MODE_REPLICATED else self.num_parts()):
-            raise ValueError("one image for a replicated handle, one per shard for a partitioned one")
+        keep, ptrs, lens = self._part_images(elements_list)
         mb = np.frombuffer(embeddings, dtype=np.uint8)
         _check(load_library().granne_b200_multi_set_rerank_embeddings(self._h, ptrs, lens, _ptr(mb), mb.size))
+
+    def _part_images(self, images):
+        """One image (`bytes`) or a list of them as (arrays that keep them alive, void*[], size_t[]): one for a
+        replicated handle, one per shard for a partitioned one."""
+        images = [images] if isinstance(images, (bytes, bytearray, memoryview)) else list(images)
+        keep = [np.frombuffer(e, dtype=np.uint8) for e in images]
+        if len(keep) != (1 if self.mode == MODE_REPLICATED else self.num_parts()):
+            raise ValueError("one image for a replicated handle, one per shard for a partitioned one")
+        return (keep, (C.c_void_p * len(keep))(*[a.ctypes.data for a in keep]),
+                (C.c_size_t * len(keep))(*[a.size for a in keep]))
 
     def search_batch_rerank(self, queries, num_candidates, max_search=DEFAULT_MAX_SEARCH,
                             num_elements=DEFAULT_NUM_ELEMENTS):
         """Two-stage search over all parts (granne_b200_multi_search_rerank_batch): GLOBAL uint64 ids."""
-        q = np.asarray(queries)
-        if q.dtype == np.int8:
-            raise ValueError("the two-stage search takes raw float32 queries")
-        q = np.ascontiguousarray(q, dtype=np.float32)
-        if q.ndim != 2:
-            raise ValueError("queries must have shape (nq, dim)")
+        q = _raw_f32_queries(queries)
         nq, k = q.shape[0], int(num_elements)
-        ids = np.empty((nq, k), dtype=np.uint64)
-        dists = np.empty((nq, k), dtype=np.float32)
-        counts = np.empty(nq, dtype=np.uint32)
+        ids, dists, counts, _ = _host_outputs(nq, k, np.uint64)
         _check(load_library().granne_b200_multi_search_rerank_batch(self._h, _ptr(q), nq, QUERY_RAW_F32,
                                                                     int(max_search), int(num_candidates), k,
                                                                     _ptr(ids), _ptr(dists), _ptr(counts)))
@@ -832,7 +786,8 @@ def _check_device_rows(kind, t):
 
 def elements_from_raw_device(element_type, raw, out=None, stream=None):
     """`Vector::from(Vec<f32>)` per row, device to device: raw = CUDA float32 [n, dim]; returns (or fills `out`) the
-    elements as a CUDA tensor [n, dim] (float32 normalised for "angular", int8 for "angular_int")."""
+    elements as a CUDA tensor [n, dim] (float32 normalised for "angular", int8 for "angular_int").  Asynchronous on
+    `stream` (a torch.cuda.Stream or a raw cudaStream_t; default: the current torch stream)."""
     import torch
 
     kind = _kind(element_type)
@@ -844,10 +799,9 @@ def elements_from_raw_device(element_type, raw, out=None, stream=None):
     _check_device_rows(kind, out)
     if tuple(out.shape) != (n, dim) or out.device != raw.device:
         raise ValueError("out must match raw's shape and device")
-    s = stream if stream is not None else torch.cuda.current_stream(raw.device).cuda_stream
     _check(load_library().granne_b200_elements_from_raw_device(kind, C.c_void_p(raw.data_ptr()), n, dim,
                                                                raw.device.index, C.c_void_p(out.data_ptr()),
-                                                               C.c_void_p(s)))
+                                                               C.c_void_p(_raw_stream(stream, raw.device))))
     return out
 
 
@@ -858,35 +812,47 @@ def _embeddings_kind(element_type):
     return kind
 
 
+def _compute_embeddings_into(kind, eb, mb, device, make_out):
+    """The two calls of granne_b200_compute_embeddings: the first learns the image's size, make_out(size) gives the
+    uint8 buffer (at least that long), the second fills it.  Returns the image's part of the buffer."""
+    L = load_library()
+    need = C.c_size_t()
+    _check(L.granne_b200_compute_embeddings(kind, _ptr(eb), eb.size, _ptr(mb), mb.size, device, None, 0,
+                                            C.byref(need)))
+    out = make_out(need.value)
+    _check(L.granne_b200_compute_embeddings(kind, _ptr(eb), eb.size, _ptr(mb), mb.size, device, _ptr(out), out.size,
+                                            C.byref(need)))
+    return out[:need.value]
+
+
 def compute_embeddings(element_type, elements_bytes, embeddings_bytes, out=None, device=0):
     """compute_embeddings_and_save_to_disk (src/elements/embeddings/parsing.rs:102-152) in memory: the elements file
     image of the sum of embeddings of every element of a SumEmbeddings container, made into "angular_int" vectors (the
     quantised raw sum; what the reference writes) or "angular" vectors (the normalised sum: SumEmbeddings::get, so that
     searching the rows searches the container).  Returns the image as a uint8 array, or fills `out` (a writable
     uint8 buffer of at least the image's size, e.g. an np.memmap) and returns the image's part of it."""
-    L = load_library()
     kind = _embeddings_kind(element_type)
     eb = np.frombuffer(elements_bytes, dtype=np.uint8)
     mb = np.frombuffer(embeddings_bytes, dtype=np.uint8)
-    need = C.c_size_t()
-    _check(L.granne_b200_compute_embeddings(kind, _ptr(eb), eb.size, _ptr(mb), mb.size, device, None, 0,
-                                            C.byref(need)))
-    if out is None:
-        out = np.empty(need.value, dtype=np.uint8)
-    elif (not isinstance(out, np.ndarray) or out.dtype != np.uint8 or out.ndim != 1 or not out.flags.c_contiguous
-          or not out.flags.writeable):
-        raise ValueError("out must be a writable contiguous 1-d uint8 array")
-    elif out.size < need.value:
-        raise ValueError("out holds %d bytes; the image needs %d" % (out.size, need.value))
-    _check(L.granne_b200_compute_embeddings(kind, _ptr(eb), eb.size, _ptr(mb), mb.size, device, _ptr(out), out.size,
-                                            C.byref(need)))
-    return out[:need.value]
+
+    def buffer(size):
+        if out is None:
+            return np.empty(size, dtype=np.uint8)
+        if (not isinstance(out, np.ndarray) or out.dtype != np.uint8 or out.ndim != 1 or not out.flags.c_contiguous
+                or not out.flags.writeable):
+            raise ValueError("out must be a writable contiguous 1-d uint8 array")
+        if out.size < size:
+            raise ValueError("out holds %d bytes; the image needs %d" % (out.size, size))
+        return out
+
+    return _compute_embeddings_into(kind, eb, mb, device, buffer)
 
 
 def compute_embeddings_device(element_type, elements_bytes, embeddings_bytes, out=None, device=None, stream=None):
     """The rows of compute_embeddings as a CUDA tensor [n, dim] (float32 for "angular", int8 for "angular_int"), or
     written into `out`; for Granne.from_device_elements / GranneBuilder.from_device_elements.  device: out's device,
-    else the current one.  Returns when the rows are written."""
+    else the current one.  stream: a torch.cuda.Stream or a raw cudaStream_t (default: the current torch stream).
+    Returns when the rows are written."""
     import torch
 
     L = load_library()
@@ -904,10 +870,9 @@ def compute_embeddings_device(element_type, elements_bytes, embeddings_bytes, ou
     _check_device_rows(kind, out)
     if tuple(out.shape) != (n.value, dim.value) or out.device != torch.device("cuda", device):
         raise ValueError("out must be a [%d, %d] tensor on cuda:%d" % (n.value, dim.value, device))
-    s = stream if stream is not None else torch.cuda.current_stream(out.device).cuda_stream
     _check(L.granne_b200_compute_embeddings_device(kind, _ptr(eb), eb.size, _ptr(mb), mb.size, device,
                                                    C.c_void_p(out.data_ptr()), C.byref(n), C.byref(dim),
-                                                   C.c_void_p(s)))
+                                                   C.c_void_p(_raw_stream(stream, out.device))))
     return out
 
 
@@ -916,21 +881,13 @@ def compute_embeddings_and_save_to_disk(elements_path, embeddings_path, output_p
     """granne.compute_embeddings_and_save_to_disk (py/src/lib.rs:132-147; parsing.rs:102-152) on the GPU, same
     argument order.  The image is written through a memory map of the output file.  show_progress is accepted and
     ignored."""
-    L = load_library()
     kind = _embeddings_kind(element_type)
     eb = np.memmap(elements_path, dtype=np.uint8, mode="r") if os.path.getsize(elements_path) else np.zeros(0, np.uint8)
     mb = (np.memmap(embeddings_path, dtype=np.uint8, mode="r") if os.path.getsize(embeddings_path)
           else np.zeros(0, np.uint8))
-    need = C.c_size_t()
-    _check(L.granne_b200_compute_embeddings(kind, _ptr(eb), eb.size, _ptr(mb), mb.size, device, None, 0,
-                                            C.byref(need)))
-    out = np.memmap(output_path, dtype=np.uint8, mode="w+", shape=(need.value,))
-    try:
-        _check(L.granne_b200_compute_embeddings(kind, _ptr(eb), eb.size, _ptr(mb), mb.size, device, _ptr(out),
-                                                out.size, C.byref(need)))
-        out.flush()
-    finally:
-        del out
+    image = _compute_embeddings_into(kind, eb, mb, device,
+                                     lambda size: np.memmap(output_path, dtype=np.uint8, mode="w+", shape=(size,)))
+    image.flush()
 
 
 class GranneBuilder:
@@ -1220,7 +1177,8 @@ def decode_layer(index_bytes, layer):
 
 def merge_topk_device(device, part_ids, part_dists, part_base, out_ids=None, out_dists=None, stream=None):
     """granne_b200_merge_topk_device over CUDA torch tensors: part_ids int32 [P, nq, k] (u32 bits), part_dists
-    float32 [P, nq, k], part_base list of P global id offsets.  Returns (int64 [nq,k] global ids, float32 dists)."""
+    float32 [P, nq, k], part_base list of P global id offsets.  Returns (int64 [nq,k] global ids, float32 dists).
+    Asynchronous on `stream` (a torch.cuda.Stream or a raw cudaStream_t; default: the current torch stream)."""
     import torch
 
     # the library takes raw pointers and indexes them as [P][nq][k]: anything else would be read out of bounds
@@ -1244,8 +1202,8 @@ def merge_topk_device(device, part_ids, part_dists, part_base, out_ids=None, out
     if not tensor_ok(out_ids, torch.int64, (nq, k)) or not tensor_ok(out_dists, torch.float32, (nq, k)):
         raise ValueError("out_ids (int64) and out_dists (float32) must be contiguous [nq, k] tensors on cuda:%d" % device)
     base = np.ascontiguousarray(part_base, dtype=np.uint64)
-    s = stream if stream is not None else torch.cuda.current_stream(part_ids.device).cuda_stream
     _check(load_library().granne_b200_merge_topk_device(
         device, C.c_void_p(part_ids.data_ptr()), C.c_void_p(part_dists.data_ptr()), _ptr(base), P, nq, k,
-        C.c_void_p(out_ids.data_ptr()), C.c_void_p(out_dists.data_ptr()), C.c_void_p(s)))
+        C.c_void_p(out_ids.data_ptr()), C.c_void_p(out_dists.data_ptr()),
+        C.c_void_p(_raw_stream(stream, part_ids.device))))
     return out_ids, out_dists

@@ -455,20 +455,27 @@ int embeddings_status(int* d_status) {
     return GRANNE_B200_OK;
 }
 
+// A pointer the caller says is device memory must be memory of `device`: the kernels would fault on anything else.
+int check_device_pointer(const void* p, int device, const char* what) {
+    cudaPointerAttributes at{};
+    if (cudaPointerGetAttributes(&at, p) != cudaSuccess || at.type != cudaMemoryTypeDevice || at.device != device) {
+        cudaGetLastError();  // a failed query must not stay behind as the thread's last error
+        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT,
+                    std::string(what) + " is not device memory of device " + std::to_string(device));
+    }
+    return GRANNE_B200_OK;
+}
+
 // Stages a dense element container whose rows already live in HBM (row-major elements: normalised f32 / i8).
 int stage_device_elements(Handle* h, int kind, const void* d_rows, uint64_t n, uint32_t dim) {
     if (kind != GRANNE_B200_ANGULAR && kind != GRANNE_B200_ANGULAR_INT)
         return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "device-resident elements: angular or angular_int only");
     if (!d_rows && n) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "elements pointer is null");
     if (dim == 0 || dim > 16384) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "vectors wider than 16384 are unsupported");
-    cudaPointerAttributes at{};
-    if (n && (cudaPointerGetAttributes(&at, d_rows) != cudaSuccess || at.type != cudaMemoryTypeDevice ||
-              at.device != h->device)) {
-        cudaGetLastError();
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "elements pointer is not device memory of the requested device");
-    }
+    int rc;
+    if (n && (rc = check_device_pointer(d_rows, h->device, "elements pointer"))) return rc;
     h->dev.kind = kind;
-    int rc = stage_dense(h, h->dev, static_cast<const uint8_t*>(d_rows), n, dim, true);
+    rc = stage_dense(h, h->dev, static_cast<const uint8_t*>(d_rows), n, dim, true);
     if (rc) return rc;
     h->dev.num_elements = n;
     return GRANNE_B200_OK;
@@ -556,6 +563,20 @@ int read_file(const char* path, std::vector<uint8_t>* out) {
     if (n > 0 && !f.read(reinterpret_cast<char*>(out->data()), n))
         return fail(GRANNE_B200_ERR_IO, std::string("Could not read ") + path);
     return GRANNE_B200_OK;
+}
+
+// Hands an encoded image to the caller: always its size; its bytes when there is a buffer, which must hold them.
+int copy_image_out(const std::vector<uint8_t>& image, void* out, size_t cap, size_t* out_len) {
+    *out_len = image.size();
+    if (!out) return GRANNE_B200_OK;
+    if (cap < image.size()) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "output buffer too small");
+    std::memcpy(out, image.data(), image.size());
+    return GRANNE_B200_OK;
+}
+
+// The header of a dense elements image: the rows' width as a little-endian u64 (FixedWidthSliceVector::write).
+void write_width_header(uint8_t* image, uint64_t dim) {
+    for (int b = 0; b < 8; ++b) image[b] = (uint8_t)(dim >> (8 * b));
 }
 
 // ---- launch configuration -----------------------------------------------------------------------------------------
@@ -799,17 +820,59 @@ int ws_reserve(Workspace* w, size_t query_bytes, size_t nq, size_t k) {
     return w->h_pinned.grow(query_bytes + nq * k * 8 + nq * 4 + nq * 32 + 128, s);
 }
 
-int validate_search(const Handle* h, const void* q, size_t nq, int fmt, uint32_t max_search, uint32_t k,
-                    const void* ids, const void* dists) {
+// One workspace per caller stream: calls on the same stream are serialised by the stream itself, so the status words /
+// slow-path buffers can be reused; the error word stays sticky until granne_b200_stream_status().
+int stream_workspace(Handle* h, cudaStream_t stream, Workspace** out) {
+    Workspace* w = nullptr;
+    {
+        std::lock_guard<std::mutex> g(h->pool_mu);
+        auto it = h->stream_ws.find(stream);
+        if (it != h->stream_ws.end()) w = it->second.get();
+    }
+    if (!w) {
+        std::unique_ptr<Workspace> fresh;
+        int rc;
+        if ((rc = ws_acquire(h, &fresh))) return rc;
+        cudaError_t e = cudaMemset(fresh->d_error, 0, 4 * sizeof(int));
+        {
+            std::lock_guard<std::mutex> g(h->pool_mu);
+            auto it = h->stream_ws.find(stream);  // two threads may meet here on the first use of a stream
+            if (it == h->stream_ws.end()) it = h->stream_ws.emplace(stream, std::move(fresh)).first;
+            w = it->second.get();
+        }
+        if (fresh) ws_release(h, std::move(fresh));  // lost that race: back to the pool
+        GB_CUDA(e);
+    }
+    *out = w;
+    return GRANNE_B200_OK;
+}
+
+// The argument rules every query call shares, in the order they are reported.  None of them reads the handle, so bad
+// arguments are reported before anything touches a device.  `own_rule`: the message of the call's own rule on its
+// sizes when the arguments break it, else nullptr.
+int validate_batch(const Handle* h, const void* q, size_t nq, int fmt, uint32_t k, const void* ids, const void* dists,
+                   const char* own_rule) {
     if (!h) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "index handle is null");
     if (fmt != GRANNE_B200_QUERY_RAW_F32 && fmt != GRANNE_B200_QUERY_ELEMENT)
         return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "unknown query format");
-    if (max_search == 0)
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT,
-                    "max_search must be >= 1 (the reference panics on 0, src/index/mod.rs:1019)");
+    if (own_rule) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, own_rule);
     if (nq > 0xFFFFFFF0ull) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "too many queries in one batch");
     if (nq && (!q || (k && (!ids || !dists)))) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null buffer");
     return GRANNE_B200_OK;
+}
+
+int validate_search(const Handle* h, const void* q, size_t nq, int fmt, uint32_t max_search, uint32_t k,
+                    const void* ids, const void* dists) {
+    return validate_batch(h, q, nq, fmt, k, ids, dists,
+                          max_search == 0 ? "max_search must be >= 1 (the reference panics on 0, src/index/mod.rs:1019)"
+                                          : nullptr);
+}
+
+int validate_exact(const Handle* h, const void* q, size_t nq, int fmt, uint32_t k, const void* ids,
+                   const void* dists) {
+    return validate_batch(h, q, nq, fmt, k, ids, dists,
+                          k > GRANNE_B200_EXACT_MAX_K ? "num_neighbors exceeds GRANNE_B200_EXACT_MAX_K (1024)"
+                                                      : nullptr);
 }
 
 gb::PeerGather device_gather(const granne_b200_peer_gather& pg, unsigned int* done_counter) {
@@ -901,24 +964,80 @@ int error_from_bits(int bits) {
     return GRANNE_B200_OK;
 }
 
+// Bytes of nq queries in `fmt`: i8 rows when they already are elements of an angular_int index, f32 rows otherwise.
+size_t query_bytes(const Handle* h, size_t nq, int fmt) {
+    const bool i8q = h->dev.kind == gb::kAngularI8 && fmt == GRANNE_B200_QUERY_ELEMENT;
+    return nq * h->dev.dim * (i8q ? 1 : 4);
+}
+
+// The host-pointer form of a query call (arguments validated, nq > 0), on a pooled workspace and its stream: the
+// queries go up through pinned memory, `enqueue(w, stream, d_stats)` queues the call's kernels from w->d_queries into
+// the workspace's result block (w->d_ids | w->d_dists | w->d_counts; d_stats is null when the caller wants no stats),
+// and one synchronise brings the results and the error word back.  A host call reports its own errors only, so the
+// error word starts the call at zero: enqueue_search zeroes it with its counters (reset_error); an `enqueue` without
+// that memset clears the word itself.
+template <class Enqueue>
+int host_batch(Handle* h, const void* queries, size_t qbytes, size_t nq, size_t k, uint32_t* out_ids,
+               float* out_dists, uint32_t* out_counts, uint64_t* out_stats, Enqueue&& enqueue) {
+    return guarded([&] {
+        GB_DEVICE(h->device);
+        std::unique_ptr<Workspace> ws;
+        int rc = ws_acquire(h, &ws);
+        if (rc) return rc;
+        Workspace* w = ws.get();
+        const int status = [&] {
+            if ((rc = ws_reserve(w, qbytes, nq, k))) return rc;
+            cudaStream_t stream = w->stream.get();
+            // pinned staging layout: queries | ids | dists | counts | error | stats, the blocks behind the queries and
+            // behind the error word on 16-byte boundaries (ws_reserve sizes the buffer with slack for both)
+            uint8_t* hp = w->h_pinned.get();
+            uint32_t* hids = reinterpret_cast<uint32_t*>(hp + ((qbytes + 15) & ~size_t(15)));
+            float* hd = reinterpret_cast<float*>(hids + nq * k);
+            uint32_t* hc = reinterpret_cast<uint32_t*>(hd + nq * k);
+            int* herr = reinterpret_cast<int*>(hc + nq);
+            unsigned long long* hstats = reinterpret_cast<unsigned long long*>(
+                hp + ((reinterpret_cast<uint8_t*>(herr + 4) - hp + 15) & ~size_t(15)));
+            std::memcpy(hp, queries, qbytes);
+            GB_CUDA(cudaMemcpyAsync(w->d_queries.get(), hp, qbytes, cudaMemcpyHostToDevice, stream));
+            if ((rc = enqueue(w, stream, out_stats ? w->d_stats.get() : nullptr))) return rc;
+            // one packed copy: ids | dists | counts (device and pinned layouts match), then the 16-byte error word
+            GB_CUDA(cudaMemcpyAsync(hids, w->d_ids.get(), (2 * nq * k + nq) * 4, cudaMemcpyDeviceToHost, stream));
+            GB_CUDA(cudaMemcpyAsync(herr, w->d_error, 4 * sizeof(int), cudaMemcpyDeviceToHost, stream));
+            if (out_stats) GB_CUDA(cudaMemcpyAsync(hstats, w->d_stats.get(), nq * 32, cudaMemcpyDeviceToHost, stream));
+            GB_CUDA(cudaStreamSynchronize(stream));
+            if (out_stats) std::memcpy(out_stats, hstats, nq * 32);
+            if (k) {
+                std::memcpy(out_ids, hids, nq * k * 4);
+                std::memcpy(out_dists, hd, nq * k * 4);
+            }
+            if (out_counts) std::memcpy(out_counts, hc, nq * 4);
+            return error_from_bits(herr[0]);
+        }();
+        ws_release(h, std::move(ws));  // back to the pool on every path
+        return status;
+    });
+}
+
+// The device-pointer form of a query call (arguments validated, nq > 0): `enqueue(w, stream)` queues the call's
+// kernels on the caller's stream with that stream's workspace.  Asynchronous; errors stay in the workspace's error
+// word until granne_b200_stream_status().
+template <class Enqueue>
+int device_batch(Handle* h, void* cuda_stream, Enqueue&& enqueue) {
+    return guarded([&] {
+        GB_DEVICE(h->device);
+        cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+        Workspace* w = nullptr;
+        int rc = stream_workspace(h, stream, &w);
+        if (rc) return rc;
+        return enqueue(w, stream);
+    });
+}
+
 // ---- exact k-NN (exact_kernels.cuh) -------------------------------------------------------------------------------
 // The slab buffer holds at most kExactSlabFloats distances (256 MB) and a slab at most kExactMaxSlabRows rows, so the
 // workspace of a call is bounded whatever nq and n are.
 constexpr uint64_t kExactSlabFloats = 64ull << 20;
 constexpr uint64_t kExactMaxSlabRows = 1ull << 20;
-
-// validate_search's rules without max_search, plus the bound on k.
-int validate_exact(const Handle* h, const void* q, size_t nq, int fmt, uint32_t k, const void* ids,
-                   const void* dists) {
-    if (!h) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "index handle is null");
-    if (fmt != GRANNE_B200_QUERY_RAW_F32 && fmt != GRANNE_B200_QUERY_ELEMENT)
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "unknown query format");
-    if (k > GRANNE_B200_EXACT_MAX_K)
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "num_neighbors exceeds GRANNE_B200_EXACT_MAX_K (1024)");
-    if (nq > 0xFFFFFFF0ull) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "too many queries in one batch");
-    if (nq && (!q || (k && (!ids || !dists)))) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null buffer");
-    return GRANNE_B200_OK;
-}
 
 // Distances of the prepared query chunk (qc queries in w->d_exact_q) to `nrows` rows, slab by slab, each slab's keys
 // merged into the running lists.  Row r has id base + r.
@@ -1541,33 +1660,6 @@ int granne_b200_get_element(const granne_b200_index* hc, uint64_t idx, void* out
     });
 }
 
-// One workspace per caller stream: calls on the same stream are serialised by the stream itself, so the status words /
-// slow-path buffers can be reused; the error word stays sticky until granne_b200_stream_status().
-static int stream_workspace(granne_b200_index* h, cudaStream_t stream, Workspace** out) {
-    Workspace* w = nullptr;
-    {
-        std::lock_guard<std::mutex> g(h->pool_mu);
-        auto it = h->stream_ws.find(stream);
-        if (it != h->stream_ws.end()) w = it->second.get();
-    }
-    if (!w) {
-        std::unique_ptr<Workspace> fresh;
-        int rc;
-        if ((rc = ws_acquire(h, &fresh))) return rc;
-        cudaError_t e = cudaMemset(fresh->d_error, 0, 4 * sizeof(int));
-        {
-            std::lock_guard<std::mutex> g(h->pool_mu);
-            auto it = h->stream_ws.find(stream);  // two threads may meet here on the first use of a stream
-            if (it == h->stream_ws.end()) it = h->stream_ws.emplace(stream, std::move(fresh)).first;
-            w = it->second.get();
-        }
-        if (fresh) ws_release(h, std::move(fresh));  // lost that race: back to the pool
-        GB_CUDA(e);
-    }
-    *out = w;
-    return GRANNE_B200_OK;
-}
-
 static int search_device_impl(granne_b200_index* h, const void* d_queries, size_t nq, int query_format,
                               uint32_t max_search, uint32_t num_neighbors, uint32_t* d_out_ids, float* d_out_dists,
                               uint32_t* d_out_counts, uint64_t* d_out_stats, void* cuda_stream,
@@ -1583,17 +1675,15 @@ static int search_device_impl(granne_b200_index* h, const void* d_queries, size_
                 return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "peer gather: null peer pointer");
     }
     if (nq == 0 && !pg) return GRANNE_B200_OK;
-    return guarded([&] {
-        GB_DEVICE(h->device);
-        cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
-        if (nq == 0) {  // nothing to store, but the peers wait for this call's sequence number all the same
-            gb::publish_seq_kernel<<<1, 1, 0, stream>>>(device_gather(*pg, nullptr));
+    if (nq == 0)  // nothing to store, but the peers wait for this call's sequence number all the same
+        return guarded([&] {
+            GB_DEVICE(h->device);
+            gb::publish_seq_kernel<<<1, 1, 0, static_cast<cudaStream_t>(cuda_stream)>>>(device_gather(*pg, nullptr));
             h->launches++;
             GB_CUDA(cudaGetLastError());
             return GRANNE_B200_OK;
-        }
-        Workspace* w = nullptr;
-        if ((rc = stream_workspace(h, stream, &w))) return rc;
+        });
+    return device_batch(h, cuda_stream, [&](Workspace* w, cudaStream_t stream) {
         return enqueue_search(h, w, d_queries, nq, query_format, max_search, num_neighbors, d_out_ids, d_out_dists,
                               d_out_counts, reinterpret_cast<unsigned long long*>(d_out_stats), stream, false, pg);
     });
@@ -1663,48 +1753,11 @@ int granne_b200_search_batch(granne_b200_index* h, const void* queries, size_t n
     int rc = validate_search(h, queries, nq, query_format, max_search, num_neighbors, out_ids, out_dists);
     if (rc) return rc;
     if (nq == 0) return GRANNE_B200_OK;
-    return guarded([&] {
-        GB_DEVICE(h->device);
-        const size_t k = num_neighbors;
-        const bool i8q = h->dev.kind == gb::kAngularI8 && query_format == GRANNE_B200_QUERY_ELEMENT;
-        const size_t qbytes = nq * h->dev.dim * (i8q ? 1 : 4);
-        std::unique_ptr<Workspace> ws;
-        if ((rc = ws_acquire(h, &ws))) return rc;
-        Workspace* w = ws.get();
-        const int status = [&] {
-            if ((rc = ws_reserve(w, qbytes, nq, k))) return rc;
-            cudaStream_t stream = w->stream.get();
-            // pinned staging layout: queries | ids | dists | counts | stats | error
-            uint8_t* hp = w->h_pinned.get();
-            uint8_t* hq = hp;
-            uint32_t* hids = reinterpret_cast<uint32_t*>(hp + ((qbytes + 15) & ~size_t(15)));
-            float* hd = reinterpret_cast<float*>(hids + nq * k);
-            uint32_t* hc = reinterpret_cast<uint32_t*>(hd + nq * k);
-            int* herr = reinterpret_cast<int*>(hc + nq);
-            unsigned long long* hstats = reinterpret_cast<unsigned long long*>(
-                reinterpret_cast<uint8_t*>(hp) + ((reinterpret_cast<uint8_t*>(herr + 4) - hp + 15) & ~size_t(15)));
-            // (the pinned buffer was sized with slack for the alignment above)
-            std::memcpy(hq, queries, qbytes);
-            GB_CUDA(cudaMemcpyAsync(w->d_queries.get(), hq, qbytes, cudaMemcpyHostToDevice, stream));
-            rc = enqueue_search(h, w, w->d_queries.get(), nq, query_format, max_search, num_neighbors, w->d_ids.get(),
-                                w->d_dists, w->d_counts, out_stats ? w->d_stats.get() : nullptr, stream, true);
-            if (rc) return rc;
-            // one packed copy: ids | dists | counts (device and pinned layouts match), then the 16-byte error word
-            GB_CUDA(cudaMemcpyAsync(hids, w->d_ids.get(), (2 * nq * k + nq) * 4, cudaMemcpyDeviceToHost, stream));
-            GB_CUDA(cudaMemcpyAsync(herr, w->d_error, 4 * sizeof(int), cudaMemcpyDeviceToHost, stream));
-            if (out_stats) GB_CUDA(cudaMemcpyAsync(hstats, w->d_stats.get(), nq * 32, cudaMemcpyDeviceToHost, stream));
-            GB_CUDA(cudaStreamSynchronize(stream));
-            if (out_stats) std::memcpy(out_stats, hstats, nq * 32);
-            if (k) {
-                std::memcpy(out_ids, hids, nq * k * 4);
-                std::memcpy(out_dists, hd, nq * k * 4);
-            }
-            if (out_counts) std::memcpy(out_counts, hc, nq * 4);
-            return error_from_bits(herr[0]);
-        }();
-        ws_release(h, std::move(ws));  // back to the pool on every path
-        return status;
-    });
+    return host_batch(h, queries, query_bytes(h, nq, query_format), nq, num_neighbors, out_ids, out_dists, out_counts,
+                      out_stats, [&](Workspace* w, cudaStream_t stream, unsigned long long* d_stats) {
+                          return enqueue_search(h, w, w->d_queries.get(), nq, query_format, max_search, num_neighbors,
+                                                w->d_ids.get(), w->d_dists, w->d_counts, d_stats, stream, true);
+                      });
 }
 
 int granne_b200_exact_search_batch(granne_b200_index* h, const void* queries, size_t nq, int query_format,
@@ -1712,42 +1765,13 @@ int granne_b200_exact_search_batch(granne_b200_index* h, const void* queries, si
     int rc = validate_exact(h, queries, nq, query_format, num_neighbors, out_ids, out_dists);
     if (rc) return rc;
     if (nq == 0) return GRANNE_B200_OK;
-    return guarded([&] {
-        GB_DEVICE(h->device);
-        const size_t k = num_neighbors;
-        const bool i8q = h->dev.kind == gb::kAngularI8 && query_format == GRANNE_B200_QUERY_ELEMENT;
-        const size_t qbytes = nq * h->dev.dim * (i8q ? 1 : 4);
-        std::unique_ptr<Workspace> ws;
-        if ((rc = ws_acquire(h, &ws))) return rc;
-        Workspace* w = ws.get();
-        const int status = [&] {
-            if ((rc = ws_reserve(w, qbytes, nq, k))) return rc;
-            cudaStream_t stream = w->stream.get();
-            // pinned staging layout: queries | ids | dists | counts | error
-            uint8_t* hp = w->h_pinned.get();
-            uint32_t* hids = reinterpret_cast<uint32_t*>(hp + ((qbytes + 15) & ~size_t(15)));
-            float* hd = reinterpret_cast<float*>(hids + nq * k);
-            uint32_t* hc = reinterpret_cast<uint32_t*>(hd + nq * k);
-            int* herr = reinterpret_cast<int*>(hc + nq);
-            std::memcpy(hp, queries, qbytes);
-            GB_CUDA(cudaMemcpyAsync(w->d_queries.get(), hp, qbytes, cudaMemcpyHostToDevice, stream));
-            GB_CUDA(cudaMemsetAsync(w->d_error, 0, 4 * sizeof(int), stream));
-            rc = enqueue_exact(h, w, w->d_queries.get(), nq, query_format, num_neighbors, w->d_ids.get(), w->d_dists,
-                               w->d_counts, stream);
-            if (rc) return rc;
-            GB_CUDA(cudaMemcpyAsync(hids, w->d_ids.get(), (2 * nq * k + nq) * 4, cudaMemcpyDeviceToHost, stream));
-            GB_CUDA(cudaMemcpyAsync(herr, w->d_error, 4 * sizeof(int), cudaMemcpyDeviceToHost, stream));
-            GB_CUDA(cudaStreamSynchronize(stream));
-            if (k) {
-                std::memcpy(out_ids, hids, nq * k * 4);
-                std::memcpy(out_dists, hd, nq * k * 4);
-            }
-            if (out_counts) std::memcpy(out_counts, hc, nq * 4);
-            return error_from_bits(herr[0]);
-        }();
-        ws_release(h, std::move(ws));  // back to the pool on every path
-        return status;
-    });
+    return host_batch(h, queries, query_bytes(h, nq, query_format), nq, num_neighbors, out_ids, out_dists, out_counts,
+                      nullptr, [&](Workspace* w, cudaStream_t stream, unsigned long long*) {
+                          // enqueue_exact has no memset that zeroes the error word (host_batch)
+                          GB_CUDA(cudaMemsetAsync(w->d_error, 0, 4 * sizeof(int), stream));
+                          return enqueue_exact(h, w, w->d_queries.get(), nq, query_format, num_neighbors,
+                                               w->d_ids.get(), w->d_dists, w->d_counts, stream);
+                      });
 }
 
 int granne_b200_exact_search_batch_device(granne_b200_index* h, const void* d_queries, size_t nq, int query_format,
@@ -1756,11 +1780,7 @@ int granne_b200_exact_search_batch_device(granne_b200_index* h, const void* d_qu
     int rc = validate_exact(h, d_queries, nq, query_format, num_neighbors, d_out_ids, d_out_dists);
     if (rc) return rc;
     if (nq == 0) return GRANNE_B200_OK;
-    return guarded([&] {
-        GB_DEVICE(h->device);
-        cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
-        Workspace* w = nullptr;
-        if ((rc = stream_workspace(h, stream, &w))) return rc;
+    return device_batch(h, cuda_stream, [&](Workspace* w, cudaStream_t stream) {
         return enqueue_exact(h, w, d_queries, nq, query_format, num_neighbors, d_out_ids, d_out_dists, d_out_counts,
                              stream);
     });
@@ -1788,12 +1808,7 @@ int granne_b200_set_rerank_elements_device(granne_b200_index* h, const float* d_
     if ((rc = check_rerank_shape(h, n, dim))) return rc;
     return guarded([&] {
         GB_DEVICE(h->device);
-        cudaPointerAttributes at{};
-        if (n && (cudaPointerGetAttributes(&at, d_rows) != cudaSuccess || at.type != cudaMemoryTypeDevice ||
-                  at.device != h->device)) {
-            cudaGetLastError();
-            return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "elements pointer is not device memory of the index's device");
-        }
+        if (n && (rc = check_device_pointer(d_rows, h->device, "elements pointer"))) return rc;
         return stage_rerank_rows(h, reinterpret_cast<const uint8_t*>(d_rows), n, dim, true);
     });
 }
@@ -1819,45 +1834,12 @@ int granne_b200_search_rerank_batch(granne_b200_index* h, const float* queries, 
                              out_dists);
     if (rc) return rc;
     if (nq == 0) return GRANNE_B200_OK;
-    return guarded([&] {
-        GB_DEVICE(h->device);
-        const size_t k = num_neighbors;
-        const size_t qbytes = nq * h->dev.dim * 4;
-        std::unique_ptr<Workspace> ws;
-        if ((rc = ws_acquire(h, &ws))) return rc;
-        Workspace* w = ws.get();
-        const int status = [&] {
-            if ((rc = ws_reserve(w, qbytes, nq, k))) return rc;
-            cudaStream_t stream = w->stream.get();
-            // pinned staging layout as in granne_b200_search_batch: queries | ids | dists | counts | error | stats
-            uint8_t* hp = w->h_pinned.get();
-            uint32_t* hids = reinterpret_cast<uint32_t*>(hp + ((qbytes + 15) & ~size_t(15)));
-            float* hd = reinterpret_cast<float*>(hids + nq * k);
-            uint32_t* hc = reinterpret_cast<uint32_t*>(hd + nq * k);
-            int* herr = reinterpret_cast<int*>(hc + nq);
-            unsigned long long* hstats = reinterpret_cast<unsigned long long*>(
-                hp + ((reinterpret_cast<uint8_t*>(herr + 4) - hp + 15) & ~size_t(15)));
-            std::memcpy(hp, queries, qbytes);
-            GB_CUDA(cudaMemcpyAsync(w->d_queries.get(), hp, qbytes, cudaMemcpyHostToDevice, stream));
-            rc = enqueue_rerank(h, w, w->d_queries.get(), nq, max_search, num_candidates, num_neighbors,
-                                w->d_ids.get(), w->d_dists, w->d_counts, out_stats ? w->d_stats.get() : nullptr,
-                                stream, true);
-            if (rc) return rc;
-            GB_CUDA(cudaMemcpyAsync(hids, w->d_ids.get(), (2 * nq * k + nq) * 4, cudaMemcpyDeviceToHost, stream));
-            GB_CUDA(cudaMemcpyAsync(herr, w->d_error, 4 * sizeof(int), cudaMemcpyDeviceToHost, stream));
-            if (out_stats) GB_CUDA(cudaMemcpyAsync(hstats, w->d_stats.get(), nq * 32, cudaMemcpyDeviceToHost, stream));
-            GB_CUDA(cudaStreamSynchronize(stream));
-            if (out_stats) std::memcpy(out_stats, hstats, nq * 32);
-            if (k) {
-                std::memcpy(out_ids, hids, nq * k * 4);
-                std::memcpy(out_dists, hd, nq * k * 4);
-            }
-            if (out_counts) std::memcpy(out_counts, hc, nq * 4);
-            return error_from_bits(herr[0]);
-        }();
-        ws_release(h, std::move(ws));  // back to the pool on every path
-        return status;
-    });
+    return host_batch(h, queries, query_bytes(h, nq, query_format), nq, num_neighbors, out_ids, out_dists, out_counts,
+                      out_stats, [&](Workspace* w, cudaStream_t stream, unsigned long long* d_stats) {
+                          return enqueue_rerank(h, w, w->d_queries.get(), nq, max_search, num_candidates,
+                                                num_neighbors, w->d_ids.get(), w->d_dists, w->d_counts, d_stats,
+                                                stream, true);
+                      });
 }
 
 int granne_b200_search_rerank_batch_device(granne_b200_index* h, const float* d_queries, size_t nq, int query_format,
@@ -1868,11 +1850,7 @@ int granne_b200_search_rerank_batch_device(granne_b200_index* h, const float* d_
                              d_out_dists);
     if (rc) return rc;
     if (nq == 0) return GRANNE_B200_OK;
-    return guarded([&] {
-        GB_DEVICE(h->device);
-        cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
-        Workspace* w = nullptr;
-        if ((rc = stream_workspace(h, stream, &w))) return rc;
+    return device_batch(h, cuda_stream, [&](Workspace* w, cudaStream_t stream) {
         return enqueue_rerank(h, w, d_queries, nq, max_search, num_candidates, num_neighbors, d_out_ids, d_out_dists,
                               d_out_counts, reinterpret_cast<unsigned long long*>(d_out_stats), stream, false);
     });
@@ -2108,11 +2086,7 @@ int granne_b200_write_index(const granne_b200_index* h, void* out, size_t cap, s
         std::vector<uint8_t> image;
         std::string err;
         if (!gb::encode_index(views, &image, &err)) return fail(GRANNE_B200_ERR_FORMAT, err);
-        *out_len = image.size();
-        if (!out) return GRANNE_B200_OK;
-        if (cap < image.size()) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "output buffer too small");
-        std::memcpy(out, image.data(), image.size());
-        return GRANNE_B200_OK;
+        return copy_image_out(image, out, cap, out_len);
     });
 }
 
@@ -2166,7 +2140,7 @@ int granne_b200_elements_from_raw(int element_kind, const float* raw, uint64_t n
     if (rc) return rc;
     GB_DEVICE(device);
     uint8_t* o = static_cast<uint8_t*>(out);
-    for (int b8 = 0; b8 < 8; ++b8) o[b8] = (uint8_t)((uint64_t)dim >> (8 * b8));
+    write_width_header(o, dim);
     const uint64_t slab = std::max<uint64_t>(1, (256ull << 20) / ((size_t)dim * 4));
     const uint64_t rows_alloc = std::min<uint64_t>(slab, std::max<uint64_t>(n, 1));
     Buffer<float> d_raw;
@@ -2226,7 +2200,7 @@ int granne_b200_compute_embeddings(int element_kind, const void* elements_bytes,
         if ((rc = check_device(device, &sms, &optin))) return rc;
         GB_DEVICE(device);
         uint8_t* o = static_cast<uint8_t*>(out);
-        for (int b = 0; b < 8; ++b) o[b] = (uint8_t)((uint64_t)in.dim >> (8 * b));  // FixedWidthSliceVector::write
+        write_width_header(o, in.dim);
         if (in.dim == 0) return GRANNE_B200_OK;
 
         const uint64_t* off = in.el.offsets.data();
@@ -2309,12 +2283,7 @@ int granne_b200_compute_embeddings_device(int element_kind, const void* elements
         if ((rc = check_device(device, &sms, &optin))) return rc;
         GB_DEVICE(device);
         if (in.dim == 0) return GRANNE_B200_OK;
-        cudaPointerAttributes at{};
-        if (cudaPointerGetAttributes(&at, d_out) != cudaSuccess || at.type != cudaMemoryTypeDevice ||
-            at.device != device) {
-            cudaGetLastError();
-            return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "d_out is not device memory of the requested device");
-        }
+        if ((rc = check_device_pointer(d_out, device, "d_out"))) return rc;
         const cudaStream_t s = static_cast<cudaStream_t>(cuda_stream);
         const uint64_t rows = std::min(in.n, emb_window_rows(in.dim));
         Buffer<float> d_table, d_raw;
@@ -2405,11 +2374,7 @@ int granne_b200_reencode_index(const void* index_bytes, size_t index_len, void* 
         for (const gb::HostLayer& L : graph.layers) views.push_back({L.rows.data(), L.num_nodes, L.width});
         std::vector<uint8_t> image;
         if (!gb::encode_index(views, &image, &err)) return fail(GRANNE_B200_ERR_FORMAT, err);
-        *out_len = image.size();
-        if (!out) return GRANNE_B200_OK;
-        if (cap < image.size()) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "output buffer too small");
-        std::memcpy(out, image.data(), image.size());
-        return GRANNE_B200_OK;
+        return copy_image_out(image, out, cap, out_len);
     });
 }
 

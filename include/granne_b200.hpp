@@ -54,6 +54,32 @@ inline std::vector<uint8_t> read_file(const std::string& path) {
     return std::vector<uint8_t>(std::istreambuf_iterator<char>(f), std::istreambuf_iterator<char>());
 }
 
+namespace detail {
+
+// The bytes of a C ABI call that reports the size of what it writes and writes only into a buffer it is given:
+// `call(out, cap, &len)` once without a buffer for the size, once with one of that size.
+template <class Call>
+std::vector<uint8_t> sized_bytes(Call&& call) {
+    size_t need = 0;
+    check(call(nullptr, 0, &need));
+    std::vector<uint8_t> out(need);
+    check(call(out.data(), out.size(), &need));
+    out.resize(need);
+    return out;
+}
+
+// One result list per query from the C ABI's (ids, dists, counts) with k slots per query: its first counts[q] pairs.
+template <class Result, class Id>
+std::vector<Result> result_lists(const std::vector<Id>& ids, const std::vector<float>& dists,
+                                 const std::vector<uint32_t>& counts, size_t k) {
+    std::vector<Result> out(counts.size());
+    for (size_t q = 0; q < counts.size(); ++q)
+        for (uint32_t j = 0; j < counts[q]; ++j) out[q].emplace_back(ids[q * k + j], dists[q * k + j]);
+    return out;
+}
+
+}  // namespace detail
+
 // An element container as the file image granne writes (`ElementContainer` + `io::Writeable`): u64 width + rows for
 // the vector types; offsets + 3-byte ids (and the embeddings table) for SumEmbeddings.
 struct Elements {
@@ -65,10 +91,9 @@ struct Elements {
     static Elements from_raw(ElementKind kind, const float* rows, uint64_t n, uint32_t dim, int device = 0) {
         Elements e;
         e.kind = kind;
-        size_t need = 0;
-        check(granne_b200_elements_from_raw(static_cast<int>(kind), nullptr, n, dim, device, nullptr, 0, &need));
-        e.bytes.resize(need);
-        check(granne_b200_elements_from_raw(static_cast<int>(kind), rows, n, dim, device, e.bytes.data(), need, &need));
+        e.bytes = detail::sized_bytes([&](void* out, size_t cap, size_t* len) {
+            return granne_b200_elements_from_raw(static_cast<int>(kind), rows, n, dim, device, out, cap, len);
+        });
         return e;
     }
     // compute_embeddings_and_save_to_disk (src/elements/embeddings/parsing.rs:102-152): the sum of embeddings of every
@@ -77,13 +102,10 @@ struct Elements {
     static Elements compute_embeddings(ElementKind kind, const Elements& sum, int device = 0) {
         Elements e;
         e.kind = kind;
-        size_t need = 0;
-        check(granne_b200_compute_embeddings(static_cast<int>(kind), sum.bytes.data(), sum.bytes.size(),
-                                             sum.embeddings.data(), sum.embeddings.size(), device, nullptr, 0, &need));
-        e.bytes.resize(need);
-        check(granne_b200_compute_embeddings(static_cast<int>(kind), sum.bytes.data(), sum.bytes.size(),
-                                             sum.embeddings.data(), sum.embeddings.size(), device, e.bytes.data(),
-                                             need, &need));
+        e.bytes = detail::sized_bytes([&](void* out, size_t cap, size_t* len) {
+            return granne_b200_compute_embeddings(static_cast<int>(kind), sum.bytes.data(), sum.bytes.size(),
+                                                  sum.embeddings.data(), sum.embeddings.size(), device, out, cap, len);
+        });
         return e;
     }
     // Vectors::from_file / SumEmbeddings::from_files
@@ -155,12 +177,8 @@ public:
         return std::vector<size_t>(buf, buf + n);
     }
     std::vector<uint8_t> write_index() const {  // Index::write_index (io.rs:11-70)
-        size_t need = 0;
-        check(granne_b200_write_index(h_, nullptr, 0, &need));
-        std::vector<uint8_t> out(need);
-        check(granne_b200_write_index(h_, out.data(), out.size(), &need));
-        out.resize(need);
-        return out;
+        return detail::sized_bytes(
+            [&](void* out, size_t cap, size_t* len) { return granne_b200_write_index(h_, out, cap, len); });
     }
 
     // ElementContainer
@@ -200,11 +218,7 @@ public:
         check(granne_b200_search_batch(h_, queries, nq, query_format, static_cast<uint32_t>(max_search),
                                        static_cast<uint32_t>(num_neighbors), ids.data(), dists.data(), counts.data(),
                                        nullptr));
-        std::vector<SearchResult> out(nq);
-        for (size_t q = 0; q < nq; ++q)
-            for (uint32_t j = 0; j < counts[q]; ++j)
-                out[q].emplace_back(ids[q * num_neighbors + j], dists[q * num_neighbors + j]);
-        return out;
+        return detail::result_lists<SearchResult>(ids, dists, counts, num_neighbors);
     }
     // Exact k nearest neighbours (granne_b200_exact_search_batch): the first min(k, len()) elements by (distance, id),
     // the reference's distance bit for bit.  Not a reference function: the ground truth of recall.
@@ -214,11 +228,7 @@ public:
         std::vector<float> dists(nq * num_neighbors);
         check(granne_b200_exact_search_batch(h_, queries, nq, query_format, static_cast<uint32_t>(num_neighbors),
                                              ids.data(), dists.data(), counts.data()));
-        std::vector<SearchResult> out(nq);
-        for (size_t q = 0; q < nq; ++q)
-            for (uint32_t j = 0; j < counts[q]; ++j)
-                out[q].emplace_back(ids[q * num_neighbors + j], dists[q * num_neighbors + j]);
-        return out;
+        return detail::result_lists<SearchResult>(ids, dists, counts, num_neighbors);
     }
 
     // Two-stage search (granne_b200_search_rerank_batch): attach the container of this angular_int index's elements
@@ -243,11 +253,7 @@ public:
                                               static_cast<uint32_t>(max_search), static_cast<uint32_t>(num_candidates),
                                               static_cast<uint32_t>(num_neighbors), ids.data(), dists.data(),
                                               counts.data(), nullptr));
-        std::vector<SearchResult> out(nq);
-        for (size_t q = 0; q < nq; ++q)
-            for (uint32_t j = 0; j < counts[q]; ++j)
-                out[q].emplace_back(ids[q * num_neighbors + j], dists[q * num_neighbors + j]);
-        return out;
+        return detail::result_lists<SearchResult>(ids, dists, counts, num_neighbors);
     }
 
     // Granne::reorder (reorder.rs:59-82) / reorder_by_keys (:89-124): reorders index and elements, returns the order
@@ -363,10 +369,7 @@ public:
         check(granne_b200_multi_search_batch(h_, queries.data(), nq, GRANNE_B200_QUERY_RAW_F32,
                                              static_cast<uint32_t>(max_search), static_cast<uint32_t>(num_neighbors),
                                              ids.data(), d.data(), c.data()));
-        std::vector<Result> out(nq);
-        for (size_t i = 0; i < nq; ++i)
-            for (uint32_t j = 0; j < c[i]; ++j) out[i].emplace_back(ids[i * num_neighbors + j], d[i * num_neighbors + j]);
-        return out;
+        return detail::result_lists<Result>(ids, d, c, num_neighbors);
     }
     // exact k nearest neighbours over every shard for nq raw f32 queries (granne_b200_multi_exact_search_batch)
     std::vector<Result> exact_search_batch_raw(const std::vector<float>& queries, size_t num_neighbors) const {
@@ -377,10 +380,7 @@ public:
         check(granne_b200_multi_exact_search_batch(h_, queries.data(), nq, GRANNE_B200_QUERY_RAW_F32,
                                                    static_cast<uint32_t>(num_neighbors), ids.data(), d.data(),
                                                    c.data()));
-        std::vector<Result> out(nq);
-        for (size_t i = 0; i < nq; ++i)
-            for (uint32_t j = 0; j < c[i]; ++j) out[i].emplace_back(ids[i * num_neighbors + j], d[i * num_neighbors + j]);
-        return out;
+        return detail::result_lists<Result>(ids, d, c, num_neighbors);
     }
 
 private:
@@ -464,12 +464,8 @@ public:
         return std::vector<size_t>(buf, buf + n);
     }
     std::vector<uint8_t> write_index() const {  // Index::write_index (:358-361)
-        size_t need = 0;
-        check(granne_b200_builder_write_index(b_, nullptr, 0, &need));
-        std::vector<uint8_t> out(need);
-        check(granne_b200_builder_write_index(b_, out.data(), out.size(), &need));
-        out.resize(need);
-        return out;
+        return detail::sized_bytes(
+            [&](void* out, size_t cap, size_t* len) { return granne_b200_builder_write_index(b_, out, cap, len); });
     }
     const Elements& get_elements() const { return elements_; }
     Granne get_index() const {  // GranneBuilder::get_index (:483-488): a searchable snapshot
