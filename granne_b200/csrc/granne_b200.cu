@@ -157,6 +157,16 @@ struct Workspace {
     Buffer<uint32_t> d_rerank;
 };
 
+// The owners of the arrays a DeviceIndex points to, one slot per pointer: the memory and the bytes allocated for it.
+// A copy shares the memory (get_index snapshots), which is freed once no slot holds it.
+struct Staged {
+    struct Slot {
+        std::shared_ptr<void> mem;
+        uint64_t bytes = 0;
+    };
+    Slot vectors, sum_offsets, sum_terms, layer_rows[gb::kMaxLayers];
+};
+
 }  // namespace
 
 struct granne_b200_index {
@@ -164,19 +174,18 @@ struct granne_b200_index {
     int num_sms = 0;
     size_t smem_optin = 0;
     gb::DeviceIndex dev{};
+    Staged dev_mem;
     // the container that re-ranks the candidates of an angular_int index: angular f32 rows
     // (granne_b200_set_rerank_elements*) or a SumEmbeddings container (granne_b200_set_rerank_embeddings);
-    // vectors == nullptr until one is attached.  rerank_bytes: its share of device_bytes.
+    // vectors == nullptr until one is attached
     gb::DeviceIndex rerank{};
-    uint64_t rerank_bytes = 0;
-    std::vector<std::shared_ptr<void>> allocations;  // device memory (shared with builder snapshots)
-    uint64_t device_bytes = 0;
+    Staged rerank_mem;
     uint64_t index_len = 0;  // Index::len
     std::vector<uint32_t> layer_max_degree;
     std::atomic<uint64_t> launches{0};
     std::atomic<int> sticky_error{0};
     std::mutex pool_mu;
-    std::mutex rerank_mu;  // serialises the attaches of re-rank containers (granne_b200_set_rerank_*)
+    mutable std::mutex rerank_mu;  // serialises the re-rank attaches (granne_b200_set_rerank_*) and device_bytes
     std::vector<std::unique_ptr<Workspace>> pool;                     // host-pointer API: one per concurrent call
     std::map<cudaStream_t, std::unique_ptr<Workspace>> stream_ws;     // device-pointer API: one per caller stream
     // fast-pass visited tables are sized max_search x degree x vis_scale; the scale doubles (up to 8) when more than
@@ -217,23 +226,26 @@ int dev_alloc(Buffer<T>* mem, size_t count) {
     return mem->grow(std::max<size_t>(count, 16 / sizeof(T)), nullptr);
 }
 
-// Hands the filled buffer `mem` to the handle, which counts it in device_bytes, and returns its address.  `old`: the
-// staged buffer (`old_bytes` long) that `mem` replaces.  The handle drops its reference to it; get_index snapshots
-// keep theirs.
+// Puts the filled buffer `mem` into `slot`, replacing whatever the slot held, and returns its address.
 template <class T>
-T* stage(Handle* h, Buffer<T> mem, const void* old = nullptr, size_t old_bytes = 0) {
+T* stage(Staged::Slot* slot, Buffer<T> mem) {
     T* p = mem.get();
-    h->device_bytes += mem.cap * sizeof(T);
-    std::shared_ptr<void> owner(std::move(mem.p));
-    auto it = std::find_if(h->allocations.begin(), h->allocations.end(),
-                           [&](const std::shared_ptr<void>& a) { return old && a.get() == old; });
-    if (it == h->allocations.end()) {
-        h->allocations.push_back(std::move(owner));
-    } else {
-        h->device_bytes -= std::max<size_t>(old_bytes, 16);
-        *it = std::move(owner);
-    }
+    slot->bytes = mem.cap * sizeof(T);
+    slot->mem = std::shared_ptr<void>(std::move(mem.p));
     return p;
+}
+
+// Stages layer l of h's index: `num_nodes` rows of `width` u32 from host memory.
+int stage_layer(Handle* h, int l, const uint32_t* rows, uint64_t num_nodes, uint32_t width) {
+    const size_t n = (size_t)num_nodes * width;
+    Buffer<uint32_t> mem;
+    int rc = dev_alloc(&mem, n);
+    if (rc) return rc;
+    if (n) GB_CUDA(cudaMemcpy(mem.get(), rows, n * 4, cudaMemcpyHostToDevice));
+    h->dev.layer_rows[l] = stage(&h->dev_mem.layer_rows[l], std::move(mem));
+    h->dev.layer_width[l] = width;
+    h->dev.layer_len[l] = num_nodes;
+    return GRANNE_B200_OK;
 }
 
 // Which distance engine serves an index: calls f.template run<Dist>() for the engine of `d`'s element kind and chunk
@@ -307,9 +319,9 @@ int upload_rows(Handle* h, const gb::DeviceIndex& d, const uint8_t* src, uint64_
     return GRANNE_B200_OK;
 }
 
-// Stages `nrows` dense rows of d's kind (host memory, or device memory if `device_src`) as d's vectors: the handle's
-// own container (h->dev) or the re-rank rows (h->rerank).  The handle owns the memory and counts it.
-int stage_dense(Handle* h, gb::DeviceIndex& d, const uint8_t* rows, uint64_t nrows, uint32_t dim,
+// Stages `nrows` dense rows of d's kind (host memory, or device memory if `device_src`) as d's vectors, owned by
+// `mem`: the handle's own container (h->dev) or the re-rank rows (h->rerank).
+int stage_dense(Handle* h, gb::DeviceIndex& d, Staged& mem, const uint8_t* rows, uint64_t nrows, uint32_t dim,
                 bool device_src = false) {
     d.dim = dim;
     d.full = dim / 32;
@@ -330,7 +342,7 @@ int stage_dense(Handle* h, gb::DeviceIndex& d, const uint8_t* rows, uint64_t nro
     int rc;
     if ((rc = dev_alloc(&dst, (size_t)nrows * d.row_stride * (i8 ? 1 : 4)))) return rc;
     if ((rc = upload_rows(h, d, rows, nrows, device_src, dst.get()))) return rc;
-    d.vectors = stage(h, std::move(dst));
+    d.vectors = stage(&mem.vectors, std::move(dst));
     return GRANNE_B200_OK;
 }
 
@@ -347,11 +359,11 @@ int parse_sum_container(const uint8_t* el, size_t el_len, const uint8_t* emb, si
     return GRANNE_B200_OK;
 }
 
-// Stages a parsed SumEmbeddings container (parse_sum_container) as d's embedding table, element offsets and term ids:
-// the handle's own container (h->dev) or its re-rank container (h->rerank).  The handle owns the memory and counts it.
-int stage_sum(Handle* h, gb::DeviceIndex& d, const gb::DenseView& ev, const gb::SumElements& se) {
+// Stages a parsed SumEmbeddings container (parse_sum_container) as d's embedding table, element offsets and term ids,
+// owned by `mem`: the handle's own container (h->dev) or its re-rank container (h->rerank).
+int stage_sum(Handle* h, gb::DeviceIndex& d, Staged& mem, const gb::DenseView& ev, const gb::SumElements& se) {
     d.kind = gb::kSumEmbeddings;
-    int rc = stage_dense(h, d, ev.data, ev.num, (uint32_t)ev.dim);
+    int rc = stage_dense(h, d, mem, ev.data, ev.num, (uint32_t)ev.dim);
     if (rc) return rc;
     d.num_elements = se.offsets.size() - 1;
     Buffer<unsigned long long> doff;
@@ -360,8 +372,8 @@ int stage_sum(Handle* h, gb::DeviceIndex& d, const gb::DenseView& ev, const gb::
     GB_CUDA(cudaMemcpy(doff.get(), se.offsets.data(), se.offsets.size() * 8, cudaMemcpyHostToDevice));
     if (!se.terms.empty())
         GB_CUDA(cudaMemcpy(dterms.get(), se.terms.data(), se.terms.size() * 4, cudaMemcpyHostToDevice));
-    d.sum_offsets = stage(h, std::move(doff));
-    d.sum_terms = stage(h, std::move(dterms));
+    d.sum_offsets = stage(&mem.sum_offsets, std::move(doff));
+    d.sum_terms = stage(&mem.sum_terms, std::move(dterms));
     return GRANNE_B200_OK;
 }
 
@@ -375,13 +387,13 @@ int stage_elements(Handle* h, int kind, const uint8_t* el, size_t el_len, const 
         gb::DenseView ev;
         gb::SumElements se;
         if ((rc = parse_sum_container(el, el_len, emb, emb_len, &ev, &se))) return rc;
-        if ((rc = stage_sum(h, d, ev, se))) return rc;
+        if ((rc = stage_sum(h, d, h->dev_mem, ev, se))) return rc;
     } else {
         gb::DenseView dv;
         const bool i8 = kind == GRANNE_B200_ANGULAR_INT;
         if (!gb::parse_dense(el, el_len, i8 ? 1 : 4, &dv, &err)) return fail(GRANNE_B200_ERR_FORMAT, err);
         if (dv.dim > 16384) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "vectors wider than 16384 are unsupported");
-        rc = stage_dense(h, d, dv.data, dv.num, (uint32_t)dv.dim);
+        rc = stage_dense(h, d, h->dev_mem, dv.data, dv.num, (uint32_t)dv.dim);
         if (rc) return rc;
         d.num_elements = dv.num;
     }
@@ -475,7 +487,7 @@ int stage_device_elements(Handle* h, int kind, const void* d_rows, uint64_t n, u
     int rc;
     if (n && (rc = check_device_pointer(d_rows, h->device, "elements pointer"))) return rc;
     h->dev.kind = kind;
-    rc = stage_dense(h, h->dev, static_cast<const uint8_t*>(d_rows), n, dim, true);
+    rc = stage_dense(h, h->dev, h->dev_mem, static_cast<const uint8_t*>(d_rows), n, dim, true);
     if (rc) return rc;
     h->dev.num_elements = n;
     return GRANNE_B200_OK;
@@ -540,12 +552,7 @@ int open_impl(const uint8_t* index_bytes, size_t index_len, int kind, const uint
         const gb::HostLayer& L = graph.layers[l];
         if (L.num_nodes > d.num_elements)
             return fail(GRANNE_B200_ERR_FORMAT, "index refers to more elements than the container holds");
-        Buffer<uint32_t> rows;
-        if ((rc = dev_alloc(&rows, L.rows.size()))) return rc;
-        if (!L.rows.empty()) GB_CUDA(cudaMemcpy(rows.get(), L.rows.data(), L.rows.size() * 4, cudaMemcpyHostToDevice));
-        d.layer_rows[l] = stage(h.get(), std::move(rows));
-        d.layer_width[l] = L.width;
-        d.layer_len[l] = L.num_nodes;
+        if ((rc = stage_layer(h.get(), l, L.rows.data(), L.num_nodes, L.width))) return rc;
         h->layer_max_degree.push_back(L.max_degree);
     }
     finish_handle(h.get());
@@ -1174,43 +1181,28 @@ int check_rerank_shape(const Handle* h, uint64_t n, uint64_t dim) {
     return GRANNE_B200_OK;
 }
 
-// Drops the device allocations of the view r (its rows or table, and a sum view's offsets and terms), which hold
-// `bytes` of h->device_bytes.
-void drop_rerank_view(Handle* h, const gb::DeviceIndex& r, uint64_t bytes) {
-    for (const void* p : {r.vectors, static_cast<const void*>(r.sum_offsets), static_cast<const void*>(r.sum_terms)}) {
-        if (!p) continue;
-        auto it = std::find_if(h->allocations.begin(), h->allocations.end(),
-                               [&](const std::shared_ptr<void>& a) { return a.get() == p; });
-        if (it != h->allocations.end()) h->allocations.erase(it);
-    }
-    h->device_bytes -= bytes;
-}
-
-// Stages h's re-rank container with stage_into(r) (stage_dense or stage_sum into an empty view r).  It becomes visible
-// to searches only once fully staged; a container that fails part-way gives its memory back.  The target check is
-// repeated under the handle's attach lock, so that of two concurrent attaches one stages its container and the other
-// fails.
+// Stages h's re-rank container with stage_into(r, mem) (stage_dense or stage_sum into an empty view r and its owners
+// mem).  It becomes visible to searches only once fully staged; a container that fails part-way frees its memory
+// when mem goes out of scope.  The target check is repeated under the handle's attach lock, so that of two concurrent
+// attaches one stages its container and the other fails.
 template <class StageInto>
 int stage_rerank(Handle* h, StageInto&& stage_into) {
     std::lock_guard<std::mutex> g(h->rerank_mu);
     int rc = check_rerank_target(h);
     if (rc) return rc;
     gb::DeviceIndex r{};
-    const uint64_t before = h->device_bytes;
-    if ((rc = stage_into(r))) {
-        drop_rerank_view(h, r, h->device_bytes - before);
-        return rc;
-    }
+    Staged mem;
+    if ((rc = stage_into(r, mem))) return rc;
     h->rerank = r;
-    h->rerank_bytes = h->device_bytes - before;
+    h->rerank_mem = std::move(mem);
     return GRANNE_B200_OK;
 }
 
 // Stages n angular f32 element rows as h's re-rank rows, laid out for the engine DistDispatch picks for their width.
 int stage_rerank_rows(Handle* h, const uint8_t* rows, uint64_t n, uint32_t dim, bool device_src) {
-    return stage_rerank(h, [&](gb::DeviceIndex& r) {
+    return stage_rerank(h, [&](gb::DeviceIndex& r, Staged& mem) {
         r.kind = gb::kAngularF32;
-        const int rc = stage_dense(h, r, rows, n, dim, device_src);
+        const int rc = stage_dense(h, r, mem, rows, n, dim, device_src);
         r.num_elements = n;
         return rc;
     });
@@ -1232,10 +1224,8 @@ int check_rerank_sum(const Handle* h, const void* el, size_t el_len, const void*
 // makes h's device current.
 void release_rerank(Handle* h) {
     std::lock_guard<std::mutex> g(h->rerank_mu);
-    if (!h->rerank.vectors) return;
-    drop_rerank_view(h, h->rerank, h->rerank_bytes);
     h->rerank = gb::DeviceIndex{};
-    h->rerank_bytes = 0;
+    h->rerank_mem = Staged{};
 }
 
 // validate_search's rules plus the two-stage ones.
@@ -1362,7 +1352,6 @@ struct granne_b200_builder {
     std::unique_ptr<Handle> h;  // search view over the layers built so far (+ the one under construction)
     granne_b200_build_config cfg{};
     uint32_t stride = 0;  // physical row stride (node_width rounded up to 8)
-    std::vector<std::shared_ptr<void>> layer_mem;
     std::unique_ptr<Workspace> ws;
     // batch scratch
     Buffer<uint32_t> d_ids;
@@ -1477,20 +1466,26 @@ int builder_index_last_layer(Builder* b, uint64_t max_num_elements) {
     uint32_t layer_m = b->cfg.num_neighbors;
     if (ideal < total) layer_m = std::max<uint32_t>(1, layer_m / 2);  // half num_neighbors on upper layers
     // the layer grows: fresh allocation (snapshots handed out by get_index keep the old one alive)
-    uint32_t* grown = nullptr;
-    GB_CUDA(cudaMalloc(&grown, std::max<size_t>((size_t)num * b->stride * 4, 16)));
-    std::shared_ptr<void> mem(grown, DeviceFree{});
+    Buffer<uint32_t> mem;
+    int rc = dev_alloc(&mem, (size_t)num * b->stride);
+    if (rc) return rc;
+    uint32_t* grown = mem.get();
     cudaStream_t stream = b->ws->stream.get();
     gb::fill_u32_kernel<<<h->num_sms * 4, 256, 0, stream>>>(grown, (unsigned long long)num * b->stride, gb::kUnusedId);
     h->launches++;
     if (have) GB_CUDA(cudaMemcpyAsync(grown, d.layer_rows[cur], (size_t)have * b->stride * 4, cudaMemcpyDeviceToDevice, stream));
-    b->layer_mem[cur] = mem;
-    d.layer_rows[cur] = grown;
+    // the replaced rows stay alive until the copy out of them has completed: the first pass below synchronises the
+    // stream before it returns OK, and a failed pass is synchronised here
+    Staged::Slot old = std::move(h->dev_mem.layer_rows[cur]);
+    d.layer_rows[cur] = stage(&h->dev_mem.layer_rows[cur], std::move(mem));
     d.layer_len[cur] = num;
     h->layer_max_degree[cur] = b->cfg.num_neighbors;
     finish_handle(h);
-    int rc = builder_index_elements(b, layer_m, b->cfg.max_search, have, num, false);
-    if (rc) return rc;
+    if ((rc = builder_index_elements(b, layer_m, b->cfg.max_search, have, num, false))) {
+        cudaStreamSynchronize(stream);
+        return rc;
+    }
+    old = {};  // the copy is done
     if (b->cfg.reinsert_elements) {
         // use half max_search when reindexing (:698-699)
         rc = builder_index_elements(b, layer_m, std::max<uint32_t>(1, b->cfg.max_search / 2), 0, num, true);
@@ -1516,10 +1511,10 @@ int builder_build_partial(Builder* b, uint64_t num_elements) {
         // new layer = clone of the previous one (:392-398)
         const int l = d.num_layers;
         d.layer_rows[l] = l ? d.layer_rows[l - 1] : nullptr;
+        h->dev_mem.layer_rows[l] = l ? h->dev_mem.layer_rows[l - 1] : Staged::Slot{};
         d.layer_len[l] = l ? d.layer_len[l - 1] : 0;
         d.layer_width[l] = b->stride;
         d.num_layers = l + 1;
-        b->layer_mem.push_back(l ? b->layer_mem[l - 1] : std::shared_ptr<void>());
         h->layer_max_degree.push_back(b->cfg.num_neighbors);
         finish_handle(h);
         if ((rc = builder_index_last_layer(b, num_elements))) return rc;
@@ -1544,14 +1539,8 @@ int builder_load_layers(Builder* b, const gb::HostGraph& graph) {
         rows.assign((size_t)L.num_nodes * b->stride, gb::kUnusedId);
         for (uint64_t i = 0; i < L.num_nodes; ++i)
             std::copy_n(L.rows.data() + i * L.width, keep, rows.data() + i * b->stride);
-        Buffer<uint32_t> mem;
-        int rc;
-        if ((rc = dev_alloc(&mem, rows.size()))) return rc;
-        if (!rows.empty()) GB_CUDA(cudaMemcpy(mem.get(), rows.data(), rows.size() * 4, cudaMemcpyHostToDevice));
-        d.layer_rows[l] = mem.get();
-        d.layer_len[l] = L.num_nodes;
-        d.layer_width[l] = b->stride;
-        b->layer_mem.push_back(std::shared_ptr<void>(std::move(mem.p)));
+        const int rc = stage_layer(h, (int)l, rows.data(), L.num_nodes, b->stride);
+        if (rc) return rc;
         h->layer_max_degree.push_back(m);
     }
     d.num_layers = (int)graph.layers.size();
@@ -1623,7 +1612,24 @@ uint64_t granne_b200_num_elements(const granne_b200_index* h) { return h ? h->de
 uint64_t granne_b200_dim(const granne_b200_index* h) { return h ? h->dev.dim : 0; }
 int granne_b200_element_kind(const granne_b200_index* h) { return h ? h->dev.kind : -1; }
 uint64_t granne_b200_launch_count(const granne_b200_index* h) { return h ? h->launches.load() : 0; }
-uint64_t granne_b200_device_bytes(const granne_b200_index* h) { return h ? h->device_bytes : 0; }
+// Counts each allocation once: a builder's new layer shares its rows with the layer above until it grows.
+uint64_t granne_b200_device_bytes(const granne_b200_index* h) {
+    if (!h) return 0;
+    std::lock_guard<std::mutex> g(h->rerank_mu);
+    const void* counted[2 * (3 + gb::kMaxLayers)];
+    size_t n = 0;
+    uint64_t bytes = 0;
+    auto count = [&](const Staged::Slot& s) {
+        if (!s.mem || std::find(counted, counted + n, s.mem.get()) != counted + n) return;
+        counted[n++] = s.mem.get();
+        bytes += s.bytes;
+    };
+    for (const Staged* m : {&h->dev_mem, &h->rerank_mem}) {
+        for (const Staged::Slot* s : {&m->vectors, &m->sum_offsets, &m->sum_terms}) count(*s);
+        for (const Staged::Slot& s : m->layer_rows) count(s);
+    }
+    return bytes;
+}
 
 int granne_b200_get_neighbors(const granne_b200_index* h, uint64_t idx, uint64_t layer, uint32_t* out, size_t cap,
                               size_t* out_n) {
@@ -1823,7 +1829,7 @@ int granne_b200_set_rerank_embeddings(granne_b200_index* h, const void* elements
         if ((rc = check_rerank_sum(h, elements_bytes, elements_len, embeddings_bytes, embeddings_len, &ev, &se)))
             return rc;
         GB_DEVICE(h->device);
-        return stage_rerank(h, [&](gb::DeviceIndex& r) { return stage_sum(h, r, ev, se); });
+        return stage_rerank(h, [&](gb::DeviceIndex& r, Staged& mem) { return stage_sum(h, r, mem, ev, se); });
     });
 }
 
@@ -2019,8 +2025,8 @@ int granne_b200_builder_append(granne_b200_builder* b, const void* elements_byte
             if (!se.terms.empty())
                 GB_CUDA(cudaMemcpy(dterms.get() + old_terms, se.terms.data(), se.terms.size() * 4,
                                    cudaMemcpyHostToDevice));
-            d.sum_offsets = stage(h, std::move(doff), d.sum_offsets, (size_t)(old_n + 1) * 8);
-            d.sum_terms = stage(h, std::move(dterms), d.sum_terms, (size_t)old_terms * 4);
+            d.sum_offsets = stage(&h->dev_mem.sum_offsets, std::move(doff));
+            d.sum_terms = stage(&h->dev_mem.sum_terms, std::move(dterms));
             d.num_elements = new_n;
             return GRANNE_B200_OK;
         }
@@ -2044,7 +2050,7 @@ int granne_b200_builder_append(granne_b200_builder* b, const void* elements_byte
         if ((rc = dev_alloc(&rows, (size_t)new_n * row_bytes))) return rc;
         if (old_n) GB_CUDA(cudaMemcpy(rows.get(), d.vectors, (size_t)old_n * row_bytes, cudaMemcpyDeviceToDevice));
         if ((rc = upload_rows(h, d, dv.data, dv.num, false, rows.get() + (size_t)old_n * row_bytes))) return rc;
-        d.vectors = stage(h, std::move(rows), d.vectors, (size_t)old_n * row_bytes);
+        d.vectors = stage(&h->dev_mem.vectors, std::move(rows));
         d.num_vectors = new_n;
         d.num_elements = new_n;
         return GRANNE_B200_OK;
@@ -2104,10 +2110,7 @@ int granne_b200_builder_get_index(granne_b200_builder* b, granne_b200_index** ou
         h->num_sms = src->num_sms;
         h->smem_optin = src->smem_optin;
         h->dev = src->dev;
-        h->allocations = src->allocations;  // shared ownership of the staged elements
-        for (const auto& m : b->layer_mem)
-            if (m) h->allocations.push_back(m);
-        h->device_bytes = src->device_bytes;
+        h->dev_mem = src->dev_mem;  // shared ownership of the staged elements and layers
         h->layer_max_degree = src->layer_max_degree;
         finish_handle(h.get());
         *out = h.release();

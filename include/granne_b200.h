@@ -493,7 +493,9 @@ int granne_b200_apply_order(const void* index_bytes, size_t index_len, int eleme
 /* Number of kernels this library launched on behalf of `h` since it was opened (bench.py's gpu_launches). */
 uint64_t granne_b200_launch_count(const granne_b200_index* h);
 
-/* Bytes of device memory the staged index occupies (layer graph + vectors). */
+/* Bytes of device memory the staged index occupies: layer rows + element container + attached re-rank container, for
+ * every way a handle is made (granne_b200_open*, granne_b200_builder_get_index).  Memory a handle shares with a
+ * builder or another snapshot is counted by every handle that holds it.  Workspaces are not counted. */
 uint64_t granne_b200_device_bytes(const granne_b200_index* h);
 
 #ifdef __cplusplus
