@@ -28,9 +28,7 @@ struct BuildArgs {
     uint32_t node_width;        // node.len() == the builder's num_neighbors (row width of every layer, :394)
     uint32_t max_neighbors;     // config.num_neighbors of THIS layer (halved on upper layers, :665-668)
     int* locks;                 // one spin lock per node
-    uint32_t stg_rows;
-    uint32_t stg_row_bytes;
-    uint32_t tile_rows;
+    WarpTiles tiles;
     unsigned int* work_counter;
     uint32_t num_nodes;         // prune pass: nodes in the layer
 };
@@ -78,10 +76,34 @@ __host__ __device__ constexpr uint32_t link_cand_cap(uint32_t cand_stride, uint3
     return cand_stride > node_width + 8 ? (cand_stride > 40 ? cand_stride : 40)
                                         : (node_width + 8 > 40 ? node_width + 8 : 40);
 }
-// bytes of shared memory the link scratch needs behind the search context
-__host__ __device__ constexpr size_t link_scratch_bytes(uint32_t cand_cap, uint32_t node_width) {
-    return (size_t)cand_cap * 8 + (size_t)link_node_slots(node_width) * 16 + (size_t)(link_node_slots(node_width) + 8) * 8;
-}
+// The link scratch behind SmemLayout::end, walked from `base` in the address type P like SmemLayout: the host sizes the
+// build launches with its `end` (P = size_t), the kernels place LinkScratch with it (P = unsigned char*).
+template <class P>
+struct LinkLayout {
+    P cid, cd, sid, sd, oid, od, tid, td, end;
+
+    __host__ __device__ __forceinline__ LinkLayout(P base, uint32_t cand_cap, uint32_t node_width) {
+        const uint32_t slots = link_node_slots(node_width);
+        P sp = base;
+        cid = sp;
+        sp += (size_t)cand_cap * 4;
+        cd = sp;
+        sp += (size_t)cand_cap * 4;
+        sid = sp;
+        sp += slots * 4;
+        sd = sp;
+        sp += slots * 4;
+        oid = sp;
+        sp += slots * 4;
+        od = sp;
+        sp += slots * 4;
+        tid = sp;
+        sp += (slots + 8) * 4;
+        td = sp;
+        sp += (slots + 8) * 4;
+        end = sp;
+    }
+};
 
 // select_neighbors (:849-883) over candidates cid/cd[0..nc) sorted by distance; result in sid/sd, returns count.
 template <class Dist>
@@ -194,33 +216,24 @@ __device__ __forceinline__ void connect_nodes(const DeviceIndex& ix, WarpCtx& c,
     add_and_limit(ix, c, dist, s, rows, stride, node_width, i, true, j, d, (int)node_width);
 }
 
-// The search context (SmemLayout) followed by the link scratch (link_scratch_bytes).
+// The search context (SmemLayout) followed by the link scratch (LinkLayout).
 __device__ __forceinline__ void setup_ctx(const DeviceIndex& ix, WarpCtx& c, LinkScratch& s, unsigned char* smem_raw,
-                                          uint32_t stg_rows, uint32_t stg_row_bytes, uint32_t tile_rows,
-                                          uint32_t cand_cap, uint32_t node_width = 32) {
+                                          const WarpTiles& t, uint32_t cand_cap, uint32_t node_width = 32) {
     c.lane = threadIdx.x;
-    unsigned char* sp = place_warp_smem(c, smem_raw, ix, tile_rows, stg_rows, stg_row_bytes);
+    const LinkLayout<unsigned char*> L(place_warp_smem(c, smem_raw, ix, t), cand_cap, node_width);
     c.status = 0;
     c.q_norm_i8 = 0;
     c.n_dist = c.n_expand = c.n_nbr = 0;
     c.list = nullptr;
     c.visited = nullptr;
-    s.cid = reinterpret_cast<uint32_t*>(sp);
-    sp += (size_t)cand_cap * 4;
-    s.cd = reinterpret_cast<float*>(sp);
-    sp += (size_t)cand_cap * 4;
-    const uint32_t slots = link_node_slots(node_width);
-    s.sid = reinterpret_cast<uint32_t*>(sp);
-    sp += slots * 4;
-    s.sd = reinterpret_cast<float*>(sp);
-    sp += slots * 4;
-    s.oid = reinterpret_cast<uint32_t*>(sp);
-    sp += slots * 4;
-    s.od = reinterpret_cast<float*>(sp);
-    sp += slots * 4;
-    s.tid = reinterpret_cast<uint32_t*>(sp);
-    sp += (slots + 8) * 4;
-    s.td = reinterpret_cast<float*>(sp);
+    s.cid = reinterpret_cast<uint32_t*>(L.cid);
+    s.cd = reinterpret_cast<float*>(L.cd);
+    s.sid = reinterpret_cast<uint32_t*>(L.sid);
+    s.sd = reinterpret_cast<float*>(L.sd);
+    s.oid = reinterpret_cast<uint32_t*>(L.oid);
+    s.od = reinterpret_cast<float*>(L.od);
+    s.tid = reinterpret_cast<uint32_t*>(L.tid);
+    s.td = reinterpret_cast<float*>(L.td);
 }
 
 // index_element (:805-846) after the candidate search, one warp per element of the batch.
@@ -230,7 +243,7 @@ __global__ void __launch_bounds__(32) build_link_kernel(const DeviceIndex ix, co
     WarpCtx c;
     LinkScratch s;
     const uint32_t cand_cap = link_cand_cap(a.cand_stride, a.node_width);
-    setup_ctx(ix, c, s, smem_raw, a.stg_rows, a.stg_row_bytes, a.tile_rows, cand_cap, a.node_width);
+    setup_ctx(ix, c, s, smem_raw, a.tiles, cand_cap, a.node_width);
     Dist dist;
     const int lane = c.lane;
     while (true) {
@@ -302,8 +315,7 @@ __global__ void __launch_bounds__(32) build_prune_kernel(const DeviceIndex ix, c
     extern __shared__ __align__(16) unsigned char smem_raw[];
     WarpCtx c;
     LinkScratch s;
-    setup_ctx(ix, c, s, smem_raw, a.stg_rows, a.stg_row_bytes, a.tile_rows, link_cand_cap(0, a.node_width),
-                    a.node_width);
+    setup_ctx(ix, c, s, smem_raw, a.tiles, link_cand_cap(0, a.node_width), a.node_width);
     Dist dist;
     while (true) {
         unsigned int w0 = 0;
@@ -322,9 +334,7 @@ struct PairArgs {
     uint32_t n;
     float* out;           // n distances
     int* error_flag;
-    uint32_t stg_rows;
-    uint32_t stg_row_bytes;
-    uint32_t tile_rows;
+    WarpTiles tiles;
 };
 
 template <class Dist>
@@ -332,7 +342,7 @@ __global__ void __launch_bounds__(32) pair_distance_kernel(const DeviceIndex ix,
     extern __shared__ __align__(16) unsigned char smem_raw[];
     WarpCtx c;
     LinkScratch s;
-    setup_ctx(ix, c, s, smem_raw, a.stg_rows, a.stg_row_bytes, a.tile_rows, 8);
+    setup_ctx(ix, c, s, smem_raw, a.tiles, 8);
     Dist dist;
     SearchArgs q{};
     q.queries = a.queries;

@@ -248,27 +248,33 @@ int stage_layer(Handle* h, int l, const uint32_t* rows, uint64_t num_nodes, uint
     return GRANNE_B200_OK;
 }
 
-// Which distance engine serves an index: calls f.template run<Dist>() for the engine of `d`'s element kind and chunk
+// The type tag DistDispatch passes: Engine<Dist>::type is the engine.
+template <class Dist>
+struct Engine {
+    using type = Dist;
+};
+
+// Which distance engine serves an index: returns f(Engine<Dist>{}) for the engine of `d`'s element kind and chunk
 // count (d.full = dim / 32) — DistF32<full> for the chunk counts it is compiled for, DistF32Generic for every other
-// f32 width.  This is the only place that decides it; the row layout (stage_dense) and the launch plan (make_plan)
+// f32 width.  This is the only place that decides it; the row layout (stage_dense) and the tiles (engine_tiles)
 // follow from the engine it picks (fixed_f32_chunks).
 struct DistDispatch {
     template <class F>
     static int call(const gb::DeviceIndex& d, F&& f) {
         switch (d.kind) {
-            case gb::kAngularI8: return f.template run<gb::DistI8>();
-            case gb::kSumEmbeddings: return f.template run<gb::DistSum>();
+            case gb::kAngularI8: return f(Engine<gb::DistI8>{});
+            case gb::kSumEmbeddings: return f(Engine<gb::DistSum>{});
             default: break;
         }
         switch (d.full) {
-            case 0: return f.template run<gb::DistF32<0>>();
-            case 1: return f.template run<gb::DistF32<1>>();
-            case 2: return f.template run<gb::DistF32<2>>();
-            case 3: return f.template run<gb::DistF32<3>>();
-            case 4: return f.template run<gb::DistF32<4>>();
-            case 6: return f.template run<gb::DistF32<6>>();
-            case 8: return f.template run<gb::DistF32<8>>();
-            default: return f.template run<gb::DistF32Generic>();
+            case 0: return f(Engine<gb::DistF32<0>>{});
+            case 1: return f(Engine<gb::DistF32<1>>{});
+            case 2: return f(Engine<gb::DistF32<2>>{});
+            case 3: return f(Engine<gb::DistF32<3>>{});
+            case 4: return f(Engine<gb::DistF32<4>>{});
+            case 6: return f(Engine<gb::DistF32<6>>{});
+            case 8: return f(Engine<gb::DistF32<8>>{});
+            default: return f(Engine<gb::DistF32Generic>{});
         }
     }
 };
@@ -279,11 +285,9 @@ template <class Dist>
 constexpr int kFixedChunks = -1;
 template <int FULL>
 constexpr int kFixedChunks<gb::DistF32<FULL>> = FULL;
-struct FixedChunksProbe {
-    template <class Dist>
-    int run() const { return kFixedChunks<Dist>; }
-};
-int fixed_f32_chunks(const gb::DeviceIndex& d) { return DistDispatch::call(d, FixedChunksProbe{}); }
+int fixed_f32_chunks(const gb::DeviceIndex& d) {
+    return DistDispatch::call(d, [](auto e) { return kFixedChunks<typename decltype(e)::type>; });
+}
 
 // Writes `nrows` dense rows of d's kind and width from `src` (host memory, or device memory if `device_src`) to the
 // staged rows at `dst`: in 64 MB slabs through a temporary device buffer, re-laid out on the device by
@@ -587,20 +591,57 @@ void write_width_header(uint8_t* image, uint64_t dim) {
 }
 
 // ---- launch configuration -----------------------------------------------------------------------------------------
+// What every one-warp kernel over a container places first in its shared window: the tiles of the engine that serves
+// it, and where its SmemLayout ends.  Behind that the search kernels put their list (and visited set), rerank_kernel
+// its keys, the build kernels their link scratch.
+struct EngineTiles {
+    gb::WarpTiles tiles;
+    size_t base_smem;  // gb::SmemLayout::end: tile + id scratch + reserved + query (+ embeddings scratch) + staging
+};
+
+EngineTiles engine_tiles(const gb::DeviceIndex& d) {
+    EngineTiles e{};
+    gb::WarpTiles& t = e.tiles;
+    const int fixed_chunks = fixed_f32_chunks(d);
+    if (d.kind == gb::kAngularI8) {
+        // DistI8: no ordered sums; the staging tile is a set of 512-byte pass slots (32 lanes x one 16-byte chunk each)
+        t.tile_rows = 0;
+        t.stg_row_bytes = 512;
+        t.stg_rows = std::max<uint32_t>(2, (unsigned)GB_STG_BYTES / 512u);
+    } else if (d.kind == gb::kSumEmbeddings) {
+        // DistSum: the staging tile holds the summed vectors of a batch of candidates (one row each)
+        t.tile_rows = 8;
+        t.stg_row_bytes = ((d.dim + 3u) & ~3u) * 4u;
+        t.stg_rows = std::min<uint32_t>(8u, std::max<uint32_t>(4, (8192u / t.stg_row_bytes) & ~3u));
+    } else if (fixed_chunks > 0) {
+        // DistF32<full>: the ordered-sum tile has one row per staged candidate row of a batch
+        t.stg_row_bytes = d.full * 128u;
+        t.stg_rows = std::min<uint32_t>(8u, std::max<uint32_t>(4, ((unsigned)GB_STG_BYTES / t.stg_row_bytes) & ~3u));
+        t.tile_rows = t.stg_rows;
+    } else if (fixed_chunks < 0 && d.full <= 64) {
+        // DistF32Generic stages rows of up to 8 KB (dim < 2080), at most 8 (the tile rows) per batch
+        t.tile_rows = 8;
+        t.stg_row_bytes = d.full * 128u;
+        t.stg_rows = std::min<uint32_t>(8u, std::max<uint32_t>(2, (unsigned)(2 * GB_STG_BYTES) / t.stg_row_bytes));
+    } else {
+        // DistF32<0> (dim < 32) and DistF32Generic on wider rows load directly; the generic engine then parks the lane
+        // partials of up to 32 candidates in the tile
+        t.tile_rows = 32;
+    }
+    e.base_smem = gb::SmemLayout<size_t>(0, d.kind, d.dim, d.row_stride, t).end;
+    return e;
+}
+
+// The search passes' sizes for h's own container.
 struct LaunchPlan {
     uint32_t list_cap, vis_slots, vis_upper;
     uint32_t vis_retry;  // visited slots per CTA of the retry pass
     int rows;           // fast list rows R (capacity 32*R), 0 = generic list
-    uint32_t stg_rows;  // candidate rows per staged batch (0: the engine loads rows directly)
-    uint32_t stg_row_bytes;
-    uint32_t tile_rows;  // ordered-sum tile rows: one per staged row (f32), 8 embeddings, 32 direct loads, 0 for i8
-    size_t base_smem;   // gb::SmemLayout::end: tile + id scratch + reserved + query (+ embeddings scratch) + staging
+    EngineTiles engine;
     size_t smem;        // fast pass total
 };
 
-// `view`: the staged container the kernels read, when it is not the handle's own (the re-rank container)
-LaunchPlan make_plan(const Handle* h, uint32_t max_search, const gb::DeviceIndex* view = nullptr) {
-    const gb::DeviceIndex& d = view ? *view : h->dev;
+LaunchPlan make_plan(const Handle* h, uint32_t max_search) {
     LaunchPlan p{};
     // fast list: capacity 32*R with R odd (conflict-free lane-major access); slack >= 16 entries over max_search
     p.rows = 0;
@@ -617,38 +658,8 @@ LaunchPlan make_plan(const Handle* h, uint32_t max_search, const gb::DeviceIndex
     const uint64_t cap_slots = 1ull << 20;
     p.vis_retry = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(want * 8, want), std::max<uint64_t>(cap_slots, want));
     want = std::min<uint64_t>(want * h->vis_scale.load(), std::max<uint64_t>(cap_slots, want));
-    // the staging tile and the ordered-sum tile of the engine that serves the index
-    const int fixed_chunks = fixed_f32_chunks(d);
-    p.stg_rows = 0;
-    p.stg_row_bytes = 0;
-    if (d.kind == gb::kAngularI8) {
-        // DistI8: no ordered sums; the staging tile is a set of 512-byte pass slots (32 lanes x one 16-byte chunk each)
-        p.tile_rows = 0;
-        p.stg_row_bytes = 512;
-        p.stg_rows = std::max<uint32_t>(2, (unsigned)GB_STG_BYTES / 512u);
-    } else if (d.kind == gb::kSumEmbeddings) {
-        // DistSum: the staging tile holds the summed vectors of a batch of candidates (one row each)
-        p.tile_rows = 8;
-        p.stg_row_bytes = ((d.dim + 3u) & ~3u) * 4u;
-        p.stg_rows = std::min<uint32_t>(8u, std::max<uint32_t>(4, (8192u / p.stg_row_bytes) & ~3u));
-    } else if (fixed_chunks > 0) {
-        // DistF32<full>: the ordered-sum tile has one row per staged candidate row of a batch
-        p.stg_row_bytes = d.full * 128u;
-        p.stg_rows = std::min<uint32_t>(8u, std::max<uint32_t>(4, ((unsigned)GB_STG_BYTES / p.stg_row_bytes) & ~3u));
-        p.tile_rows = p.stg_rows;
-    } else if (fixed_chunks < 0 && d.full <= 64) {
-        // DistF32Generic stages rows of up to 8 KB (dim < 2080), at most 8 (the tile rows) per batch
-        p.tile_rows = 8;
-        p.stg_row_bytes = d.full * 128u;
-        p.stg_rows = std::min<uint32_t>(8u, std::max<uint32_t>(2, (unsigned)(2 * GB_STG_BYTES) / p.stg_row_bytes));
-    } else {
-        // DistF32<0> (dim < 32) and DistF32Generic on wider rows load directly; the generic engine then parks the lane
-        // partials of up to 32 candidates in the tile
-        p.tile_rows = 32;
-    }
-    const size_t base =
-        gb::SmemLayout<size_t>(0, d.kind, d.dim, d.row_stride, p.tile_rows, p.stg_rows, p.stg_row_bytes).end;
-    p.base_smem = base;
+    p.engine = engine_tiles(h->dev);
+    const size_t base = p.engine.base_smem;
     const size_t budget = h->smem_optin;
     if (p.rows) {
         // fast pass: list in shared memory, visited set in global memory
@@ -673,11 +684,49 @@ LaunchPlan make_plan(const Handle* h, uint32_t max_search, const gb::DeviceIndex
 // next longer fast list for the retry pass (0 = none: go straight to the slow pass)
 constexpr int retry_rows(int R) { return R == 3 ? 7 : (R == 7 ? 15 : (R == 15 ? 31 : 0)); }
 
-template <class Kern>
-int set_smem_attr(Kern kern, Handle* h, std::atomic<bool>* done) {
-    if (!done->load()) {
-        GB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_optin));
-        done->store(true);
+// Raises Kern's dynamic shared-memory limit to the device's opt-in maximum, once per (kernel, device): function
+// attributes are per device.  One flag per device ordinal (every handle's device is one, check_device), so the check
+// takes no lock.
+template <auto Kern>
+int raise_smem_limit(const Handle* h) {
+    static std::vector<std::atomic<bool>> raised([] {
+        int n = 0;
+        cudaGetDeviceCount(&n);
+        return (size_t)n;
+    }());
+    std::atomic<bool>& done = raised[h->device];
+    if (!done.load()) {
+        GB_CUDA(cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_optin));
+        done.store(true);
+    }
+    return GRANNE_B200_OK;
+}
+
+// Launches the one-warp kernel Kern<<<grid, 32, smem, stream>>>(d, a) over the staged container d and counts it.
+template <auto Kern, class Args>
+int launch_warps(Handle* h, unsigned grid, size_t smem, cudaStream_t stream, const gb::DeviceIndex& d, const Args& a) {
+    const int rc = raise_smem_limit<Kern>(h);
+    if (rc) return rc;
+    Kern<<<grid, 32, smem, stream>>>(d, a);
+    h->launches++;
+    GB_CUDA(cudaGetLastError());
+    return GRANNE_B200_OK;
+}
+
+// Resident one-warp CTAs per SM of Kern with `smem` bytes of dynamic shared memory, queried once per (kernel, smem).
+template <auto Kern>
+int resident_ctas(const Handle* h, size_t smem, int* occ) {
+    const int rc = raise_smem_limit<Kern>(h);  // the query counts the CTAs the raised limit admits
+    if (rc) return rc;
+    static std::mutex mu;
+    static std::map<size_t, int> cache;
+    std::lock_guard<std::mutex> g(mu);
+    auto it = cache.find(smem);
+    if (it == cache.end()) {
+        GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ, Kern, 32, smem));
+        cache[smem] = *occ;
+    } else {
+        *occ = it->second;
     }
     return GRANNE_B200_OK;
 }
@@ -686,29 +735,13 @@ template <class Dist, int R>
 int launch_kernels(Handle* h, Workspace* w, gb::SearchArgs a, const LaunchPlan& plan, cudaStream_t stream,
                    const gb::DeviceIndex& dv) {
     constexpr int RR = retry_rows(R);
-    auto kern = gb::search_kernel<Dist, R>;
-    auto retry = gb::search_kernel<Dist, (RR > 0 ? RR : 1)>;
-    auto slow = gb::search_kernel<Dist, 0>;
-    static std::atomic<bool> attr_set[64][3];  // function attributes are per device
-    const int dslot = h->device & 63;
-    int rc;
-    if ((rc = set_smem_attr(kern, h, &attr_set[dslot][0]))) return rc;
-    if (RR > 0 && (rc = set_smem_attr(retry, h, &attr_set[dslot][1]))) return rc;
-    if ((rc = set_smem_attr(slow, h, &attr_set[dslot][2]))) return rc;
+    constexpr auto kern = gb::search_kernel<Dist, R>;
+    constexpr auto retry = gb::search_kernel<Dist, (RR > 0 ? RR : 1)>;
+    constexpr auto slow = gb::search_kernel<Dist, 0>;
     // fast pass
-    static std::mutex occ_mu;
-    static std::map<size_t, int> occ_cache;
     int occ = 0;
-    {
-        std::lock_guard<std::mutex> g(occ_mu);
-        auto it = occ_cache.find(plan.smem);
-        if (it == occ_cache.end()) {
-            GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, 32, plan.smem));
-            occ_cache[plan.smem] = occ;
-        } else {
-            occ = it->second;
-        }
-    }
+    int rc = resident_ctas<kern>(h, plan.smem, &occ);
+    if (rc) return rc;
     if (occ < 1) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "max_search too large for the shared-memory workspace");
     static const int occ_cap = [] {  // tuning/diagnostic knob: cap the resident one-warp CTAs per SM
         const char* e = std::getenv("GRANNE_B200_MAX_CTAS_PER_SM");
@@ -728,9 +761,7 @@ int launch_kernels(Handle* h, Workspace* w, gb::SearchArgs a, const LaunchPlan& 
     a.final_pass = 0;
     a.gate_in = nullptr;
     a.gate_out = w->d_counters.get() + 3;
-    kern<<<grid, 32, plan.smem, stream>>>(dv, a);
-    h->launches++;
-    GB_CUDA(cudaGetLastError());
+    if ((rc = launch_warps<kern>(h, grid, plan.smem, stream, dv, a))) return rc;
     if (have_retry) {
         // retry pass: only the queries the fast pass flagged (exits at once if none) on a full-size grid of its own,
         // with the next longer list and 8x larger visited tables — so a batch of heavy queries (e.g. the reference's
@@ -745,10 +776,8 @@ int launch_kernels(Handle* h, Workspace* w, gb::SearchArgs a, const LaunchPlan& 
         const unsigned rgrid = (unsigned)std::min<unsigned long long>(a.nq, (unsigned long long)h->num_sms * 4);
         if ((rc = w->d_vis_retry.grow((size_t)h->num_sms * 4 * r.vis_slots, stream))) return rc;
         r.vis_global = w->d_vis_retry.get();
-        const size_t rsmem = plan.base_smem + gb::fast_list_bytes(RR > 0 ? RR : 1);
-        retry<<<rgrid, 32, rsmem, stream>>>(dv, r);
-        h->launches++;
-        GB_CUDA(cudaGetLastError());
+        const size_t rsmem = plan.engine.base_smem + gb::fast_list_bytes(RR > 0 ? RR : 1);
+        if ((rc = launch_warps<retry>(h, rgrid, rsmem, stream, dv, r))) return rc;
     }
     // slow pass: re-runs only the queries that are still flagged (exits immediately if none)
     gb::SearchArgs s = a;
@@ -758,32 +787,8 @@ int launch_kernels(Handle* h, Workspace* w, gb::SearchArgs a, const LaunchPlan& 
     s.work_counter = w->d_counters.get() + 2;
     s.gate_in = w->d_counters.get() + (have_retry ? 4 : 3);
     s.gate_out = nullptr;
-    slow<<<h->slow_ctas, 32, plan.base_smem, stream>>>(dv, s);
-    h->launches++;
-    GB_CUDA(cudaGetLastError());
-    return GRANNE_B200_OK;
+    return launch_warps<slow>(h, h->slow_ctas, plan.engine.base_smem, stream, dv, s);
 }
-
-// The search passes for the engine DistDispatch picks.  `d`: the staged index the kernels see — the handle's own, or a
-// private view of it (compute_order searches single layers without touching the shared handle)
-struct SearchLaunch {
-    Handle* h;
-    Workspace* w;
-    const gb::SearchArgs& a;
-    const LaunchPlan& plan;
-    cudaStream_t stream;
-    const gb::DeviceIndex& d;
-    template <class Dist>
-    int run() {
-        switch (plan.rows) {
-            case 3: return launch_kernels<Dist, 3>(h, w, a, plan, stream, d);
-            case 7: return launch_kernels<Dist, 7>(h, w, a, plan, stream, d);
-            case 15: return launch_kernels<Dist, 15>(h, w, a, plan, stream, d);
-            case 31: return launch_kernels<Dist, 31>(h, w, a, plan, stream, d);
-            default: return launch_kernels<Dist, 0>(h, w, a, plan, stream, d);
-        }
-    }
-};
 
 // ---- workspace pool -----------------------------------------------------------------------------------------------
 int ws_acquire(Handle* h, std::unique_ptr<Workspace>* out) {
@@ -952,12 +957,21 @@ int enqueue_search(Handle* h, Workspace* w, const void* d_queries, size_t nq, in
     a.slow_vis_slots = h->slow_vis_slots;
     a.pass = a.slow_pass = a.final_pass = 0;
     a.pg = pg ? device_gather(*pg, w->d_counters.get() + 5) : gb::PeerGather{};
-    a.stg_rows = plan.stg_rows;
-    a.stg_row_bytes = plan.stg_row_bytes;
-    a.tile_rows = plan.tile_rows;
+    a.tiles = plan.engine.tiles;
     a.vis_global = nullptr;
+    // the staged index the kernels see: the handle's own, or a private view of it (compute_order searches single
+    // layers without touching the shared handle)
     const gb::DeviceIndex& dv = view ? *view : h->dev;
-    rc = DistDispatch::call(dv, SearchLaunch{h, w, a, plan, stream, dv});
+    rc = DistDispatch::call(dv, [&](auto e) {
+        using Dist = typename decltype(e)::type;
+        switch (plan.rows) {
+            case 3: return launch_kernels<Dist, 3>(h, w, a, plan, stream, dv);
+            case 7: return launch_kernels<Dist, 7>(h, w, a, plan, stream, dv);
+            case 15: return launch_kernels<Dist, 15>(h, w, a, plan, stream, dv);
+            case 31: return launch_kernels<Dist, 31>(h, w, a, plan, stream, dv);
+            default: return launch_kernels<Dist, 0>(h, w, a, plan, stream, dv);
+        }
+    });
     if (rc) return rc;
     GB_CUDA(cudaMemcpyAsync(w->h_retried.get(), w->d_retried.get(), 8, cudaMemcpyDeviceToHost, stream));
     return GRANNE_B200_OK;
@@ -1243,34 +1257,6 @@ int validate_rerank(const Handle* h, const void* q, size_t nq, int fmt, uint32_t
     return GRANNE_B200_OK;
 }
 
-// rerank_kernel for the engine DistDispatch picks for the re-rank container: the f32 engine for the width of angular
-// rows, DistSum for a SumEmbeddings container (never the i8 engine: no container is staged as angular_int).
-struct RerankLaunch {
-    Handle* h;
-    const gb::RerankArgs& a;
-    size_t smem;
-    cudaStream_t stream;
-    template <class Dist>
-    int run() {
-        if constexpr (std::is_same<Dist, gb::DistI8>::value) {
-            return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "re-rank container must be angular f32 rows or SumEmbeddings");
-        } else {
-            auto kern = gb::rerank_kernel<Dist>;
-            static std::atomic<bool> attr_set[64];  // function attributes are per device
-            int rc = set_smem_attr(kern, h, &attr_set[h->device & 63]);
-            if (rc) return rc;
-            int occ = 0;
-            GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, 32, smem));
-            if (occ < 1) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "re-rank workspace exceeds shared memory");
-            const unsigned grid = (unsigned)std::min<unsigned long long>(a.nq, (unsigned long long)occ * h->num_sms);
-            kern<<<grid, 32, smem, stream>>>(h->rerank, a);
-            h->launches++;
-            GB_CUDA(cudaGetLastError());
-            return GRANNE_B200_OK;
-        }
-    }
-};
-
 // Enqueues one two-stage search on `stream`: stage 1 is enqueue_search with k = C into the workspace's candidate
 // block, stage 2 is rerank_kernel over h->rerank into the caller's outputs.  Stage 1 writes `d_stats` as search does.
 int enqueue_rerank(Handle* h, Workspace* w, const void* d_queries, size_t nq, uint32_t max_search, uint32_t c,
@@ -1283,7 +1269,7 @@ int enqueue_rerank(Handle* h, Workspace* w, const void* d_queries, size_t nq, ui
     if ((rc = enqueue_search(h, w, d_queries, nq, GRANNE_B200_QUERY_RAW_F32, max_search, c, cand_ids,
                              reinterpret_cast<float*>(cand_ids + nq * c), cand_counts, d_stats, stream, reset_error)))
         return rc;
-    const LaunchPlan plan = make_plan(h, 1, &h->rerank);
+    const EngineTiles eng = engine_tiles(h->rerank);
     gb::RerankArgs a{};
     a.queries = static_cast<const float*>(d_queries);
     a.nq = nq;
@@ -1296,58 +1282,28 @@ int enqueue_rerank(Handle* h, Workspace* w, const void* d_queries, size_t nq, ui
     a.out_counts = d_counts;
     a.work_counter = w->d_counters.get() + 6;  // zeroed by enqueue_search's memset on this stream
     a.error_flag = w->d_error;
-    a.stg_rows = plan.stg_rows;
-    a.stg_row_bytes = plan.stg_row_bytes;
-    a.tile_rows = plan.tile_rows;
-    // the keys start on the first 16-byte boundary behind the engine's SmemLayout (rerank_kernel)
-    const size_t smem = ((plan.base_smem + 15) & ~size_t(15)) + (size_t)gb::rerank_key_slots(c) * 8;
-    return DistDispatch::call(h->rerank, RerankLaunch{h, a, smem, stream});
-}
-
-// ---- GranneBuilder (src/index/mod.rs:295-531, 645-960) on the device ---------------------------------------------
-struct PairLaunch {
-    Handle* h;
-    gb::PairArgs a;
-    size_t smem;
-    unsigned grid;
-    cudaStream_t stream;
-    template <class Dist>
-    int run() {
-        auto k = gb::pair_distance_kernel<Dist>;
-        GB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_optin));
-        k<<<grid, 32, smem, stream>>>(h->dev, a);
-        h->launches++;
-        GB_CUDA(cudaGetLastError());
-        return GRANNE_B200_OK;
-    }
-};
-
-struct LinkLaunch {
-    Handle* h;
-    gb::BuildArgs a;
-    size_t smem;
-    unsigned grid;
-    cudaStream_t stream;
-    bool prune;
-    template <class Dist>
-    int run() {
-        if (prune) {
-            auto k = gb::build_prune_kernel<Dist>;
-            GB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_optin));
-            k<<<grid, 32, smem, stream>>>(h->dev, a);
+    a.tiles = eng.tiles;
+    const size_t smem = gb::rerank_keys_offset(eng.base_smem) + (size_t)gb::rerank_key_slots(c) * 8;
+    // the f32 engine for the width of angular rows, DistSum for a SumEmbeddings container (never the i8 engine: no
+    // container is staged as angular_int)
+    return DistDispatch::call(h->rerank, [&](auto e) {
+        using Dist = typename decltype(e)::type;
+        if constexpr (std::is_same<Dist, gb::DistI8>::value) {
+            return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "re-rank container must be angular f32 rows or SumEmbeddings");
         } else {
-            auto k = gb::build_link_kernel<Dist>;
-            GB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_optin));
-            k<<<grid, 32, smem, stream>>>(h->dev, a);
+            int occ = 0;
+            const int err = resident_ctas<gb::rerank_kernel<Dist>>(h, smem, &occ);
+            if (err) return err;
+            if (occ < 1) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "re-rank workspace exceeds shared memory");
+            const unsigned grid = (unsigned)std::min<unsigned long long>(a.nq, (unsigned long long)occ * h->num_sms);
+            return launch_warps<gb::rerank_kernel<Dist>>(h, grid, smem, stream, h->rerank, a);
         }
-        h->launches++;
-        GB_CUDA(cudaGetLastError());
-        return GRANNE_B200_OK;
-    }
-};
+    });
+}
 
 }  // namespace
 
+// ---- GranneBuilder (src/index/mod.rs:295-531, 645-960) on the device ---------------------------------------------
 struct granne_b200_builder {
     std::unique_ptr<Handle> h;  // search view over the layers built so far (+ the one under construction)
     granne_b200_build_config cfg{};
@@ -1373,8 +1329,7 @@ int builder_index_elements(Builder* b, uint32_t layer_m, uint32_t ef, uint64_t a
     const int cur = d.num_layers - 1;
     uint32_t* rows = const_cast<uint32_t*>(d.layer_rows[cur]);
     cudaStream_t stream = b->ws->stream.get();
-    const LaunchPlan plan = make_plan(h, ef);
-    if (plan.smem == 0) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "max_search too large");
+    if (make_plan(h, ef).smem == 0) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "max_search too large");
     const uint64_t first = reinsert ? 0 : already;
     const uint64_t total = num - first;
     // test knob: GRANNE_B200_BUILD_MAX_BATCH=1 makes every insertion see all earlier links, i.e. the reference's
@@ -1393,8 +1348,26 @@ int builder_index_elements(Builder* b, uint32_t layer_m, uint32_t ef, uint64_t a
         (rc = b->d_locks.grow(num, stream)) || (rc = b->d_counter.grow(4, stream)))
         return rc;
     GB_CUDA(cudaMemsetAsync(b->d_locks.get(), 0, num * sizeof(int), stream));
-    const size_t link_smem = plan.base_smem + gb::link_scratch_bytes(gb::link_cand_cap(ef, b->cfg.num_neighbors),
-                                                                      b->cfg.num_neighbors);
+    // shared memory: the engine's SmemLayout, then the link scratch for ef candidates (link) or a node's row (prune)
+    const uint32_t nn = b->cfg.num_neighbors;
+    const EngineTiles eng = engine_tiles(d);
+    const size_t link_smem = gb::LinkLayout<size_t>(eng.base_smem, gb::link_cand_cap(ef, nn), nn).end;
+    const size_t prune_smem = gb::LinkLayout<size_t>(eng.base_smem, gb::link_cand_cap(0, nn), nn).end;
+    gb::BuildArgs prune{};
+    prune.rows = rows;
+    prune.stride = b->stride;
+    prune.node_width = nn;
+    prune.max_neighbors = layer_m;
+    prune.tiles = eng.tiles;
+    prune.work_counter = b->d_counter.get();
+    prune.num_nodes = (uint32_t)num;
+    gb::BuildArgs link = prune;  // the prune pass's arguments and a batch's candidates
+    link.ids = b->d_ids.get();
+    link.cand_ids = b->d_cand_ids.get();
+    link.cand_dists = b->d_cand_d.get();
+    link.cand_counts = b->d_cand_cnt.get();
+    link.cand_stride = ef;
+    link.locks = b->d_locks.get();
     uint64_t pos = 0;
     while (pos < total) {
         // nodes already linked into this layer: a batch never exceeds 1/16 of them (its members do not see each other)
@@ -1409,42 +1382,21 @@ int builder_index_elements(Builder* b, uint32_t layer_m, uint32_t ef, uint64_t a
                             b->d_cand_d.get(), b->d_cand_cnt.get(), nullptr, stream, false);
         if (rc) return rc;
         GB_CUDA(cudaMemsetAsync(b->d_counter.get(), 0, 16, stream));
-        LinkLaunch L{h, {}, link_smem, 0, stream, false};
-        L.a.ids = b->d_ids.get();
-        L.a.n_batch = (uint32_t)bsz;
-        L.a.cand_ids = b->d_cand_ids.get();
-        L.a.cand_dists = b->d_cand_d.get();
-        L.a.cand_counts = b->d_cand_cnt.get();
-        L.a.cand_stride = ef;
-        L.a.rows = rows;
-        L.a.stride = b->stride;
-        L.a.node_width = b->cfg.num_neighbors;
-        L.a.max_neighbors = layer_m;
-        L.a.locks = b->d_locks.get();
-        L.a.stg_rows = plan.stg_rows;
-        L.a.stg_row_bytes = plan.stg_row_bytes;
-        L.a.tile_rows = plan.tile_rows;
-        L.a.work_counter = b->d_counter.get();
-        L.a.num_nodes = (uint32_t)num;
-        L.grid = (unsigned)std::min<uint64_t>(bsz, link_warps);
-        if ((rc = DistDispatch::call(d, L))) return rc;
+        link.n_batch = (uint32_t)bsz;
+        const unsigned grid = (unsigned)std::min<uint64_t>(bsz, link_warps);
+        rc = DistDispatch::call(d, [&](auto e) {
+            return launch_warps<gb::build_link_kernel<typename decltype(e)::type>>(h, grid, link_smem, stream, d, link);
+        });
+        if (rc) return rc;
         pos += bsz;
     }
     // limit number of neighbors (:794-797)
     GB_CUDA(cudaMemsetAsync(b->d_counter.get(), 0, 16, stream));
-    LinkLaunch P{h, {}, plan.base_smem + gb::link_scratch_bytes(gb::link_cand_cap(0, b->cfg.num_neighbors),
-                                                               b->cfg.num_neighbors), 0, stream, true};
-    P.a.rows = rows;
-    P.a.stride = b->stride;
-    P.a.node_width = b->cfg.num_neighbors;
-    P.a.max_neighbors = layer_m;
-    P.a.stg_rows = plan.stg_rows;
-    P.a.stg_row_bytes = plan.stg_row_bytes;
-    P.a.tile_rows = plan.tile_rows;
-    P.a.work_counter = b->d_counter.get();
-    P.a.num_nodes = (uint32_t)num;
-    P.grid = (unsigned)std::min<uint64_t>(num, (uint64_t)h->num_sms * 8);
-    if ((rc = DistDispatch::call(d, P))) return rc;
+    const unsigned grid = (unsigned)std::min<uint64_t>(num, (uint64_t)h->num_sms * 8);
+    rc = DistDispatch::call(d, [&](auto e) {
+        return launch_warps<gb::build_prune_kernel<typename decltype(e)::type>>(h, grid, prune_smem, stream, d, prune);
+    });
+    if (rc) return rc;
     GB_CUDA(cudaStreamSynchronize(stream));
     int herr[4] = {0, 0, 0, 0};
     GB_CUDA(cudaMemcpy(herr, b->ws->d_error, sizeof(herr), cudaMemcpyDeviceToHost));
@@ -2340,7 +2292,6 @@ int granne_b200_compute_distances(int element_kind, const float* a, const float*
                             &raw_h)))
             return rc;
         std::unique_ptr<Handle, void (*)(Handle*)> h(raw_h, [](Handle* p) { granne_b200_close(p); });
-        const LaunchPlan plan = make_plan(h.get(), 1);
         GB_DEVICE(device);
         Buffer<float> d_a, d_out;
         Buffer<int> d_err;
@@ -2348,16 +2299,20 @@ int granne_b200_compute_distances(int element_kind, const float* a, const float*
             return rc;
         GB_CUDA(cudaMemcpy(d_a.get(), a, (size_t)n * dim * 4, cudaMemcpyHostToDevice));
         GB_CUDA(cudaMemset(d_err.get(), 0, 4));
-        PairLaunch L{h.get(), {}, plan.base_smem + gb::link_scratch_bytes(8, 32), 0, nullptr};
-        L.a.queries = d_a.get();
-        L.a.n = (uint32_t)n;
-        L.a.out = d_out.get();
-        L.a.error_flag = d_err.get();
-        L.a.stg_rows = plan.stg_rows;
-        L.a.stg_row_bytes = plan.stg_row_bytes;
-        L.a.tile_rows = plan.tile_rows;
-        L.grid = (unsigned)std::min<uint64_t>(n, (uint64_t)h->num_sms * 16);
-        if ((rc = DistDispatch::call(h->dev, L))) return rc;
+        const EngineTiles eng = engine_tiles(h->dev);
+        gb::PairArgs args{};
+        args.queries = d_a.get();
+        args.n = (uint32_t)n;
+        args.out = d_out.get();
+        args.error_flag = d_err.get();
+        args.tiles = eng.tiles;
+        const unsigned grid = (unsigned)std::min<uint64_t>(n, (uint64_t)h->num_sms * 16);
+        const size_t smem = gb::LinkLayout<size_t>(eng.base_smem, 8, 32).end;  // pair_distance_kernel's setup_ctx
+        rc = DistDispatch::call(h->dev, [&](auto e) {
+            return launch_warps<gb::pair_distance_kernel<typename decltype(e)::type>>(h.get(), grid, smem, nullptr,
+                                                                                     h->dev, args);
+        });
+        if (rc) return rc;
         GB_CUDA(cudaDeviceSynchronize());
         int herr = 0;
         GB_CUDA(cudaMemcpy(&herr, d_err.get(), 4, cudaMemcpyDeviceToHost));

@@ -27,6 +27,10 @@ __host__ __device__ constexpr uint32_t rerank_key_slots(uint32_t c) {
     return p;
 }
 
+// Where a warp's keys start in its shared window: the first 16-byte boundary behind the engine's SmemLayout, which
+// ends `layout_end` bytes in.
+__host__ __device__ constexpr size_t rerank_keys_offset(size_t layout_end) { return (layout_end + 15) & ~(size_t)15; }
+
 struct RerankArgs {
     const float* queries;        // nq x dim raw f32
     unsigned long long nq;
@@ -39,7 +43,7 @@ struct RerankArgs {
     uint32_t* out_counts;        // nq (or null)
     unsigned int* work_counter;  // zeroed before the launch
     int* error_flag;             // kStatusNotFinite is or-ed in on a NaN distance
-    uint32_t stg_rows, stg_row_bytes, tile_rows;  // the engine's staging and ordered-sum tiles (make_plan)
+    WarpTiles tiles;
 };
 
 // Ascending sort of keys[0, p) (p a power of two) by the warp.  The pairs (i, i ^ j) of one step are disjoint, so a
@@ -67,8 +71,8 @@ __global__ void __launch_bounds__(32) rerank_kernel(const DeviceIndex ix, const 
     extern __shared__ __align__(16) unsigned char smem_raw[];
     WarpCtx c;
     c.lane = threadIdx.x;
-    const unsigned char* end = place_warp_smem(c, smem_raw, ix, a.tile_rows, a.stg_rows, a.stg_row_bytes);
-    unsigned long long* keys = reinterpret_cast<unsigned long long*>(smem_raw + (((end - smem_raw) + 15) & ~15));
+    const unsigned char* end = place_warp_smem(c, smem_raw, ix, a.tiles);
+    unsigned long long* keys = reinterpret_cast<unsigned long long*>(smem_raw + rerank_keys_offset(end - smem_raw));
     SearchArgs q{};
     q.queries = a.queries;
     q.query_format = kQueryRawF32;

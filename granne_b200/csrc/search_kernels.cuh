@@ -62,13 +62,21 @@ __host__ __device__ constexpr uint32_t tile_bytes_for_rows(uint32_t rows) {
 enum ElementKind : int { kAngularF32 = 0, kAngularI8 = 1, kSumEmbeddings = 2 };
 enum QueryFormat : int { kQueryRawF32 = 0, kQueryElement = 1, kQueryById = 2 };  // ById: builder only (u32 ids)
 
-// Shared-memory layout of one warp in the dynamic window: the host sizes every launch from it, the build kernels place
-// their pointers with it (place_warp_smem), and search_kernel spells out the same walk:
+// The staging and ordered-sum tiles of the engine that serves a container (picked on the host by engine_tiles); the
+// argument struct of every one-warp kernel carries them.
+struct WarpTiles {
+    uint32_t stg_rows;       // candidate rows per staged batch (0 = this element kind loads directly)
+    uint32_t stg_row_bytes;  // bytes of one staged row (f32: 128*FULL, i8: a 512-byte pass slot, embeddings: one sum)
+    uint32_t tile_rows;      // rows of the ordered-sum tile (0 for i8, which has none)
+};
+
+// Shared-memory layout of one warp in the dynamic window: the host sizes every launch from it, the build and re-rank
+// kernels place their pointers with it (place_warp_smem), and search_kernel spells out the same walk:
 //   tile (ordered-sum rows) + id scratch | reserved 16 bytes | qs | xs (embeddings only) | staging tile | end
 // qs holds the query (f32 dim rounded up to 4 floats, or the row_stride bytes of an i8 row), xs one element of the same
 // size; both start on 16-byte boundaries, the staging tile (stg_rows x stg_row_bytes) on a 128-byte boundary.  Behind
-// `end` each kernel appends its own: the fast list, or the generic list and visited set (search_kernel), or the link
-// scratch (build kernels).
+// `end` each kernel appends its own: the fast list, or the generic list and visited set (search_kernel), the link
+// scratch (build kernels: LinkLayout), or the sort keys (rerank_kernel: rerank_keys_offset).
 // The layout is walked from `base` in the address type P: the host walks byte offsets (P = size_t, base = 0), the
 // kernels walk their shared window (P = unsigned char*, base = smem_raw), so that every pointer is smem_raw + offset
 // and the compiler keeps the accesses in the shared address space (LDS/STS with 32-bit addresses).
@@ -80,10 +88,10 @@ struct SmemLayout {
     P ids, qs, xs, stg, end;  // stg = P() without a staging tile
 
     __host__ __device__ __forceinline__ SmemLayout(P base, int kind, uint32_t dim, uint32_t row_stride,
-                                                   uint32_t tile_rows, uint32_t stg_rows, uint32_t stg_row_bytes) {
+                                                   const WarpTiles& t) {
         P sp = base;  // the tile starts at base
-        ids = sp + tile_bytes_for_rows(tile_rows) - kIdScratchBytes;
-        sp += tile_bytes_for_rows(tile_rows);
+        ids = sp + tile_bytes_for_rows(t.tile_rows) - kIdScratchBytes;
+        sp += tile_bytes_for_rows(t.tile_rows);
         sp += kReservedBytes;
         const uint32_t slot_bytes = (kind == kAngularI8) ? row_stride : ((dim + 3u) & ~3u) * 4u;
         qs = sp;
@@ -91,10 +99,10 @@ struct SmemLayout {
         xs = sp;
         if (kind == kSumEmbeddings) sp += (slot_bytes + 15u) & ~15u;
         stg = P();
-        if (stg_rows) {
+        if (t.stg_rows) {
             sp = base + (((size_t)(sp - base) + 127u) & ~(size_t)127u);
             stg = sp;
-            sp += (size_t)stg_rows * stg_row_bytes;
+            sp += (size_t)t.stg_rows * t.stg_row_bytes;
         }
         end = sp;
     }
@@ -149,9 +157,7 @@ struct SearchArgs {
     uint32_t vis_slots;       // visited slots for the bottom layer
     uint32_t vis_slots_upper; // visited slots for the max_search = 1 descents
     uint32_t* vis_global;     // fast pass: one table of vis_slots u32 per CTA in global memory (L2 resident)
-    uint32_t stg_rows;        // candidate rows per staged batch (0 = this element kind loads directly)
-    uint32_t stg_row_bytes;   // bytes of one staged row (f32: 128*FULL, i8: row_stride)
-    uint32_t tile_rows;       // rows of the ordered-sum tile (8 for the staged f32 engine, 32 generic, 0 unused)
+    WarpTiles tiles;
     uint32_t* out_ids;
     float* out_dists;
     uint32_t* out_counts;
@@ -239,16 +245,16 @@ __device__ __forceinline__ unsigned long long make_policy_evict_last() {
 
 // Points the warp's shared buffers into smem_raw as SmemLayout places them; returns the first byte behind them.
 __device__ __forceinline__ unsigned char* place_warp_smem(WarpCtx& c, unsigned char* smem_raw, const DeviceIndex& ix,
-                                                          uint32_t tile_rows, uint32_t stg_rows, uint32_t stg_row_bytes) {
-    const SmemLayout<unsigned char*> L(smem_raw, ix.kind, ix.dim, ix.row_stride, tile_rows, stg_rows, stg_row_bytes);
+                                                          const WarpTiles& t) {
+    const SmemLayout<unsigned char*> L(smem_raw, ix.kind, ix.dim, ix.row_stride, t);
     c.tile = reinterpret_cast<float*>(smem_raw);
     c.ids = reinterpret_cast<uint32_t*>(L.ids);
     c.pol_keep = make_policy_evict_last();
     c.qs = reinterpret_cast<float*>(L.qs);
     c.xs = reinterpret_cast<float*>(L.xs);
     c.stg = L.stg;
-    c.stg_rows = stg_rows;
-    c.stg_row_bytes = stg_row_bytes;
+    c.stg_rows = t.stg_rows;
+    c.stg_row_bytes = t.stg_row_bytes;
     return L.end;
 }
 
@@ -1539,8 +1545,8 @@ __global__ void __launch_bounds__(32, R > 0 ? GB_MIN_BLOCKS : 1) search_kernel(c
     // differently scheduled prologue, and this kernel runs at its register cap.
     unsigned char* sp = smem_raw;
     c.tile = reinterpret_cast<float*>(sp);
-    c.ids = reinterpret_cast<uint32_t*>(sp + tile_bytes_for_rows(a.tile_rows) - kIdScratchBytes);
-    sp += tile_bytes_for_rows(a.tile_rows);
+    c.ids = reinterpret_cast<uint32_t*>(sp + tile_bytes_for_rows(a.tiles.tile_rows) - kIdScratchBytes);
+    sp += tile_bytes_for_rows(a.tiles.tile_rows);
     c.pol_keep = make_policy_evict_last();
     sp += SmemLayout<unsigned char*>::kReservedBytes;
     const uint32_t qbytes = (ix.kind == kAngularI8) ? ix.row_stride : ((ix.dim + 3u) & ~3u) * 4u;
@@ -1549,12 +1555,12 @@ __global__ void __launch_bounds__(32, R > 0 ? GB_MIN_BLOCKS : 1) search_kernel(c
     c.xs = reinterpret_cast<float*>(sp);
     if (ix.kind == kSumEmbeddings) sp += (qbytes + 15u) & ~15u;
     c.stg = nullptr;
-    c.stg_rows = a.stg_rows;
-    c.stg_row_bytes = a.stg_row_bytes;
-    if (a.stg_rows) {  // staging tile: gathered candidate rows (f32 / i8) or summed candidate vectors (embeddings)
+    c.stg_rows = a.tiles.stg_rows;
+    c.stg_row_bytes = a.tiles.stg_row_bytes;
+    if (a.tiles.stg_rows) {  // staging tile: gathered candidate rows (f32 / i8) or summed candidates (embeddings)
         sp = smem_raw + (((size_t)(sp - smem_raw) + 127u) & ~(size_t)127u);
         c.stg = sp;
-        sp += (size_t)a.stg_rows * a.stg_row_bytes;
+        sp += (size_t)a.tiles.stg_rows * a.tiles.stg_row_bytes;
     }
     // the fast list always lives in this CTA's shared window (derived from smem_raw only, so that the compiler keeps
     // its accesses in the shared address space: LDS/STS with 32-bit addresses)

@@ -2,7 +2,7 @@
 reach (GPU).  Each case runs raw queries and `already_element` queries through search_kernel and compares them with
 the oracle: same ids, bit-identical distances, same counts and counters.
 
-Engine selection (granne_b200.cu, make_plan / dispatch_search): f32 rows use DistF32<FULL> (FULL = dim / 32 in
+Engine selection (granne_b200.cu, DistDispatch / engine_tiles): f32 rows use DistF32<FULL> (FULL = dim / 32 in
 {0..4, 6, 8} with 4-float groups), else DistF32Generic, which stages rows of up to 64 32-float chunks (dim < 2080) and
 loads wider rows directly; i8 rows use DistI8 (lanes per row by row bytes, a separate path beyond 512 bytes); sums of
 embeddings use DistSum (128 floats per pass, 32 terms per id load)."""
