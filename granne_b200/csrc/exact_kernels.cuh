@@ -7,9 +7,9 @@
 //
 // A call runs in query chunks (at most kExactMaxChunk queries) and row slabs (rows whose distances fit the slab
 // buffer):
-//   exact_prepare_kernel    the queries as elements (prepare_query's arithmetic: normalise or quantise)
+//   exact_prepare_kernel    the queries as elements (prepare_query: normalise or quantise)
 //   exact_scan_f32_kernel   distances of a chunk x slab into the slab buffer, CUDA-core FMAs in the reference order
-//   exact_scan_i8_kernel    the same for i8 rows: exact integer dot products, DistI8::finish's epilogue
+//   exact_scan_i8_kernel    the same for i8 rows: exact integer dot products, then finish_angular_i8
 //   exact_select_kernel     per query: keys of the slab below the running k-th key join the running top-k list
 //   exact_write_kernel      the lists into the search_batch output layout
 // EMBEDDINGS rows are materialised window by window by sum_embeddings_kernel + make_elements_kernel and scanned as
@@ -47,63 +47,27 @@ struct ExactScanArgs {
     int* error;           // kStatusNotFinite is or-ed in on a NaN distance
 };
 
-// The queries of a chunk as elements, one warp per query: prepare_query's arithmetic.  f32 kinds: [nq][dim] (RAW_F32
-// normalised with normalize_f32); i8: [nq][row_stride] zero padded (RAW_F32 quantised with quantize_i8) and dy.
+// The queries of a chunk as elements, one warp per query: prepare_query writes each one to its row of `out` instead
+// of a search warp's query slot.  f32 kinds: [nq][dim]; i8: [nq][row_stride] zero padded, and dy.
 __global__ void __launch_bounds__(32) exact_prepare_kernel(const DeviceIndex ix, const void* __restrict__ queries,
                                                             int fmt, uint32_t nq, void* __restrict__ out,
                                                             int* __restrict__ qnorm, int* __restrict__ error) {
-    const int lane = threadIdx.x;
-    const uint32_t dim = ix.dim;
+    const bool i8 = ix.kind == kAngularI8;
+    SearchArgs q{};
+    q.queries = queries;
+    q.query_format = fmt;  // kQueryRawF32 or kQueryElement
+    WarpCtx c;
+    c.lane = threadIdx.x;
     for (uint32_t qi = blockIdx.x; qi < nq; qi += gridDim.x) {
-        if (ix.kind == kAngularI8) {
-            int8_t* qb = static_cast<int8_t*>(out) + (size_t)qi * ix.row_stride;
-            int* qw = reinterpret_cast<int*>(qb);
-            const int words = ix.row_stride / 4;
-            for (int w = lane; w < words; w += 32) qw[w] = 0;
-            __syncwarp();
-            int status = 0;
-            if (fmt == kQueryElement) {
-                const int8_t* src = static_cast<const int8_t*>(queries) + (size_t)qi * dim;
-                for (uint32_t i = lane; i < dim; i += 32) qb[i] = src[i];
-            } else {
-                quantize_i8(static_cast<const float*>(queries) + (size_t)qi * dim, qb, dim, lane, &status);
-            }
-            __syncwarp();
-            int dy = 0;
-            for (int w = lane; w < words; w += 32) dy = __dp4a(qw[w], qw[w], dy);
-            dy = __reduce_add_sync(kFullMask, dy);
-            if (lane == 0) {
-                qnorm[qi] = dy;
-                if (status) atomicOr(error, status);
-            }
-        } else {
-            float* x = static_cast<float*>(out) + (size_t)qi * dim;
-            const float* src = static_cast<const float*>(queries) + (size_t)qi * dim;
-            for (uint32_t i = lane; i < dim; i += 32) x[i] = src[i];
-            __syncwarp();
-            if (fmt == kQueryRawF32) normalize_f32(x, dim, (int)ix.full, lane);  // Vector::from (angular.rs:55-61)
+        c.qs = i8 ? reinterpret_cast<float*>(static_cast<int8_t*>(out) + (size_t)qi * ix.row_stride)
+                  : static_cast<float*>(out) + (size_t)qi * ix.dim;
+        c.status = 0;
+        prepare_query(ix, q, c, qi);
+        if (c.lane == 0 && i8) {
+            qnorm[qi] = c.q_norm_i8;
+            if (c.status) atomicOr(error, c.status);
         }
     }
-}
-
-// finish_angular (search_kernels.cuh) restated: cmp::max(0.0, 1.0 - r) with NaN detection (angular.rs:70-73).
-__device__ __forceinline__ float exact_finish_angular(float r, int* status) {
-    float d = __fsub_rn(1.0f, r);
-    if (d != d) {
-        *status |= kStatusNotFinite;
-        return 0.0f;
-    }
-    return (0.0f <= d) ? d : 0.0f;
-}
-
-// DistI8::finish (search_kernels.cuh) restated: 1 - r / (sqrt(dx) * sqrt(dy)) in IEEE f32, NaN -> 0, max(0, .)
-// (angular_int.rs:47-59).
-__device__ __forceinline__ float exact_finish_i8(int r, int dx, int dy) {
-    const float rf = (float)r, dxf = (float)dx, dyf = (float)dy;
-    float qq = __fdiv_rn(rf, __fmul_rn(__fsqrt_rn(dxf), __fsqrt_rn(dyf)));
-    if (qq != qq) qq = 0.0f;  // NotNan::new(..).unwrap_or_else(|_| 0.0)
-    const float dd = __fsub_rn(1.0f, qq);
-    return (0.0f <= dd) ? dd : 0.0f;
 }
 
 // f32 distances of kExactQB queries x kExactRB rows per block; thread (tq, tr) owns 4 queries x 8 rows.
@@ -200,7 +164,7 @@ __global__ void __launch_bounds__(256, 2) exact_scan_f32_kernel(const ExactScanA
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
             const unsigned long long row = r0 + tr * 8 + j;
-            const float d = exact_finish_angular(r[i][j], &status);
+            const float d = finish_angular(r[i][j], &status);
             if (q < a.nq && row < a.nrows) a.dists[(size_t)q * a.ld + row] = d;
         }
     }
@@ -210,7 +174,7 @@ __global__ void __launch_bounds__(256, 2) exact_scan_f32_kernel(const ExactScanA
 
 // i8 distances of kExactQB queries x kExactRB rows per block: r over the 32-bit words of the padded rows with dp4a
 // (integer sums: any order is exact), dx of every row computed once per block by the warp that stages it, then
-// DistI8::finish's IEEE sequence.  dx is computed per tile rather than cached per handle: it costs one dp4a per staged
+// finish_angular_i8, DistI8's IEEE sequence.  dx is computed per tile rather than cached per handle: it costs one dp4a per staged
 // word, needs no state on the handle and stays right when a builder appends rows.
 __global__ void __launch_bounds__(256, 2) exact_scan_i8_kernel(const ExactScanArgs a) {
     __shared__ __align__(16) int Qs[kExactBK][kExactQB + 4];
@@ -277,7 +241,7 @@ __global__ void __launch_bounds__(256, 2) exact_scan_i8_kernel(const ExactScanAr
         for (int j = 0; j < 8; ++j) {
             const int row = tr * 8 + j;
             if (q < a.nq && r0 + row < a.nrows)
-                a.dists[(size_t)q * a.ld + r0 + row] = exact_finish_i8(acc[i][j], dxs[row], dy);
+                a.dists[(size_t)q * a.ld + r0 + row] = finish_angular_i8(acc[i][j], dxs[row], dy);
         }
     }
 }

@@ -218,6 +218,16 @@ __device__ __forceinline__ float finish_angular(float r, int* status) {
     return (0.0f <= d) ? d : 0.0f;
 }
 
+// The angular_int distance from r = dot(x, y), dx = dot(x, x) and dy = dot(y, y): 1 - r / (sqrt(dx) * sqrt(dy)) in
+// IEEE f32, NaN -> 0, max(0, .) (angular_int.rs:47-59).
+__device__ __forceinline__ float finish_angular_i8(int r, int dx, int dy) {
+    const float rf = (float)r, dxf = (float)dx, dyf = (float)dy;
+    float qq = __fdiv_rn(rf, __fmul_rn(__fsqrt_rn(dxf), __fsqrt_rn(dyf)));
+    if (qq != qq) qq = 0.0f;  // NotNan::new(..).unwrap_or_else(|_| 0.0)
+    const float dd = __fsub_rn(1.0f, qq);
+    return (0.0f <= dd) ? dd : 0.0f;
+}
+
 // Per-warp working set (pointers may be shared or global memory: the slow path uses global workspaces).
 struct WarpCtx {
     unsigned long long* list;  // L
@@ -583,13 +593,7 @@ struct DistI8 {
 
     __device__ __forceinline__ float finish(const WarpCtx& c, int my_r, int my_dx, bool live) const {
         float d = 0.0f;
-        if (live) {
-            const float rf = (float)my_r, dxf = (float)my_dx, dyf = (float)c.q_norm_i8;
-            float qq = __fdiv_rn(rf, __fmul_rn(__fsqrt_rn(dxf), __fsqrt_rn(dyf)));
-            if (qq != qq) qq = 0.0f;  // NotNan::new(..).unwrap_or_else(|_| 0.0)
-            const float dd = __fsub_rn(1.0f, qq);
-            d = (0.0f <= dd) ? dd : 0.0f;
-        }
+        if (live) d = finish_angular_i8(my_r, my_dx, c.q_norm_i8);
         return d;
     }
 
