@@ -106,6 +106,14 @@ extern "C" {
         m: *mut RawMulti, queries: *const c_void, nq: usize, query_format: c_int, num_neighbors: u32,
         out_ids: *mut u64, out_dists: *mut f32, out_counts: *mut u32,
     ) -> c_int;
+    fn granne_b200_exact_search_within_batch(
+        h: *mut RawIndex, queries: *const c_void, nq: usize, query_format: c_int, offsets: *const u64,
+        ids: *const u32, num_neighbors: u32, out_ids: *mut u32, out_dists: *mut f32, out_counts: *mut u32,
+    ) -> c_int;
+    fn granne_b200_multi_exact_search_within_batch(
+        m: *mut RawMulti, queries: *const c_void, nq: usize, query_format: c_int, offsets: *const u64,
+        ids: *const u64, num_neighbors: u32, out_ids: *mut u64, out_dists: *mut f32, out_counts: *mut u32,
+    ) -> c_int;
     fn granne_b200_set_rerank_elements(h: *mut RawIndex, elements: *const c_void, elements_len: usize) -> c_int;
     fn granne_b200_search_rerank_batch(
         h: *mut RawIndex, queries: *const f32, nq: usize, query_format: c_int, max_search: u32, num_candidates: u32,
@@ -273,6 +281,38 @@ impl GpuGranne {
             granne_b200_exact_search_batch(
                 self.h, queries.as_ptr() as *const c_void, nq, query_format, num_neighbors as u32, ids.as_mut_ptr(),
                 dists.as_mut_ptr(), counts.as_mut_ptr(),
+            )
+        });
+        (0..nq)
+            .map(|q| {
+                (0..counts[q] as usize)
+                    .map(|j| (ids[q * num_neighbors + j] as usize, dists[q * num_neighbors + j]))
+                    .collect()
+            })
+            .collect()
+    }
+
+    /// Exact k nearest neighbours of each query within its own candidate list (not a reference function):
+    /// `lists[q]` holds query q's ids (< `len()`; duplicates count once); the first min(k, |set(lists[q])|) by
+    /// (distance, id), the reference's distance bit for bit.
+    pub fn exact_search_within(
+        &self, queries: &[f32], nq: usize, query_format: c_int, lists: &[Vec<u32>], num_neighbors: usize,
+    ) -> Vec<Vec<(usize, f32)>> {
+        assert_eq!(queries.len(), nq * self.dim);
+        assert_eq!(lists.len(), nq);
+        let mut offsets = vec![0u64];
+        let mut cand = Vec::new();
+        for l in lists {
+            cand.extend_from_slice(l);
+            offsets.push(cand.len() as u64);
+        }
+        let mut ids = vec![0u32; nq * num_neighbors];
+        let mut dists = vec![0f32; nq * num_neighbors];
+        let mut counts = vec![0u32; nq];
+        check(unsafe {
+            granne_b200_exact_search_within_batch(
+                self.h, queries.as_ptr() as *const c_void, nq, query_format, offsets.as_ptr(), cand.as_ptr(),
+                num_neighbors as u32, ids.as_mut_ptr(), dists.as_mut_ptr(), counts.as_mut_ptr(),
             )
         });
         (0..nq)
@@ -476,6 +516,29 @@ impl GpuMultiGranne {
             granne_b200_multi_exact_search_batch(self.m, elements.as_ptr() as *const c_void, nq, QUERY_ELEMENT,
                                                  num_neighbors as u32, ids.as_mut_ptr(), d.as_mut_ptr(),
                                                  c.as_mut_ptr())
+        });
+        (0..nq)
+            .map(|i| (0..c[i] as usize).map(|j| (ids[i * num_neighbors + j] as usize, d[i * num_neighbors + j])).collect())
+            .collect()
+    }
+
+    /// `exact_search_within` over every part: GLOBAL ids in the lists and in the results.
+    pub fn exact_search_within(
+        &self, elements: &[f32], lists: &[Vec<u64>], num_neighbors: usize,
+    ) -> Vec<Vec<(usize, f32)>> {
+        let nq = elements.len() / self.dim;
+        assert_eq!(lists.len(), nq);
+        let mut offsets = vec![0u64];
+        let mut cand = Vec::new();
+        for l in lists {
+            cand.extend_from_slice(l);
+            offsets.push(cand.len() as u64);
+        }
+        let (mut ids, mut d, mut c) = (vec![0u64; nq * num_neighbors], vec![0f32; nq * num_neighbors], vec![0u32; nq]);
+        check(unsafe {
+            granne_b200_multi_exact_search_within_batch(self.m, elements.as_ptr() as *const c_void, nq, QUERY_ELEMENT,
+                                                        offsets.as_ptr(), cand.as_ptr(), num_neighbors as u32,
+                                                        ids.as_mut_ptr(), d.as_mut_ptr(), c.as_mut_ptr())
         });
         (0..nq)
             .map(|i| (0..c[i] as usize).map(|j| (ids[i * num_neighbors + j] as usize, d[i * num_neighbors + j])).collect())

@@ -1,4 +1,5 @@
 """ctypes binding over include/granne_b200.h."""
+import collections
 import ctypes as C
 import os
 
@@ -101,6 +102,9 @@ def load_library():
         "granne_b200_exact_search_batch": (i32, [vp, vp, sz, i32, u32, vp, vp, vp]),
         "granne_b200_exact_search_batch_device": (i32, [vp, vp, sz, i32, u32, vp, vp, vp, vp]),
         "granne_b200_multi_exact_search_batch": (i32, [vp, vp, sz, i32, u32, vp, vp, vp]),
+        "granne_b200_exact_search_within_batch": (i32, [vp, vp, sz, i32, vp, vp, u32, vp, vp, vp]),
+        "granne_b200_exact_search_within_batch_device": (i32, [vp, vp, sz, i32, vp, vp, u32, vp, vp, vp, vp]),
+        "granne_b200_multi_exact_search_within_batch": (i32, [vp, vp, sz, i32, vp, vp, u32, vp, vp, vp]),
         "granne_b200_set_rerank_elements": (i32, [vp, vp, sz]),
         "granne_b200_set_rerank_elements_device": (i32, [vp, vp, u64, u32]),
         "granne_b200_search_rerank_batch": (i32, [vp, vp, sz, i32, u32, u32, u32, vp, vp, vp, vp]),
@@ -160,6 +164,44 @@ def _host_outputs(nq, k, id_dtype, with_stats=False):
     shape = (nq, k)
     return (np.empty(shape, dtype=id_dtype), np.empty(shape, dtype=np.float32), np.empty(nq, dtype=np.uint32),
             np.zeros((nq, STATS_PER_QUERY), dtype=np.uint64) if with_stats else None)
+
+
+class CsrLists(collections.namedtuple("CsrLists", ["offsets", "ids"])):
+    """The candidate lists of nq queries in CSR form: query q's list is ids[offsets[q]:offsets[q + 1]] (offsets: nq + 1
+    values, offsets[0] == 0, non-decreasing).  A plain tuple of arrays is a sequence of per-query lists, never this."""
+
+
+def _candidate_lists(candidates, nq, id_dtype):
+    """(offsets u64 [nq + 1], ids) of the candidate lists of nq queries: a sequence of nq 1-D integer arrays, or a
+    CsrLists.  Ids must be non-negative and fit id_dtype, and a CsrLists' ids must hold offsets[-1] of them; the
+    library checks the offsets' shape and the ids against the index."""
+    if isinstance(candidates, CsrLists):
+        offsets, ids = np.asarray(candidates.offsets), np.asarray(candidates.ids)
+        if offsets.ndim != 1 or offsets.shape[0] != nq + 1:
+            raise ValueError("offsets must have shape (nq + 1,)")
+        if ids.ndim != 1:
+            raise ValueError("ids must be 1-D")
+        if offsets.dtype.kind in "iu" and int(offsets[-1]) > ids.shape[0]:
+            # the library reads offsets[-1] ids from the buffer: more than it holds is out of bounds
+            raise ValueError("offsets[-1] = %d exceeds the %d ids given" % (int(offsets[-1]), ids.shape[0]))
+    else:
+        lists = [np.asarray(c) for c in candidates]
+        lists = [c.astype(id_dtype) if c.size == 0 else c for c in lists]  # an empty Python list is float64
+        if len(lists) != nq:
+            raise ValueError("one candidate list per query: got %d lists for %d queries" % (len(lists), nq))
+        if any(c.ndim != 1 for c in lists):
+            raise ValueError("each candidate list must be 1-D")
+        offsets = np.zeros(nq + 1, dtype=np.uint64)
+        np.cumsum([c.shape[0] for c in lists], out=offsets[1:])
+        ids = np.concatenate(lists) if lists else np.zeros(0, dtype=id_dtype)
+    for a, what in ((offsets, "offsets"), (ids, "ids")):
+        if a.size and a.dtype.kind not in "iu":
+            raise ValueError("%s must be integers" % what)
+        if a.size and a.dtype.kind == "i" and a.min() < 0:
+            raise ValueError("%s must be non-negative" % what)
+    if ids.size and int(ids.max()) > np.iinfo(id_dtype).max:
+        raise ValueError("ids must fit %s" % np.dtype(id_dtype).name)
+    return (np.ascontiguousarray(offsets, dtype=np.uint64), np.ascontiguousarray(ids, dtype=id_dtype))
 
 
 def _device_outputs(q, k, out):
@@ -420,6 +462,46 @@ class Granne:
             C.c_void_p(counts.data_ptr()), C.c_void_p(_raw_stream(stream, q.device))))
         return ids, dists, counts
 
+    def exact_search_within(self, queries, candidates, num_elements=DEFAULT_NUM_ELEMENTS, already_element=False):
+        """Exact k nearest neighbours of each query within its own candidate list: the first min(k, |set(list)|) ids
+        of the list by (distance, id), with the reference's distance bit for bit (granne_b200_exact_search_within_batch).
+        Not a reference function.  `candidates`: one 1-D integer array of ids per query, or a CsrLists(offsets, ids)
+        (offsets [nq + 1], offsets[0] == 0, non-decreasing).  Duplicates count once; every id must be
+        < len(self).  Queries as in exact_search_batch; k <= EXACT_MAX_K.  Returns (ids, dists, counts) in
+        search_batch's layout."""
+        q, fmt = self._host_queries(queries, already_element)
+        nq, k = q.shape[0], int(num_elements)
+        offsets, cand = _candidate_lists(candidates, nq, np.uint32)
+        ids, dists, counts, _ = _host_outputs(nq, k, np.uint32)
+        _check(load_library().granne_b200_exact_search_within_batch(
+            self._h, _ptr(q), nq, fmt, _ptr(offsets), _ptr(cand), k, _ptr(ids), _ptr(dists), _ptr(counts)))
+        return ids, dists, counts
+
+    def exact_search_within_device(self, queries, offsets, ids, num_elements=DEFAULT_NUM_ELEMENTS,
+                                   already_element=False, out=None, stream=None):
+        """Device-resident exact_search_within: CUDA tensors in (queries; offsets int64 [nq + 1]; ids int32 view of
+        u32 ids) and out, asynchronous on `stream` (a torch.cuda.Stream or a raw cudaStream_t; default: the current
+        torch stream).  The kernels check the lists: a bad list gives its query count 0 and padding, and
+        stream_status() raises; so does a NaN distance.  `ids` must hold offsets[-1] ids: the kernels read that many,
+        and checking it here would wait for the device."""
+        import torch
+
+        q = self._check_device_queries(queries)
+        fmt = QUERY_ELEMENT if already_element or q.dtype == torch.int8 else QUERY_RAW_F32
+        nq, k = q.shape[0], int(num_elements)
+        for t, dt, what in ((offsets, torch.int64, "offsets"), (ids, torch.int32, "ids")):
+            if (not isinstance(t, torch.Tensor) or not t.is_cuda or t.device != q.device or t.dtype != dt
+                    or t.dim() != 1 or not t.is_contiguous()):
+                raise ValueError("%s must be a contiguous 1-D %s CUDA tensor on the queries' device" % (what, dt))
+        if offsets.shape[0] != nq + 1:
+            raise ValueError("offsets must have shape (nq + 1,)")
+        out_ids, dists, counts = _device_outputs(q, k, out)
+        _check(load_library().granne_b200_exact_search_within_batch_device(
+            self._h, C.c_void_p(q.data_ptr()), nq, fmt, C.c_void_p(offsets.data_ptr()), C.c_void_p(ids.data_ptr()),
+            k, C.c_void_p(out_ids.data_ptr()), C.c_void_p(dists.data_ptr()), C.c_void_p(counts.data_ptr()),
+            C.c_void_p(_raw_stream(stream, q.device))))
+        return out_ids, dists, counts
+
     # ---- two-stage search (granne_b200_search_rerank_batch*) ----
     def set_rerank_elements(self, elements):
         """Attaches the angular f32 rows (an angular elements file image, `bytes`) that re-rank the candidates of
@@ -662,6 +744,17 @@ class MultiGranne:
         ids, dists, counts, _ = _host_outputs(nq, k, np.uint64)
         _check(load_library().granne_b200_multi_exact_search_batch(self._h, _ptr(q), nq, fmt, k, _ptr(ids),
                                                                    _ptr(dists), _ptr(counts)))
+        return ids, dists, counts
+
+    def exact_search_within(self, queries, candidates, num_elements=DEFAULT_NUM_ELEMENTS, already_element=False):
+        """Granne.exact_search_within over all parts (granne_b200_multi_exact_search_within_batch): GLOBAL ids in the
+        candidate lists (uint64) and in the results."""
+        q, fmt = _host_queries(queries, already_element)
+        nq, k = q.shape[0], int(num_elements)
+        offsets, cand = _candidate_lists(candidates, nq, np.uint64)
+        ids, dists, counts, _ = _host_outputs(nq, k, np.uint64)
+        _check(load_library().granne_b200_multi_exact_search_within_batch(
+            self._h, _ptr(q), nq, fmt, _ptr(offsets), _ptr(cand), k, _ptr(ids), _ptr(dists), _ptr(counts)))
         return ids, dists, counts
 
     def set_rerank_elements(self, elements):

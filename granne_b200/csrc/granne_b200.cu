@@ -28,6 +28,7 @@
 #include "search_kernels.cuh"
 #include "exact_kernels.cuh"
 #include "rerank_kernels.cuh"
+#include "within_kernels.cuh"
 
 namespace gb = granne_b200;
 
@@ -155,6 +156,9 @@ struct Workspace {
     Buffer<float> d_exact_table;
     // two-stage search: stage 1's candidates, one block ids | dists | counts for the current call's nq x C
     Buffer<uint32_t> d_rerank;
+    // exact search within lists: a chunk's running lists | segment prefix; its locks | query flags
+    Buffer<unsigned long long> d_within;
+    Buffer<int> d_within_flags;
 };
 
 // The owners of the arrays a DeviceIndex points to, one slot per pointer: the memory and the bytes allocated for it.
@@ -982,6 +986,8 @@ int error_from_bits(int bits) {
         return fail(GRANNE_B200_ERR_NOT_FINITE, "a NaN distance occurred (non-finite query or element)");
     if (bits & gb::kStatusOverflow)
         return fail(GRANNE_B200_ERR_CAPACITY, "exact search workspace exhausted even on the slow path");
+    if (bits & gb::kStatusBadList)
+        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "a candidate list has bad offsets or an id >= Index::len");
     return GRANNE_B200_OK;
 }
 
@@ -1298,6 +1304,97 @@ int enqueue_rerank(Handle* h, Workspace* w, const void* d_queries, size_t nq, ui
             const unsigned grid = (unsigned)std::min<unsigned long long>(a.nq, (unsigned long long)occ * h->num_sms);
             return launch_warps<gb::rerank_kernel<Dist>>(h, grid, smem, stream, h->rerank, a);
         }
+    });
+}
+
+// ---- exact search within candidate lists (within_kernels.cuh) -----------------------------------------------------
+// validate_exact's rules, then the lists' pointers: offsets when nq > 0 and, when the lists are in host memory, ids
+// when offsets[nq] > 0 (a device call's kernels check a null ids pointer against the lists they are given).
+int validate_within(const Handle* h, const void* q, size_t nq, int fmt, uint32_t k, const void* out_ids,
+                    const void* out_dists, const uint64_t* offsets, const void* ids, bool host_lists) {
+    const int rc = validate_exact(h, q, nq, fmt, k, out_ids, out_dists);
+    if (rc || nq == 0) return rc;
+    if (!offsets) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "offsets is null");
+    if (host_lists && offsets[nq] > 0 && !ids) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "ids is null");
+    return GRANNE_B200_OK;
+}
+
+// The host checks of nq lists in host memory: the shape of the offsets (which reads no handle), then every id
+// against n.
+int check_within_offsets(const uint64_t* offsets, size_t nq) {
+    if (offsets[0] != 0) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "offsets must start at 0 and not decrease");
+    for (size_t q = 0; q < nq; ++q)
+        if (offsets[q + 1] < offsets[q])
+            return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "offsets must start at 0 and not decrease");
+    return GRANNE_B200_OK;
+}
+template <class Id>
+int check_within_ids(const uint64_t* offsets, size_t nq, const Id* ids, uint64_t n) {
+    for (uint64_t i = 0; i < offsets[nq]; ++i)
+        if ((uint64_t)ids[i] >= n) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "candidate id >= Index::len");
+    return GRANNE_B200_OK;
+}
+
+// Enqueues one exact search within lists on `stream`: nq queries (device memory, the caller's format), their lists
+// d_offsets / d_ids (device memory), results in search_batch's layout.  Query chunks of at most kExactMaxChunk: the
+// segments kernel, then within_kernel over the chunk's segments, then the rows of the lists of other than one segment.
+// A NaN distance sets kStatusNotFinite in w->d_error, a bad list kStatusBadList.
+int enqueue_within(Handle* h, Workspace* w, const void* d_queries, size_t nq, int fmt, const uint64_t* d_offsets,
+                   const uint32_t* d_ids, uint32_t k, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts,
+                   cudaStream_t stream) {
+    const gb::DeviceIndex& d = h->dev;
+    const size_t in_row = query_bytes(h, 1, fmt);
+    const size_t qc_max = std::min<size_t>(nq, gb::kExactMaxChunk);
+    int rc;
+    if ((rc = w->d_within.grow(qc_max * k + qc_max + 2, stream)) || (rc = w->d_within_flags.grow(2 * qc_max, stream)))
+        return rc;
+    unsigned long long* lists = w->d_within.get();
+    unsigned long long* prefix = lists + qc_max * k;
+    unsigned long long* counter = prefix + qc_max + 1;
+    int* locks = w->d_within_flags.get();
+    int* qflags = locks + qc_max;
+    const EngineTiles eng = engine_tiles(d);
+    const size_t smem = gb::rerank_keys_offset(eng.base_smem) + (size_t)gb::within_key_slots(k) * 8;
+    return DistDispatch::call(d, [&](auto e) {
+        using Dist = typename decltype(e)::type;
+        constexpr auto kern = gb::within_kernel<Dist>;
+        int occ = 0;
+        int err = resident_ctas<kern>(h, smem, &occ);
+        if (err) return err;
+        if (occ < 1) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "exact search within lists exceeds shared memory");
+        for (size_t c0 = 0; c0 < nq; c0 += gb::kExactMaxChunk) {
+            const uint32_t qc = (uint32_t)std::min<size_t>(gb::kExactMaxChunk, nq - c0);
+            const unsigned long long* offs = reinterpret_cast<const unsigned long long*>(d_offsets) + c0;
+            gb::within_segments_kernel<<<1, gb::kExactMaxChunk, 0, stream>>>(offs, qc, c0 == 0, d_ids, prefix, locks,
+                                                                            qflags, counter, w->d_error);
+            h->launches++;
+            GB_CUDA(cudaGetLastError());
+            if (k) GB_CUDA(cudaMemsetAsync(lists, 0xFF, (size_t)qc * k * 8, stream));
+            gb::WithinArgs a{};
+            a.queries = static_cast<const uint8_t*>(d_queries) + c0 * in_row;
+            a.query_format = fmt;
+            a.nq = qc;
+            a.offsets = offs;
+            a.ids = d_ids;
+            a.len = h->index_len;
+            a.num_neighbors = k;
+            a.seg_prefix = prefix;
+            a.lists = lists;
+            a.locks = locks;
+            a.qflags = qflags;
+            a.work_counter = counter;
+            a.out_ids = d_out_ids ? d_out_ids + c0 * k : nullptr;
+            a.out_dists = d_out_dists ? d_out_dists + c0 * k : nullptr;
+            a.out_counts = d_out_counts ? d_out_counts + c0 : nullptr;
+            a.error_flag = w->d_error;
+            a.tiles = eng.tiles;
+            if ((err = launch_warps<kern>(h, (unsigned)occ * h->num_sms, smem, stream, d, a))) return err;
+            gb::within_write_kernel<<<qc, 128, 0, stream>>>(lists, prefix, qflags, k, a.out_ids, a.out_dists,
+                                                            a.out_counts);
+            h->launches++;
+            GB_CUDA(cudaGetLastError());
+        }
+        return (int)GRANNE_B200_OK;
     });
 }
 
@@ -1741,6 +1838,54 @@ int granne_b200_exact_search_batch_device(granne_b200_index* h, const void* d_qu
     return device_batch(h, cuda_stream, [&](Workspace* w, cudaStream_t stream) {
         return enqueue_exact(h, w, d_queries, nq, query_format, num_neighbors, d_out_ids, d_out_dists, d_out_counts,
                              stream);
+    });
+}
+
+int granne_b200_exact_search_within_batch(granne_b200_index* h, const void* queries, size_t nq, int query_format,
+                                          const uint64_t* offsets, const uint32_t* ids, uint32_t num_neighbors,
+                                          uint32_t* out_ids, float* out_dists, uint32_t* out_counts) {
+    int rc = validate_within(h, queries, nq, query_format, num_neighbors, out_ids, out_dists, offsets, ids, true);
+    if (rc) return rc;
+    if (nq == 0) return GRANNE_B200_OK;
+    if ((rc = check_within_offsets(offsets, nq)) || (rc = check_within_ids(offsets, nq, ids, h->index_len))) return rc;
+    const uint64_t total = offsets[nq];
+    return host_batch(h, queries, query_bytes(h, nq, query_format), nq, num_neighbors, out_ids, out_dists, out_counts,
+                      nullptr, [&](Workspace* w, cudaStream_t stream, unsigned long long*) {
+                          // enqueue_within has no memset that zeroes the error word (host_batch)
+                          GB_CUDA(cudaMemsetAsync(w->d_error, 0, 4 * sizeof(int), stream));
+                          // the lists are the caller's input, not workspace: a stream-ordered allocation for this call
+                          // only, freed behind its kernels, so that a long list leaves no device memory held by the
+                          // pooled workspace
+                          const size_t obytes = (nq + 1) * 8;
+                          void* mem = nullptr;
+                          GB_CUDA(cudaMallocAsync(&mem, obytes + total * 4, stream));
+                          uint64_t* d_offsets = static_cast<uint64_t*>(mem);
+                          uint32_t* d_ids = reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(mem) + obytes);
+                          const int r = [&] {
+                              GB_CUDA(cudaMemcpyAsync(d_offsets, offsets, obytes, cudaMemcpyHostToDevice, stream));
+                              if (total)
+                                  GB_CUDA(cudaMemcpyAsync(d_ids, ids, total * 4, cudaMemcpyHostToDevice, stream));
+                              return enqueue_within(h, w, w->d_queries.get(), nq, query_format, d_offsets, d_ids,
+                                                    num_neighbors, w->d_ids.get(), w->d_dists, w->d_counts, stream);
+                          }();
+                          const cudaError_t fe = cudaFreeAsync(mem, stream);
+                          if (r) return r;
+                          GB_CUDA(fe);
+                          return (int)GRANNE_B200_OK;
+                      });
+}
+
+int granne_b200_exact_search_within_batch_device(granne_b200_index* h, const void* d_queries, size_t nq,
+                                                 int query_format, const uint64_t* d_offsets, const uint32_t* d_ids,
+                                                 uint32_t num_neighbors, uint32_t* d_out_ids, float* d_out_dists,
+                                                 uint32_t* d_out_counts, void* cuda_stream) {
+    int rc = validate_within(h, d_queries, nq, query_format, num_neighbors, d_out_ids, d_out_dists, d_offsets, d_ids,
+                             false);
+    if (rc) return rc;
+    if (nq == 0) return GRANNE_B200_OK;
+    return device_batch(h, cuda_stream, [&](Workspace* w, cudaStream_t stream) {
+        return enqueue_within(h, w, d_queries, nq, query_format, d_offsets, d_ids, num_neighbors, d_out_ids,
+                              d_out_dists, d_out_counts, stream);
     });
 }
 
@@ -2738,6 +2883,58 @@ int granne_b200_multi_exact_search_batch(granne_b200_multi* m, const void* queri
                        [&](granne_b200_index* h, const void* q, size_t cnt, uint32_t* ids, float* ds, uint32_t* c) {
                            return granne_b200_exact_search_batch(h, q, cnt, query_format, num_neighbors, ids, ds, c);
                        });
+}
+
+// REPLICATED: each device runs its slice of the queries on their lists, offsets rebased to the slice.
+// RANGE_PARTITIONED: each global id goes to the shard that owns it as a local id, every shard runs every query on its
+// local lists, and multi_batch merges the shard lists by (distance, global id) as for the exact search.
+int granne_b200_multi_exact_search_within_batch(granne_b200_multi* m, const void* queries, size_t nq,
+                                                int query_format, const uint64_t* offsets, const uint64_t* ids,
+                                                uint32_t num_neighbors, uint64_t* out_ids, float* out_dists,
+                                                uint32_t* out_counts) {
+    if (!m) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "multi handle is null");
+    int rc = validate_within(m->parts[0], queries, nq, query_format, num_neighbors, out_ids, out_dists, offsets, ids,
+                             true);
+    if (rc) return rc;
+    if (nq == 0) return GRANNE_B200_OK;
+    if ((rc = check_within_offsets(offsets, nq)) || (rc = check_within_ids(offsets, nq, ids, m->total_len))) return rc;
+    return guarded([&] {
+        const size_t n = m->parts.size();
+        const bool range = m->mode == GRANNE_B200_MODE_RANGE_PARTITIONED;
+        std::vector<std::vector<uint64_t>> loff(range ? n : 0, std::vector<uint64_t>(1, 0));
+        std::vector<std::vector<uint32_t>> lids(range ? n : 0);
+        for (size_t q = 0; range && q < nq; ++q) {
+            for (uint64_t i = offsets[q]; i < offsets[q + 1]; ++i) {
+                const size_t s = std::upper_bound(m->base.begin(), m->base.end(), ids[i]) - m->base.begin() - 1;
+                const uint64_t local = ids[i] - m->base[s];
+                if (local >= m->parts[s]->index_len)
+                    return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "candidate id is in no shard's Index::len range");
+                lids[s].push_back((uint32_t)local);
+            }
+            for (size_t s = 0; s < n; ++s) loff[s].push_back(lids[s].size());
+        }
+        const bool i8q = m->kind == GRANNE_B200_ANGULAR_INT && query_format == GRANNE_B200_QUERY_ELEMENT;
+        const size_t qrow = (size_t)m->dim * (i8q ? 1 : 4);
+        return multi_batch(m, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts,
+                           [&](granne_b200_index* h, const void* q, size_t cnt, uint32_t* pids, float* ds, uint32_t* c) {
+                               if (range) {
+                                   const size_t s = std::find(m->parts.begin(), m->parts.end(), h) - m->parts.begin();
+                                   return granne_b200_exact_search_within_batch(h, q, cnt, query_format, loff[s].data(),
+                                                                                lids[s].data(), num_neighbors, pids, ds,
+                                                                                c);
+                               }
+                               // the slice of queries [b, b + cnt) and their lists
+                               const size_t b =
+                                   (static_cast<const uint8_t*>(q) - static_cast<const uint8_t*>(queries)) / qrow;
+                               return guarded([&] {
+                                   std::vector<uint64_t> off(cnt + 1);
+                                   for (size_t j = 0; j <= cnt; ++j) off[j] = offsets[b + j] - offsets[b];
+                                   const std::vector<uint32_t> sl(ids + offsets[b], ids + offsets[b + cnt]);
+                                   return granne_b200_exact_search_within_batch(h, q, cnt, query_format, off.data(),
+                                                                                sl.data(), num_neighbors, pids, ds, c);
+                               });
+                           });
+    });
 }
 
 // Every image is checked on the host against its part before any part stages rows (multi_attach_rerank).

@@ -191,6 +191,40 @@ int granne_b200_exact_search_batch_device(granne_b200_index* h, const void* d_qu
                                           uint32_t num_neighbors, uint32_t* d_out_ids, float* d_out_dists,
                                           uint32_t* d_out_counts, void* cuda_stream);
 
+/* ---- exact search within caller-given candidate lists ---------------------------------------------------------------
+ * NOT a reference function: the exact answer within a list of ids per query — a restricted search (ids admitted by a
+ * category, tenant, time range or ACL), the ranking of a lexical engine's candidates, the union of several indexes'
+ * results, or ground truth inside a subset.  For n = granne_b200_len(h) (Index::len), a query q and its list L_q of
+ * u32 ids the result is the first min(k, |set(L_q)|) entries of
+ *     sort ascending { (dist_to_element(q, i), i) : i in set(L_q) }
+ * with dist_to_element and the order exactly as in granne_b200_exact_search_batch (an angular_int handle ranks by its
+ * i8 distance).  The result depends only on the set of ids, not on their order or multiplicity.  L_q = [0, n) gives
+ * granne_b200_exact_search_batch(q, k); L_q = the ids of granne_b200_search_batch(q, ef, ef) gives
+ * granne_b200_search_batch(q, ef, k) for k <= ef.
+ *   queries        as granne_b200_exact_search_batch (RAW_F32 or ELEMENT)
+ *   offsets        nq + 1 u64, offsets[0] == 0, non-decreasing: L_q = ids[offsets[q], offsets[q + 1])
+ *   ids            offsets[nq] u32 ids, each < n (ids in [n, num_elements) of a container larger than its index are
+ *                  rejected too); may be NULL when offsets[nq] == 0
+ *   num_neighbors  k, 0..GRANNE_B200_EXACT_MAX_K
+ *   out_*          as granne_b200_exact_search_batch; out_counts[q] = min(k, |set(L_q)|)
+ * nq == 0, k == 0 and empty lists are valid.  Only listed elements are read: a NaN distance of a listed element (or a
+ * NaN query with a non-empty list and k > 0) returns ERR_NOT_FINITE; one of an element no list names does not.
+ * ERR_INVALID_ARGUMENT, in this order: a rule of granne_b200_exact_search_batch; offsets NULL with nq > 0; ids NULL with
+ * offsets[nq] > 0; offsets that do not start at 0 or go backwards; an id >= n.  The host call checks all of them on
+ * the host before any device call; its lists are copied to the device with the queries, in the one round trip of the
+ * call, into memory held only until the call's kernels have run.  Workspace is bounded (query chunks of 1024, k keys per query) whatever the lists' lengths. */
+int granne_b200_exact_search_within_batch(granne_b200_index* h, const void* queries, size_t nq, int query_format,
+                                          const uint64_t* offsets, const uint32_t* ids, uint32_t num_neighbors,
+                                          uint32_t* out_ids, float* out_dists, uint32_t* out_counts);
+/* Same with DEVICE pointers (queries, offsets, ids, outputs) on cuda_stream (NULL = the default stream), asynchronous
+ * like granne_b200_exact_search_batch_device and without a host synchronisation.  The host checks the arguments up to
+ * offsets NULL; the kernels check the offsets and the ids: a bad list writes count 0 and padding for its query, and
+ * granne_b200_stream_status reports ERR_INVALID_ARGUMENT (ERR_NOT_FINITE for a NaN distance). */
+int granne_b200_exact_search_within_batch_device(granne_b200_index* h, const void* d_queries, size_t nq,
+                                                 int query_format, const uint64_t* d_offsets, const uint32_t* d_ids,
+                                                 uint32_t num_neighbors, uint32_t* d_out_ids, float* d_out_dists,
+                                                 uint32_t* d_out_counts, void* cuda_stream);
+
 /* ---- two-stage search: traverse angular_int rows, re-rank by exact f32 angular distance ----------------------------
  * NOT a reference function: what a user of granne assembles by hand from two containers over one index.  For an
  * angular_int handle h with an attached container F (angular rows or SumEmbeddings) and a raw f32 query q:
@@ -241,7 +275,8 @@ int granne_b200_search_rerank_batch_device(granne_b200_index* h, const float* d_
 int granne_b200_release_stream(granne_b200_index* h, void* cuda_stream);
 
 /* After synchronising a stream used with granne_b200_search_batch_device: GRANNE_B200_OK, or the first error
- * (ERR_NOT_FINITE / ERR_CAPACITY) any query of the calls issued since the previous check raised. */
+ * (ERR_NOT_FINITE / ERR_CAPACITY, or ERR_INVALID_ARGUMENT for a bad candidate list of
+ * granne_b200_exact_search_within_batch_device) any query of the calls issued since the previous check raised. */
 int granne_b200_stream_status(granne_b200_index* h);
 
 /* Range-partitioned mode (SURVEY.md §8e mode 2; granne shards elements into independent indexes,
@@ -291,6 +326,15 @@ int granne_b200_multi_search_batch(granne_b200_multi* m, const void* queries, si
 int granne_b200_multi_exact_search_batch(granne_b200_multi* m, const void* queries, size_t nq, int query_format,
                                          uint32_t num_neighbors, uint64_t* out_ids, float* out_dists,
                                          uint32_t* out_counts);
+/* granne_b200_exact_search_within_batch over a multi handle: u64 GLOBAL ids in the lists and in the results.
+ * REPLICATED slices the queries together with their lists over the devices; RANGE_PARTITIONED routes each id to the
+ * shard that owns it (shard_base[s] <= id < shard_base[s] + that shard's Index::len), runs every shard on its local
+ * lists and merges by (distance, global id).  An id >= granne_b200_multi_len(m), or one in no shard's Index::len range,
+ * is ERR_INVALID_ARGUMENT, checked on the host before any device call. */
+int granne_b200_multi_exact_search_within_batch(granne_b200_multi* m, const void* queries, size_t nq,
+                                                int query_format, const uint64_t* offsets, const uint64_t* ids,
+                                                uint32_t num_neighbors, uint64_t* out_ids, float* out_dists,
+                                                uint32_t* out_counts);
 /* granne_b200_set_rerank_elements on every part: REPLICATED takes one image (elements_bytes[0]) and stages it on every
  * device; RANGE_PARTITIONED takes one image per shard.  Every image is checked before any is staged; if a part then fails to
  * stage its rows (a device error), the parts this call attached release theirs again, so the call can be repeated. */

@@ -230,6 +230,26 @@ public:
                                              ids.data(), dists.data(), counts.data()));
         return detail::result_lists<SearchResult>(ids, dists, counts, num_neighbors);
     }
+    // Exact k nearest neighbours of each query within its own candidate list (granne_b200_exact_search_within_batch):
+    // lists[q] holds query q's ids (< len(); duplicates count once); the first min(k, |set(lists[q])|) by (distance,
+    // id), the reference's distance bit for bit.  Not a reference function.
+    std::vector<SearchResult> exact_search_within(const void* queries, size_t nq, int query_format,
+                                                  const std::vector<std::vector<uint32_t>>& lists,
+                                                  size_t num_neighbors) const {
+        if (lists.size() != nq) throw Error(GRANNE_B200_ERR_INVALID_ARGUMENT, "one candidate list per query");
+        std::vector<uint64_t> offsets(1, 0);
+        std::vector<uint32_t> cand;
+        for (const auto& l : lists) {
+            cand.insert(cand.end(), l.begin(), l.end());
+            offsets.push_back(cand.size());
+        }
+        std::vector<uint32_t> ids(nq * num_neighbors), counts(nq);
+        std::vector<float> dists(nq * num_neighbors);
+        check(granne_b200_exact_search_within_batch(h_, queries, nq, query_format, offsets.data(), cand.data(),
+                                                    static_cast<uint32_t>(num_neighbors), ids.data(), dists.data(),
+                                                    counts.data()));
+        return detail::result_lists<SearchResult>(ids, dists, counts, num_neighbors);
+    }
 
     // Two-stage search (granne_b200_search_rerank_batch): attach the container of this angular_int index's elements
     // once (angular f32 rows, or the SumEmbeddings container the rows were computed from), then search_rerank
@@ -380,6 +400,27 @@ public:
         check(granne_b200_multi_exact_search_batch(h_, queries.data(), nq, GRANNE_B200_QUERY_RAW_F32,
                                                    static_cast<uint32_t>(num_neighbors), ids.data(), d.data(),
                                                    c.data()));
+        return detail::result_lists<Result>(ids, d, c, num_neighbors);
+    }
+    // Granne::exact_search_within over every part for nq raw f32 queries (nq x dim, row-major, as the *_raw calls
+    // take them), GLOBAL ids in the lists and the results (granne_b200_multi_exact_search_within_batch)
+    std::vector<Result> exact_search_within(const std::vector<float>& queries,
+                                                const std::vector<std::vector<uint64_t>>& lists,
+                                                size_t num_neighbors) const {
+        const size_t nq = dim_ ? queries.size() / dim_ : 0;
+        if (lists.size() != nq) throw Error(GRANNE_B200_ERR_INVALID_ARGUMENT, "one candidate list per query");
+        std::vector<uint64_t> offsets(1, 0), cand;
+        for (const auto& l : lists) {
+            cand.insert(cand.end(), l.begin(), l.end());
+            offsets.push_back(cand.size());
+        }
+        std::vector<uint64_t> ids(nq * num_neighbors);
+        std::vector<float> d(nq * num_neighbors);
+        std::vector<uint32_t> c(nq);
+        check(granne_b200_multi_exact_search_within_batch(h_, queries.data(), nq, GRANNE_B200_QUERY_RAW_F32,
+                                                          offsets.data(), cand.data(),
+                                                          static_cast<uint32_t>(num_neighbors), ids.data(), d.data(),
+                                                          c.data()));
         return detail::result_lists<Result>(ids, d, c, num_neighbors);
     }
 
