@@ -114,6 +114,16 @@ extern "C" {
         m: *mut RawMulti, queries: *const c_void, nq: usize, query_format: c_int, offsets: *const u64,
         ids: *const u64, num_neighbors: u32, out_ids: *mut u64, out_dists: *mut f32, out_counts: *mut u32,
     ) -> c_int;
+    fn granne_b200_search_filtered_batch(
+        h: *mut RawIndex, queries: *const c_void, nq: usize, query_format: c_int, max_search: u32, num_neighbors: u32,
+        filters: *const u32, num_filters: u32, filter_words: u64, query_filter: *const u32, out_ids: *mut u32,
+        out_dists: *mut f32, out_counts: *mut u32, out_stats: *mut u64,
+    ) -> c_int;
+    fn granne_b200_multi_search_filtered_batch(
+        m: *mut RawMulti, queries: *const c_void, nq: usize, query_format: c_int, max_search: u32, num_neighbors: u32,
+        filters: *const u32, num_filters: u32, filter_words: u64, query_filter: *const u32, out_ids: *mut u64,
+        out_dists: *mut f32, out_counts: *mut u32,
+    ) -> c_int;
     fn granne_b200_set_rerank_elements(h: *mut RawIndex, elements: *const c_void, elements_len: usize) -> c_int;
     fn granne_b200_search_rerank_batch(
         h: *mut RawIndex, queries: *const f32, nq: usize, query_format: c_int, max_search: u32, num_candidates: u32,
@@ -313,6 +323,39 @@ impl GpuGranne {
             granne_b200_exact_search_within_batch(
                 self.h, queries.as_ptr() as *const c_void, nq, query_format, offsets.as_ptr(), cand.as_ptr(),
                 num_neighbors as u32, ids.as_mut_ptr(), dists.as_mut_ptr(), counts.as_mut_ptr(),
+            )
+        });
+        (0..nq)
+            .map(|q| {
+                (0..counts[q] as usize)
+                    .map(|j| (ids[q * num_neighbors + j] as usize, dists[q * num_neighbors + j]))
+                    .collect()
+            })
+            .collect()
+    }
+
+    /// Filtered search (not a reference function): `search`'s traversal, unchanged, keeping the first k elements by
+    /// (distance, id) among those it scores in the bottom layer that the query's filter admits.  `filters` holds
+    /// `filters.len() / filter_words` bitmaps (id i: bit i % 32 of word i / 32, `filter_words >= ceil(len() / 32)`);
+    /// `query_filter` picks each query's bitmap (None: bitmap 0).  k <= GRANNE_B200_EXACT_MAX_K.
+    pub fn search_filtered(
+        &self, queries: &[f32], nq: usize, query_format: c_int, max_search: usize, num_neighbors: usize,
+        filters: &[u32], filter_words: usize, query_filter: Option<&[u32]>,
+    ) -> Vec<Vec<(usize, f32)>> {
+        assert_eq!(queries.len(), nq * self.dim);
+        assert!(filter_words > 0 && filters.len() % filter_words == 0);
+        if let Some(f) = query_filter {
+            assert_eq!(f.len(), nq);
+        }
+        let mut ids = vec![0u32; nq * num_neighbors];
+        let mut dists = vec![0f32; nq * num_neighbors];
+        let mut counts = vec![0u32; nq];
+        check(unsafe {
+            granne_b200_search_filtered_batch(
+                self.h, queries.as_ptr() as *const c_void, nq, query_format, max_search as u32, num_neighbors as u32,
+                filters.as_ptr(), (filters.len() / filter_words) as u32, filter_words as u64,
+                query_filter.map_or(std::ptr::null(), |f| f.as_ptr()), ids.as_mut_ptr(), dists.as_mut_ptr(),
+                counts.as_mut_ptr(), std::ptr::null_mut(),
             )
         });
         (0..nq)
@@ -539,6 +582,29 @@ impl GpuMultiGranne {
             granne_b200_multi_exact_search_within_batch(self.m, elements.as_ptr() as *const c_void, nq, QUERY_ELEMENT,
                                                         offsets.as_ptr(), cand.as_ptr(), num_neighbors as u32,
                                                         ids.as_mut_ptr(), d.as_mut_ptr(), c.as_mut_ptr())
+        });
+        (0..nq)
+            .map(|i| (0..c[i] as usize).map(|j| (ids[i * num_neighbors + j] as usize, d[i * num_neighbors + j])).collect())
+            .collect()
+    }
+
+    /// `search_filtered` over every part: the bitmaps are over GLOBAL ids, and so are the results.
+    pub fn search_filtered(
+        &self, elements: &[f32], max_search: usize, num_neighbors: usize, filters: &[u32], filter_words: usize,
+        query_filter: Option<&[u32]>,
+    ) -> Vec<Vec<(usize, f32)>> {
+        let nq = elements.len() / self.dim;
+        assert!(filter_words > 0 && filters.len() % filter_words == 0);
+        if let Some(f) = query_filter {
+            assert_eq!(f.len(), nq);
+        }
+        let (mut ids, mut d, mut c) = (vec![0u64; nq * num_neighbors], vec![0f32; nq * num_neighbors], vec![0u32; nq]);
+        check(unsafe {
+            granne_b200_multi_search_filtered_batch(self.m, elements.as_ptr() as *const c_void, nq, QUERY_ELEMENT,
+                                                    max_search as u32, num_neighbors as u32, filters.as_ptr(),
+                                                    (filters.len() / filter_words) as u32, filter_words as u64,
+                                                    query_filter.map_or(std::ptr::null(), |f| f.as_ptr()),
+                                                    ids.as_mut_ptr(), d.as_mut_ptr(), c.as_mut_ptr())
         });
         (0..nq)
             .map(|i| (0..c[i] as usize).map(|j| (ids[i * num_neighbors + j] as usize, d[i * num_neighbors + j])).collect())

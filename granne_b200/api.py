@@ -105,6 +105,10 @@ def load_library():
         "granne_b200_exact_search_within_batch": (i32, [vp, vp, sz, i32, vp, vp, u32, vp, vp, vp]),
         "granne_b200_exact_search_within_batch_device": (i32, [vp, vp, sz, i32, vp, vp, u32, vp, vp, vp, vp]),
         "granne_b200_multi_exact_search_within_batch": (i32, [vp, vp, sz, i32, vp, vp, u32, vp, vp, vp]),
+        "granne_b200_search_filtered_batch": (i32, [vp, vp, sz, i32, u32, u32, vp, u32, u64, vp, vp, vp, vp, vp]),
+        "granne_b200_search_filtered_batch_device": (i32, [vp, vp, sz, i32, u32, u32, vp, u32, u64, vp, vp, vp, vp, vp,
+                                                           vp]),
+        "granne_b200_multi_search_filtered_batch": (i32, [vp, vp, sz, i32, u32, u32, vp, u32, u64, vp, vp, vp, vp]),
         "granne_b200_set_rerank_elements": (i32, [vp, vp, sz]),
         "granne_b200_set_rerank_elements_device": (i32, [vp, vp, u64, u32]),
         "granne_b200_search_rerank_batch": (i32, [vp, vp, sz, i32, u32, u32, u32, vp, vp, vp, vp]),
@@ -202,6 +206,47 @@ def _candidate_lists(candidates, nq, id_dtype):
     if ids.size and int(ids.max()) > np.iinfo(id_dtype).max:
         raise ValueError("ids must fit %s" % np.dtype(id_dtype).name)
     return (np.ascontiguousarray(offsets, dtype=np.uint64), np.ascontiguousarray(ids, dtype=id_dtype))
+
+
+def _filter_words(filters, n):
+    """The packed bitmaps (uint32 [F, W], C-contiguous) of a filtered search over ids [0, n): a bool mask of shape (n,)
+    or (F, n), packed LSB first (id i is bit i % 32 of word i // 32), or uint32 words of shape (F, W) with
+    W >= ceil(n / 32), passed as they are."""
+    f = np.asarray(filters)
+    if f.dtype == np.bool_:
+        if f.ndim == 1:
+            f = f[None, :]
+        if f.ndim != 2 or f.shape[1] != n:
+            raise ValueError("a bool filter mask must have shape (%d,) or (F, %d)" % (n, n))
+        w = (n + 31) // 32
+        b = np.zeros((f.shape[0], 4 * w), dtype=np.uint8)
+        b[:, :(n + 7) // 8] = np.packbits(f, axis=1, bitorder="little")
+        words = b.view("<u4").astype(np.uint32, copy=False)
+    elif f.dtype == np.uint32:
+        if f.ndim != 2:
+            raise ValueError("filter words must have shape (F, W)")
+        if f.shape[1] < (n + 31) // 32:
+            raise ValueError("filter words: W = %d is less than ceil(%d / 32) = %d" % (f.shape[1], n, (n + 31) // 32))
+        words = f
+    else:
+        raise ValueError("filters must be a bool mask or uint32 words, not %s" % f.dtype)
+    if words.shape[0] == 0:
+        raise ValueError("filters must hold at least one filter")
+    return np.ascontiguousarray(words)
+
+
+def _query_filter(query_filter, nq):
+    """query_filter as uint32 [nq] (the library checks each entry against the number of filters), or None."""
+    if query_filter is None:
+        return None
+    qf = np.asarray(query_filter)
+    if qf.ndim != 1 or qf.shape[0] != nq:
+        raise ValueError("query_filter must have shape (nq,) = (%d,)" % nq)
+    if qf.size and qf.dtype.kind not in "iu":
+        raise ValueError("query_filter must be integers")
+    if qf.size and (qf.min() < 0 or int(qf.max()) > 0xFFFFFFFF):
+        raise ValueError("query_filter entries must be non-negative and fit uint32")
+    return np.ascontiguousarray(qf, dtype=np.uint32)
 
 
 def _device_outputs(q, k, out):
@@ -503,6 +548,56 @@ class Granne:
         return out_ids, dists, counts
 
     # ---- two-stage search (granne_b200_search_rerank_batch*) ----
+    def search_batch_filtered(self, queries, filters, query_filter=None, max_search=DEFAULT_MAX_SEARCH,
+                              num_elements=DEFAULT_NUM_ELEMENTS, already_element=False, with_stats=False):
+        """Filtered search (granne_b200_search_filtered_batch): search_batch's traversal, unchanged, returning the first
+        k admitted elements among those it scores in the bottom layer, by (distance, id).  Not a reference function.
+        `filters`: a bool mask of shape (len,) or (F, len), or packed uint32 words (F, W), W >= ceil(len / 32) (id i
+        is bit i % 32 of word i // 32); query_filter: one filter index per query (None: filter 0 for all).  k <=
+        EXACT_MAX_K and may exceed max_search; no exact fallback, so a selective filter may return fewer than k.
+        Returns search_batch's (ids, dists, counts[, stats]); stats columns 0..2 equal search_batch's."""
+        q, fmt = self._host_queries(queries, already_element)
+        nq, k = q.shape[0], int(num_elements)
+        words = _filter_words(filters, len(self))
+        qf = _query_filter(query_filter, nq)
+        ids, dists, counts, stats = _host_outputs(nq, k, np.uint32, with_stats)
+        _check(load_library().granne_b200_search_filtered_batch(
+            self._h, _ptr(q), nq, fmt, int(max_search), k, _ptr(words), words.shape[0], words.shape[1],
+            _ptr(qf) if qf is not None else None, _ptr(ids), _ptr(dists), _ptr(counts),
+            _ptr(stats) if with_stats else None))
+        if with_stats:
+            return ids, dists, counts, stats
+        return ids, dists, counts
+
+    def search_batch_filtered_device(self, queries, filters, query_filter=None, max_search=DEFAULT_MAX_SEARCH,
+                                     num_elements=DEFAULT_NUM_ELEMENTS, already_element=False, out=None, stats=None,
+                                     stream=None):
+        """Device-resident search_batch_filtered: CUDA tensors in (queries; filters int32 [F, W] holding the uint32
+        words; query_filter int32 [nq] or None) and out, asynchronous on `stream` like search_batch_device.  The kernel
+        checks query_filter: an entry >= F gives its query count 0 and padding, and stream_status() raises."""
+        import torch
+
+        q = self._check_device_queries(queries)
+        fmt = QUERY_ELEMENT if already_element or q.dtype == torch.int8 else QUERY_RAW_F32
+        nq, k = q.shape[0], int(num_elements)
+        for t, shape, what in ((filters, None, "filters"), (query_filter, (nq,), "query_filter")):
+            if t is None and what == "query_filter":
+                continue
+            if (not isinstance(t, torch.Tensor) or not t.is_cuda or t.device != q.device or t.dtype != torch.int32
+                    or not t.is_contiguous() or (shape is None and t.dim() != 2)
+                    or (shape is not None and tuple(t.shape) != shape)):
+                raise ValueError("%s must be a contiguous int32 CUDA tensor of shape %s on the queries' device"
+                                 % (what, "(F, W)" if shape is None else "(nq,)"))
+        ids, dists, counts = _device_outputs(q, k, out)
+        _check_stats(stats, q)
+        _check(load_library().granne_b200_search_filtered_batch_device(
+            self._h, C.c_void_p(q.data_ptr()), nq, fmt, int(max_search), k, C.c_void_p(filters.data_ptr()),
+            filters.shape[0], filters.shape[1],
+            C.c_void_p(query_filter.data_ptr()) if query_filter is not None else None, C.c_void_p(ids.data_ptr()),
+            C.c_void_p(dists.data_ptr()), C.c_void_p(counts.data_ptr()),
+            C.c_void_p(stats.data_ptr()) if stats is not None else None, C.c_void_p(_raw_stream(stream, q.device))))
+        return ids, dists, counts
+
     def set_rerank_elements(self, elements):
         """Attaches the angular f32 rows (an angular elements file image, `bytes`) that re-rank the candidates of
         this angular_int index: at least len(self) rows of its width.  Once, before searching."""
@@ -755,6 +850,20 @@ class MultiGranne:
         ids, dists, counts, _ = _host_outputs(nq, k, np.uint64)
         _check(load_library().granne_b200_multi_exact_search_within_batch(
             self._h, _ptr(q), nq, fmt, _ptr(offsets), _ptr(cand), k, _ptr(ids), _ptr(dists), _ptr(counts)))
+        return ids, dists, counts
+
+    def search_batch_filtered(self, queries, filters, query_filter=None, max_search=DEFAULT_MAX_SEARCH,
+                              num_elements=DEFAULT_NUM_ELEMENTS, already_element=False):
+        """Granne.search_batch_filtered over all parts (granne_b200_multi_search_filtered_batch): the filters are over
+        GLOBAL ids (a bool mask of shape (len,) or (F, len), or uint32 words), the results are GLOBAL uint64 ids."""
+        q, fmt = _host_queries(queries, already_element)
+        nq, k = q.shape[0], int(num_elements)
+        words = _filter_words(filters, len(self))
+        qf = _query_filter(query_filter, nq)
+        ids, dists, counts, _ = _host_outputs(nq, k, np.uint64)
+        _check(load_library().granne_b200_multi_search_filtered_batch(
+            self._h, _ptr(q), nq, fmt, int(max_search), k, _ptr(words), words.shape[0], words.shape[1],
+            _ptr(qf) if qf is not None else None, _ptr(ids), _ptr(dists), _ptr(counts)))
         return ids, dists, counts
 
     def set_rerank_elements(self, elements):

@@ -643,9 +643,12 @@ struct LaunchPlan {
     int rows;           // fast list rows R (capacity 32*R), 0 = generic list
     EngineTiles engine;
     size_t smem;        // fast pass total
+    size_t extra;       // bytes every pass appends behind its own shared memory (a filtered search's admitted list)
 };
 
-LaunchPlan make_plan(const Handle* h, uint32_t max_search) {
+// extra: shared memory a pass needs behind its own (0 for an unfiltered search); the generic pass's visited set
+// shrinks to leave room for it.
+LaunchPlan make_plan(const Handle* h, uint32_t max_search, size_t extra = 0) {
     LaunchPlan p{};
     // fast list: capacity 32*R with R odd (conflict-free lane-major access); slack >= 16 entries over max_search
     p.rows = 0;
@@ -663,13 +666,14 @@ LaunchPlan make_plan(const Handle* h, uint32_t max_search) {
     p.vis_retry = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(want * 8, want), std::max<uint64_t>(cap_slots, want));
     want = std::min<uint64_t>(want * h->vis_scale.load(), std::max<uint64_t>(cap_slots, want));
     p.engine = engine_tiles(h->dev);
+    p.extra = extra;
     const size_t base = p.engine.base_smem;
-    const size_t budget = h->smem_optin;
+    const size_t budget = h->smem_optin - extra;
     if (p.rows) {
         // fast pass: list in shared memory, visited set in global memory
         p.vis_slots = (uint32_t)want;
         p.vis_upper = std::min<uint32_t>(1024, p.vis_slots);
-        p.smem = base + gb::fast_list_bytes(p.rows);
+        p.smem = base + gb::fast_list_bytes(p.rows) + extra;
         return p;
     }
     const size_t fixed = base + (size_t)p.list_cap * 8;
@@ -681,7 +685,7 @@ LaunchPlan make_plan(const Handle* h, uint32_t max_search) {
     if (fixed + want * 4 > budget) want = (budget - fixed) / 4 / 32 * 32;  // huge max_search: overflow -> slow path
     p.vis_slots = (uint32_t)want;
     p.vis_upper = std::min<uint32_t>(1024, p.vis_slots);
-    p.smem = fixed + (size_t)p.vis_slots * 4;
+    p.smem = fixed + (size_t)p.vis_slots * 4 + extra;
     return p;
 }
 
@@ -735,13 +739,13 @@ int resident_ctas(const Handle* h, size_t smem, int* occ) {
     return GRANNE_B200_OK;
 }
 
-template <class Dist, int R>
+template <class Dist, int R, bool FILT>
 int launch_kernels(Handle* h, Workspace* w, gb::SearchArgs a, const LaunchPlan& plan, cudaStream_t stream,
                    const gb::DeviceIndex& dv) {
     constexpr int RR = retry_rows(R);
-    constexpr auto kern = gb::search_kernel<Dist, R>;
-    constexpr auto retry = gb::search_kernel<Dist, (RR > 0 ? RR : 1)>;
-    constexpr auto slow = gb::search_kernel<Dist, 0>;
+    constexpr auto kern = gb::search_kernel<Dist, R, FILT>;
+    constexpr auto retry = gb::search_kernel<Dist, (RR > 0 ? RR : 1), FILT>;
+    constexpr auto slow = gb::search_kernel<Dist, 0, FILT>;
     // fast pass
     int occ = 0;
     int rc = resident_ctas<kern>(h, plan.smem, &occ);
@@ -780,7 +784,7 @@ int launch_kernels(Handle* h, Workspace* w, gb::SearchArgs a, const LaunchPlan& 
         const unsigned rgrid = (unsigned)std::min<unsigned long long>(a.nq, (unsigned long long)h->num_sms * 4);
         if ((rc = w->d_vis_retry.grow((size_t)h->num_sms * 4 * r.vis_slots, stream))) return rc;
         r.vis_global = w->d_vis_retry.get();
-        const size_t rsmem = plan.engine.base_smem + gb::fast_list_bytes(RR > 0 ? RR : 1);
+        const size_t rsmem = plan.engine.base_smem + gb::fast_list_bytes(RR > 0 ? RR : 1) + plan.extra;
         if ((rc = launch_warps<retry>(h, rgrid, rsmem, stream, dv, r))) return rc;
     }
     // slow pass: re-runs only the queries that are still flagged (exits immediately if none)
@@ -791,7 +795,7 @@ int launch_kernels(Handle* h, Workspace* w, gb::SearchArgs a, const LaunchPlan& 
     s.work_counter = w->d_counters.get() + 2;
     s.gate_in = w->d_counters.get() + (have_retry ? 4 : 3);
     s.gate_out = nullptr;
-    return launch_warps<slow>(h, h->slow_ctas, plan.engine.base_smem, stream, dv, s);
+    return launch_warps<slow>(h, h->slow_ctas, plan.engine.base_smem + plan.extra, stream, dv, s);
 }
 
 // ---- workspace pool -----------------------------------------------------------------------------------------------
@@ -877,11 +881,11 @@ int validate_batch(const Handle* h, const void* q, size_t nq, int fmt, uint32_t 
     return GRANNE_B200_OK;
 }
 
+constexpr const char* kMaxSearchRule = "max_search must be >= 1 (the reference panics on 0, src/index/mod.rs:1019)";
+
 int validate_search(const Handle* h, const void* q, size_t nq, int fmt, uint32_t max_search, uint32_t k,
                     const void* ids, const void* dists) {
-    return validate_batch(h, q, nq, fmt, k, ids, dists,
-                          max_search == 0 ? "max_search must be >= 1 (the reference panics on 0, src/index/mod.rs:1019)"
-                                          : nullptr);
+    return validate_batch(h, q, nq, fmt, k, ids, dists, max_search == 0 ? kMaxSearchRule : nullptr);
 }
 
 int validate_exact(const Handle* h, const void* q, size_t nq, int fmt, uint32_t k, const void* ids,
@@ -906,12 +910,23 @@ gb::PeerGather device_gather(const granne_b200_peer_gather& pg, unsigned int* do
     return d;
 }
 
-// Enqueues one batch on `stream` with device pointers.  Needs a workspace for status words / slow path.
+// The filters of a filtered search, in device memory (granne_b200_search_filtered_batch_device's arguments).
+struct DeviceFilters {
+    const uint32_t* words;         // num_filters x filter_words u32
+    const uint32_t* query_filter;  // nq entries, or null (every query uses filter 0)
+    uint64_t filter_words;
+    uint32_t num_filters;
+    uint64_t bit_base;             // bit of element 0 (a shard's base in a range-partitioned multi handle)
+};
+
+// Enqueues one batch on `stream` with device pointers.  Needs a workspace for status words / slow path.  `filt`: a
+// filtered search (search_kernel<Dist, R, true>), whose passes each append round_up(k, 32) keys of shared memory.
 int enqueue_search(Handle* h, Workspace* w, const void* d_queries, size_t nq, int fmt, uint32_t max_search,
                    uint32_t k, uint32_t* d_ids, float* d_dists, uint32_t* d_counts, unsigned long long* d_stats,
                    cudaStream_t stream, bool reset_error, const granne_b200_peer_gather* pg = nullptr,
-                   const gb::DeviceIndex* view = nullptr) {
-    const LaunchPlan plan = make_plan(h, max_search);
+                   const gb::DeviceIndex* view = nullptr, const DeviceFilters* filt = nullptr) {
+    const uint32_t filter_cap = (k + 31u) & ~31u;
+    const LaunchPlan plan = make_plan(h, max_search, filt ? (size_t)filter_cap * 8 : 0);
     if (plan.smem == 0 || max_search + 64 > h->slow_list_cap)
         return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "max_search exceeds the supported maximum (about 27000)");
     int rc = w->d_status.grow(nq, stream);
@@ -963,19 +978,31 @@ int enqueue_search(Handle* h, Workspace* w, const void* d_queries, size_t nq, in
     a.pg = pg ? device_gather(*pg, w->d_counters.get() + 5) : gb::PeerGather{};
     a.tiles = plan.engine.tiles;
     a.vis_global = nullptr;
+    if (filt) {
+        a.filters = filt->words;
+        a.query_filter = filt->query_filter;
+        a.filter_words = filt->filter_words;
+        a.filter_bit_base = filt->bit_base;
+        a.num_filters = filt->num_filters;
+        a.filter_cap = filter_cap;
+    }
     // the staged index the kernels see: the handle's own, or a private view of it (compute_order searches single
     // layers without touching the shared handle)
     const gb::DeviceIndex& dv = view ? *view : h->dev;
-    rc = DistDispatch::call(dv, [&](auto e) {
-        using Dist = typename decltype(e)::type;
-        switch (plan.rows) {
-            case 3: return launch_kernels<Dist, 3>(h, w, a, plan, stream, dv);
-            case 7: return launch_kernels<Dist, 7>(h, w, a, plan, stream, dv);
-            case 15: return launch_kernels<Dist, 15>(h, w, a, plan, stream, dv);
-            case 31: return launch_kernels<Dist, 31>(h, w, a, plan, stream, dv);
-            default: return launch_kernels<Dist, 0>(h, w, a, plan, stream, dv);
-        }
-    });
+    auto launch = [&](auto filtered) {
+        constexpr bool FILT = decltype(filtered)::value;
+        return DistDispatch::call(dv, [&](auto e) {
+            using Dist = typename decltype(e)::type;
+            switch (plan.rows) {
+                case 3: return launch_kernels<Dist, 3, FILT>(h, w, a, plan, stream, dv);
+                case 7: return launch_kernels<Dist, 7, FILT>(h, w, a, plan, stream, dv);
+                case 15: return launch_kernels<Dist, 15, FILT>(h, w, a, plan, stream, dv);
+                case 31: return launch_kernels<Dist, 31, FILT>(h, w, a, plan, stream, dv);
+                default: return launch_kernels<Dist, 0, FILT>(h, w, a, plan, stream, dv);
+            }
+        });
+    };
+    rc = filt ? launch(std::true_type{}) : launch(std::false_type{});
     if (rc) return rc;
     GB_CUDA(cudaMemcpyAsync(w->h_retried.get(), w->d_retried.get(), 8, cudaMemcpyDeviceToHost, stream));
     return GRANNE_B200_OK;
@@ -988,6 +1015,8 @@ int error_from_bits(int bits) {
         return fail(GRANNE_B200_ERR_CAPACITY, "exact search workspace exhausted even on the slow path");
     if (bits & gb::kStatusBadList)
         return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "a candidate list has bad offsets or an id >= Index::len");
+    if (bits & gb::kStatusBadFilter)
+        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "a query_filter entry is >= num_filters");
     return GRANNE_B200_OK;
 }
 
@@ -1396,6 +1425,68 @@ int enqueue_within(Handle* h, Workspace* w, const void* d_queries, size_t nq, in
         }
         return (int)GRANNE_B200_OK;
     });
+}
+
+// ---- filtered search (search_kernel<Dist, R, true>) -----------------------------------------------------------------
+// The rules of a filtered call that read no handle, in the order they are reported: validate_batch's, with
+// max_search >= 1 and k <= GRANNE_B200_EXACT_MAX_K as the call's own; then, when nq > 0, the filters' pointer and count.
+int validate_filtered(const Handle* h, const void* q, size_t nq, int fmt, uint32_t max_search, uint32_t k,
+                      const void* ids, const void* dists, const void* filters, uint32_t num_filters) {
+    const int rc = validate_batch(h, q, nq, fmt, k, ids, dists,
+                                  max_search == 0                ? kMaxSearchRule
+                                  : k > GRANNE_B200_EXACT_MAX_K ? "num_neighbors exceeds GRANNE_B200_EXACT_MAX_K (1024)"
+                                                                 : nullptr);
+    if (rc || nq == 0) return rc;
+    if (!filters || num_filters == 0) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "filters is null or num_filters is 0");
+    return GRANNE_B200_OK;
+}
+
+// A bitmap of filter_words words must hold a bit for every id in [0, span).
+int check_filter_words(uint64_t filter_words, uint64_t span) {
+    if (filter_words < (span + 31) / 32)
+        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "filter_words is less than ceil(Index::len / 32)");
+    return GRANNE_B200_OK;
+}
+
+// The host check of a host call's query_filter (null: every query uses filter 0).
+int check_query_filter(const uint32_t* query_filter, size_t nq, uint32_t num_filters) {
+    for (size_t q = 0; query_filter && q < nq; ++q)
+        if (query_filter[q] >= num_filters)
+            return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "a query_filter entry is >= num_filters");
+    return GRANNE_B200_OK;
+}
+
+// A filtered search from host buffers (arguments checked, nq > 0): the filters and query_filter go up in the call's
+// stream order into memory held only until its kernels have run, like the lists of an exact search within lists.
+// bit_base: the bit of element 0 in the bitmaps (a range-partitioned shard reads the global bitmap).
+int search_filtered_host(Handle* h, const void* queries, size_t nq, int fmt, uint32_t max_search, uint32_t k,
+                         const uint32_t* filters, uint32_t num_filters, uint64_t filter_words,
+                         const uint32_t* query_filter, uint64_t bit_base, uint32_t* out_ids, float* out_dists,
+                         uint32_t* out_counts, uint64_t* out_stats) {
+    return host_batch(h, queries, query_bytes(h, nq, fmt), nq, k, out_ids, out_dists, out_counts, out_stats,
+                      [&](Workspace* w, cudaStream_t stream, unsigned long long* d_stats) {
+                          const size_t fbytes = (size_t)num_filters * filter_words * 4;
+                          const size_t qbytes = query_filter ? nq * 4 : 0;
+                          void* mem = nullptr;
+                          GB_CUDA(cudaMallocAsync(&mem, fbytes + qbytes, stream));
+                          uint8_t* m8 = static_cast<uint8_t*>(mem);
+                          const DeviceFilters f{reinterpret_cast<const uint32_t*>(m8),
+                                                query_filter ? reinterpret_cast<const uint32_t*>(m8 + fbytes) : nullptr,
+                                                filter_words, num_filters, bit_base};
+                          const int r = [&] {
+                              GB_CUDA(cudaMemcpyAsync(m8, filters, fbytes, cudaMemcpyHostToDevice, stream));
+                              if (qbytes)
+                                  GB_CUDA(cudaMemcpyAsync(m8 + fbytes, query_filter, qbytes, cudaMemcpyHostToDevice,
+                                                          stream));
+                              return enqueue_search(h, w, w->d_queries.get(), nq, fmt, max_search, k, w->d_ids.get(),
+                                                    w->d_dists, w->d_counts, d_stats, stream, true, nullptr, nullptr,
+                                                    &f);
+                          }();
+                          const cudaError_t fe = cudaFreeAsync(mem, stream);
+                          if (r) return r;
+                          GB_CUDA(fe);
+                          return (int)GRANNE_B200_OK;
+                      });
 }
 
 }  // namespace
@@ -1886,6 +1977,37 @@ int granne_b200_exact_search_within_batch_device(granne_b200_index* h, const voi
     return device_batch(h, cuda_stream, [&](Workspace* w, cudaStream_t stream) {
         return enqueue_within(h, w, d_queries, nq, query_format, d_offsets, d_ids, num_neighbors, d_out_ids,
                               d_out_dists, d_out_counts, stream);
+    });
+}
+
+int granne_b200_search_filtered_batch(granne_b200_index* h, const void* queries, size_t nq, int query_format,
+                                      uint32_t max_search, uint32_t num_neighbors, const uint32_t* filters,
+                                      uint32_t num_filters, uint64_t filter_words, const uint32_t* query_filter,
+                                      uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint64_t* out_stats) {
+    int rc = validate_filtered(h, queries, nq, query_format, max_search, num_neighbors, out_ids, out_dists, filters,
+                               num_filters);
+    if (rc || nq == 0) return rc;
+    if ((rc = check_filter_words(filter_words, h->index_len)) ||
+        (rc = check_query_filter(query_filter, nq, num_filters)))
+        return rc;
+    return search_filtered_host(h, queries, nq, query_format, max_search, num_neighbors, filters, num_filters,
+                                filter_words, query_filter, 0, out_ids, out_dists, out_counts, out_stats);
+}
+
+int granne_b200_search_filtered_batch_device(granne_b200_index* h, const void* d_queries, size_t nq, int query_format,
+                                             uint32_t max_search, uint32_t num_neighbors, const uint32_t* d_filters,
+                                             uint32_t num_filters, uint64_t filter_words,
+                                             const uint32_t* d_query_filter, uint32_t* d_out_ids, float* d_out_dists,
+                                             uint32_t* d_out_counts, uint64_t* d_out_stats, void* cuda_stream) {
+    int rc = validate_filtered(h, d_queries, nq, query_format, max_search, num_neighbors, d_out_ids, d_out_dists,
+                               d_filters, num_filters);
+    if (rc || nq == 0) return rc;
+    if ((rc = check_filter_words(filter_words, h->index_len))) return rc;
+    return device_batch(h, cuda_stream, [&](Workspace* w, cudaStream_t stream) {
+        const DeviceFilters f{d_filters, d_query_filter, filter_words, num_filters, 0};
+        return enqueue_search(h, w, d_queries, nq, query_format, max_search, num_neighbors, d_out_ids, d_out_dists,
+                              d_out_counts, reinterpret_cast<unsigned long long*>(d_out_stats), stream, false, nullptr,
+                              nullptr, &f);
     });
 }
 
@@ -2935,6 +3057,37 @@ int granne_b200_multi_exact_search_within_batch(granne_b200_multi* m, const void
                                });
                            });
     });
+}
+
+// REPLICATED: each device runs its slice of the queries with their query_filter entries.  RANGE_PARTITIONED: every
+// shard runs every query on the global bitmaps, reading bit shard_base[s] + local id, and multi_batch merges the shard
+// lists by (distance, global id): shard s scores S_s(q), so the result is the first k of the union of the shards'
+// admitted lists.
+int granne_b200_multi_search_filtered_batch(granne_b200_multi* m, const void* queries, size_t nq, int query_format,
+                                            uint32_t max_search, uint32_t num_neighbors, const uint32_t* filters,
+                                            uint32_t num_filters, uint64_t filter_words, const uint32_t* query_filter,
+                                            uint64_t* out_ids, float* out_dists, uint32_t* out_counts) {
+    if (!m) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "multi handle is null");
+    int rc = validate_filtered(m->parts[0], queries, nq, query_format, max_search, num_neighbors, out_ids, out_dists,
+                               filters, num_filters);
+    if (rc || nq == 0) return rc;
+    const bool range = m->mode == GRANNE_B200_MODE_RANGE_PARTITIONED;
+    uint64_t span = m->total_len;  // ids [0, span) are global ids of some part
+    for (size_t s = 0; range && s < m->parts.size(); ++s) span = std::max(span, m->base[s] + m->parts[s]->index_len);
+    if ((rc = check_filter_words(filter_words, span)) || (rc = check_query_filter(query_filter, nq, num_filters)))
+        return rc;
+    const bool i8q = m->kind == GRANNE_B200_ANGULAR_INT && query_format == GRANNE_B200_QUERY_ELEMENT;
+    const size_t qrow = (size_t)m->dim * (i8q ? 1 : 4);
+    return multi_batch(m, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts,
+                       [&](granne_b200_index* h, const void* q, size_t cnt, uint32_t* ids, float* ds, uint32_t* c) {
+                           const size_t s = std::find(m->parts.begin(), m->parts.end(), h) - m->parts.begin();
+                           const size_t b =
+                               (static_cast<const uint8_t*>(q) - static_cast<const uint8_t*>(queries)) / qrow;
+                           return search_filtered_host(h, q, cnt, query_format, max_search, num_neighbors, filters,
+                                                       num_filters, filter_words,
+                                                       query_filter ? query_filter + b : nullptr,
+                                                       range ? m->base[s] : 0, ids, ds, c, nullptr);
+                       });
 }
 
 // Every image is checked on the host against its part before any part stages rows (multi_attach_rerank).

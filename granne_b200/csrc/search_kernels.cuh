@@ -111,6 +111,7 @@ struct SmemLayout {
 // per-query status bits (device side)
 constexpr int kStatusOverflow = 1;   // workspace too small for an exact answer -> slow path
 constexpr int kStatusNotFinite = 2;  // NaN distance (reference panics)
+constexpr int kStatusBadFilter = 16; // filtered search: a query_filter entry >= num_filters (ERR_INVALID_ARGUMENT)
 
 // The staged index in HBM.
 struct DeviceIndex {
@@ -180,6 +181,16 @@ struct SearchArgs {
     int slow_pass;   // this pass uses the global slow workspaces (list + visited set)
     int final_pass;  // nothing comes after this pass
     PeerGather pg;
+    // filtered search only (search_kernel<Dist, R, true>): num_filters bitmaps of filter_words u32 words each; query
+    // q keeps the scored bottom-layer candidates i whose bit filter_bit_base + i is set in bitmap query_filter[q]
+    // (query_filter null: bitmap 0), in a sorted list of filter_cap = round_up(k, 32) keys behind the pass's own
+    // shared memory
+    const uint32_t* filters;
+    const uint32_t* query_filter;
+    unsigned long long filter_words;
+    unsigned long long filter_bit_base;
+    uint32_t num_filters;
+    uint32_t filter_cap;
 };
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -916,10 +927,69 @@ __device__ __forceinline__ bool vis_bucket_insert(uint32_t* tab, uint32_t nbucke
 // ------------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t warp_min_u32(unsigned mask, uint32_t v) { return __reduce_min_sync(mask, v); }
 
-template <class Dist>
+// ------------------------------------------------------------------------------------------------------------------
+// Filtered search: the admitted list.  Beside the traversal (which it never influences) the bottom layer's search
+// offers every candidate it scores to a sorted list of the `cap` smallest make_key keys among those whose filter bit
+// is set; the kernel then reports the first k of that list instead of the expanded entries of L.  The ids a layer
+// search scores are distinct (the visited set), so keys are unique and the list is exactly the first cap keys of
+// S(q) ∩ A in (distance, id) order.  The keys live in shared memory; all fields are warp-uniform.
+// ------------------------------------------------------------------------------------------------------------------
+struct AdmitList {
+    unsigned long long* keys;  // sorted ascending, n valid
+    const uint32_t* bits;      // the query's filter bitmap, bit (bit_base + id) LSB first
+    unsigned long long bit_base;
+    uint32_t cap, n;
+};
+
+// Lane l offers (id, d) when `scored`: admitted keys below the list's last (or all, while it is not full) are merged
+// in, every lane of the warp takes part.  The merge is search_layer's: each offered key's rank is its lower bound in the
+// list plus the offered keys below it, and the entries at or after the first rank move up row by row, top-down.
+__device__ __forceinline__ void admit_offer(AdmitList& A, uint32_t id, float d, bool scored, int lane) {
+    bool pass = false;
+    if (scored) {
+        const unsigned long long b = A.bit_base + id;
+        pass = (__ldg(A.bits + (b >> 5)) >> (uint32_t)(b & 31u)) & 1u;
+    }
+    const unsigned long long key = make_key(d, id);
+    if (A.n == A.cap) pass = pass && key < A.keys[A.cap - 1];
+    const unsigned pm = __ballot_sync(kFullMask, pass);
+    if (pm == 0) return;
+    uint32_t lo = 0, hi = A.n;
+    for (int it = 32 - __clz(A.n); it > 0; --it) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (lo < hi) {
+            if (A.keys[mid] < key)
+                lo = mid + 1;
+            else
+                hi = mid;
+        }
+    }
+    uint32_t rank_n = 0;
+    for (unsigned t = pm; t; t &= t - 1) rank_n += (__shfl_sync(kFullMask, key, __ffs(t) - 1) < key) ? 1u : 0u;
+    const uint32_t new_pos = lo + rank_n;
+    const uint32_t min_rank = warp_min_u32(kFullMask, pass ? lo : 0xFFFFFFFFu);
+    for (int base = (int)((A.n - 1) & ~31u); base >= (int)(min_rank & ~31u); base -= 32) {
+        const uint32_t j = base + lane;
+        const bool in = (j < A.n) && (j >= min_rank);
+        unsigned long long v = 0;
+        if (in) v = A.keys[j];
+        uint32_t sh = 0;
+        for (unsigned t = pm; t; t &= t - 1) sh += (__shfl_sync(kFullMask, lo, __ffs(t) - 1) <= j) ? 1u : 0u;
+        __syncwarp();
+        if (in && j + sh < A.cap) A.keys[j + sh] = v;
+    }
+    __syncwarp();
+    if (pass && new_pos < A.cap) A.keys[new_pos] = key;
+    __syncwarp();
+    A.n = min(A.n + (uint32_t)__popc(pm), A.cap);
+}
+
+// FILT: when `admit` (the bottom layer), `adm` receives every candidate this layer scores (admit_offer).
+template <class Dist, bool FILT = false>
 __device__ __forceinline__ void search_layer(const DeviceIndex& ix, WarpCtx& c, Dist& dist, const uint32_t* rows,
                                              const uint32_t width, const uint32_t entrypoint, const uint32_t ef,
-                                             const uint32_t cap, const uint32_t vis_slots, uint32_t* out_n) {
+                                             const uint32_t cap, const uint32_t vis_slots, uint32_t* out_n,
+                                             AdmitList* adm = nullptr, bool admit = false) {
     unsigned long long* L = c.list;
     const int lane = c.lane;
     for (uint32_t i = lane; i < vis_slots; i += 32) c.visited[i] = kUnusedId;
@@ -941,6 +1011,12 @@ __device__ __forceinline__ void search_layer(const DeviceIndex& ix, WarpCtx& c, 
             vis_insert(c.visited, vis_slots, entrypoint);
         }
         __syncwarp();
+        if constexpr (FILT) {
+            if (admit) {
+                adm->n = 0;
+                admit_offer(*adm, entrypoint, d0, lane == 0, lane);
+            }
+        }
     }
     uint32_t n = 1;
     uint32_t n_exp = 0;
@@ -1028,6 +1104,9 @@ __device__ __forceinline__ void search_layer(const DeviceIndex& ix, WarpCtx& c, 
                 c.status |= kStatusNotFinite;
                 *out_n = n;
                 return;
+            }
+            if constexpr (FILT) {
+                if (admit) admit_offer(*adm, my_id, d, lane < k, lane);
             }
             const unsigned long long my_key = make_key(d, my_id);
             // !res.is_full() || distance < res.peek().0   (:1029)
@@ -1146,11 +1225,13 @@ __host__ __device__ constexpr uint32_t fast_list_pow2(int R) {
 // bytes of shared memory the fast list needs: Ld[P] + Li[32*R]
 __host__ __device__ constexpr uint32_t fast_list_bytes(int R) { return (fast_list_pow2(R) + 32u * (uint32_t)R) * 4u; }
 
-template <class Dist, int R>
+// FILT: `adm` receives every candidate this layer scores (admit_offer); only the bottom layer is searched with it.
+template <class Dist, int R, bool FILT = false>
 __device__ __forceinline__ void search_layer_fast(const DeviceIndex& ix, WarpCtx& c, Dist& dist, uint32_t* Ld,
                                                   const uint32_t* rows, const uint32_t width,
                                                   const uint32_t entrypoint, const uint32_t ef,
-                                                  const uint32_t vis_slots, uint32_t* out_n) {
+                                                  const uint32_t vis_slots, uint32_t* out_n,
+                                                  AdmitList* adm = nullptr) {
     constexpr uint32_t cap = 32u * R;
     constexpr uint32_t P = fast_list_pow2(R);  // Ld is padded to a power of two > cap with sentinels
     constexpr uint32_t kFlag = 0x80000000u, kDMask = 0x7FFFFFFFu;
@@ -1184,6 +1265,10 @@ __device__ __forceinline__ void search_layer_fast(const DeviceIndex& ix, WarpCtx
             Li[0] = entrypoint;
         }
         __syncwarp();
+        if constexpr (FILT) {
+            adm->n = 0;
+            admit_offer(*adm, entrypoint, d0, lane == 0, lane);
+        }
     }
     uint32_t n = 1, n_exp = 0, cursor = 0, pos_thr = 0, thr_bits = 0;
     uint32_t spec_id = kUnusedId, spec_slot = 0;
@@ -1314,6 +1399,7 @@ __device__ __forceinline__ void search_layer_fast(const DeviceIndex& ix, WarpCtx
                 *out_n = n;
                 return;
             }
+            if constexpr (FILT) admit_offer(*adm, my_id, d, lane < k, lane);
             const uint32_t my_d = __float_as_uint(d);
             // !res.is_full() || distance < res.peek().0   (:1029)
             bool pass = (lane < k) && (n_exp < ef || my_d < thr_bits);
@@ -1536,10 +1622,29 @@ __global__ void publish_seq_kernel(const PeerGather pg) {
     publish_seq(pg);
 }
 
+// Resident one-warp CTAs per SM the filtered fast kernel is register-limited to.  The admitted list's state costs a
+// few registers, which the widest fixed f32 engine and the embeddings engine cannot spare under GB_MIN_BLOCKS's cap
+// without spilling to local memory (DistSum already spills there unfiltered).
+template <class Dist>
+struct FilteredMinBlocks {
+    static constexpr int value = GB_MIN_BLOCKS;
+};
+template <>
+struct FilteredMinBlocks<DistF32<8>> {
+    static constexpr int value = 20;
+};
+template <>
+struct FilteredMinBlocks<DistSum> {
+    static constexpr int value = 16;
+};
+
 // R == 0: generic list (64-bit keys, any capacity, shared or global memory) — the slow pass and very large max_search.
 // R  > 0: fast list with capacity 32*R for the bottom layer (upper layers always use R = 1).
-template <class Dist, int R>
-__global__ void __launch_bounds__(32, R > 0 ? GB_MIN_BLOCKS : 1) search_kernel(const DeviceIndex ix, const SearchArgs a) {
+// FILT: filtered search (SearchArgs' filter fields): the same traversal, counters and pass ladder, with the bottom
+// layer's scored candidates offered to an admitted list (AdmitList) that the results are written from.
+template <class Dist, int R, bool FILT = false>
+__global__ void __launch_bounds__(32, R > 0 ? (FILT ? FilteredMinBlocks<Dist>::value : GB_MIN_BLOCKS) : 1)
+    search_kernel(const DeviceIndex ix, const SearchArgs a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     WarpCtx c;
     c.lane = threadIdx.x;
@@ -1588,6 +1693,17 @@ __global__ void __launch_bounds__(32, R > 0 ? GB_MIN_BLOCKS : 1) search_kernel(c
             c.visited = reinterpret_cast<uint32_t*>(sp);
         }
     }
+    AdmitList adm;
+    if constexpr (FILT) {
+        // behind the pass's own shared memory: the fast list, or the generic list and visited set (the slow pass
+        // keeps both in global memory)
+        unsigned char* ap = sp;
+        if (!a.slow_pass) ap += R > 0 ? (size_t)fast_list_bytes(R > 0 ? R : 1) : (size_t)a.vis_slots * 4u;
+        adm.keys = reinterpret_cast<unsigned long long*>(ap);
+        adm.cap = a.filter_cap;
+        adm.bit_base = a.filter_bit_base;
+        adm.n = 0;
+    }
     Dist dist;
     if (a.pass && *reinterpret_cast<volatile unsigned int*>(a.gate_in) == 0u) {  // nothing flagged
         if (a.final_pass) signal_peers(a, c.lane);
@@ -1607,11 +1723,17 @@ __global__ void __launch_bounds__(32, R > 0 ? GB_MIN_BLOCKS : 1) search_kernel(c
         c.q_norm_i8 = 0;
         prepare_query(ix, a, c, qi);
         dist.load_query(ix, c);
+        if constexpr (FILT) {
+            const uint32_t f = a.query_filter ? a.query_filter[qi] : 0u;
+            if (f >= a.num_filters) c.status |= kStatusBadFilter;
+            adm.bits = a.filters + (size_t)(f < a.num_filters ? f : 0u) * a.filter_words;
+            adm.n = 0;
+        }
 
         uint32_t n = 0;
         const uint32_t k = a.num_neighbors;
         uint32_t found = 0;
-        if (ix.num_layers > 0 && !(c.status & kStatusNotFinite)) {
+        if (ix.num_layers > 0 && !(c.status & (FILT ? kStatusNotFinite | kStatusBadFilter : kStatusNotFinite))) {
             // find_entrypoint (:984-997): max_search = 1 descent through the upper layers, then the bottom layer
             // with the caller's max_search (:970-973).
             uint32_t entrypoint = 0;
@@ -1620,9 +1742,9 @@ __global__ void __launch_bounds__(32, R > 0 ? GB_MIN_BLOCKS : 1) search_kernel(c
                 const uint32_t cap1 = list_cap < 32 ? list_cap : 32;
                 for (int l = 0; l <= bl && c.status == 0; ++l) {
                     const bool bottom = (l == bl);
-                    search_layer(ix, c, dist, ix.layer_rows[l], ix.layer_width[l], entrypoint,
-                                 bottom ? a.max_search : 1u, bottom ? list_cap : cap1,
-                                 bottom ? vis_slots : vis_upper, &n);
+                    search_layer<Dist, FILT>(ix, c, dist, ix.layer_rows[l], ix.layer_width[l], entrypoint,
+                                             bottom ? a.max_search : 1u, bottom ? list_cap : cap1,
+                                             bottom ? vis_slots : vis_upper, &n, &adm, bottom);
                     if (bottom || c.status) break;
                     uint32_t ep = 0;  // res[0]: first expanded entry
                     for (uint32_t base = 0; base < n; base += 32) {
@@ -1635,7 +1757,7 @@ __global__ void __launch_bounds__(32, R > 0 ? GB_MIN_BLOCKS : 1) search_kernel(c
                     }
                     entrypoint = ep;
                 }
-                if (c.status == 0) {
+                if (c.status == 0 && !FILT) {
                     // res.into_sorted_vec().take(num_neighbors) (:974-977, :1036)
                     const uint32_t limit = a.max_search < k ? a.max_search : k;
                     uint32_t cnt = 0;
@@ -1664,9 +1786,9 @@ __global__ void __launch_bounds__(32, R > 0 ? GB_MIN_BLOCKS : 1) search_kernel(c
                     entrypoint = ep;
                 }
                 if (c.status == 0)
-                    search_layer_fast<Dist, RB>(ix, c, dist, fast_list, ix.layer_rows[bl], ix.layer_width[bl],
-                                                entrypoint, a.max_search, vis_slots, &n);
-                if (c.status == 0) {
+                    search_layer_fast<Dist, RB, FILT>(ix, c, dist, fast_list, ix.layer_rows[bl], ix.layer_width[bl],
+                                                      entrypoint, a.max_search, vis_slots, &n, &adm);
+                if (c.status == 0 && !FILT) {
                     const uint32_t* Li = Ld + fast_list_pow2(RB);
                     const uint32_t limit = a.max_search < k ? a.max_search : k;
                     uint32_t cnt = 0;
@@ -1682,6 +1804,22 @@ __global__ void __launch_bounds__(32, R > 0 ? GB_MIN_BLOCKS : 1) search_kernel(c
                     }
                     found = cnt < limit ? cnt : limit;
                 }
+            }
+            if constexpr (FILT) {
+                // the first min(k, n) admitted keys (k may exceed max_search)
+                if (c.status == 0) {
+                    found = adm.n < k ? adm.n : k;
+                    for (uint32_t r = c.lane; r < found; r += 32) {
+                        const unsigned long long v = adm.keys[r];
+                        store_result(a, qi, k, r, key_id(v), __uint_as_float(key_dbits(v)));
+                    }
+                }
+            }
+        }
+        if constexpr (FILT) {
+            if (c.status & kStatusBadFilter) {
+                found = 0;
+                if (c.lane == 0) atomicOr(a.error_flag, kStatusBadFilter);
             }
         }
         if (c.status & kStatusOverflow) {

@@ -225,6 +225,46 @@ int granne_b200_exact_search_within_batch_device(granne_b200_index* h, const voi
                                                  uint32_t num_neighbors, uint32_t* d_out_ids, float* d_out_dists,
                                                  uint32_t* d_out_counts, void* cuda_stream);
 
+/* ---- filtered search: the k nearest admitted elements among those the graph search scores ---------------------------
+ * NOT a reference function: granne_b200_search_batch's traversal, unchanged, with its scored candidates filtered by an
+ * id bitmap — a tenant's, a category's or an ACL's ids.  For a query q let B be the bottom layer and S(q) the elements
+ * whose distance granne_b200_search_batch(q, max_search) computes in B: B's entry point and every layer-B neighbour of
+ * every element its layer-B search expands.  With A the ids the query's filter admits, the result is the first
+ * min(k, |S(q) ∩ A|) elements of S(q) ∩ A ordered by (distance, id), distances as the handle's search computes them,
+ * bit for bit.  The expansions, the visited set and stats columns 0..2 (n_dist, n_expand, n_nbr) are
+ * granne_b200_search_batch's for the same query and max_search, whatever the filter; a larger max_search widens S(q).
+ * Every element of S(q) strictly closer than the last of search_batch(q, max_search, max_search) is among its results,
+ * so an all-admitting filter returns search_batch(q, max_search, k) (k <= max_search) whenever that call's k-th
+ * distance is strictly below its max_search-th, or it returns fewer than max_search results.  There
+ * is no exact fallback: a selective filter may return fewer than k (granne_b200_exact_search_within_batch ranks a
+ * list of ids exactly).
+ *   filters        num_filters bitmaps of filter_words u32 words each, bitmap f at filters + f * filter_words; id i is
+ *                  admitted by filter f iff bit i % 32 (LSB first) of word i / 32 of bitmap f is set.  Bits at or
+ *                  beyond Index::len are ignored.
+ *   filter_words   >= ceil(Index::len / 32)
+ *   query_filter   nq u32 in [0, num_filters): the filter of each query; NULL: every query uses filter 0
+ *   num_neighbors  k, 0..GRANNE_B200_EXACT_MAX_K; k may exceed max_search
+ *   out_*          as granne_b200_search_batch (ids padded with 0xFFFFFFFF, dists with +inf); out_stats' column 3 is
+ *                  the answering pass of the filtered call's own ladder
+ * ERR_INVALID_ARGUMENT, in this order: the handle is NULL; an unknown query format; max_search == 0; k >
+ * GRANNE_B200_EXACT_MAX_K; nq above the batch limit; a NULL queries or output buffer; then, when nq > 0: filters NULL or
+ * num_filters == 0; filter_words < ceil(Index::len / 32); and (host call) a query_filter entry >= num_filters.  The
+ * host call checks all of them before any device call and copies the filters and query_filter to the device in its one
+ * round trip, into memory held only until its kernels have run.  ERR_NOT_FINITE / ERR_CAPACITY as in search. */
+int granne_b200_search_filtered_batch(granne_b200_index* h, const void* queries, size_t nq, int query_format,
+                                      uint32_t max_search, uint32_t num_neighbors, const uint32_t* filters,
+                                      uint32_t num_filters, uint64_t filter_words, const uint32_t* query_filter,
+                                      uint32_t* out_ids, float* out_dists, uint32_t* out_counts, uint64_t* out_stats);
+/* Same with DEVICE pointers (queries, filters, query_filter, outputs) on cuda_stream (NULL = the default stream),
+ * asynchronous like granne_b200_search_batch_device.  The host checks the rules up to filter_words; the kernel checks
+ * query_filter: a query whose entry is >= num_filters gets count 0 and padding, and granne_b200_stream_status reports
+ * ERR_INVALID_ARGUMENT. */
+int granne_b200_search_filtered_batch_device(granne_b200_index* h, const void* d_queries, size_t nq, int query_format,
+                                             uint32_t max_search, uint32_t num_neighbors, const uint32_t* d_filters,
+                                             uint32_t num_filters, uint64_t filter_words,
+                                             const uint32_t* d_query_filter, uint32_t* d_out_ids, float* d_out_dists,
+                                             uint32_t* d_out_counts, uint64_t* d_out_stats, void* cuda_stream);
+
 /* ---- two-stage search: traverse angular_int rows, re-rank by exact f32 angular distance ----------------------------
  * NOT a reference function: what a user of granne assembles by hand from two containers over one index.  For an
  * angular_int handle h with an attached container F (angular rows or SumEmbeddings) and a raw f32 query q:
@@ -335,6 +375,16 @@ int granne_b200_multi_exact_search_within_batch(granne_b200_multi* m, const void
                                                 int query_format, const uint64_t* offsets, const uint64_t* ids,
                                                 uint32_t num_neighbors, uint64_t* out_ids, float* out_dists,
                                                 uint32_t* out_counts);
+/* granne_b200_search_filtered_batch over a multi handle: the bitmaps are over GLOBAL ids, results are u64 GLOBAL ids.
+ * REPLICATED slices the queries together with their query_filter entries over the devices; RANGE_PARTITIONED runs
+ * every query on every shard, shard s reading bit shard_base[s] + local id of the same bitmaps, and merges the shard
+ * lists by (distance, global id).  filter_words must cover every part's ids: >= ceil(max_s(shard_base[s] + Index::len
+ * of shard s) / 32) (REPLICATED: ceil(Index::len / 32)).  The rules and their order are the single-device call's,
+ * with "multi handle is null" first; all are checked on the host before any device call. */
+int granne_b200_multi_search_filtered_batch(granne_b200_multi* m, const void* queries, size_t nq, int query_format,
+                                            uint32_t max_search, uint32_t num_neighbors, const uint32_t* filters,
+                                            uint32_t num_filters, uint64_t filter_words, const uint32_t* query_filter,
+                                            uint64_t* out_ids, float* out_dists, uint32_t* out_counts);
 /* granne_b200_set_rerank_elements on every part: REPLICATED takes one image (elements_bytes[0]) and stages it on every
  * device; RANGE_PARTITIONED takes one image per shard.  Every image is checked before any is staged; if a part then fails to
  * stage its rows (a device error), the parts this call attached release theirs again, so the call can be repeated. */

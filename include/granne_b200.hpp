@@ -250,6 +250,22 @@ public:
                                                     counts.data()));
         return detail::result_lists<SearchResult>(ids, dists, counts, num_neighbors);
     }
+    // Filtered search (granne_b200_search_filtered_batch): search_batch's traversal, unchanged, keeping the first k
+    // elements by (distance, id) among those it scores in the bottom layer that the query's filter admits.  `filters`
+    // holds num_filters bitmaps of filter_words u32 words (id i: bit i % 32 of word i / 32, filter_words >=
+    // ceil(len() / 32)); query_filter (may be null) picks each query's bitmap.  k <= GRANNE_B200_EXACT_MAX_K.  Not a
+    // reference function.
+    std::vector<SearchResult> search_filtered(const void* queries, size_t nq, int query_format, size_t max_search,
+                                              size_t num_neighbors, const uint32_t* filters, uint32_t num_filters,
+                                              uint64_t filter_words, const uint32_t* query_filter = nullptr) const {
+        std::vector<uint32_t> ids(nq * num_neighbors), counts(nq);
+        std::vector<float> dists(nq * num_neighbors);
+        check(granne_b200_search_filtered_batch(h_, queries, nq, query_format, static_cast<uint32_t>(max_search),
+                                                static_cast<uint32_t>(num_neighbors), filters, num_filters,
+                                                filter_words, query_filter, ids.data(), dists.data(), counts.data(),
+                                                nullptr));
+        return detail::result_lists<SearchResult>(ids, dists, counts, num_neighbors);
+    }
 
     // Two-stage search (granne_b200_search_rerank_batch): attach the container of this angular_int index's elements
     // once (angular f32 rows, or the SumEmbeddings container the rows were computed from), then search_rerank
@@ -421,6 +437,21 @@ public:
                                                           offsets.data(), cand.data(),
                                                           static_cast<uint32_t>(num_neighbors), ids.data(), d.data(),
                                                           c.data()));
+        return detail::result_lists<Result>(ids, d, c, num_neighbors);
+    }
+    // Granne::search_filtered over every part for nq raw f32 queries: the bitmaps are over GLOBAL ids, and so are the
+    // results (granne_b200_multi_search_filtered_batch)
+    std::vector<Result> search_filtered(const std::vector<float>& queries, size_t max_search, size_t num_neighbors,
+                                        const uint32_t* filters, uint32_t num_filters, uint64_t filter_words,
+                                        const uint32_t* query_filter = nullptr) const {
+        const size_t nq = dim_ ? queries.size() / dim_ : 0;
+        std::vector<uint64_t> ids(nq * num_neighbors);
+        std::vector<float> d(nq * num_neighbors);
+        std::vector<uint32_t> c(nq);
+        check(granne_b200_multi_search_filtered_batch(h_, queries.data(), nq, GRANNE_B200_QUERY_RAW_F32,
+                                                      static_cast<uint32_t>(max_search),
+                                                      static_cast<uint32_t>(num_neighbors), filters, num_filters,
+                                                      filter_words, query_filter, ids.data(), d.data(), c.data()));
         return detail::result_lists<Result>(ids, d, c, num_neighbors);
     }
 
