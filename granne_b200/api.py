@@ -496,10 +496,7 @@ class Granne:
                                   stream=None):
         """Device-resident exact_search_batch: CUDA tensors in and out, asynchronous on `stream` (a torch.cuda.Stream
         or a raw cudaStream_t; default: the current torch stream); a NaN distance is reported by stream_status()."""
-        import torch
-
-        q = self._check_device_queries(queries)
-        fmt = QUERY_ELEMENT if already_element or q.dtype == torch.int8 else QUERY_RAW_F32
+        q, fmt = self._device_queries(queries, already_element)
         nq, k = q.shape[0], int(num_elements)
         ids, dists, counts = _device_outputs(q, k, out)
         _check(load_library().granne_b200_exact_search_batch_device(
@@ -531,8 +528,7 @@ class Granne:
         and checking it here would wait for the device."""
         import torch
 
-        q = self._check_device_queries(queries)
-        fmt = QUERY_ELEMENT if already_element or q.dtype == torch.int8 else QUERY_RAW_F32
+        q, fmt = self._device_queries(queries, already_element)
         nq, k = q.shape[0], int(num_elements)
         for t, dt, what in ((offsets, torch.int64, "offsets"), (ids, torch.int32, "ids")):
             if (not isinstance(t, torch.Tensor) or not t.is_cuda or t.device != q.device or t.dtype != dt
@@ -577,8 +573,7 @@ class Granne:
         checks query_filter: an entry >= F gives its query count 0 and padding, and stream_status() raises."""
         import torch
 
-        q = self._check_device_queries(queries)
-        fmt = QUERY_ELEMENT if already_element or q.dtype == torch.int8 else QUERY_RAW_F32
+        q, fmt = self._device_queries(queries, already_element)
         nq, k = q.shape[0], int(num_elements)
         for t, shape, what in ((filters, None, "filters"), (query_filter, (nq,), "query_filter")):
             if t is None and what == "query_filter":
@@ -713,10 +708,7 @@ class Granne:
         """Device-resident variant: `queries` is a CUDA torch tensor on this index's device; returns CUDA tensors
         (ids int32 view of u32 bits, dists float32, counts int32).  Asynchronous on `stream` (a torch.cuda.Stream or a
         raw cudaStream_t; default: the current torch stream)."""
-        import torch
-
-        q = self._check_device_queries(queries)
-        fmt = QUERY_ELEMENT if already_element or q.dtype == torch.int8 else QUERY_RAW_F32
+        q, fmt = self._device_queries(queries, already_element)
         nq, k = q.shape[0], int(num_elements)
         ids, dists, counts = _device_outputs(q, k, out)
         _check_stats(stats, q)
@@ -731,15 +723,19 @@ class Granne:
                                    stream=None):
         """Like search_batch_device, but the result rows are stored by the kernels straight into every peer's
         gathered buffer described by `gather` (a PeerGather).  stream: as for search_batch_device."""
-        import torch
-
-        q = self._check_device_queries(queries)
-        fmt = QUERY_ELEMENT if already_element or q.dtype == torch.int8 else QUERY_RAW_F32
+        q, fmt = self._device_queries(queries, already_element)
         _check_stats(stats, q)
         _check(load_library().granne_b200_search_batch_device_gather(
             self._h, C.c_void_p(q.data_ptr()), q.shape[0], fmt, int(max_search), int(num_elements), C.byref(gather),
             C.c_void_p(counts.data_ptr()) if counts is not None else None,
             C.c_void_p(stats.data_ptr()) if stats is not None else None, C.c_void_p(_raw_stream(stream, q.device))))
+
+    def _device_queries(self, queries, already_element):
+        """(checked queries, query format) of a device call, as _host_queries gives them for a host call."""
+        import torch
+
+        q = self._check_device_queries(queries)
+        return q, QUERY_ELEMENT if already_element or q.dtype == torch.int8 else QUERY_RAW_F32
 
     def _check_device_queries(self, q):
         """Same checks as the host path (search_batch): a wrong dtype, width, device or a strided view would make the

@@ -120,6 +120,8 @@ struct Buffer {
 template <class T>
 using Pinned = Buffer<T, true>;
 
+constexpr size_t kSearchCounterBytes = 32, kHostCallBytes = 64;  // the start-of-call words (Workspace::d_counters)
+
 // Per-call scratch: device copies of queries/results, status words, stream.  Pooled per handle so that several host
 // threads can search concurrently (the reference's `search` is `&self` and reentrant).
 struct Workspace {
@@ -130,9 +132,11 @@ struct Workspace {
     uint32_t* d_counts = nullptr;
     Buffer<unsigned long long> d_stats;
     Buffer<int> d_status;  // nq ints
-    // one 64-byte block, zeroed once per call: [0..2] work counters of the three passes, [3] fast pass flagged
-    // something, [4] retry pass flagged something, [5] done counter (fused gather), [6] work counter of the re-rank
-    // kernel; d_error = words [8..11]
+    // one 64-byte block: [0..2] work counters of the three passes, [3] fast pass flagged something, [4] retry pass
+    // flagged something, [5] done counter (fused gather), [6] work counter of the re-rank kernel; d_error = words
+    // [8..11].  A call zeroes its words with one memset before its kernels: a host call the whole block, since it
+    // reports the errors of its own kernels only (kHostCallBytes, host_batch); a device call or a builder batch the
+    // counters when it searches, leaving the error word sticky (kSearchCounterBytes).
     Buffer<unsigned int> d_counters;
     int* d_error = nullptr;              // [0]=sticky error bits of this call (inside the counters block)
     Buffer<unsigned long long> d_retried;  // cumulative: queries that needed more than the fast pass
@@ -882,6 +886,7 @@ int validate_batch(const Handle* h, const void* q, size_t nq, int fmt, uint32_t 
 }
 
 constexpr const char* kMaxSearchRule = "max_search must be >= 1 (the reference panics on 0, src/index/mod.rs:1019)";
+constexpr const char* kExactKRule = "num_neighbors exceeds GRANNE_B200_EXACT_MAX_K (1024)";
 
 int validate_search(const Handle* h, const void* q, size_t nq, int fmt, uint32_t max_search, uint32_t k,
                     const void* ids, const void* dists) {
@@ -890,9 +895,7 @@ int validate_search(const Handle* h, const void* q, size_t nq, int fmt, uint32_t
 
 int validate_exact(const Handle* h, const void* q, size_t nq, int fmt, uint32_t k, const void* ids,
                    const void* dists) {
-    return validate_batch(h, q, nq, fmt, k, ids, dists,
-                          k > GRANNE_B200_EXACT_MAX_K ? "num_neighbors exceeds GRANNE_B200_EXACT_MAX_K (1024)"
-                                                      : nullptr);
+    return validate_batch(h, q, nq, fmt, k, ids, dists, k > GRANNE_B200_EXACT_MAX_K ? kExactKRule : nullptr);
 }
 
 gb::PeerGather device_gather(const granne_b200_peer_gather& pg, unsigned int* done_counter) {
@@ -919,11 +922,21 @@ struct DeviceFilters {
     uint64_t bit_base;             // bit of element 0 (a shard's base in a range-partitioned multi handle)
 };
 
-// Enqueues one batch on `stream` with device pointers.  Needs a workspace for status words / slow path.  `filt`: a
-// filtered search (search_kernel<Dist, R, true>), whose passes each append round_up(k, 32) keys of shared memory.
+// The device outputs of a query call, in search_batch's layout: nq x k ids and distances, nq counts, nq x 4 stats (a
+// null pointer: not wanted, where the call allows it).
+struct QueryOut {
+    uint32_t* ids;
+    float* dists;
+    uint32_t* counts;
+    uint64_t* stats;
+};
+
+// Enqueues one batch on `stream` with device pointers.  Needs a workspace for status words / slow path, whose counters
+// the caller has zeroed on `stream` (Workspace::d_counters; the per-query status words need no reset: the fast pass
+// writes every one of them).  `filt`: a filtered search (search_kernel<Dist, R, true>), whose passes each append
+// round_up(k, 32) keys of shared memory.
 int enqueue_search(Handle* h, Workspace* w, const void* d_queries, size_t nq, int fmt, uint32_t max_search,
-                   uint32_t k, uint32_t* d_ids, float* d_dists, uint32_t* d_counts, unsigned long long* d_stats,
-                   cudaStream_t stream, bool reset_error, const granne_b200_peer_gather* pg = nullptr,
+                   uint32_t k, const QueryOut& out, cudaStream_t stream, const granne_b200_peer_gather* pg = nullptr,
                    const gb::DeviceIndex* view = nullptr, const DeviceFilters* filt = nullptr) {
     const uint32_t filter_cap = (k + 31u) & ~31u;
     const LaunchPlan plan = make_plan(h, max_search, filt ? (size_t)filter_cap * 8 : 0);
@@ -950,9 +963,6 @@ int enqueue_search(Handle* h, Workspace* w, const void* d_queries, size_t nq, in
             w->seen_retried = retried;
         }
     }
-    // one memset per call: the work counters / gates of the three passes (and the error word of a host-API call);
-    // the per-query status words need no reset: the fast pass writes every one of them
-    GB_CUDA(cudaMemsetAsync(w->d_counters.get(), 0, reset_error ? 64 : 32, stream));
     gb::SearchArgs a{};
     a.queries = d_queries;
     a.query_format = fmt;
@@ -962,10 +972,10 @@ int enqueue_search(Handle* h, Workspace* w, const void* d_queries, size_t nq, in
     a.list_cap = plan.list_cap;
     a.vis_slots = plan.vis_slots;
     a.vis_slots_upper = plan.vis_upper;
-    a.out_ids = d_ids;
-    a.out_dists = d_dists;
-    a.out_counts = d_counts;
-    a.out_stats = d_stats;
+    a.out_ids = out.ids;
+    a.out_dists = out.dists;
+    a.out_counts = out.counts;
+    a.out_stats = reinterpret_cast<unsigned long long*>(out.stats);
     a.query_status = w->d_status.get();
     a.work_counter = w->d_counters.get();
     a.retried = w->d_retried.get();
@@ -1020,27 +1030,26 @@ int error_from_bits(int bits) {
     return GRANNE_B200_OK;
 }
 
-// Bytes of nq queries in `fmt`: i8 rows when they already are elements of an angular_int index, f32 rows otherwise.
-size_t query_bytes(const Handle* h, size_t nq, int fmt) {
-    const bool i8q = h->dev.kind == gb::kAngularI8 && fmt == GRANNE_B200_QUERY_ELEMENT;
-    return nq * h->dev.dim * (i8q ? 1 : 4);
+// Bytes of one query row in `fmt` for an index of `kind` (gb::ElementKind) and width `dim`: i8 when the queries already
+// are elements of an angular_int index, f32 otherwise.
+size_t query_row_bytes(int kind, uint32_t dim, int fmt) {
+    return (size_t)dim * (kind == gb::kAngularI8 && fmt == GRANNE_B200_QUERY_ELEMENT ? 1 : 4);
 }
 
 // The host-pointer form of a query call (arguments validated, nq > 0), on a pooled workspace and its stream: the
-// queries go up through pinned memory, `enqueue(w, stream, d_stats)` queues the call's kernels from w->d_queries into
-// the workspace's result block (w->d_ids | w->d_dists | w->d_counts; d_stats is null when the caller wants no stats),
-// and one synchronise brings the results and the error word back.  A host call reports its own errors only, so the
-// error word starts the call at zero: enqueue_search zeroes it with its counters (reset_error); an `enqueue` without
-// that memset clears the word itself.
+// queries go up through pinned memory, the call's words are zeroed (Workspace::d_counters), `enqueue(w, stream, out)`
+// queues the call's kernels from w->d_queries into the workspace's result block (w->d_ids | w->d_dists | w->d_counts;
+// out.stats is null when the caller wants no stats), and one synchronise brings the results and the error word back.
 template <class Enqueue>
-int host_batch(Handle* h, const void* queries, size_t qbytes, size_t nq, size_t k, uint32_t* out_ids,
-               float* out_dists, uint32_t* out_counts, uint64_t* out_stats, Enqueue&& enqueue) {
+int host_batch(Handle* h, const void* queries, size_t nq, int fmt, size_t k, uint32_t* out_ids, float* out_dists,
+               uint32_t* out_counts, uint64_t* out_stats, Enqueue&& enqueue) {
     return guarded([&] {
         GB_DEVICE(h->device);
         std::unique_ptr<Workspace> ws;
         int rc = ws_acquire(h, &ws);
         if (rc) return rc;
         Workspace* w = ws.get();
+        const size_t qbytes = nq * query_row_bytes(h->dev.kind, h->dev.dim, fmt);
         const int status = [&] {
             if ((rc = ws_reserve(w, qbytes, nq, k))) return rc;
             cudaStream_t stream = w->stream.get();
@@ -1055,7 +1064,9 @@ int host_batch(Handle* h, const void* queries, size_t qbytes, size_t nq, size_t 
                 hp + ((reinterpret_cast<uint8_t*>(herr + 4) - hp + 15) & ~size_t(15)));
             std::memcpy(hp, queries, qbytes);
             GB_CUDA(cudaMemcpyAsync(w->d_queries.get(), hp, qbytes, cudaMemcpyHostToDevice, stream));
-            if ((rc = enqueue(w, stream, out_stats ? w->d_stats.get() : nullptr))) return rc;
+            GB_CUDA(cudaMemsetAsync(w->d_counters.get(), 0, kHostCallBytes, stream));
+            uint64_t* d_stats = out_stats ? reinterpret_cast<uint64_t*>(w->d_stats.get()) : nullptr;
+            if ((rc = enqueue(w, stream, QueryOut{w->d_ids.get(), w->d_dists, w->d_counts, d_stats}))) return rc;
             // one packed copy: ids | dists | counts (device and pinned layouts match), then the 16-byte error word
             GB_CUDA(cudaMemcpyAsync(hids, w->d_ids.get(), (2 * nq * k + nq) * 4, cudaMemcpyDeviceToHost, stream));
             GB_CUDA(cudaMemcpyAsync(herr, w->d_error, 4 * sizeof(int), cudaMemcpyDeviceToHost, stream));
@@ -1075,18 +1086,47 @@ int host_batch(Handle* h, const void* queries, size_t qbytes, size_t nq, size_t 
 }
 
 // The device-pointer form of a query call (arguments validated, nq > 0): `enqueue(w, stream)` queues the call's
-// kernels on the caller's stream with that stream's workspace.  Asynchronous; errors stay in the workspace's error
-// word until granne_b200_stream_status().
+// kernels on the caller's stream with that stream's workspace, after zeroing its search counters when the call
+// `searches` (Workspace::d_counters).  Asynchronous; errors stay in the workspace's error word until
+// granne_b200_stream_status().
 template <class Enqueue>
-int device_batch(Handle* h, void* cuda_stream, Enqueue&& enqueue) {
+int device_batch(Handle* h, void* cuda_stream, bool searches, Enqueue&& enqueue) {
     return guarded([&] {
         GB_DEVICE(h->device);
         cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
         Workspace* w = nullptr;
         int rc = stream_workspace(h, stream, &w);
         if (rc) return rc;
+        if (searches) GB_CUDA(cudaMemsetAsync(w->d_counters.get(), 0, kSearchCounterBytes, stream));
         return enqueue(w, stream);
     });
+}
+
+struct HostInput { const void* data; size_t bytes; };  // a caller's array that a host call copies to the device
+
+// Runs `enqueue(d)` with the arrays `in` copied up on `stream`, d[i] the device copy of in[i], all in one stream-ordered
+// allocation freed behind the call's kernels: they are the caller's inputs, not workspace, so that long lists or large
+// bitmaps leave no device memory held by the pooled workspace.  An error of the enqueue is reported before one of the
+// free.
+template <size_t N, class Enqueue>
+int with_call_inputs(cudaStream_t stream, const HostInput (&in)[N], Enqueue&& enqueue) {
+    size_t total = 0;
+    for (const HostInput& a : in) total += a.bytes;
+    void* mem = nullptr;
+    GB_CUDA(cudaMallocAsync(&mem, total, stream));
+    const int rc = [&] {
+        const void* d[N];
+        uint8_t* p = static_cast<uint8_t*>(mem);
+        for (size_t i = 0; i < N; p += in[i].bytes, ++i) {
+            d[i] = p;
+            if (in[i].bytes) GB_CUDA(cudaMemcpyAsync(p, in[i].data, in[i].bytes, cudaMemcpyHostToDevice, stream));
+        }
+        return enqueue(d);
+    }();
+    const cudaError_t fe = cudaFreeAsync(mem, stream);
+    if (rc) return rc;
+    GB_CUDA(fe);
+    return GRANNE_B200_OK;
 }
 
 // ---- exact k-NN (exact_kernels.cuh) -------------------------------------------------------------------------------
@@ -1136,14 +1176,14 @@ int exact_scan_rows(Handle* h, Workspace* w, uint32_t qc, uint32_t k, const void
 
 // Enqueues one exact search on `stream`: nq queries (device memory, the caller's format) against [0, Index::len),
 // results in search_batch's layout.  A NaN distance or query sets kStatusNotFinite in w->d_error.
-int enqueue_exact(Handle* h, Workspace* w, const void* d_queries, size_t nq, int fmt, uint32_t k, uint32_t* d_ids,
-                  float* d_dists, uint32_t* d_counts, cudaStream_t stream) {
+int enqueue_exact(Handle* h, Workspace* w, const void* d_queries, size_t nq, int fmt, uint32_t k, const QueryOut& out,
+                  cudaStream_t stream) {
     const gb::DeviceIndex& d = h->dev;
     const uint64_t n = h->index_len;
     const uint32_t count = (uint32_t)std::min<uint64_t>(k, n);
     const bool i8 = d.kind == gb::kAngularI8, emb = d.kind == gb::kSumEmbeddings;
     const bool scan = k > 0 && n > 0;
-    const size_t in_row = (i8 && fmt == GRANNE_B200_QUERY_ELEMENT) ? d.dim : (size_t)d.dim * 4;
+    const size_t in_row = query_row_bytes(d.kind, d.dim, fmt);
     const size_t qc_max = std::min<size_t>(nq, gb::kExactMaxChunk);
     uint64_t slab = 0;
     const float* table = static_cast<const float*>(d.vectors);
@@ -1198,11 +1238,11 @@ int enqueue_exact(Handle* h, Workspace* w, const void* d_queries, size_t nq, int
                 return rc;
             }
         }
-        const uint64_t outs = std::max<uint64_t>((uint64_t)qc * k, d_counts ? qc : 0);
+        const uint64_t outs = std::max<uint64_t>((uint64_t)qc * k, out.counts ? qc : 0);
         if (outs == 0) continue;
         gb::exact_write_kernel<<<(unsigned)((outs + 255) / 256), 256, 0, stream>>>(
-            w->d_exact_lists.get(), qc, k, count, d_ids ? d_ids + c0 * k : nullptr, d_dists ? d_dists + c0 * k : nullptr,
-            d_counts ? d_counts + c0 : nullptr);
+            w->d_exact_lists.get(), qc, k, count, out.ids ? out.ids + c0 * k : nullptr,
+            out.dists ? out.dists + c0 * k : nullptr, out.counts ? out.counts + c0 : nullptr);
         h->launches++;
         GB_CUDA(cudaGetLastError());
     }
@@ -1293,16 +1333,15 @@ int validate_rerank(const Handle* h, const void* q, size_t nq, int fmt, uint32_t
 }
 
 // Enqueues one two-stage search on `stream`: stage 1 is enqueue_search with k = C into the workspace's candidate
-// block, stage 2 is rerank_kernel over h->rerank into the caller's outputs.  Stage 1 writes `d_stats` as search does.
+// block, stage 2 is rerank_kernel over h->rerank into the caller's outputs.  Stage 1 writes out.stats as search does.
 int enqueue_rerank(Handle* h, Workspace* w, const void* d_queries, size_t nq, uint32_t max_search, uint32_t c,
-                   uint32_t k, uint32_t* d_ids, float* d_dists, uint32_t* d_counts, unsigned long long* d_stats,
-                   cudaStream_t stream, bool reset_error) {
+                   uint32_t k, const QueryOut& out, cudaStream_t stream) {
     int rc = w->d_rerank.grow(2 * nq * c + nq, stream);
     if (rc) return rc;
     uint32_t* cand_ids = w->d_rerank.get();
     uint32_t* cand_counts = cand_ids + 2 * nq * c;
-    if ((rc = enqueue_search(h, w, d_queries, nq, GRANNE_B200_QUERY_RAW_F32, max_search, c, cand_ids,
-                             reinterpret_cast<float*>(cand_ids + nq * c), cand_counts, d_stats, stream, reset_error)))
+    if ((rc = enqueue_search(h, w, d_queries, nq, GRANNE_B200_QUERY_RAW_F32, max_search, c,
+                             {cand_ids, reinterpret_cast<float*>(cand_ids + nq * c), cand_counts, out.stats}, stream)))
         return rc;
     const EngineTiles eng = engine_tiles(h->rerank);
     gb::RerankArgs a{};
@@ -1312,10 +1351,10 @@ int enqueue_rerank(Handle* h, Workspace* w, const void* d_queries, size_t nq, ui
     a.cand_counts = cand_counts;
     a.cand_stride = c;
     a.num_neighbors = k;
-    a.out_ids = d_ids;
-    a.out_dists = d_dists;
-    a.out_counts = d_counts;
-    a.work_counter = w->d_counters.get() + 6;  // zeroed by enqueue_search's memset on this stream
+    a.out_ids = out.ids;
+    a.out_dists = out.dists;
+    a.out_counts = out.counts;
+    a.work_counter = w->d_counters.get() + 6;  // zeroed with the search counters before stage 1, on this stream
     a.error_flag = w->d_error;
     a.tiles = eng.tiles;
     const size_t smem = gb::rerank_keys_offset(eng.base_smem) + (size_t)gb::rerank_key_slots(c) * 8;
@@ -1369,10 +1408,9 @@ int check_within_ids(const uint64_t* offsets, size_t nq, const Id* ids, uint64_t
 // segments kernel, then within_kernel over the chunk's segments, then the rows of the lists of other than one segment.
 // A NaN distance sets kStatusNotFinite in w->d_error, a bad list kStatusBadList.
 int enqueue_within(Handle* h, Workspace* w, const void* d_queries, size_t nq, int fmt, const uint64_t* d_offsets,
-                   const uint32_t* d_ids, uint32_t k, uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts,
-                   cudaStream_t stream) {
+                   const uint32_t* d_ids, uint32_t k, const QueryOut& out, cudaStream_t stream) {
     const gb::DeviceIndex& d = h->dev;
-    const size_t in_row = query_bytes(h, 1, fmt);
+    const size_t in_row = query_row_bytes(d.kind, d.dim, fmt);
     const size_t qc_max = std::min<size_t>(nq, gb::kExactMaxChunk);
     int rc;
     if ((rc = w->d_within.grow(qc_max * k + qc_max + 2, stream)) || (rc = w->d_within_flags.grow(2 * qc_max, stream)))
@@ -1412,9 +1450,9 @@ int enqueue_within(Handle* h, Workspace* w, const void* d_queries, size_t nq, in
             a.locks = locks;
             a.qflags = qflags;
             a.work_counter = counter;
-            a.out_ids = d_out_ids ? d_out_ids + c0 * k : nullptr;
-            a.out_dists = d_out_dists ? d_out_dists + c0 * k : nullptr;
-            a.out_counts = d_out_counts ? d_out_counts + c0 : nullptr;
+            a.out_ids = out.ids ? out.ids + c0 * k : nullptr;
+            a.out_dists = out.dists ? out.dists + c0 * k : nullptr;
+            a.out_counts = out.counts ? out.counts + c0 : nullptr;
             a.error_flag = w->d_error;
             a.tiles = eng.tiles;
             if ((err = launch_warps<kern>(h, (unsigned)occ * h->num_sms, smem, stream, d, a))) return err;
@@ -1433,9 +1471,7 @@ int enqueue_within(Handle* h, Workspace* w, const void* d_queries, size_t nq, in
 int validate_filtered(const Handle* h, const void* q, size_t nq, int fmt, uint32_t max_search, uint32_t k,
                       const void* ids, const void* dists, const void* filters, uint32_t num_filters) {
     const int rc = validate_batch(h, q, nq, fmt, k, ids, dists,
-                                  max_search == 0                ? kMaxSearchRule
-                                  : k > GRANNE_B200_EXACT_MAX_K ? "num_neighbors exceeds GRANNE_B200_EXACT_MAX_K (1024)"
-                                                                 : nullptr);
+                                  max_search == 0 ? kMaxSearchRule : k > GRANNE_B200_EXACT_MAX_K ? kExactKRule : nullptr);
     if (rc || nq == 0) return rc;
     if (!filters || num_filters == 0) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "filters is null or num_filters is 0");
     return GRANNE_B200_OK;
@@ -1456,36 +1492,24 @@ int check_query_filter(const uint32_t* query_filter, size_t nq, uint32_t num_fil
     return GRANNE_B200_OK;
 }
 
-// A filtered search from host buffers (arguments checked, nq > 0): the filters and query_filter go up in the call's
-// stream order into memory held only until its kernels have run, like the lists of an exact search within lists.
-// bit_base: the bit of element 0 in the bitmaps (a range-partitioned shard reads the global bitmap).
+// A filtered search from host buffers (arguments checked, nq > 0), the filters and query_filter copied up for the call
+// only (with_call_inputs).  bit_base: the bit of element 0 in the bitmaps (a range-partitioned shard reads the global
+// bitmap).
 int search_filtered_host(Handle* h, const void* queries, size_t nq, int fmt, uint32_t max_search, uint32_t k,
                          const uint32_t* filters, uint32_t num_filters, uint64_t filter_words,
                          const uint32_t* query_filter, uint64_t bit_base, uint32_t* out_ids, float* out_dists,
                          uint32_t* out_counts, uint64_t* out_stats) {
-    return host_batch(h, queries, query_bytes(h, nq, fmt), nq, k, out_ids, out_dists, out_counts, out_stats,
-                      [&](Workspace* w, cudaStream_t stream, unsigned long long* d_stats) {
-                          const size_t fbytes = (size_t)num_filters * filter_words * 4;
-                          const size_t qbytes = query_filter ? nq * 4 : 0;
-                          void* mem = nullptr;
-                          GB_CUDA(cudaMallocAsync(&mem, fbytes + qbytes, stream));
-                          uint8_t* m8 = static_cast<uint8_t*>(mem);
-                          const DeviceFilters f{reinterpret_cast<const uint32_t*>(m8),
-                                                query_filter ? reinterpret_cast<const uint32_t*>(m8 + fbytes) : nullptr,
-                                                filter_words, num_filters, bit_base};
-                          const int r = [&] {
-                              GB_CUDA(cudaMemcpyAsync(m8, filters, fbytes, cudaMemcpyHostToDevice, stream));
-                              if (qbytes)
-                                  GB_CUDA(cudaMemcpyAsync(m8 + fbytes, query_filter, qbytes, cudaMemcpyHostToDevice,
-                                                          stream));
-                              return enqueue_search(h, w, w->d_queries.get(), nq, fmt, max_search, k, w->d_ids.get(),
-                                                    w->d_dists, w->d_counts, d_stats, stream, true, nullptr, nullptr,
-                                                    &f);
-                          }();
-                          const cudaError_t fe = cudaFreeAsync(mem, stream);
-                          if (r) return r;
-                          GB_CUDA(fe);
-                          return (int)GRANNE_B200_OK;
+    return host_batch(h, queries, nq, fmt, k, out_ids, out_dists, out_counts, out_stats,
+                      [&](Workspace* w, cudaStream_t stream, const QueryOut& out) {
+                          const HostInput in[] = {{filters, (size_t)num_filters * filter_words * 4},
+                                                  {query_filter, query_filter ? nq * 4 : 0}};
+                          return with_call_inputs(stream, in, [&](const void* const* d) {
+                              const DeviceFilters f{static_cast<const uint32_t*>(d[0]),
+                                                    query_filter ? static_cast<const uint32_t*>(d[1]) : nullptr,
+                                                    filter_words, num_filters, bit_base};
+                              return enqueue_search(h, w, w->d_queries.get(), nq, fmt, max_search, k, out, stream,
+                                                    nullptr, nullptr, &f);
+                          });
                       });
 }
 
@@ -1566,8 +1590,9 @@ int builder_index_elements(Builder* b, uint32_t layer_m, uint32_t ef, uint64_t a
                                                                             reinsert ? -1 : 1);
         h->launches++;
         // candidates = search_for_neighbors(layer, prev_layers.search(e,1,1), e, max_search) (:819-820)
-        rc = enqueue_search(h, b->ws.get(), b->d_ids.get(), bsz, gb::kQueryById, ef, ef, b->d_cand_ids.get(),
-                            b->d_cand_d.get(), b->d_cand_cnt.get(), nullptr, stream, false);
+        GB_CUDA(cudaMemsetAsync(b->ws->d_counters.get(), 0, kSearchCounterBytes, stream));
+        rc = enqueue_search(h, b->ws.get(), b->d_ids.get(), bsz, gb::kQueryById, ef, ef,
+                            {b->d_cand_ids.get(), b->d_cand_d.get(), b->d_cand_cnt.get(), nullptr}, stream);
         if (rc) return rc;
         GB_CUDA(cudaMemsetAsync(b->d_counter.get(), 0, 16, stream));
         link.n_batch = (uint32_t)bsz;
@@ -1829,9 +1854,9 @@ static int search_device_impl(granne_b200_index* h, const void* d_queries, size_
             GB_CUDA(cudaGetLastError());
             return GRANNE_B200_OK;
         });
-    return device_batch(h, cuda_stream, [&](Workspace* w, cudaStream_t stream) {
-        return enqueue_search(h, w, d_queries, nq, query_format, max_search, num_neighbors, d_out_ids, d_out_dists,
-                              d_out_counts, reinterpret_cast<unsigned long long*>(d_out_stats), stream, false, pg);
+    return device_batch(h, cuda_stream, true, [&](Workspace* w, cudaStream_t stream) {
+        return enqueue_search(h, w, d_queries, nq, query_format, max_search, num_neighbors,
+                              {d_out_ids, d_out_dists, d_out_counts, d_out_stats}, stream, pg);
     });
 }
 
@@ -1899,10 +1924,10 @@ int granne_b200_search_batch(granne_b200_index* h, const void* queries, size_t n
     int rc = validate_search(h, queries, nq, query_format, max_search, num_neighbors, out_ids, out_dists);
     if (rc) return rc;
     if (nq == 0) return GRANNE_B200_OK;
-    return host_batch(h, queries, query_bytes(h, nq, query_format), nq, num_neighbors, out_ids, out_dists, out_counts,
-                      out_stats, [&](Workspace* w, cudaStream_t stream, unsigned long long* d_stats) {
+    return host_batch(h, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts, out_stats,
+                      [&](Workspace* w, cudaStream_t stream, const QueryOut& out) {
                           return enqueue_search(h, w, w->d_queries.get(), nq, query_format, max_search, num_neighbors,
-                                                w->d_ids.get(), w->d_dists, w->d_counts, d_stats, stream, true);
+                                                out, stream);
                       });
 }
 
@@ -1911,12 +1936,9 @@ int granne_b200_exact_search_batch(granne_b200_index* h, const void* queries, si
     int rc = validate_exact(h, queries, nq, query_format, num_neighbors, out_ids, out_dists);
     if (rc) return rc;
     if (nq == 0) return GRANNE_B200_OK;
-    return host_batch(h, queries, query_bytes(h, nq, query_format), nq, num_neighbors, out_ids, out_dists, out_counts,
-                      nullptr, [&](Workspace* w, cudaStream_t stream, unsigned long long*) {
-                          // enqueue_exact has no memset that zeroes the error word (host_batch)
-                          GB_CUDA(cudaMemsetAsync(w->d_error, 0, 4 * sizeof(int), stream));
-                          return enqueue_exact(h, w, w->d_queries.get(), nq, query_format, num_neighbors,
-                                               w->d_ids.get(), w->d_dists, w->d_counts, stream);
+    return host_batch(h, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts, nullptr,
+                      [&](Workspace* w, cudaStream_t stream, const QueryOut& out) {
+                          return enqueue_exact(h, w, w->d_queries.get(), nq, query_format, num_neighbors, out, stream);
                       });
 }
 
@@ -1926,9 +1948,9 @@ int granne_b200_exact_search_batch_device(granne_b200_index* h, const void* d_qu
     int rc = validate_exact(h, d_queries, nq, query_format, num_neighbors, d_out_ids, d_out_dists);
     if (rc) return rc;
     if (nq == 0) return GRANNE_B200_OK;
-    return device_batch(h, cuda_stream, [&](Workspace* w, cudaStream_t stream) {
-        return enqueue_exact(h, w, d_queries, nq, query_format, num_neighbors, d_out_ids, d_out_dists, d_out_counts,
-                             stream);
+    return device_batch(h, cuda_stream, false, [&](Workspace* w, cudaStream_t stream) {
+        return enqueue_exact(h, w, d_queries, nq, query_format, num_neighbors,
+                             {d_out_ids, d_out_dists, d_out_counts, nullptr}, stream);
     });
 }
 
@@ -1939,30 +1961,14 @@ int granne_b200_exact_search_within_batch(granne_b200_index* h, const void* quer
     if (rc) return rc;
     if (nq == 0) return GRANNE_B200_OK;
     if ((rc = check_within_offsets(offsets, nq)) || (rc = check_within_ids(offsets, nq, ids, h->index_len))) return rc;
-    const uint64_t total = offsets[nq];
-    return host_batch(h, queries, query_bytes(h, nq, query_format), nq, num_neighbors, out_ids, out_dists, out_counts,
-                      nullptr, [&](Workspace* w, cudaStream_t stream, unsigned long long*) {
-                          // enqueue_within has no memset that zeroes the error word (host_batch)
-                          GB_CUDA(cudaMemsetAsync(w->d_error, 0, 4 * sizeof(int), stream));
-                          // the lists are the caller's input, not workspace: a stream-ordered allocation for this call
-                          // only, freed behind its kernels, so that a long list leaves no device memory held by the
-                          // pooled workspace
-                          const size_t obytes = (nq + 1) * 8;
-                          void* mem = nullptr;
-                          GB_CUDA(cudaMallocAsync(&mem, obytes + total * 4, stream));
-                          uint64_t* d_offsets = static_cast<uint64_t*>(mem);
-                          uint32_t* d_ids = reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(mem) + obytes);
-                          const int r = [&] {
-                              GB_CUDA(cudaMemcpyAsync(d_offsets, offsets, obytes, cudaMemcpyHostToDevice, stream));
-                              if (total)
-                                  GB_CUDA(cudaMemcpyAsync(d_ids, ids, total * 4, cudaMemcpyHostToDevice, stream));
-                              return enqueue_within(h, w, w->d_queries.get(), nq, query_format, d_offsets, d_ids,
-                                                    num_neighbors, w->d_ids.get(), w->d_dists, w->d_counts, stream);
-                          }();
-                          const cudaError_t fe = cudaFreeAsync(mem, stream);
-                          if (r) return r;
-                          GB_CUDA(fe);
-                          return (int)GRANNE_B200_OK;
+    return host_batch(h, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts, nullptr,
+                      [&](Workspace* w, cudaStream_t stream, const QueryOut& out) {
+                          const HostInput in[] = {{offsets, (nq + 1) * 8}, {ids, offsets[nq] * 4}};
+                          return with_call_inputs(stream, in, [&](const void* const* d) {
+                              return enqueue_within(h, w, w->d_queries.get(), nq, query_format,
+                                                    static_cast<const uint64_t*>(d[0]),
+                                                    static_cast<const uint32_t*>(d[1]), num_neighbors, out, stream);
+                          });
                       });
 }
 
@@ -1974,9 +1980,9 @@ int granne_b200_exact_search_within_batch_device(granne_b200_index* h, const voi
                              false);
     if (rc) return rc;
     if (nq == 0) return GRANNE_B200_OK;
-    return device_batch(h, cuda_stream, [&](Workspace* w, cudaStream_t stream) {
-        return enqueue_within(h, w, d_queries, nq, query_format, d_offsets, d_ids, num_neighbors, d_out_ids,
-                              d_out_dists, d_out_counts, stream);
+    return device_batch(h, cuda_stream, false, [&](Workspace* w, cudaStream_t stream) {
+        return enqueue_within(h, w, d_queries, nq, query_format, d_offsets, d_ids, num_neighbors,
+                              {d_out_ids, d_out_dists, d_out_counts, nullptr}, stream);
     });
 }
 
@@ -2003,11 +2009,10 @@ int granne_b200_search_filtered_batch_device(granne_b200_index* h, const void* d
                                d_filters, num_filters);
     if (rc || nq == 0) return rc;
     if ((rc = check_filter_words(filter_words, h->index_len))) return rc;
-    return device_batch(h, cuda_stream, [&](Workspace* w, cudaStream_t stream) {
+    return device_batch(h, cuda_stream, true, [&](Workspace* w, cudaStream_t stream) {
         const DeviceFilters f{d_filters, d_query_filter, filter_words, num_filters, 0};
-        return enqueue_search(h, w, d_queries, nq, query_format, max_search, num_neighbors, d_out_ids, d_out_dists,
-                              d_out_counts, reinterpret_cast<unsigned long long*>(d_out_stats), stream, false, nullptr,
-                              nullptr, &f);
+        return enqueue_search(h, w, d_queries, nq, query_format, max_search, num_neighbors,
+                              {d_out_ids, d_out_dists, d_out_counts, d_out_stats}, stream, nullptr, nullptr, &f);
     });
 }
 
@@ -2059,11 +2064,10 @@ int granne_b200_search_rerank_batch(granne_b200_index* h, const float* queries, 
                              out_dists);
     if (rc) return rc;
     if (nq == 0) return GRANNE_B200_OK;
-    return host_batch(h, queries, query_bytes(h, nq, query_format), nq, num_neighbors, out_ids, out_dists, out_counts,
-                      out_stats, [&](Workspace* w, cudaStream_t stream, unsigned long long* d_stats) {
+    return host_batch(h, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts, out_stats,
+                      [&](Workspace* w, cudaStream_t stream, const QueryOut& out) {
                           return enqueue_rerank(h, w, w->d_queries.get(), nq, max_search, num_candidates,
-                                                num_neighbors, w->d_ids.get(), w->d_dists, w->d_counts, d_stats,
-                                                stream, true);
+                                                num_neighbors, out, stream);
                       });
 }
 
@@ -2075,9 +2079,9 @@ int granne_b200_search_rerank_batch_device(granne_b200_index* h, const float* d_
                              d_out_dists);
     if (rc) return rc;
     if (nq == 0) return GRANNE_B200_OK;
-    return device_batch(h, cuda_stream, [&](Workspace* w, cudaStream_t stream) {
-        return enqueue_rerank(h, w, d_queries, nq, max_search, num_candidates, num_neighbors, d_out_ids, d_out_dists,
-                              d_out_counts, reinterpret_cast<unsigned long long*>(d_out_stats), stream, false);
+    return device_batch(h, cuda_stream, true, [&](Workspace* w, cudaStream_t stream) {
+        return enqueue_rerank(h, w, d_queries, nq, max_search, num_candidates, num_neighbors,
+                              {d_out_ids, d_out_dists, d_out_counts, d_out_stats}, stream);
     });
 }
 
@@ -2646,8 +2650,9 @@ int granne_b200_compute_order(granne_b200_index* h, uint64_t* order_out, uint64_
                     gb::iota_kernel<<<(unsigned)((bsz + 255) / 256), 256, 0, stream>>>(d_q.get(), (uint32_t)bsz,
                                                                                         (uint32_t)base, 1);
                     h->launches++;
-                    rc = enqueue_search(h, w, d_q.get(), bsz, gb::kQueryById, 1, 1, d_ids.get(), d_d.get(), d_cnt.get(),
-                                        nullptr, stream, true, nullptr, &view);
+                    GB_CUDA(cudaMemsetAsync(w->d_counters.get(), 0, kHostCallBytes, stream));
+                    rc = enqueue_search(h, w, d_q.get(), bsz, gb::kQueryById, 1, 1,
+                                        {d_ids.get(), d_d.get(), d_cnt.get(), nullptr}, stream, nullptr, &view);
                     if (rc) return rc;
                     GB_CUDA(cudaMemcpyAsync(eps[j].data() + (base - layer_lens[j]), d_ids.get(), bsz * 4,
                                             cudaMemcpyDeviceToHost, stream));
@@ -2878,15 +2883,15 @@ uint64_t granne_b200_multi_shard_base(const granne_b200_multi* m, size_t s) {
 
 namespace {
 
-// A batch on a multi handle: `part(handle, queries, nq, ids, dists, counts)` runs the single-device call.  REPLICATED
-// slices the queries over the devices; RANGE_PARTITIONED runs every query on every shard and merges the shard lists.
+// A batch on a multi handle: `part(i, b, q, cnt, ids, dists, counts)` runs the single-device call on part i for the
+// queries [b, b + cnt), whose rows start at q.  REPLICATED slices the queries over the devices; RANGE_PARTITIONED runs
+// every query on every shard (b = 0, cnt = nq) and merges the shard lists.
 template <class Part>
 int multi_batch(granne_b200_multi* m, const void* queries, size_t nq, int query_format, uint32_t num_neighbors,
                 uint64_t* out_ids, float* out_dists, uint32_t* out_counts, Part&& part) {
     return guarded([&] {
         const size_t n = m->parts.size(), k = num_neighbors;
-        const bool i8q = m->kind == GRANNE_B200_ANGULAR_INT && query_format == GRANNE_B200_QUERY_ELEMENT;
-        const size_t qrow = (size_t)m->dim * (i8q ? 1 : 4);
+        const size_t qrow = query_row_bytes(m->kind, m->dim, query_format);
         const uint8_t* q = static_cast<const uint8_t*>(queries);
         if (m->mode == GRANNE_B200_MODE_REPLICATED) {
             // contiguous, balanced query slices (the first nq % n devices take one more)
@@ -2896,7 +2901,7 @@ int multi_batch(granne_b200_multi* m, const void* queries, size_t nq, int query_
             int rc = for_each_part(n, [&](size_t i) {
                 const size_t b = i * per + std::min(i, extra), cntq = per + (i < extra ? 1 : 0);
                 if (cntq == 0) return (int)GRANNE_B200_OK;
-                return part(m->parts[i], q + b * qrow, cntq, ids.data() + b * k, out_dists + b * k, cnt.data() + b);
+                return part(i, b, q + b * qrow, cntq, ids.data() + b * k, out_dists + b * k, cnt.data() + b);
             });
             if (rc) return rc;
             for (size_t i = 0; i < nq * k; ++i) out_ids[i] = ids[i] == gb::kUnusedId ? ~0ull : (uint64_t)ids[i];
@@ -2907,7 +2912,7 @@ int multi_batch(granne_b200_multi* m, const void* queries, size_t nq, int query_
         std::vector<uint32_t> ids(n * nq * k);
         std::vector<float> ds(n * nq * k);
         int rc = for_each_part(n, [&](size_t i) {
-            return part(m->parts[i], q, nq, ids.data() + i * nq * k, ds.data() + i * nq * k, nullptr);
+            return part(i, 0, q, nq, ids.data() + i * nq * k, ds.data() + i * nq * k, nullptr);
         });
         if (rc) return rc;
         std::vector<size_t> cur(n);
@@ -2982,13 +2987,12 @@ int granne_b200_multi_search_batch(granne_b200_multi* m, const void* queries, si
                                    uint32_t max_search, uint32_t num_neighbors, uint64_t* out_ids, float* out_dists,
                                    uint32_t* out_counts) {
     if (!m) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "multi handle is null");
-    if (nq == 0) return GRANNE_B200_OK;
-    if (!queries || (num_neighbors && (!out_ids || !out_dists)))
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null buffer");
+    int rc = validate_search(m->parts[0], queries, nq, query_format, max_search, num_neighbors, out_ids, out_dists);
+    if (rc || nq == 0) return rc;
     return multi_batch(m, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts,
-                       [&](granne_b200_index* h, const void* q, size_t cnt, uint32_t* ids, float* ds, uint32_t* c) {
-                           return granne_b200_search_batch(h, q, cnt, query_format, max_search, num_neighbors, ids,
-                                                           ds, c, nullptr);
+                       [&](size_t i, size_t, const void* q, size_t cnt, uint32_t* ids, float* ds, uint32_t* c) {
+                           return granne_b200_search_batch(m->parts[i], q, cnt, query_format, max_search,
+                                                           num_neighbors, ids, ds, c, nullptr);
                        });
 }
 
@@ -2999,11 +3003,11 @@ int granne_b200_multi_exact_search_batch(granne_b200_multi* m, const void* queri
                                          uint32_t* out_counts) {
     if (!m) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "multi handle is null");
     int rc = validate_exact(m->parts[0], queries, nq, query_format, num_neighbors, out_ids, out_dists);
-    if (rc) return rc;
-    if (nq == 0) return GRANNE_B200_OK;
+    if (rc || nq == 0) return rc;
     return multi_batch(m, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts,
-                       [&](granne_b200_index* h, const void* q, size_t cnt, uint32_t* ids, float* ds, uint32_t* c) {
-                           return granne_b200_exact_search_batch(h, q, cnt, query_format, num_neighbors, ids, ds, c);
+                       [&](size_t i, size_t, const void* q, size_t cnt, uint32_t* ids, float* ds, uint32_t* c) {
+                           return granne_b200_exact_search_batch(m->parts[i], q, cnt, query_format, num_neighbors,
+                                                                 ids, ds, c);
                        });
 }
 
@@ -3035,25 +3039,20 @@ int granne_b200_multi_exact_search_within_batch(granne_b200_multi* m, const void
             }
             for (size_t s = 0; s < n; ++s) loff[s].push_back(lids[s].size());
         }
-        const bool i8q = m->kind == GRANNE_B200_ANGULAR_INT && query_format == GRANNE_B200_QUERY_ELEMENT;
-        const size_t qrow = (size_t)m->dim * (i8q ? 1 : 4);
         return multi_batch(m, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts,
-                           [&](granne_b200_index* h, const void* q, size_t cnt, uint32_t* pids, float* ds, uint32_t* c) {
-                               if (range) {
-                                   const size_t s = std::find(m->parts.begin(), m->parts.end(), h) - m->parts.begin();
-                                   return granne_b200_exact_search_within_batch(h, q, cnt, query_format, loff[s].data(),
-                                                                                lids[s].data(), num_neighbors, pids, ds,
-                                                                                c);
-                               }
+                           [&](size_t i, size_t b, const void* q, size_t cnt, uint32_t* pids, float* ds, uint32_t* c) {
+                               if (range)
+                                   return granne_b200_exact_search_within_batch(m->parts[i], q, cnt, query_format,
+                                                                                loff[i].data(), lids[i].data(),
+                                                                                num_neighbors, pids, ds, c);
                                // the slice of queries [b, b + cnt) and their lists
-                               const size_t b =
-                                   (static_cast<const uint8_t*>(q) - static_cast<const uint8_t*>(queries)) / qrow;
                                return guarded([&] {
                                    std::vector<uint64_t> off(cnt + 1);
                                    for (size_t j = 0; j <= cnt; ++j) off[j] = offsets[b + j] - offsets[b];
                                    const std::vector<uint32_t> sl(ids + offsets[b], ids + offsets[b + cnt]);
-                                   return granne_b200_exact_search_within_batch(h, q, cnt, query_format, off.data(),
-                                                                                sl.data(), num_neighbors, pids, ds, c);
+                                   return granne_b200_exact_search_within_batch(m->parts[i], q, cnt, query_format,
+                                                                                off.data(), sl.data(), num_neighbors,
+                                                                                pids, ds, c);
                                });
                            });
     });
@@ -3076,17 +3075,12 @@ int granne_b200_multi_search_filtered_batch(granne_b200_multi* m, const void* qu
     for (size_t s = 0; range && s < m->parts.size(); ++s) span = std::max(span, m->base[s] + m->parts[s]->index_len);
     if ((rc = check_filter_words(filter_words, span)) || (rc = check_query_filter(query_filter, nq, num_filters)))
         return rc;
-    const bool i8q = m->kind == GRANNE_B200_ANGULAR_INT && query_format == GRANNE_B200_QUERY_ELEMENT;
-    const size_t qrow = (size_t)m->dim * (i8q ? 1 : 4);
     return multi_batch(m, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts,
-                       [&](granne_b200_index* h, const void* q, size_t cnt, uint32_t* ids, float* ds, uint32_t* c) {
-                           const size_t s = std::find(m->parts.begin(), m->parts.end(), h) - m->parts.begin();
-                           const size_t b =
-                               (static_cast<const uint8_t*>(q) - static_cast<const uint8_t*>(queries)) / qrow;
-                           return search_filtered_host(h, q, cnt, query_format, max_search, num_neighbors, filters,
-                                                       num_filters, filter_words,
-                                                       query_filter ? query_filter + b : nullptr,
-                                                       range ? m->base[s] : 0, ids, ds, c, nullptr);
+                       [&](size_t i, size_t b, const void* q, size_t cnt, uint32_t* ids, float* ds, uint32_t* c) {
+                           return search_filtered_host(m->parts[i], q, cnt, query_format, max_search, num_neighbors,
+                                                       filters, num_filters, filter_words,
+                                                       query_filter ? query_filter + b : nullptr, m->base[i], ids, ds,
+                                                       c, nullptr);
                        });
 }
 
@@ -3142,13 +3136,12 @@ int granne_b200_multi_search_rerank_batch(granne_b200_multi* m, const float* que
     if (!m) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "multi handle is null");
     int rc = validate_rerank(m->parts[0], queries, nq, query_format, max_search, num_candidates, num_neighbors,
                              out_ids, out_dists);
-    if (rc) return rc;
-    if (nq == 0) return GRANNE_B200_OK;
+    if (rc || nq == 0) return rc;
     return multi_batch(m, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts,
-                       [&](granne_b200_index* h, const void* q, size_t cnt, uint32_t* ids, float* ds, uint32_t* c) {
-                           return granne_b200_search_rerank_batch(h, static_cast<const float*>(q), cnt, query_format,
-                                                                  max_search, num_candidates, num_neighbors, ids, ds,
-                                                                  c, nullptr);
+                       [&](size_t i, size_t, const void* q, size_t cnt, uint32_t* ids, float* ds, uint32_t* c) {
+                           return granne_b200_search_rerank_batch(m->parts[i], static_cast<const float*>(q), cnt,
+                                                                  query_format, max_search, num_candidates,
+                                                                  num_neighbors, ids, ds, c, nullptr);
                        });
 }
 

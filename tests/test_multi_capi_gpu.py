@@ -14,6 +14,7 @@ from granne_b200.distributed import merge_topk_host
 from helpers.data import build_fixture, random_vectors
 
 pytestmark = pytest.mark.gpu
+INVALID = -1  # GRANNE_B200_ERR_INVALID_ARGUMENT
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -80,3 +81,62 @@ def test_multi_open_reports_errors_as_status(oracle):
     with pytest.raises(granne_b200.GranneError):
         m.search_batch(random_vectors(4, 16, seed=1), 0, 5)                    # max_search == 0 panics in the reference
     m.close()
+
+
+def test_multi_calls_report_the_single_device_rules(oracle):
+    """Each multi call checks the rules of its single-device call before any part runs: on a one-device replicated
+    handle, the same bad arguments give the single-device call's status and message, nq == 0 included."""
+    from granne_b200 import api
+
+    el, g, ib, eb, _ = build_fixture(oracle, "angular", 500, 16, seed=3, num_neighbors=8, max_search=20)
+    L = granne_b200.load_library()
+    s = granne_b200.Granne.from_bytes(ib, "angular", eb)
+    m = granne_b200.MultiGranne.replicated(ib, "angular", eb, [0])
+    q = random_vectors(2, 16, seed=1)
+    ids32, ids64, dists = np.zeros(4000, np.uint32), np.zeros(4000, np.uint64), np.zeros(4000, np.float32)
+    offsets, words = np.array([0, 2, 3], np.uint64), np.ones((1, 16), np.uint32)
+    cand32, cand64 = np.array([0, 1, 2], np.uint32), np.array([0, 1, 2], np.uint64)
+
+    def run(call, multi, nq=2, fmt=api.QUERY_RAW_F32, ef=20, k=5, queries=True, out=True, offs=True, cand=True,
+            filters=True, nf=1):
+        h = m._h if multi else s._h
+        pq = api._ptr(q) if queries else None
+        pi = api._ptr(ids64 if multi else ids32) if out else None
+        pd = api._ptr(dists)
+        stats = () if multi else (None,)
+        if call == "search":
+            fn = L.granne_b200_multi_search_batch if multi else L.granne_b200_search_batch
+            rc = fn(h, pq, nq, fmt, ef, k, pi, pd, None, *stats)
+        elif call == "exact":
+            fn = L.granne_b200_multi_exact_search_batch if multi else L.granne_b200_exact_search_batch
+            rc = fn(h, pq, nq, fmt, k, pi, pd, None)
+        elif call == "within":
+            fn = L.granne_b200_multi_exact_search_within_batch if multi else L.granne_b200_exact_search_within_batch
+            rc = fn(h, pq, nq, fmt, api._ptr(offsets) if offs else None,
+                    api._ptr(cand64 if multi else cand32) if cand else None, k, pi, pd, None)
+        elif call == "filtered":
+            fn = L.granne_b200_multi_search_filtered_batch if multi else L.granne_b200_search_filtered_batch
+            rc = fn(h, pq, nq, fmt, ef, k, api._ptr(words) if filters else None, nf, 16, None, pi, pd, None, *stats)
+        else:
+            fn = L.granne_b200_multi_search_rerank_batch if multi else L.granne_b200_search_rerank_batch
+            rc = fn(h, pq, nq, fmt, ef, 10, k, pi, pd, None, *stats)
+        return rc, L.granne_b200_last_error().decode()
+
+    shared = [dict(fmt=7), dict(nq=0, fmt=7), dict(nq=0xFFFFFFF1, queries=False), dict(queries=False), dict(out=False)]
+    max_search = [dict(ef=0), dict(nq=0, ef=0), dict(ef=0, fmt=7)]
+    exact_k = [dict(k=1025), dict(nq=0, k=1025)]
+    cases = {
+        "search": shared + max_search,
+        "exact": shared + exact_k,
+        "within": shared + exact_k + [dict(offs=False), dict(offs=False, cand=False), dict(cand=False)],
+        "filtered": shared + max_search + exact_k + [dict(filters=False), dict(nf=0), dict(ef=0, k=1025)],
+        # no re-rank container is attached: the rule reads the handle, the multi call reads its first part's
+        "rerank": shared + max_search + [dict(), dict(fmt=api.QUERY_ELEMENT)],
+    }
+    for call, args in cases.items():
+        for a in args:
+            want = run(call, False, **a)
+            assert want[0] == INVALID, (call, a, want)
+            assert run(call, True, **a) == want, (call, a)
+    m.close()
+    s.close()
