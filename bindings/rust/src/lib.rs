@@ -50,6 +50,9 @@ extern "C" {
     ) -> c_int;
     fn granne_b200_dim(h: *const RawIndex) -> u64;
     fn granne_b200_get_element(h: *const RawIndex, idx: u64, out: *mut c_void) -> c_int;
+    fn granne_b200_get_elements(h: *mut RawIndex, ids: *const u32, n: usize, out: *mut c_void) -> c_int;
+    fn granne_b200_get_elements_device(h: *mut RawIndex, d_ids: *const u32, n: usize, d_out: *mut c_void,
+                                       cuda_stream: *mut c_void) -> c_int;
     fn granne_b200_search_batch(
         h: *mut RawIndex, queries: *const c_void, nq: usize, query_format: c_int, max_search: u32, num_neighbors: u32,
         out_ids: *mut u32, out_dists: *mut f32, out_counts: *mut u32, out_stats: *mut u64,
@@ -94,6 +97,7 @@ extern "C" {
     fn granne_b200_multi_close(m: *mut RawMulti);
     fn granne_b200_multi_len(m: *const RawMulti) -> u64;
     fn granne_b200_multi_shard_base(m: *const RawMulti, s: usize) -> u64;
+    fn granne_b200_multi_part_len(m: *const RawMulti, s: usize) -> u64;
     fn granne_b200_multi_search_batch(
         m: *mut RawMulti, queries: *const c_void, nq: usize, query_format: c_int, max_search: u32, num_neighbors: u32,
         out_ids: *mut u64, out_dists: *mut f32, out_counts: *mut u32,
@@ -151,6 +155,8 @@ pub const ANGULAR_INT: c_int = 1; // angular_int::Vectors
 pub const EMBEDDINGS: c_int = 2; // embeddings::SumEmbeddings
 const QUERY_RAW_F32: c_int = 0; // the library applies Vector::from
 const QUERY_ELEMENT: c_int = 1; // the caller passes an Elements::Element
+pub const QUERY_ID: c_int = 2; // u32 element ids (u64 global ids on a multi handle): the query is get_element(id)
+pub const QUERY_ID_EXCLUDING: c_int = 3; // QUERY_ID without the element itself (k + 1 searched, self dropped)
 
 fn last_error() -> String {
     unsafe { CStr::from_ptr(granne_b200_last_error()).to_string_lossy().into_owned() }

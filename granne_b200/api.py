@@ -9,7 +9,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = os.environ.get("GRANNE_B200_LIB") or os.path.join(_HERE, "libgranne_b200.so")  # env: tuning variants
 
 ANGULAR, ANGULAR_INT, EMBEDDINGS = 0, 1, 2
-QUERY_RAW_F32, QUERY_ELEMENT = 0, 1
+QUERY_RAW_F32, QUERY_ELEMENT, QUERY_ID, QUERY_ID_EXCLUDING = 0, 1, 2, 3
 _ELEMENT_TYPES = {"angular": ANGULAR, "angular_int": ANGULAR_INT, "embeddings": EMBEDDINGS}
 STATS_PER_QUERY = 4
 EXACT_MAX_K = 1024  # GRANNE_B200_EXACT_MAX_K
@@ -61,10 +61,14 @@ def load_library():
         "granne_b200_dim": (u64, [vp]),
         "granne_b200_element_kind": (i32, [vp]),
         "granne_b200_get_element": (i32, [vp, u64, vp]),
+        "granne_b200_get_elements": (i32, [vp, vp, sz, vp]),
+        "granne_b200_get_elements_device": (i32, [vp, vp, sz, vp, vp]),
         "granne_b200_search_batch": (i32, [vp, vp, sz, i32, u32, u32, vp, vp, vp, vp]),
         "granne_b200_search_batch_device": (i32, [vp, vp, sz, i32, u32, u32, vp, vp, vp, vp, vp]),
         "granne_b200_search_batch_device_gather": (i32, [vp, vp, sz, i32, u32, u32, vp, vp, vp, vp]),
         "granne_b200_stream_status": (i32, [vp]),
+        "granne_b200_stream_status_of": (i32, [vp, vp]),
+        "granne_b200_multi_part_len": (u64, [vp, sz]),
         "granne_b200_release_stream": (i32, [vp, vp]),
         "granne_b200_merge_topk_device": (i32, [i32, vp, vp, vp, sz, sz, u32, vp, vp, vp]),
         "granne_b200_inspect_index": (i32, [vp, sz, vp, vp, vp, vp, sz]),
@@ -154,6 +158,21 @@ def _host_queries(queries, already_element, dim=None):
     if q.ndim != 2 or (dim is not None and q.shape[1] != dim):
         raise ValueError("queries must have shape (nq, %s)" % ("dim" if dim is None else dim))
     return q, fmt
+
+
+def _id_queries(ids, exclude_self, id_dtype):
+    """(contiguous ids, query format) of a host call by element id: a 1-D array of non-negative integers that fit
+    id_dtype (uint32 for one index, uint64 global ids for a MultiGranne)."""
+    a = np.asarray(ids)
+    if a.ndim != 1:
+        raise ValueError("ids must be a 1-D integer array")
+    if a.size and a.dtype.kind not in "iu":
+        raise ValueError("ids must be integers, not %s" % a.dtype)
+    if a.size and a.dtype.kind == "i" and a.min() < 0:
+        raise ValueError("ids must be non-negative")
+    if a.size and int(a.max()) > np.iinfo(id_dtype).max:
+        raise ValueError("ids must fit %s" % np.dtype(id_dtype).name)
+    return np.ascontiguousarray(a, dtype=id_dtype), QUERY_ID_EXCLUDING if exclude_self else QUERY_ID
 
 
 def _raw_f32_queries(queries, dim=None):
@@ -452,15 +471,82 @@ class Granne:
         _check(load_library().granne_b200_get_element(self._h, idx, _ptr(out)))
         return out
 
+    def get_elements(self, ids):
+        """get_element for a 1-D integer array of ids in one launch: (n, dim) float32 (int8 for angular_int), row i
+        bit for bit get_element(ids[i]).  Every id must be < num_elements()."""
+        q, _ = _id_queries(ids, False, np.uint32)
+        out = np.empty((q.shape[0], self.dim), dtype=np.int8 if self.element_kind == ANGULAR_INT else np.float32)
+        _check(load_library().granne_b200_get_elements(self._h, _ptr(q), q.shape[0], _ptr(out)))
+        return out
+
+    def get_elements_device(self, ids, out=None, stream=None):
+        """Device-resident get_elements: `ids` a contiguous 1-D int32 CUDA tensor (the u32 ids' bits) on this index's
+        device; returns (n, dim) float32 (int8 for angular_int) CUDA rows, asynchronous on `stream`.  A bad id's row
+        is zeros and stream_status() raises."""
+        import torch
+
+        q, _ = self._device_queries(ids, False, by_id=True)
+        dt = torch.int8 if self.element_kind == ANGULAR_INT else torch.float32
+        if out is None:
+            out = torch.empty((q.shape[0], self.dim), dtype=dt, device=q.device)
+        elif (not isinstance(out, torch.Tensor) or out.device != q.device or out.dtype != dt
+              or tuple(out.shape) != (q.shape[0], self.dim) or not out.is_contiguous()):
+            raise ValueError("out must be a contiguous %s CUDA tensor of shape (n, dim) on the ids' device" % dt)
+        _check(load_library().granne_b200_get_elements_device(self._h, C.c_void_p(q.data_ptr()), q.shape[0],
+                                                              C.c_void_p(out.data_ptr()),
+                                                              C.c_void_p(_raw_stream(stream, q.device))))
+        return out
+
+    def knn_graph(self, max_search=DEFAULT_MAX_SEARCH, num_elements=DEFAULT_NUM_ELEMENTS, exclude_self=True,
+                  exact=False, chunk=65536, out="host"):
+        """The k-nearest-neighbour graph of the index: for every element i < len(self), search_batch(by_id) of i (or
+        exact_search_batch with exact=True), without i itself when exclude_self.  The ids stream through the device
+        calls in chunks made on the device, so no id array of length len(self) exists on the host.  The calls run on a
+        stream of their own, and only their errors are reported (stream_status(stream)): other threads' device calls
+        on this handle keep theirs.  Returns (ids, dists, counts) of shape [len, k]: uint32 / float32 / uint32 numpy
+        arrays (out="host") or int32 / float32 / int32 CUDA tensors (out="device")."""
+        import torch
+
+        if out not in ("host", "device"):
+            raise ValueError('out must be "host" or "device"')
+        if int(chunk) < 1:
+            raise ValueError("chunk must be >= 1")
+        n, k, dev = len(self), int(num_elements), torch.device("cuda", self.device)
+        s = torch.cuda.Stream(device=dev)
+        s.wait_stream(torch.cuda.current_stream(dev))
+        try:
+            with torch.cuda.stream(s):
+                ids = torch.empty((n, k), dtype=torch.int32, device=dev)
+                dists = torch.empty((n, k), dtype=torch.float32, device=dev)
+                counts = torch.empty((n,), dtype=torch.int32, device=dev)
+                for c0 in range(0, n, int(chunk)):
+                    c1 = min(n, c0 + int(chunk))
+                    q = torch.arange(c0, c1, dtype=torch.int64, device=dev).to(torch.int32)  # the u32 ids' bits
+                    part = (ids[c0:c1], dists[c0:c1], counts[c0:c1])
+                    if exact:
+                        self.exact_search_batch_device(q, k, by_id=True, exclude_self=exclude_self, out=part, stream=s)
+                    else:
+                        self.search_batch_device(q, max_search, k, by_id=True, exclude_self=exclude_self, out=part,
+                                                 stream=s)
+            self.stream_status(s)  # synchronises s and raises what any chunk reported
+        finally:
+            self.release_stream(s)
+        if out == "device":
+            return ids, dists, counts
+        return ids.cpu().numpy().view(np.uint32), dists.cpu().numpy(), counts.cpu().numpy().view(np.uint32)
+
     # ---- search ----
     def search_batch(self, queries, max_search=DEFAULT_MAX_SEARCH, num_elements=DEFAULT_NUM_ELEMENTS,
-                     already_element=False, with_stats=False):
+                     already_element=False, with_stats=False, by_id=False, exclude_self=False):
         """nq independent Granne::search calls (src/index/mod.rs:140-150) in one launch; host buffers in and out.
 
         queries: (nq, dim) float32 raw vectors (normalised / quantised by the library like the reference's Python
         binding), or with already_element=True rows that already are elements (normalised f32; int8 for
-        angular_int).  Returns (ids uint32 [nq,k] padded 0xFFFFFFFF, dists float32 [nq,k] padded +inf, counts)."""
-        q, fmt = self._host_queries(queries, already_element)
+        angular_int).  With by_id=True, a 1-D integer array of element ids < num_elements(): the query of row q is
+        get_element(ids[q]), with results bit-identical to passing those rows as elements; exclude_self=True (which
+        implies by_id) searches k + 1 and drops each query's own id.  The other query calls take the same keywords.
+        Returns (ids uint32 [nq,k] padded 0xFFFFFFFF, dists float32 [nq,k] padded +inf, counts)."""
+        q, fmt = self._host_queries(queries, already_element, by_id, exclude_self)
         nq, k = q.shape[0], int(num_elements)
         ids, dists, counts, stats = _host_outputs(nq, k, np.uint32, with_stats)
         _check(load_library().granne_b200_search_batch(self._h, _ptr(q), nq, fmt, int(max_search), k, _ptr(ids),
@@ -470,8 +556,11 @@ class Granne:
             return ids, dists, counts, stats
         return ids, dists, counts
 
-    def _host_queries(self, queries, already_element):
-        """_host_queries for this index: its width, and its rules on int8 rows."""
+    def _host_queries(self, queries, already_element, by_id=False, exclude_self=False):
+        """_host_queries for this index: its width, and its rules on int8 rows; element ids with by_id or
+        exclude_self."""
+        if by_id or exclude_self:
+            return _id_queries(queries, exclude_self, np.uint32)
         q = np.asarray(queries)
         if q.dtype == np.int8:
             if self.element_kind != ANGULAR_INT:
@@ -480,12 +569,13 @@ class Granne:
             raise ValueError("angular_int elements are int8")
         return _host_queries(q, already_element, self.dim)
 
-    def exact_search_batch(self, queries, num_elements=DEFAULT_NUM_ELEMENTS, already_element=False):
+    def exact_search_batch(self, queries, num_elements=DEFAULT_NUM_ELEMENTS, already_element=False, by_id=False,
+                           exclude_self=False):
         """Exact k nearest neighbours: the first min(k, len(self)) of all elements i < len(self) by (distance, id),
         with the reference's distance bit for bit (granne_b200_exact_search_batch) — the ground truth of recall.
         Not a reference function.  Queries as in search_batch; k <= EXACT_MAX_K.  Returns (ids, dists, counts) in
         search_batch's layout."""
-        q, fmt = self._host_queries(queries, already_element)
+        q, fmt = self._host_queries(queries, already_element, by_id, exclude_self)
         nq, k = q.shape[0], int(num_elements)
         ids, dists, counts, _ = _host_outputs(nq, k, np.uint32)
         _check(load_library().granne_b200_exact_search_batch(self._h, _ptr(q), nq, fmt, k, _ptr(ids), _ptr(dists),
@@ -493,10 +583,10 @@ class Granne:
         return ids, dists, counts
 
     def exact_search_batch_device(self, queries, num_elements=DEFAULT_NUM_ELEMENTS, already_element=False, out=None,
-                                  stream=None):
+                                  stream=None, by_id=False, exclude_self=False):
         """Device-resident exact_search_batch: CUDA tensors in and out, asynchronous on `stream` (a torch.cuda.Stream
         or a raw cudaStream_t; default: the current torch stream); a NaN distance is reported by stream_status()."""
-        q, fmt = self._device_queries(queries, already_element)
+        q, fmt = self._device_queries(queries, already_element, by_id, exclude_self)
         nq, k = q.shape[0], int(num_elements)
         ids, dists, counts = _device_outputs(q, k, out)
         _check(load_library().granne_b200_exact_search_batch_device(
@@ -504,14 +594,15 @@ class Granne:
             C.c_void_p(counts.data_ptr()), C.c_void_p(_raw_stream(stream, q.device))))
         return ids, dists, counts
 
-    def exact_search_within(self, queries, candidates, num_elements=DEFAULT_NUM_ELEMENTS, already_element=False):
+    def exact_search_within(self, queries, candidates, num_elements=DEFAULT_NUM_ELEMENTS, already_element=False,
+                            by_id=False, exclude_self=False):
         """Exact k nearest neighbours of each query within its own candidate list: the first min(k, |set(list)|) ids
         of the list by (distance, id), with the reference's distance bit for bit (granne_b200_exact_search_within_batch).
         Not a reference function.  `candidates`: one 1-D integer array of ids per query, or a CsrLists(offsets, ids)
         (offsets [nq + 1], offsets[0] == 0, non-decreasing).  Duplicates count once; every id must be
         < len(self).  Queries as in exact_search_batch; k <= EXACT_MAX_K.  Returns (ids, dists, counts) in
         search_batch's layout."""
-        q, fmt = self._host_queries(queries, already_element)
+        q, fmt = self._host_queries(queries, already_element, by_id, exclude_self)
         nq, k = q.shape[0], int(num_elements)
         offsets, cand = _candidate_lists(candidates, nq, np.uint32)
         ids, dists, counts, _ = _host_outputs(nq, k, np.uint32)
@@ -520,7 +611,7 @@ class Granne:
         return ids, dists, counts
 
     def exact_search_within_device(self, queries, offsets, ids, num_elements=DEFAULT_NUM_ELEMENTS,
-                                   already_element=False, out=None, stream=None):
+                                   already_element=False, out=None, stream=None, by_id=False, exclude_self=False):
         """Device-resident exact_search_within: CUDA tensors in (queries; offsets int64 [nq + 1]; ids int32 view of
         u32 ids) and out, asynchronous on `stream` (a torch.cuda.Stream or a raw cudaStream_t; default: the current
         torch stream).  The kernels check the lists: a bad list gives its query count 0 and padding, and
@@ -528,7 +619,7 @@ class Granne:
         and checking it here would wait for the device."""
         import torch
 
-        q, fmt = self._device_queries(queries, already_element)
+        q, fmt = self._device_queries(queries, already_element, by_id, exclude_self)
         nq, k = q.shape[0], int(num_elements)
         for t, dt, what in ((offsets, torch.int64, "offsets"), (ids, torch.int32, "ids")):
             if (not isinstance(t, torch.Tensor) or not t.is_cuda or t.device != q.device or t.dtype != dt
@@ -545,14 +636,15 @@ class Granne:
 
     # ---- two-stage search (granne_b200_search_rerank_batch*) ----
     def search_batch_filtered(self, queries, filters, query_filter=None, max_search=DEFAULT_MAX_SEARCH,
-                              num_elements=DEFAULT_NUM_ELEMENTS, already_element=False, with_stats=False):
+                              num_elements=DEFAULT_NUM_ELEMENTS, already_element=False, with_stats=False, by_id=False,
+                              exclude_self=False):
         """Filtered search (granne_b200_search_filtered_batch): search_batch's traversal, unchanged, returning the first
         k admitted elements among those it scores in the bottom layer, by (distance, id).  Not a reference function.
         `filters`: a bool mask of shape (len,) or (F, len), or packed uint32 words (F, W), W >= ceil(len / 32) (id i
         is bit i % 32 of word i // 32); query_filter: one filter index per query (None: filter 0 for all).  k <=
         EXACT_MAX_K and may exceed max_search; no exact fallback, so a selective filter may return fewer than k.
         Returns search_batch's (ids, dists, counts[, stats]); stats columns 0..2 equal search_batch's."""
-        q, fmt = self._host_queries(queries, already_element)
+        q, fmt = self._host_queries(queries, already_element, by_id, exclude_self)
         nq, k = q.shape[0], int(num_elements)
         words = _filter_words(filters, len(self))
         qf = _query_filter(query_filter, nq)
@@ -567,13 +659,13 @@ class Granne:
 
     def search_batch_filtered_device(self, queries, filters, query_filter=None, max_search=DEFAULT_MAX_SEARCH,
                                      num_elements=DEFAULT_NUM_ELEMENTS, already_element=False, out=None, stats=None,
-                                     stream=None):
+                                     stream=None, by_id=False, exclude_self=False):
         """Device-resident search_batch_filtered: CUDA tensors in (queries; filters int32 [F, W] holding the uint32
         words; query_filter int32 [nq] or None) and out, asynchronous on `stream` like search_batch_device.  The kernel
         checks query_filter: an entry >= F gives its query count 0 and padding, and stream_status() raises."""
         import torch
 
-        q, fmt = self._device_queries(queries, already_element)
+        q, fmt = self._device_queries(queries, already_element, by_id, exclude_self)
         nq, k = q.shape[0], int(num_elements)
         for t, shape, what in ((filters, None, "filters"), (query_filter, (nq,), "query_filter")):
             if t is None and what == "query_filter":
@@ -704,11 +796,13 @@ class Granne:
         return [(int(ids[0, i]), float(dists[0, i])) for i in range(int(counts[0]))]
 
     def search_batch_device(self, queries, max_search=DEFAULT_MAX_SEARCH, num_elements=DEFAULT_NUM_ELEMENTS,
-                            already_element=False, out=None, stats=None, stream=None):
+                            already_element=False, out=None, stats=None, stream=None, by_id=False, exclude_self=False):
         """Device-resident variant: `queries` is a CUDA torch tensor on this index's device; returns CUDA tensors
         (ids int32 view of u32 bits, dists float32, counts int32).  Asynchronous on `stream` (a torch.cuda.Stream or a
-        raw cudaStream_t; default: the current torch stream)."""
-        q, fmt = self._device_queries(queries, already_element)
+        raw cudaStream_t; default: the current torch stream).  With by_id / exclude_self, `queries` is a contiguous
+        1-D int32 tensor of element ids (the u32 bits); a query whose id is >= num_elements() gets count 0, padding
+        and zero stats, and stream_status() raises."""
+        q, fmt = self._device_queries(queries, already_element, by_id, exclude_self)
         nq, k = q.shape[0], int(num_elements)
         ids, dists, counts = _device_outputs(q, k, out)
         _check_stats(stats, q)
@@ -730,10 +824,16 @@ class Granne:
             C.c_void_p(counts.data_ptr()) if counts is not None else None,
             C.c_void_p(stats.data_ptr()) if stats is not None else None, C.c_void_p(_raw_stream(stream, q.device))))
 
-    def _device_queries(self, queries, already_element):
+    def _device_queries(self, queries, already_element, by_id=False, exclude_self=False):
         """(checked queries, query format) of a device call, as _host_queries gives them for a host call."""
         import torch
 
+        if by_id or exclude_self:
+            if (not isinstance(queries, torch.Tensor) or not queries.is_cuda or queries.device.index != self.device
+                    or queries.dtype != torch.int32 or queries.dim() != 1 or not queries.is_contiguous()):
+                raise ValueError("ids must be a contiguous 1-D int32 CUDA tensor (the u32 ids' bits) on cuda:%d"
+                                 % self.device)
+            return queries, QUERY_ID_EXCLUDING if exclude_self else QUERY_ID
         q = self._check_device_queries(queries)
         return q, QUERY_ELEMENT if already_element or q.dtype == torch.int8 else QUERY_RAW_F32
 
@@ -755,8 +855,15 @@ class Granne:
             raise ValueError("queries must be float32 (or int8 elements for angular_int)")
         return q.contiguous()
 
-    def stream_status(self):
-        _check(load_library().granne_b200_stream_status(self._h))
+    def stream_status(self, stream=None):
+        """Raises the first error of the device calls issued since the previous check: of every stream of this handle
+        (after synchronising the device), or, given `stream` (a torch.cuda.Stream or a raw cudaStream_t), of that
+        stream's calls only, after synchronising it."""
+        if stream is None:
+            _check(load_library().granne_b200_stream_status(self._h))
+        else:
+            raw = getattr(stream, "cuda_stream", stream)
+            _check(load_library().granne_b200_stream_status_of(self._h, C.c_void_p(raw)))
 
     def release_stream(self, stream):
         """Returns the workspace the library keeps for a caller stream (a raw cudaStream_t or a torch stream)."""
@@ -819,28 +926,76 @@ class MultiGranne:
     def shard_base(self, s):
         return int(load_library().granne_b200_multi_shard_base(self._h, s))
 
+    def part_len(self, s):
+        """Index::len of part s: its global ids are [shard_base(s), shard_base(s) + part_len(s))."""
+        return int(load_library().granne_b200_multi_part_len(self._h, s))
+
+    def global_ids(self):
+        """The global ids of every indexed element, in order: [0, len) for a replicated handle, each shard's
+        [shard_base, shard_base + part_len) for a partitioned one (equal to [0, len) when every shard's index covers
+        its whole container)."""
+        parts = [(0, len(self))] if self.mode == MODE_REPLICATED else \
+            [(self.shard_base(s), self.part_len(s)) for s in range(self.num_parts())]
+        return np.concatenate([np.arange(b, b + n, dtype=np.uint64) for b, n in parts] + [np.zeros(0, np.uint64)])
+
+    def knn_graph(self, max_search=DEFAULT_MAX_SEARCH, num_elements=DEFAULT_NUM_ELEMENTS, exclude_self=True,
+                  exact=False, chunk=65536):
+        """Granne.knn_graph over all parts: for every global id of global_ids(), search_batch (exact_search_batch with
+        exact=True) of that element by id, without itself when exclude_self.  The ids go through the host calls in
+        chunks of `chunk`, each made as it is needed.  Returns (ids uint64 GLOBAL ids [len, k] padded with
+        0xFFFF_FFFF_FFFF_FFFF, dists float32 [len, k], counts uint32 [len]); row r belongs to global_ids()[r]."""
+        if int(chunk) < 1:
+            raise ValueError("chunk must be >= 1")
+        k = int(num_elements)
+        parts = [(0, len(self))] if self.mode == MODE_REPLICATED else \
+            [(self.shard_base(s), self.part_len(s)) for s in range(self.num_parts())]
+        total = sum(n for _, n in parts)
+        ids, dists, counts, _ = _host_outputs(total, k, np.uint64)
+        row = 0
+        for base, n in parts:
+            for c0 in range(0, n, int(chunk)):
+                q = np.arange(base + c0, base + min(n, c0 + int(chunk)), dtype=np.uint64)
+                if exact:
+                    r = self.exact_search_batch(q, k, by_id=True, exclude_self=exclude_self)
+                else:
+                    r = self.search_batch(q, max_search, k, by_id=True, exclude_self=exclude_self)
+                ids[row:row + q.size], dists[row:row + q.size], counts[row:row + q.size] = r
+                row += q.size
+        return ids, dists, counts
+
+    def _host_queries(self, queries, already_element, by_id, exclude_self):
+        """(contiguous queries, query format) of a host call: rows, or GLOBAL uint64 element ids with by_id /
+        exclude_self."""
+        if by_id or exclude_self:
+            return _id_queries(queries, exclude_self, np.uint64)
+        return _host_queries(queries, already_element)
+
     def search_batch(self, queries, max_search=DEFAULT_MAX_SEARCH, num_elements=DEFAULT_NUM_ELEMENTS,
-                     already_element=False):
-        q, fmt = _host_queries(queries, already_element)
+                     already_element=False, by_id=False, exclude_self=False):
+        """Granne.search_batch over all parts: GLOBAL uint64 ids in the results, and as queries with by_id (each in
+        some part's [shard_base, shard_base + Index::len) range) — exclude_self drops each query's own global id."""
+        q, fmt = self._host_queries(queries, already_element, by_id, exclude_self)
         nq, k = q.shape[0], int(num_elements)
         ids, dists, counts, _ = _host_outputs(nq, k, np.uint64)
         _check(load_library().granne_b200_multi_search_batch(self._h, _ptr(q), nq, fmt, int(max_search), k, _ptr(ids),
                                                              _ptr(dists), _ptr(counts)))
         return ids, dists, counts
 
-    def exact_search_batch(self, queries, num_elements=DEFAULT_NUM_ELEMENTS, already_element=False):
+    def exact_search_batch(self, queries, num_elements=DEFAULT_NUM_ELEMENTS, already_element=False, by_id=False,
+                           exclude_self=False):
         """Exact k nearest neighbours over all shards (granne_b200_multi_exact_search_batch): GLOBAL uint64 ids."""
-        q, fmt = _host_queries(queries, already_element)
+        q, fmt = self._host_queries(queries, already_element, by_id, exclude_self)
         nq, k = q.shape[0], int(num_elements)
         ids, dists, counts, _ = _host_outputs(nq, k, np.uint64)
         _check(load_library().granne_b200_multi_exact_search_batch(self._h, _ptr(q), nq, fmt, k, _ptr(ids),
                                                                    _ptr(dists), _ptr(counts)))
         return ids, dists, counts
 
-    def exact_search_within(self, queries, candidates, num_elements=DEFAULT_NUM_ELEMENTS, already_element=False):
+    def exact_search_within(self, queries, candidates, num_elements=DEFAULT_NUM_ELEMENTS, already_element=False,
+                            by_id=False, exclude_self=False):
         """Granne.exact_search_within over all parts (granne_b200_multi_exact_search_within_batch): GLOBAL ids in the
         candidate lists (uint64) and in the results."""
-        q, fmt = _host_queries(queries, already_element)
+        q, fmt = self._host_queries(queries, already_element, by_id, exclude_self)
         nq, k = q.shape[0], int(num_elements)
         offsets, cand = _candidate_lists(candidates, nq, np.uint64)
         ids, dists, counts, _ = _host_outputs(nq, k, np.uint64)
@@ -849,10 +1004,11 @@ class MultiGranne:
         return ids, dists, counts
 
     def search_batch_filtered(self, queries, filters, query_filter=None, max_search=DEFAULT_MAX_SEARCH,
-                              num_elements=DEFAULT_NUM_ELEMENTS, already_element=False):
+                              num_elements=DEFAULT_NUM_ELEMENTS, already_element=False, by_id=False,
+                              exclude_self=False):
         """Granne.search_batch_filtered over all parts (granne_b200_multi_search_filtered_batch): the filters are over
         GLOBAL ids (a bool mask of shape (len,) or (F, len), or uint32 words), the results are GLOBAL uint64 ids."""
-        q, fmt = _host_queries(queries, already_element)
+        q, fmt = self._host_queries(queries, already_element, by_id, exclude_self)
         nq, k = q.shape[0], int(num_elements)
         words = _filter_words(filters, len(self))
         qf = _query_filter(query_filter, nq)

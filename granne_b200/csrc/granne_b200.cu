@@ -29,6 +29,7 @@
 #include "exact_kernels.cuh"
 #include "rerank_kernels.cuh"
 #include "within_kernels.cuh"
+#include "ids_kernels.cuh"
 
 namespace gb = granne_b200;
 
@@ -163,6 +164,11 @@ struct Workspace {
     // exact search within lists: a chunk's running lists | segment prefix; its locks | query flags
     Buffer<unsigned long long> d_within;
     Buffer<int> d_within_flags;
+    // queries by element id: the elements' rows, the bad-id flags, and (QUERY_ID_EXCLUDING) the k + 1 column block
+    // ids | dists | counts
+    Buffer<uint8_t> d_id_rows;
+    Buffer<int> d_id_bad;
+    Buffer<uint32_t> d_id_res;
 };
 
 // The owners of the arrays a DeviceIndex points to, one slot per pointer: the memory and the bytes allocated for it.
@@ -871,13 +877,15 @@ int stream_workspace(Handle* h, cudaStream_t stream, Workspace** out) {
     return GRANNE_B200_OK;
 }
 
+bool by_id(int fmt) { return fmt == GRANNE_B200_QUERY_ID || fmt == GRANNE_B200_QUERY_ID_EXCLUDING; }
+
 // The argument rules every query call shares, in the order they are reported.  None of them reads the handle, so bad
 // arguments are reported before anything touches a device.  `own_rule`: the message of the call's own rule on its
-// sizes when the arguments break it, else nullptr.
+// sizes when the arguments break it, else nullptr.  `id_formats`: the call also takes queries by element id.
 int validate_batch(const Handle* h, const void* q, size_t nq, int fmt, uint32_t k, const void* ids, const void* dists,
-                   const char* own_rule) {
+                   const char* own_rule, bool id_formats = true) {
     if (!h) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "index handle is null");
-    if (fmt != GRANNE_B200_QUERY_RAW_F32 && fmt != GRANNE_B200_QUERY_ELEMENT)
+    if (fmt != GRANNE_B200_QUERY_RAW_F32 && fmt != GRANNE_B200_QUERY_ELEMENT && !(id_formats && by_id(fmt)))
         return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "unknown query format");
     if (own_rule) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, own_rule);
     if (nq > 0xFFFFFFF0ull) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "too many queries in one batch");
@@ -889,13 +897,37 @@ constexpr const char* kMaxSearchRule = "max_search must be >= 1 (the reference p
 constexpr const char* kExactKRule = "num_neighbors exceeds GRANNE_B200_EXACT_MAX_K (1024)";
 
 int validate_search(const Handle* h, const void* q, size_t nq, int fmt, uint32_t max_search, uint32_t k,
-                    const void* ids, const void* dists) {
-    return validate_batch(h, q, nq, fmt, k, ids, dists, max_search == 0 ? kMaxSearchRule : nullptr);
+                    const void* ids, const void* dists, bool id_formats = true) {
+    return validate_batch(h, q, nq, fmt, k, ids, dists, max_search == 0 ? kMaxSearchRule : nullptr, id_formats);
 }
 
 int validate_exact(const Handle* h, const void* q, size_t nq, int fmt, uint32_t k, const void* ids,
                    const void* dists) {
     return validate_batch(h, q, nq, fmt, k, ids, dists, k > GRANNE_B200_EXACT_MAX_K ? kExactKRule : nullptr);
+}
+
+// The rule QUERY_ID_EXCLUDING adds, reported after a call's other rules: the call runs with k + 1 columns, so k + 1
+// must be within the call's cap (GRANNE_B200_EXACT_MAX_K, or the u32 range for search_batch).
+int check_exclude_k(int fmt, uint32_t k, uint64_t cap) {
+    if (fmt == GRANNE_B200_QUERY_ID_EXCLUDING && (uint64_t)k + 1 > cap)
+        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT,
+                    cap == GRANNE_B200_EXACT_MAX_K
+                        ? "num_neighbors exceeds 1023 with GRANNE_B200_QUERY_ID_EXCLUDING (the call runs k + 1)"
+                        : "num_neighbors + 1 exceeds u32 with GRANNE_B200_QUERY_ID_EXCLUDING");
+    return GRANNE_B200_OK;
+}
+
+// The host check of n element ids in host memory: each < granne_b200_num_elements(h).
+int check_element_ids(const Handle* h, const uint32_t* ids, size_t n) {
+    for (size_t i = 0; i < n; ++i)
+        if (ids[i] >= h->dev.num_elements)
+            return fail(GRANNE_B200_ERR_OUT_OF_RANGE, "element id >= granne_b200_num_elements");
+    return GRANNE_B200_OK;
+}
+
+// The host check of a host call's queries: its ids when the call is by id, else nothing.
+int check_host_query_ids(const Handle* h, const void* queries, size_t nq, int fmt) {
+    return by_id(fmt) ? check_element_ids(h, static_cast<const uint32_t*>(queries), nq) : GRANNE_B200_OK;
 }
 
 gb::PeerGather device_gather(const granne_b200_peer_gather& pg, unsigned int* done_counter) {
@@ -1027,12 +1059,15 @@ int error_from_bits(int bits) {
         return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "a candidate list has bad offsets or an id >= Index::len");
     if (bits & gb::kStatusBadFilter)
         return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "a query_filter entry is >= num_filters");
+    if (bits & gb::kStatusBadId)
+        return fail(GRANNE_B200_ERR_OUT_OF_RANGE, "an element id is >= granne_b200_num_elements");
     return GRANNE_B200_OK;
 }
 
-// Bytes of one query row in `fmt` for an index of `kind` (gb::ElementKind) and width `dim`: i8 when the queries already
-// are elements of an angular_int index, f32 otherwise.
+// Bytes of one query row in `fmt` for an index of `kind` (gb::ElementKind) and width `dim`: a u32 id for the id
+// formats, i8 when the queries already are elements of an angular_int index, f32 otherwise.
 size_t query_row_bytes(int kind, uint32_t dim, int fmt) {
+    if (by_id(fmt)) return 4;
     return (size_t)dim * (kind == gb::kAngularI8 && fmt == GRANNE_B200_QUERY_ELEMENT ? 1 : 4);
 }
 
@@ -1126,6 +1161,47 @@ int with_call_inputs(cudaStream_t stream, const HostInput (&in)[N], Enqueue&& en
     const cudaError_t fe = cudaFreeAsync(mem, stream);
     if (rc) return rc;
     GB_CUDA(fe);
+    return GRANNE_B200_OK;
+}
+
+// ---- queries by element id (ids_kernels.cuh) ------------------------------------------------------------------------
+// Enqueues a query call on `stream` whatever its format: `call(q, fmt, k, out)` queues the call's kernels for device
+// query rows q.  RAW_F32 and ELEMENT queries go straight to it.  Ids (nq u32 in device memory at d_q) are read as
+// elements first: get_elements_kernel writes their rows into the workspace (a bad id reads nothing and flags its
+// query), the call runs on those rows as ELEMENT queries, and id_results_kernel writes the caller's columns.
+// QUERY_ID runs the call into the caller's output; only a device call, whose ids no host has checked
+// (`host_checked`), needs the pass that blanks flagged queries.  QUERY_ID_EXCLUDING runs it with k + 1 columns into
+// the workspace (stats straight into the caller's: they do not depend on k) and drops each query's own id.
+template <class Call>
+int enqueue_query(Handle* h, Workspace* w, const void* d_q, size_t nq, int fmt, uint32_t k, const QueryOut& out,
+                  bool host_checked, cudaStream_t stream, Call&& call) {
+    if (!by_id(fmt)) return call(d_q, fmt, k, out);
+    const gb::DeviceIndex& d = h->dev;
+    const bool exclude = fmt == GRANNE_B200_QUERY_ID_EXCLUDING;
+    const uint32_t* ids = static_cast<const uint32_t*>(d_q);
+    const size_t row = query_row_bytes(d.kind, d.dim, GRANNE_B200_QUERY_ELEMENT);
+    int rc;
+    if ((rc = w->d_id_rows.grow(std::max<size_t>(nq * row, 16), stream)) || (rc = w->d_id_bad.grow(nq, stream)))
+        return rc;
+    const size_t smem = d.kind == gb::kSumEmbeddings ? (size_t)d.dim * 4 : 0;
+    gb::get_elements_kernel<<<(unsigned)std::min<uint64_t>(nq, (uint64_t)h->num_sms * 32), 32, smem, stream>>>(
+        d, ids, nq, d.num_elements, w->d_id_rows.get(), w->d_id_bad.get(), w->d_error);
+    h->launches++;
+    GB_CUDA(cudaGetLastError());
+    QueryOut res = out;
+    const uint32_t kk = exclude ? k + 1 : k;
+    if (exclude) {
+        if ((rc = w->d_id_res.grow(2 * nq * kk + nq, stream))) return rc;
+        uint32_t* r = w->d_id_res.get();
+        res = {r, reinterpret_cast<float*>(r + nq * kk), r + 2 * nq * kk, out.stats};
+    }
+    if ((rc = call(w->d_id_rows.get(), (int)GRANNE_B200_QUERY_ELEMENT, kk, res))) return rc;
+    if (!exclude && host_checked) return GRANNE_B200_OK;
+    gb::id_results_kernel<<<(unsigned)std::min<uint64_t>((nq + 3) / 4, (uint64_t)h->num_sms * 16), 128, 0, stream>>>(
+        res.ids, res.dists, res.counts, kk, ids, w->d_id_bad.get(), exclude, nq, k, out.ids, out.dists, out.counts,
+        reinterpret_cast<unsigned long long*>(out.stats));
+    h->launches++;
+    GB_CUDA(cudaGetLastError());
     return GRANNE_B200_OK;
 }
 
@@ -1317,10 +1393,10 @@ void release_rerank(Handle* h) {
     h->rerank_mem = Staged{};
 }
 
-// validate_search's rules plus the two-stage ones.
+// validate_search's rules (raw or element queries only) plus the two-stage ones.
 int validate_rerank(const Handle* h, const void* q, size_t nq, int fmt, uint32_t max_search, uint32_t c,
                     uint32_t k, const void* ids, const void* dists) {
-    int rc = validate_search(h, q, nq, fmt, max_search, k, ids, dists);
+    int rc = validate_search(h, q, nq, fmt, max_search, k, ids, dists, false);
     if (rc) return rc;
     if (fmt != GRANNE_B200_QUERY_RAW_F32)
         return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "the two-stage search takes raw f32 queries");
@@ -1381,10 +1457,10 @@ int enqueue_rerank(Handle* h, Workspace* w, const void* d_queries, size_t nq, ui
 int validate_within(const Handle* h, const void* q, size_t nq, int fmt, uint32_t k, const void* out_ids,
                     const void* out_dists, const uint64_t* offsets, const void* ids, bool host_lists) {
     const int rc = validate_exact(h, q, nq, fmt, k, out_ids, out_dists);
-    if (rc || nq == 0) return rc;
-    if (!offsets) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "offsets is null");
-    if (host_lists && offsets[nq] > 0 && !ids) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "ids is null");
-    return GRANNE_B200_OK;
+    if (rc) return rc;
+    if (nq > 0 && !offsets) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "offsets is null");
+    if (nq > 0 && host_lists && offsets[nq] > 0 && !ids) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "ids is null");
+    return check_exclude_k(fmt, k, GRANNE_B200_EXACT_MAX_K);
 }
 
 // The host checks of nq lists in host memory: the shape of the offsets (which reads no handle), then every id
@@ -1472,9 +1548,10 @@ int validate_filtered(const Handle* h, const void* q, size_t nq, int fmt, uint32
                       const void* ids, const void* dists, const void* filters, uint32_t num_filters) {
     const int rc = validate_batch(h, q, nq, fmt, k, ids, dists,
                                   max_search == 0 ? kMaxSearchRule : k > GRANNE_B200_EXACT_MAX_K ? kExactKRule : nullptr);
-    if (rc || nq == 0) return rc;
-    if (!filters || num_filters == 0) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "filters is null or num_filters is 0");
-    return GRANNE_B200_OK;
+    if (rc) return rc;
+    if (nq > 0 && (!filters || num_filters == 0))
+        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "filters is null or num_filters is 0");
+    return check_exclude_k(fmt, k, GRANNE_B200_EXACT_MAX_K);
 }
 
 // A bitmap of filter_words words must hold a bit for every id in [0, span).
@@ -1507,8 +1584,11 @@ int search_filtered_host(Handle* h, const void* queries, size_t nq, int fmt, uin
                               const DeviceFilters f{static_cast<const uint32_t*>(d[0]),
                                                     query_filter ? static_cast<const uint32_t*>(d[1]) : nullptr,
                                                     filter_words, num_filters, bit_base};
-                              return enqueue_search(h, w, w->d_queries.get(), nq, fmt, max_search, k, out, stream,
-                                                    nullptr, nullptr, &f);
+                              return enqueue_query(h, w, w->d_queries.get(), nq, fmt, k, out, true, stream,
+                                                   [&](const void* q, int f2, uint32_t kk, const QueryOut& o) {
+                                                       return enqueue_search(h, w, q, nq, f2, max_search, kk, o,
+                                                                             stream, nullptr, nullptr, &f);
+                                                   });
                           });
                       });
 }
@@ -1831,13 +1911,59 @@ int granne_b200_get_element(const granne_b200_index* hc, uint64_t idx, void* out
     });
 }
 
+int granne_b200_get_elements(granne_b200_index* h, const uint32_t* ids, size_t n, void* out) {
+    if (!h || (n && (!ids || !out))) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
+    int rc = check_element_ids(h, ids, n);
+    if (rc || n == 0) return rc;
+    return guarded([&] {
+        GB_DEVICE(h->device);
+        std::unique_ptr<Workspace> ws;
+        int rc = ws_acquire(h, &ws);
+        if (rc) return rc;
+        Workspace* w = ws.get();
+        const int status = [&] {
+            cudaStream_t stream = w->stream.get();
+            const size_t bytes = n * query_row_bytes(h->dev.kind, h->dev.dim, GRANNE_B200_QUERY_ELEMENT);
+            int rc;
+            if ((rc = w->d_queries.grow(n * 4, stream)) || (rc = w->d_id_rows.grow(std::max<size_t>(bytes, 16), stream)))
+                return rc;
+            GB_CUDA(cudaMemcpyAsync(w->d_queries.get(), ids, n * 4, cudaMemcpyHostToDevice, stream));
+            const size_t smem = h->dev.kind == gb::kSumEmbeddings ? (size_t)h->dev.dim * 4 : 0;
+            gb::get_elements_kernel<<<(unsigned)std::min<uint64_t>(n, (uint64_t)h->num_sms * 32), 32, smem, stream>>>(
+                h->dev, reinterpret_cast<const uint32_t*>(w->d_queries.get()), n, h->dev.num_elements,
+                w->d_id_rows.get(), nullptr, w->d_error);
+            h->launches++;
+            GB_CUDA(cudaGetLastError());
+            GB_CUDA(cudaMemcpyAsync(out, w->d_id_rows.get(), bytes, cudaMemcpyDeviceToHost, stream));
+            GB_CUDA(cudaStreamSynchronize(stream));
+            return (int)GRANNE_B200_OK;
+        }();
+        ws_release(h, std::move(ws));
+        return status;
+    });
+}
+
+int granne_b200_get_elements_device(granne_b200_index* h, const uint32_t* d_ids, size_t n, void* d_out,
+                                    void* cuda_stream) {
+    if (!h || (n && (!d_ids || !d_out))) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
+    if (n == 0) return GRANNE_B200_OK;
+    return device_batch(h, cuda_stream, false, [&](Workspace* w, cudaStream_t stream) {
+        const size_t smem = h->dev.kind == gb::kSumEmbeddings ? (size_t)h->dev.dim * 4 : 0;
+        gb::get_elements_kernel<<<(unsigned)std::min<uint64_t>(n, (uint64_t)h->num_sms * 32), 32, smem, stream>>>(
+            h->dev, d_ids, n, h->dev.num_elements, d_out, nullptr, w->d_error);
+        h->launches++;
+        GB_CUDA(cudaGetLastError());
+        return GRANNE_B200_OK;
+    });
+}
+
 static int search_device_impl(granne_b200_index* h, const void* d_queries, size_t nq, int query_format,
                               uint32_t max_search, uint32_t num_neighbors, uint32_t* d_out_ids, float* d_out_dists,
                               uint32_t* d_out_counts, uint64_t* d_out_stats, void* cuda_stream,
                               const granne_b200_peer_gather* pg) {
     int rc = validate_search(h, d_queries, nq, query_format, max_search, num_neighbors, pg ? (void*)pg : d_out_ids,
-                             pg ? (void*)pg : d_out_dists);
-    if (rc) return rc;
+                             pg ? (void*)pg : d_out_dists, !pg);
+    if (rc || (rc = check_exclude_k(query_format, num_neighbors, UINT32_MAX))) return rc;
     if (pg) {
         if (pg->n_peers < 1 || pg->n_peers > GRANNE_B200_MAX_PEERS || pg->my_rank >= pg->n_peers)
             return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "peer gather: n_peers must be 1..8 and my_rank < n_peers");
@@ -1855,8 +1981,11 @@ static int search_device_impl(granne_b200_index* h, const void* d_queries, size_
             return GRANNE_B200_OK;
         });
     return device_batch(h, cuda_stream, true, [&](Workspace* w, cudaStream_t stream) {
-        return enqueue_search(h, w, d_queries, nq, query_format, max_search, num_neighbors,
-                              {d_out_ids, d_out_dists, d_out_counts, d_out_stats}, stream, pg);
+        return enqueue_query(h, w, d_queries, nq, query_format, num_neighbors,
+                             {d_out_ids, d_out_dists, d_out_counts, d_out_stats}, false, stream,
+                             [&](const void* q, int f, uint32_t kk, const QueryOut& o) {
+                                 return enqueue_search(h, w, q, nq, f, max_search, kk, o, stream, pg);
+                             });
     });
 }
 
@@ -1901,6 +2030,22 @@ int granne_b200_release_stream(granne_b200_index* h, void* cuda_stream) {
     });
 }
 
+int granne_b200_stream_status_of(granne_b200_index* h, void* cuda_stream) {
+    if (!h) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "index handle is null");
+    return guarded([&] {
+        GB_DEVICE(h->device);
+        cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+        GB_CUDA(cudaStreamSynchronize(stream));
+        std::lock_guard<std::mutex> g(h->pool_mu);
+        auto it = h->stream_ws.find(stream);
+        if (it == h->stream_ws.end()) return (int)GRANNE_B200_OK;
+        int e[4] = {0, 0, 0, 0};
+        GB_CUDA(cudaMemcpy(e, it->second->d_error, sizeof(e), cudaMemcpyDeviceToHost));
+        GB_CUDA(cudaMemset(it->second->d_error, 0, sizeof(e)));
+        return error_from_bits(e[0]);
+    });
+}
+
 int granne_b200_stream_status(granne_b200_index* h) {
     if (!h) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "index handle is null");
     return guarded([&] {
@@ -1922,23 +2067,30 @@ int granne_b200_search_batch(granne_b200_index* h, const void* queries, size_t n
                              uint32_t max_search, uint32_t num_neighbors, uint32_t* out_ids, float* out_dists,
                              uint32_t* out_counts, uint64_t* out_stats) {
     int rc = validate_search(h, queries, nq, query_format, max_search, num_neighbors, out_ids, out_dists);
-    if (rc) return rc;
+    if (rc || (rc = check_exclude_k(query_format, num_neighbors, UINT32_MAX))) return rc;
     if (nq == 0) return GRANNE_B200_OK;
+    if ((rc = check_host_query_ids(h, queries, nq, query_format))) return rc;
     return host_batch(h, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts, out_stats,
                       [&](Workspace* w, cudaStream_t stream, const QueryOut& out) {
-                          return enqueue_search(h, w, w->d_queries.get(), nq, query_format, max_search, num_neighbors,
-                                                out, stream);
+                          return enqueue_query(h, w, w->d_queries.get(), nq, query_format, num_neighbors, out, true,
+                                               stream, [&](const void* q, int f, uint32_t kk, const QueryOut& o) {
+                                                   return enqueue_search(h, w, q, nq, f, max_search, kk, o, stream);
+                                               });
                       });
 }
 
 int granne_b200_exact_search_batch(granne_b200_index* h, const void* queries, size_t nq, int query_format,
                                    uint32_t num_neighbors, uint32_t* out_ids, float* out_dists, uint32_t* out_counts) {
     int rc = validate_exact(h, queries, nq, query_format, num_neighbors, out_ids, out_dists);
-    if (rc) return rc;
+    if (rc || (rc = check_exclude_k(query_format, num_neighbors, GRANNE_B200_EXACT_MAX_K))) return rc;
     if (nq == 0) return GRANNE_B200_OK;
+    if ((rc = check_host_query_ids(h, queries, nq, query_format))) return rc;
     return host_batch(h, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts, nullptr,
                       [&](Workspace* w, cudaStream_t stream, const QueryOut& out) {
-                          return enqueue_exact(h, w, w->d_queries.get(), nq, query_format, num_neighbors, out, stream);
+                          return enqueue_query(h, w, w->d_queries.get(), nq, query_format, num_neighbors, out, true,
+                                               stream, [&](const void* q, int f, uint32_t kk, const QueryOut& o) {
+                                                   return enqueue_exact(h, w, q, nq, f, kk, o, stream);
+                                               });
                       });
 }
 
@@ -1946,11 +2098,14 @@ int granne_b200_exact_search_batch_device(granne_b200_index* h, const void* d_qu
                                           uint32_t num_neighbors, uint32_t* d_out_ids, float* d_out_dists,
                                           uint32_t* d_out_counts, void* cuda_stream) {
     int rc = validate_exact(h, d_queries, nq, query_format, num_neighbors, d_out_ids, d_out_dists);
-    if (rc) return rc;
+    if (rc || (rc = check_exclude_k(query_format, num_neighbors, GRANNE_B200_EXACT_MAX_K))) return rc;
     if (nq == 0) return GRANNE_B200_OK;
     return device_batch(h, cuda_stream, false, [&](Workspace* w, cudaStream_t stream) {
-        return enqueue_exact(h, w, d_queries, nq, query_format, num_neighbors,
-                             {d_out_ids, d_out_dists, d_out_counts, nullptr}, stream);
+        return enqueue_query(h, w, d_queries, nq, query_format, num_neighbors,
+                             {d_out_ids, d_out_dists, d_out_counts, nullptr}, false, stream,
+                             [&](const void* q, int f, uint32_t kk, const QueryOut& o) {
+                                 return enqueue_exact(h, w, q, nq, f, kk, o, stream);
+                             });
     });
 }
 
@@ -1960,14 +2115,19 @@ int granne_b200_exact_search_within_batch(granne_b200_index* h, const void* quer
     int rc = validate_within(h, queries, nq, query_format, num_neighbors, out_ids, out_dists, offsets, ids, true);
     if (rc) return rc;
     if (nq == 0) return GRANNE_B200_OK;
-    if ((rc = check_within_offsets(offsets, nq)) || (rc = check_within_ids(offsets, nq, ids, h->index_len))) return rc;
+    if ((rc = check_within_offsets(offsets, nq)) || (rc = check_within_ids(offsets, nq, ids, h->index_len)) ||
+        (rc = check_host_query_ids(h, queries, nq, query_format)))
+        return rc;
     return host_batch(h, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts, nullptr,
                       [&](Workspace* w, cudaStream_t stream, const QueryOut& out) {
                           const HostInput in[] = {{offsets, (nq + 1) * 8}, {ids, offsets[nq] * 4}};
                           return with_call_inputs(stream, in, [&](const void* const* d) {
-                              return enqueue_within(h, w, w->d_queries.get(), nq, query_format,
-                                                    static_cast<const uint64_t*>(d[0]),
-                                                    static_cast<const uint32_t*>(d[1]), num_neighbors, out, stream);
+                              return enqueue_query(
+                                  h, w, w->d_queries.get(), nq, query_format, num_neighbors, out, true, stream,
+                                  [&](const void* q, int f, uint32_t kk, const QueryOut& o) {
+                                      return enqueue_within(h, w, q, nq, f, static_cast<const uint64_t*>(d[0]),
+                                                            static_cast<const uint32_t*>(d[1]), kk, o, stream);
+                                  });
                           });
                       });
 }
@@ -1981,8 +2141,11 @@ int granne_b200_exact_search_within_batch_device(granne_b200_index* h, const voi
     if (rc) return rc;
     if (nq == 0) return GRANNE_B200_OK;
     return device_batch(h, cuda_stream, false, [&](Workspace* w, cudaStream_t stream) {
-        return enqueue_within(h, w, d_queries, nq, query_format, d_offsets, d_ids, num_neighbors,
-                              {d_out_ids, d_out_dists, d_out_counts, nullptr}, stream);
+        return enqueue_query(h, w, d_queries, nq, query_format, num_neighbors,
+                             {d_out_ids, d_out_dists, d_out_counts, nullptr}, false, stream,
+                             [&](const void* q, int f, uint32_t kk, const QueryOut& o) {
+                                 return enqueue_within(h, w, q, nq, f, d_offsets, d_ids, kk, o, stream);
+                             });
     });
 }
 
@@ -1994,7 +2157,8 @@ int granne_b200_search_filtered_batch(granne_b200_index* h, const void* queries,
                                num_filters);
     if (rc || nq == 0) return rc;
     if ((rc = check_filter_words(filter_words, h->index_len)) ||
-        (rc = check_query_filter(query_filter, nq, num_filters)))
+        (rc = check_query_filter(query_filter, nq, num_filters)) ||
+        (rc = check_host_query_ids(h, queries, nq, query_format)))
         return rc;
     return search_filtered_host(h, queries, nq, query_format, max_search, num_neighbors, filters, num_filters,
                                 filter_words, query_filter, 0, out_ids, out_dists, out_counts, out_stats);
@@ -2011,8 +2175,12 @@ int granne_b200_search_filtered_batch_device(granne_b200_index* h, const void* d
     if ((rc = check_filter_words(filter_words, h->index_len))) return rc;
     return device_batch(h, cuda_stream, true, [&](Workspace* w, cudaStream_t stream) {
         const DeviceFilters f{d_filters, d_query_filter, filter_words, num_filters, 0};
-        return enqueue_search(h, w, d_queries, nq, query_format, max_search, num_neighbors,
-                              {d_out_ids, d_out_dists, d_out_counts, d_out_stats}, stream, nullptr, nullptr, &f);
+        return enqueue_query(h, w, d_queries, nq, query_format, num_neighbors,
+                             {d_out_ids, d_out_dists, d_out_counts, d_out_stats}, false, stream,
+                             [&](const void* q, int f2, uint32_t kk, const QueryOut& o) {
+                                 return enqueue_search(h, w, q, nq, f2, max_search, kk, o, stream, nullptr, nullptr,
+                                                       &f);
+                             });
     });
 }
 
@@ -2875,6 +3043,9 @@ void granne_b200_multi_close(granne_b200_multi* m) {
 
 uint64_t granne_b200_multi_len(const granne_b200_multi* m) { return m ? m->total_len : 0; }
 size_t granne_b200_multi_num_parts(const granne_b200_multi* m) { return m ? m->parts.size() : 0; }
+uint64_t granne_b200_multi_part_len(const granne_b200_multi* m, size_t s) {
+    return (m && s < m->parts.size()) ? m->parts[s]->index_len : 0;
+}
 uint64_t granne_b200_multi_shard_base(const granne_b200_multi* m, size_t s) {
     return (m && s < m->base.size()) ? m->base[s] : 0;
 }
@@ -2950,6 +3121,65 @@ int multi_batch(granne_b200_multi* m, const void* queries, size_t nq, int query_
     });
 }
 
+// A multi-handle call whatever its query format: `call(q, fmt, k, ids, dists, counts)` runs it for host query rows q.
+// RAW_F32 and ELEMENT queries go straight to it.  Ids are u64 global ids, each in some part's [shard_base, shard_base +
+// Index::len) (checked on the host before any device call); their rows are read from the parts that own them
+// (granne_b200_get_elements), and the call runs on those rows as ELEMENT queries: into the caller's outputs for
+// QUERY_ID, with k + 1 columns for QUERY_ID_EXCLUDING, whose entry of the query's own global id is then removed.
+template <class Call>
+int multi_query(granne_b200_multi* m, const void* queries, size_t nq, int fmt, uint32_t k, uint64_t* out_ids,
+                float* out_dists, uint32_t* out_counts, Call&& call) {
+    if (!by_id(fmt)) return call(queries, fmt, k, out_ids, out_dists, out_counts);
+    return guarded([&] {
+        const uint64_t* gids = static_cast<const uint64_t*>(queries);
+        const size_t n = m->parts.size();
+        std::vector<std::vector<uint32_t>> local(n);
+        std::vector<std::vector<size_t>> rows_of(n);
+        for (size_t q = 0; q < nq; ++q) {
+            size_t s = 0;
+            if (m->mode == GRANNE_B200_MODE_RANGE_PARTITIONED)
+                s = std::upper_bound(m->base.begin(), m->base.end(), gids[q]) - m->base.begin() - 1;
+            if (gids[q] - m->base[s] >= m->parts[s]->index_len)
+                return fail(GRANNE_B200_ERR_OUT_OF_RANGE, "element id is in no part's Index::len range");
+            local[s].push_back((uint32_t)(gids[q] - m->base[s]));
+            rows_of[s].push_back(q);
+        }
+        const size_t row = query_row_bytes(m->kind, m->dim, GRANNE_B200_QUERY_ELEMENT);
+        std::vector<uint8_t> rows(nq * row), part;
+        for (size_t s = 0; s < n; ++s) {
+            if (local[s].empty()) continue;
+            part.resize(local[s].size() * row);
+            const int rc = granne_b200_get_elements(m->parts[s], local[s].data(), local[s].size(), part.data());
+            if (rc) return rc;
+            for (size_t j = 0; j < rows_of[s].size(); ++j)
+                std::memcpy(rows.data() + rows_of[s][j] * row, part.data() + j * row, row);
+        }
+        if (fmt == GRANNE_B200_QUERY_ID)
+            return call(rows.data(), (int)GRANNE_B200_QUERY_ELEMENT, k, out_ids, out_dists, out_counts);
+        const size_t kk = (size_t)k + 1;
+        std::vector<uint64_t> ids(nq * kk);
+        std::vector<float> ds(nq * kk);
+        std::vector<uint32_t> cnt(nq);
+        const int rc = call(rows.data(), (int)GRANNE_B200_QUERY_ELEMENT, (uint32_t)kk, ids.data(), ds.data(), cnt.data());
+        if (rc) return rc;
+        for (size_t q = 0; q < nq; ++q) {
+            uint32_t r = 0;
+            for (size_t j = 0; j < cnt[q] && r < k; ++j) {
+                if (ids[q * kk + j] == gids[q]) continue;
+                out_ids[q * k + r] = ids[q * kk + j];
+                out_dists[q * k + r] = ds[q * kk + j];
+                ++r;
+            }
+            if (out_counts) out_counts[q] = r;
+            for (size_t j = r; j < k; ++j) {
+                out_ids[q * k + j] = ~0ull;
+                out_dists[q * k + j] = std::numeric_limits<float>::infinity();
+            }
+        }
+        return (int)GRANNE_B200_OK;
+    });
+}
+
 // Attaches a re-rank container to every part: check(i) runs every host check of part i's images (i: the part, whose
 // image is 0 for a replicated handle), for every part, before attach(i) stages any.  If a part then fails to stage (a
 // device error), the parts this call attached drop their containers again, so that the call can be repeated.
@@ -2988,11 +3218,15 @@ int granne_b200_multi_search_batch(granne_b200_multi* m, const void* queries, si
                                    uint32_t* out_counts) {
     if (!m) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "multi handle is null");
     int rc = validate_search(m->parts[0], queries, nq, query_format, max_search, num_neighbors, out_ids, out_dists);
-    if (rc || nq == 0) return rc;
-    return multi_batch(m, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts,
-                       [&](size_t i, size_t, const void* q, size_t cnt, uint32_t* ids, float* ds, uint32_t* c) {
-                           return granne_b200_search_batch(m->parts[i], q, cnt, query_format, max_search,
-                                                           num_neighbors, ids, ds, c, nullptr);
+    if (rc || (rc = check_exclude_k(query_format, num_neighbors, UINT32_MAX)) || nq == 0) return rc;
+    return multi_query(m, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts,
+                       [&](const void* rows, int fmt, uint32_t k, uint64_t* oi, float* od, uint32_t* oc) {
+                           return multi_batch(
+                               m, rows, nq, fmt, k, oi, od, oc,
+                               [&](size_t i, size_t, const void* q, size_t cnt, uint32_t* ids, float* ds, uint32_t* c) {
+                                   return granne_b200_search_batch(m->parts[i], q, cnt, fmt, max_search, k, ids, ds,
+                                                                   c, nullptr);
+                               });
                        });
 }
 
@@ -3003,11 +3237,14 @@ int granne_b200_multi_exact_search_batch(granne_b200_multi* m, const void* queri
                                          uint32_t* out_counts) {
     if (!m) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "multi handle is null");
     int rc = validate_exact(m->parts[0], queries, nq, query_format, num_neighbors, out_ids, out_dists);
-    if (rc || nq == 0) return rc;
-    return multi_batch(m, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts,
-                       [&](size_t i, size_t, const void* q, size_t cnt, uint32_t* ids, float* ds, uint32_t* c) {
-                           return granne_b200_exact_search_batch(m->parts[i], q, cnt, query_format, num_neighbors,
-                                                                 ids, ds, c);
+    if (rc || (rc = check_exclude_k(query_format, num_neighbors, GRANNE_B200_EXACT_MAX_K)) || nq == 0) return rc;
+    return multi_query(m, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts,
+                       [&](const void* rows, int fmt, uint32_t k, uint64_t* oi, float* od, uint32_t* oc) {
+                           return multi_batch(
+                               m, rows, nq, fmt, k, oi, od, oc,
+                               [&](size_t i, size_t, const void* q, size_t cnt, uint32_t* ids, float* ds, uint32_t* c) {
+                                   return granne_b200_exact_search_batch(m->parts[i], q, cnt, fmt, k, ids, ds, c);
+                               });
                        });
 }
 
@@ -3039,22 +3276,25 @@ int granne_b200_multi_exact_search_within_batch(granne_b200_multi* m, const void
             }
             for (size_t s = 0; s < n; ++s) loff[s].push_back(lids[s].size());
         }
-        return multi_batch(m, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts,
-                           [&](size_t i, size_t b, const void* q, size_t cnt, uint32_t* pids, float* ds, uint32_t* c) {
-                               if (range)
-                                   return granne_b200_exact_search_within_batch(m->parts[i], q, cnt, query_format,
-                                                                                loff[i].data(), lids[i].data(),
-                                                                                num_neighbors, pids, ds, c);
-                               // the slice of queries [b, b + cnt) and their lists
-                               return guarded([&] {
-                                   std::vector<uint64_t> off(cnt + 1);
-                                   for (size_t j = 0; j <= cnt; ++j) off[j] = offsets[b + j] - offsets[b];
-                                   const std::vector<uint32_t> sl(ids + offsets[b], ids + offsets[b + cnt]);
-                                   return granne_b200_exact_search_within_batch(m->parts[i], q, cnt, query_format,
-                                                                                off.data(), sl.data(), num_neighbors,
-                                                                                pids, ds, c);
-                               });
-                           });
+        return multi_query(
+            m, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts,
+            [&](const void* rows, int fmt, uint32_t k, uint64_t* oi, float* od, uint32_t* oc) {
+                return multi_batch(
+                    m, rows, nq, fmt, k, oi, od, oc,
+                    [&](size_t i, size_t b, const void* q, size_t cnt, uint32_t* pids, float* ds, uint32_t* c) {
+                        if (range)
+                            return granne_b200_exact_search_within_batch(m->parts[i], q, cnt, fmt, loff[i].data(),
+                                                                         lids[i].data(), k, pids, ds, c);
+                        // the slice of queries [b, b + cnt) and their lists
+                        return guarded([&] {
+                            std::vector<uint64_t> off(cnt + 1);
+                            for (size_t j = 0; j <= cnt; ++j) off[j] = offsets[b + j] - offsets[b];
+                            const std::vector<uint32_t> sl(ids + offsets[b], ids + offsets[b + cnt]);
+                            return granne_b200_exact_search_within_batch(m->parts[i], q, cnt, fmt, off.data(),
+                                                                         sl.data(), k, pids, ds, c);
+                        });
+                    });
+            });
     });
 }
 
@@ -3075,12 +3315,16 @@ int granne_b200_multi_search_filtered_batch(granne_b200_multi* m, const void* qu
     for (size_t s = 0; range && s < m->parts.size(); ++s) span = std::max(span, m->base[s] + m->parts[s]->index_len);
     if ((rc = check_filter_words(filter_words, span)) || (rc = check_query_filter(query_filter, nq, num_filters)))
         return rc;
-    return multi_batch(m, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts,
-                       [&](size_t i, size_t b, const void* q, size_t cnt, uint32_t* ids, float* ds, uint32_t* c) {
-                           return search_filtered_host(m->parts[i], q, cnt, query_format, max_search, num_neighbors,
-                                                       filters, num_filters, filter_words,
-                                                       query_filter ? query_filter + b : nullptr, m->base[i], ids, ds,
-                                                       c, nullptr);
+    return multi_query(m, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts,
+                       [&](const void* rows, int fmt, uint32_t k, uint64_t* oi, float* od, uint32_t* oc) {
+                           return multi_batch(
+                               m, rows, nq, fmt, k, oi, od, oc,
+                               [&](size_t i, size_t b, const void* q, size_t cnt, uint32_t* ids, float* ds, uint32_t* c) {
+                                   return search_filtered_host(m->parts[i], q, cnt, fmt, max_search, k, filters,
+                                                               num_filters, filter_words,
+                                                               query_filter ? query_filter + b : nullptr, m->base[i],
+                                                               ids, ds, c, nullptr);
+                               });
                        });
 }
 

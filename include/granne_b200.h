@@ -56,6 +56,23 @@ extern "C" {
                                        (py/src/variants/index.rs:15-16,32-33,103-108). */
 #define GRANNE_B200_QUERY_ELEMENT 1 /* already an `Elements::Element`: normalised f32 (angular, embeddings) or i8
                                        (angular_int) — what Rust callers of Granne::search pass. */
+#define GRANNE_B200_QUERY_ID 2      /* nq u32 element ids (u64 global ids on a multi handle): the query of row q is
+                                       Granne::get_element(ids[q]) (src/index/mod.rs:153-155), how the reference's
+                                       examples and self-recall tests search (examples/glove.rs).  The result is
+                                       bit-identical to the same call with those rows as QUERY_ELEMENT (ids, distance
+                                       bits, counts, stats columns 0..2).  An id must be < granne_b200_num_elements
+                                       (the container: ids in [Index::len, num_elements) of a builder snapshot are valid
+                                       queries).  Host calls check every id before any device call and return
+                                       GRANNE_B200_ERR_OUT_OF_RANGE; in device calls a query with a bad id gets count 0,
+                                       padding and zero stats, the others are unaffected, and granne_b200_stream_status
+                                       reports ERR_OUT_OF_RANGE.  Accepted by search_batch, exact_search_batch,
+                                       exact_search_within_batch and search_filtered_batch (host and device forms, and
+                                       their multi-handle forms); search_batch_device_gather and the two-stage calls
+                                       reject it as an unknown format. */
+#define GRANNE_B200_QUERY_ID_EXCLUDING 3 /* QUERY_ID without the element itself: the call's result for the same query
+                                       with num_neighbors = k + 1, the entry whose id is ids[q] removed, cut to the first
+                                       k.  Other elements at distance 0 (duplicates) stay.  Stats columns 0..2 are
+                                       QUERY_ID's.  The calls capped at GRANNE_B200_EXACT_MAX_K then take k <= 1023. */
 
 /* Per-query counters written to `out_stats` (4 x u64 per query).  n_dist / n_expand are exactly the number of
  * `dist_to_element` (src/index/mod.rs:1012,1027) and `get_neighbors` (:1025) calls the reference makes for the
@@ -113,6 +130,15 @@ int granne_b200_element_kind(const granne_b200_index* h);
 /* Granne::get_element (src/index/mod.rs:153-155) == ElementContainer::get: writes dim f32 (ANGULAR: the stored row;
  * EMBEDDINGS: the normalised sum, embeddings/mod.rs:164-166) or dim i8 (ANGULAR_INT) to `out`. */
 int granne_b200_get_element(const granne_b200_index* h, uint64_t idx, void* out);
+/* granne_b200_get_element for n ids in one launch: row i of `out` (n x dim, f32 or i8 as above) is bit for bit what
+ * granne_b200_get_element writes for ids[i].  Every id must be < granne_b200_num_elements(h): the host call checks them
+ * all before any device call (GRANNE_B200_ERR_OUT_OF_RANGE).  n == 0 is valid; ids and out may be NULL then. */
+int granne_b200_get_elements(granne_b200_index* h, const uint32_t* ids, size_t n, void* out);
+/* Same with DEVICE pointers on cuda_stream (NULL = the default stream), asynchronous like
+ * granne_b200_search_batch_device.  The kernel checks the ids: a bad id's row is zeros and granne_b200_stream_status
+ * reports ERR_OUT_OF_RANGE. */
+int granne_b200_get_elements_device(granne_b200_index* h, const uint32_t* d_ids, size_t n, void* d_out,
+                                    void* cuda_stream);
 
 /* Replaces Granne::search(&self, &element, max_search, num_neighbors) -> Vec<(usize, f32)>
  * (src/index/mod.rs:140-150, 962-1037), for a batch of `nq` independent queries (the reference has no batch API;
@@ -316,8 +342,15 @@ int granne_b200_release_stream(granne_b200_index* h, void* cuda_stream);
 
 /* After synchronising a stream used with granne_b200_search_batch_device: GRANNE_B200_OK, or the first error
  * (ERR_NOT_FINITE / ERR_CAPACITY, or ERR_INVALID_ARGUMENT for a bad candidate list of
- * granne_b200_exact_search_within_batch_device) any query of the calls issued since the previous check raised. */
+ * granne_b200_exact_search_within_batch_device, or ERR_OUT_OF_RANGE for an element id >= num_elements of a
+ * GRANNE_B200_QUERY_ID* call or of granne_b200_get_elements_device) any query of the calls issued since the previous
+ * check raised. */
 int granne_b200_stream_status(granne_b200_index* h);
+/* granne_b200_stream_status for one caller stream: synchronises cuda_stream only, and reports and clears the errors of
+ * the calls issued on it since its previous check (GRANNE_B200_OK for a stream the handle has no workspace for).  The
+ * other streams' errors stay for their own check, so a caller that shares the handle with other threads checks its
+ * own work without consuming theirs. */
+int granne_b200_stream_status_of(granne_b200_index* h, void* cuda_stream);
 
 /* Range-partitioned mode (SURVEY.md §8e mode 2; granne shards elements into independent indexes,
  * src/elements/embeddings/parsing.rs:63-100): merges `num_parts` per-shard result tiles into the global top-k, ordered by
@@ -355,8 +388,14 @@ uint64_t granne_b200_multi_len(const granne_b200_multi* m);
 size_t granne_b200_multi_num_parts(const granne_b200_multi* m);
 /* global id of shard s's element 0 (0 for REPLICATED) */
 uint64_t granne_b200_multi_shard_base(const granne_b200_multi* m, size_t s);
+/* Index::len of part s (REPLICATED: every part's is the index's); its global ids are [shard_base, shard_base + this). */
+uint64_t granne_b200_multi_part_len(const granne_b200_multi* m, size_t s);
 /* Granne::search for nq queries (HOST buffers, as granne_b200_search_batch); out_ids are u64 GLOBAL ids padded with
- * UINT64_MAX, out_dists padded with +inf, out_counts may be NULL.  Thread-safe like the single-device call. */
+ * UINT64_MAX, out_dists padded with +inf, out_counts may be NULL.  Thread-safe like the single-device call.
+ * GRANNE_B200_QUERY_ID* queries on this and the three calls below are nq u64 GLOBAL ids, each in some part's
+ * [shard_base, shard_base + Index::len) range (else ERR_OUT_OF_RANGE, checked on the host before any device call):
+ * each query's row is read from the part that owns it and the call runs as QUERY_ELEMENT (with k + 1 columns and the
+ * query's own global id removed for QUERY_ID_EXCLUDING). */
 int granne_b200_multi_search_batch(granne_b200_multi* m, const void* queries, size_t nq, int query_format,
                                    uint32_t max_search, uint32_t num_neighbors, uint64_t* out_ids, float* out_dists,
                                    uint32_t* out_counts);

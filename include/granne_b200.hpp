@@ -17,6 +17,7 @@
 // sm_90 device every constructor that stages data throws Error{GRANNE_B200_ERR_NO_DEVICE}.
 #pragma once
 
+#include <algorithm>
 #include <cstdint>
 #include <fstream>
 #include <iterator>
@@ -196,6 +197,50 @@ public:
         std::vector<int8_t> out(dim());
         check(granne_b200_get_element(h_, idx, out.data()));
         return out;
+    }
+    // get_element for every id in one launch (granne_b200_get_elements): ids.size() x dim() values, row-major
+    std::vector<float> get_elements(const std::vector<uint32_t>& ids) const {
+        if (kind() == ElementKind::AngularInt) throw Error(GRANNE_B200_ERR_INVALID_ARGUMENT, "use get_elements_i8");
+        std::vector<float> out(ids.size() * dim());
+        check(granne_b200_get_elements(h_, ids.data(), ids.size(), out.data()));
+        return out;
+    }
+    std::vector<int8_t> get_elements_i8(const std::vector<uint32_t>& ids) const {
+        if (kind() != ElementKind::AngularInt) throw Error(GRANNE_B200_ERR_INVALID_ARGUMENT, "use get_elements");
+        std::vector<int8_t> out(ids.size() * dim());
+        check(granne_b200_get_elements(h_, ids.data(), ids.size(), out.data()));
+        return out;
+    }
+
+    // Granne::search(&get_element(id), max_search, num_neighbors) for every id in one call (GRANNE_B200_QUERY_ID);
+    // with exclude_self each id's own entry is dropped from its k + 1 results (GRANNE_B200_QUERY_ID_EXCLUDING).
+    // exact_search_by_id is the same for exact_search_batch.  exact_search_within and search_filtered take ids the same
+    // way: pass ids.data(), ids.size() and GRANNE_B200_QUERY_ID or GRANNE_B200_QUERY_ID_EXCLUDING as their queries.
+    std::vector<SearchResult> search_by_id(const std::vector<uint32_t>& ids, size_t max_search, size_t num_neighbors,
+                                           bool exclude_self = false) const {
+        return search_batch(ids.data(), ids.size(), exclude_self ? GRANNE_B200_QUERY_ID_EXCLUDING : GRANNE_B200_QUERY_ID,
+                            max_search, num_neighbors);
+    }
+    std::vector<SearchResult> exact_search_by_id(const std::vector<uint32_t>& ids, size_t num_neighbors,
+                                                 bool exclude_self = false) const {
+        return exact_search_batch(ids.data(), ids.size(),
+                                  exclude_self ? GRANNE_B200_QUERY_ID_EXCLUDING : GRANNE_B200_QUERY_ID, num_neighbors);
+    }
+    // The k-nearest-neighbour graph: search_by_id (or exact_search_batch by id, `exact`) of every element of [0, len())
+    // in chunks of `chunk` ids; entry i is element i's list.
+    std::vector<SearchResult> knn_graph(size_t max_search, size_t num_neighbors, bool exclude_self = true,
+                                        bool exact = false, size_t chunk = 65536) const {
+        if (chunk == 0) throw Error(GRANNE_B200_ERR_INVALID_ARGUMENT, "chunk must be >= 1");
+        std::vector<SearchResult> graph;
+        const int fmt = exclude_self ? GRANNE_B200_QUERY_ID_EXCLUDING : GRANNE_B200_QUERY_ID;
+        for (size_t c0 = 0; c0 < len(); c0 += chunk) {
+            std::vector<uint32_t> ids(std::min(chunk, len() - c0));
+            for (size_t i = 0; i < ids.size(); ++i) ids[i] = static_cast<uint32_t>(c0 + i);
+            std::vector<SearchResult> part = exact ? exact_search_batch(ids.data(), ids.size(), fmt, num_neighbors)
+                                                   : search_batch(ids.data(), ids.size(), fmt, max_search, num_neighbors);
+            for (auto& r : part) graph.push_back(std::move(r));
+        }
+        return graph;
     }
 
     // Granne::search(&element, max_search, num_neighbors) (:140-150); `element` is an Elements::Element
