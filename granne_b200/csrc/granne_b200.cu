@@ -2521,7 +2521,7 @@ int granne_b200_elements_from_raw(int element_kind, const float* raw, uint64_t n
     if (!out_len) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
     if (element_kind != GRANNE_B200_ANGULAR && element_kind != GRANNE_B200_ANGULAR_INT)
         return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "elements_from_raw builds angular or angular_int vectors");
-    if (dim == 0 || dim > 8192) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "dim must be in 1..8192");
+    if (dim == 0 || dim > 12000) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "dim must be in 1..12000");
     const size_t esz = element_kind == GRANNE_B200_ANGULAR ? 4 : 1;
     const size_t need = 8 + (size_t)n * dim * esz;
     *out_len = need;
@@ -2558,7 +2558,7 @@ int granne_b200_elements_from_raw_device(int element_kind, const float* d_raw, u
                                          void* d_out, void* cuda_stream) {
     if (element_kind != GRANNE_B200_ANGULAR && element_kind != GRANNE_B200_ANGULAR_INT)
         return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "elements_from_raw supports angular and angular_int");
-    if (dim == 0 || dim > 12000) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "unsupported dimension");
+    if (dim == 0 || dim > 12000) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "dim must be in 1..12000");
     if (n == 0) return GRANNE_B200_OK;
     if (!d_raw || !d_out) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null argument");
     int sms = 0;

@@ -534,7 +534,8 @@ void granne_b200_builder_free(granne_b200_builder* b);
 /* Element construction on the device: `angular::Vector::from(Vec<f32>)` per row — normalise (angular.rs:55-61,
  * math.rs:124-150) or quantise to i8 (angular_int.rs:28-45) — written as an elements file image
  * (FixedWidthSliceVector::write, src/slice_vector/mod.rs:460-466: u64 dim + rows).  kind: ANGULAR or ANGULAR_INT.
- * Call with out == NULL to query the size. */
+ * dim is 1..12000: a row is staged in the kernel's default 48 KB of shared memory (wider rows: ERR_INVALID_ARGUMENT).
+ * granne_b200_compute_distances shares the limit.  Call with out == NULL to query the size. */
 int granne_b200_elements_from_raw(int element_kind, const float* raw, uint64_t n, uint32_t dim, int device, void* out,
                                   size_t cap, size_t* out_len);
 
@@ -546,7 +547,7 @@ int granne_b200_elements_from_raw(int element_kind, const float* raw, uint64_t n
  * `device`.  The rows are copied into the staged layout during the call; the caller keeps its buffer. */
 
 /* Vector::from per row (angular.rs:55-61 / angular_int.rs:28-45), device to device, asynchronous on `cuda_stream`:
- * d_raw = n x dim raw f32 rows, d_out = n x dim elements (f32 or i8). */
+ * d_raw = n x dim raw f32 rows, d_out = n x dim elements (f32 or i8); dim 1..12000 as in granne_b200_elements_from_raw. */
 int granne_b200_elements_from_raw_device(int element_kind, const float* d_raw, uint64_t n, uint32_t dim, int device,
                                          void* d_out, void* cuda_stream);
 

@@ -80,3 +80,42 @@ def index_from_lists(oracle, layers):
                                   "num_neighbors": len(layers[-1][0]) if layers else 0, "version": 2},
                                  separators=(",", ":"))
     return meta.encode().ljust(1024, b" ") + b"".join(blobs)
+
+
+def edge_raw_f32(n, dim, seed):
+    """Raw f32 rows (n >= 12) at the edges of the reference's arithmetic, the rest random: an all-zero row, duplicates,
+    -0.0 and subnormal components, rows whose squared norm underflows to 0 (normalize_f32 leaves them as they are) or
+    overflows to +inf (they normalise to +-0), rows of subnormals only, and a row of equal components."""
+    x = random_vectors(n, dim, seed)
+    rng = np.random.default_rng(seed + 1)
+    x[0] = 0.0
+    x[2] = x[1]
+    x[3] = -0.0
+    x[3, ::3] = x[1, ::3]
+    x[4, rng.random(dim) < 0.3] = np.float32(-0.0)
+    sub = rng.random(dim) < 0.3
+    x[4, sub] = np.float32(1e-40) * np.where(rng.random(int(sub.sum())) < 0.5, -1, 1).astype(np.float32)
+    x[5] = np.float32(1e-25) * np.sign(x[5])             # squares are below the smallest subnormal: norm 0
+    x[6] = np.float32(1e20) * np.sign(x[6])              # squares overflow: norm +inf
+    x[7] = np.float32(3e-39) * np.sign(x[7])             # subnormal components
+    x[8] = np.float32(0.25)
+    x[9] = x[0]
+    x[10, : dim // 2] = np.float32(1e-38)
+    x[11] = np.float32(1.7e19) * np.sign(x[11])           # the squared norm just overflows for dim > 1
+    return x
+
+
+def edge_i8_rows(n, dim, seed):
+    """int8 element rows (n >= 8): random quantised rows plus saturated rows of +-127 and of -128 (which quantize never
+    makes, but an elements image may hold), whose r, dx and dy pass 2^24 once dim > 1040, and all-zero rows."""
+    rng = np.random.default_rng(seed)
+    x = rng.integers(-127, 128, size=(n, dim)).astype(np.int8)
+    x[0] = 0
+    x[1] = 127
+    x[2] = np.where(rng.random(dim) < 0.5, 127, -127)
+    x[3] = -128
+    x[4] = np.where(rng.random(dim) < 0.5, -128, 127)
+    x[5] = x[2]
+    x[6] = -x[2]
+    x[7] = 0
+    return x
