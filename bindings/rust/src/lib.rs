@@ -110,6 +110,20 @@ extern "C" {
         m: *mut RawMulti, queries: *const c_void, nq: usize, query_format: c_int, num_neighbors: u32,
         out_ids: *mut u64, out_dists: *mut f32, out_counts: *mut u32,
     ) -> c_int;
+    fn granne_b200_exact_range_count(
+        h: *mut RawIndex, queries: *const c_void, nq: usize, query_format: c_int, radius: f32, counts: *mut u64,
+    ) -> c_int;
+    fn granne_b200_exact_range_search(
+        h: *mut RawIndex, queries: *const c_void, nq: usize, query_format: c_int, radius: f32, offsets: *const u64,
+        ids: *mut u32, dists: *mut f32,
+    ) -> c_int;
+    fn granne_b200_multi_exact_range_count(
+        m: *mut RawMulti, queries: *const c_void, nq: usize, query_format: c_int, radius: f32, counts: *mut u64,
+    ) -> c_int;
+    fn granne_b200_multi_exact_range_search(
+        m: *mut RawMulti, queries: *const c_void, nq: usize, query_format: c_int, radius: f32, offsets: *const u64,
+        ids: *mut u64, dists: *mut f32,
+    ) -> c_int;
     fn granne_b200_exact_search_within_batch(
         h: *mut RawIndex, queries: *const c_void, nq: usize, query_format: c_int, offsets: *const u64,
         ids: *const u32, num_neighbors: u32, out_ids: *mut u32, out_dists: *mut f32, out_counts: *mut u32,
@@ -305,6 +319,30 @@ impl GpuGranne {
                     .map(|j| (ids[q * num_neighbors + j] as usize, dists[q * num_neighbors + j]))
                     .collect()
             })
+            .collect()
+    }
+
+    /// Exact range search (not a reference function): every element of `[0, len())` whose distance to the query is
+    /// `<= radius`, sorted by `(dist_to_element, id)`, the reference's distance bit for bit; count, then fill.
+    pub fn exact_range_search(
+        &self, queries: &[f32], nq: usize, query_format: c_int, radius: f32,
+    ) -> Vec<Vec<(usize, f32)>> {
+        assert_eq!(queries.len(), nq * self.dim);
+        let q = queries.as_ptr() as *const c_void;
+        let mut counts = vec![0u64; nq];
+        check(unsafe { granne_b200_exact_range_count(self.h, q, nq, query_format, radius, counts.as_mut_ptr()) });
+        let mut offsets = vec![0u64; nq + 1];
+        for i in 0..nq {
+            offsets[i + 1] = offsets[i] + counts[i];
+        }
+        let mut ids = vec![0u32; offsets[nq] as usize];
+        let mut dists = vec![0f32; offsets[nq] as usize];
+        check(unsafe {
+            granne_b200_exact_range_search(self.h, q, nq, query_format, radius, offsets.as_ptr(), ids.as_mut_ptr(),
+                                           dists.as_mut_ptr())
+        });
+        (0..nq)
+            .map(|i| (offsets[i] as usize..offsets[i + 1] as usize).map(|j| (ids[j] as usize, dists[j])).collect())
             .collect()
     }
 
@@ -568,6 +606,26 @@ impl GpuMultiGranne {
         });
         (0..nq)
             .map(|i| (0..c[i] as usize).map(|j| (ids[i * num_neighbors + j] as usize, d[i * num_neighbors + j])).collect())
+            .collect()
+    }
+
+    /// `exact_range_search` over every shard for a batch of normalised vectors; ids are global.
+    pub fn exact_range_search(&self, elements: &[f32], radius: f32) -> Vec<Vec<(usize, f32)>> {
+        let nq = elements.len() / self.dim;
+        let q = elements.as_ptr() as *const c_void;
+        let mut counts = vec![0u64; nq];
+        check(unsafe { granne_b200_multi_exact_range_count(self.m, q, nq, QUERY_ELEMENT, radius, counts.as_mut_ptr()) });
+        let mut offsets = vec![0u64; nq + 1];
+        for i in 0..nq {
+            offsets[i + 1] = offsets[i] + counts[i];
+        }
+        let (mut ids, mut d) = (vec![0u64; offsets[nq] as usize], vec![0f32; offsets[nq] as usize]);
+        check(unsafe {
+            granne_b200_multi_exact_range_search(self.m, q, nq, QUERY_ELEMENT, radius, offsets.as_ptr(),
+                                                 ids.as_mut_ptr(), d.as_mut_ptr())
+        });
+        (0..nq)
+            .map(|i| (offsets[i] as usize..offsets[i + 1] as usize).map(|j| (ids[j] as usize, d[j])).collect())
             .collect()
     }
 

@@ -109,6 +109,12 @@ def load_library():
         "granne_b200_exact_search_within_batch": (i32, [vp, vp, sz, i32, vp, vp, u32, vp, vp, vp]),
         "granne_b200_exact_search_within_batch_device": (i32, [vp, vp, sz, i32, vp, vp, u32, vp, vp, vp, vp]),
         "granne_b200_multi_exact_search_within_batch": (i32, [vp, vp, sz, i32, vp, vp, u32, vp, vp, vp]),
+        "granne_b200_exact_range_count": (i32, [vp, vp, sz, i32, C.c_float, vp]),
+        "granne_b200_exact_range_count_device": (i32, [vp, vp, sz, i32, C.c_float, vp, vp]),
+        "granne_b200_exact_range_search": (i32, [vp, vp, sz, i32, C.c_float, vp, vp, vp]),
+        "granne_b200_exact_range_search_device": (i32, [vp, vp, sz, i32, C.c_float, vp, vp, vp, vp]),
+        "granne_b200_multi_exact_range_count": (i32, [vp, vp, sz, i32, C.c_float, vp]),
+        "granne_b200_multi_exact_range_search": (i32, [vp, vp, sz, i32, C.c_float, vp, vp, vp]),
         "granne_b200_search_filtered_batch": (i32, [vp, vp, sz, i32, u32, u32, vp, u32, u64, vp, vp, vp, vp, vp]),
         "granne_b200_search_filtered_batch_device": (i32, [vp, vp, sz, i32, u32, u32, vp, u32, u64, vp, vp, vp, vp, vp,
                                                            vp]),
@@ -266,6 +272,21 @@ def _query_filter(query_filter, nq):
     if qf.size and (qf.min() < 0 or int(qf.max()) > 0xFFFFFFFF):
         raise ValueError("query_filter entries must be non-negative and fit uint32")
     return np.ascontiguousarray(qf, dtype=np.uint32)
+
+
+def _radius(radius):
+    """The radius of a range call as the library takes it: a real number, rounded to float32 (NaN is the library's to
+    reject)."""
+    if isinstance(radius, (bool, np.bool_)) or not isinstance(radius, (int, float, np.integer, np.floating)):
+        raise ValueError("radius must be a real number, not %r" % (radius,))
+    return float(np.float32(radius))
+
+
+def _csr_offsets(counts):
+    """The offsets (uint64 [nq + 1]) of a range search's output: the exclusive prefix sum of its counts."""
+    offsets = np.zeros(counts.shape[0] + 1, dtype=np.uint64)
+    np.cumsum(counts, out=offsets[1:])
+    return offsets
 
 
 def _device_outputs(q, k, out):
@@ -635,6 +656,124 @@ class Granne:
         return out_ids, dists, counts
 
     # ---- two-stage search (granne_b200_search_rerank_batch*) ----
+    # ---- exact range search ----
+    def exact_range_count(self, queries, radius, already_element=False, by_id=False, exclude_self=False):
+        """|R(q)| of every query: the number of elements i < len(self) whose distance is <= radius (rounded to float32;
+        IEEE <=, so +inf counts every element), with exact_search_batch's distances bit for bit
+        (granne_b200_exact_range_count).  Not a reference function.  Queries as in search_batch; exclude_self leaves
+        the query's own id out.  Returns uint64 [nq]."""
+        q, fmt = self._host_queries(queries, already_element, by_id, exclude_self)
+        counts = np.empty(q.shape[0], dtype=np.uint64)
+        _check(load_library().granne_b200_exact_range_count(self._h, _ptr(q), q.shape[0], fmt, _radius(radius),
+                                                            _ptr(counts)))
+        return counts
+
+    def exact_range_search(self, queries, radius, already_element=False, by_id=False, exclude_self=False):
+        """Every element within radius of each query, sorted by (distance, id), with no cap on their number: the
+        count, its prefix sum, then the fill (granne_b200_exact_range_search), i.e. two exact scans.  Returns
+        (offsets uint64 [nq + 1], ids uint32, dists float32): query q's entries are ids[offsets[q]:offsets[q + 1]]."""
+        q, fmt = self._host_queries(queries, already_element, by_id, exclude_self)
+        r = _radius(radius)
+        offsets = _csr_offsets(self.exact_range_count(q, r, already_element=fmt == QUERY_ELEMENT, by_id=by_id,
+                                                      exclude_self=exclude_self))
+        ids = np.empty(int(offsets[-1]), dtype=np.uint32)
+        dists = np.empty(int(offsets[-1]), dtype=np.float32)
+        _check(load_library().granne_b200_exact_range_search(self._h, _ptr(q), q.shape[0], fmt, r, _ptr(offsets),
+                                                             _ptr(ids), _ptr(dists)))
+        return offsets, ids, dists
+
+    def exact_range_count_device(self, queries, radius, already_element=False, out=None, stream=None, by_id=False,
+                                 exclude_self=False):
+        """Device-resident exact_range_count: CUDA tensors in, int64 [nq] counts out (the u64 counts' bits),
+        asynchronous on `stream` (a torch.cuda.Stream or a raw cudaStream_t; default: the current torch stream).  A
+        bad id counts 0 and, like a NaN distance, is raised by stream_status()."""
+        import torch
+
+        q, fmt = self._device_queries(queries, already_element, by_id, exclude_self)
+        nq = q.shape[0]
+        if out is None:
+            out = torch.empty((nq,), dtype=torch.int64, device=q.device)
+        elif (not isinstance(out, torch.Tensor) or out.device != q.device or out.dtype != torch.int64
+              or tuple(out.shape) != (nq,) or not out.is_contiguous()):
+            raise ValueError("out must be a contiguous int64 [nq] CUDA tensor on the queries' device")
+        _check(load_library().granne_b200_exact_range_count_device(
+            self._h, C.c_void_p(q.data_ptr()), nq, fmt, _radius(radius), C.c_void_p(out.data_ptr()),
+            C.c_void_p(_raw_stream(stream, q.device))))
+        return out
+
+    def exact_range_search_device(self, queries, radius, offsets, out=None, stream=None, already_element=False,
+                                  by_id=False, exclude_self=False):
+        """Device-resident fill of exact_range_search: `offsets` an int64 [nq + 1] CUDA tensor (normally the prefix
+        sum of exact_range_count_device's counts), `out` (ids int32, dists float32) of offsets[-1] entries.  With
+        out=None the outputs are sized from offsets[-1], which waits for the device; a caller that keeps its work
+        asynchronous passes `out`.  A segment whose length differs from its query's count is padded and raised by
+        stream_status().  Returns (ids, dists)."""
+        import torch
+
+        q, fmt = self._device_queries(queries, already_element, by_id, exclude_self)
+        nq = q.shape[0]
+        if (not isinstance(offsets, torch.Tensor) or offsets.device != q.device or offsets.dtype != torch.int64
+                or tuple(offsets.shape) != (nq + 1,) or not offsets.is_contiguous()):
+            raise ValueError("offsets must be a contiguous int64 [nq + 1] CUDA tensor on the queries' device")
+        if out is None:
+            total = int(offsets[-1])
+            out = (torch.empty((total,), dtype=torch.int32, device=q.device),
+                   torch.empty((total,), dtype=torch.float32, device=q.device))
+        for t, dt in zip(out, (torch.int32, torch.float32)):
+            if (not isinstance(t, torch.Tensor) or t.device != q.device or t.dtype != dt or t.dim() != 1
+                    or not t.is_contiguous()):
+                raise ValueError("out must be contiguous 1-D CUDA tensors (ids int32, dists float32) on the queries' "
+                                 "device")
+        _check(load_library().granne_b200_exact_range_search_device(
+            self._h, C.c_void_p(q.data_ptr()), nq, fmt, _radius(radius), C.c_void_p(offsets.data_ptr()),
+            C.c_void_p(out[0].data_ptr()), C.c_void_p(out[1].data_ptr()), C.c_void_p(_raw_stream(stream, q.device))))
+        return out
+
+    def range_graph(self, radius, exclude_self=True, chunk=65536, out="host"):
+        """The exact range graph of the index (near duplicates at a small radius): for every element i < len(self),
+        every element within radius of i, sorted by (distance, id), without i itself when exclude_self.  The ids
+        stream through the device calls in chunks made on the device, on a stream of its own whose errors alone are
+        reported (as knn_graph).  It computes len(self)^2 distances twice (count, then fill): O(n^2) work.  Returns
+        CSR (offsets [len + 1], ids, dists): uint64 / uint32 / float32 numpy arrays (out="host") or int64 / int32 /
+        float32 CUDA tensors (out="device")."""
+        import torch
+
+        if out not in ("host", "device"):
+            raise ValueError('out must be "host" or "device"')
+        if int(chunk) < 1:
+            raise ValueError("chunk must be >= 1")
+        r, n, step, dev = _radius(radius), len(self), int(chunk), torch.device("cuda", self.device)
+        s = torch.cuda.Stream(device=dev)
+        s.wait_stream(torch.cuda.current_stream(dev))
+
+        def ids_of(c0, c1):
+            return torch.arange(c0, c1, dtype=torch.int64, device=dev).to(torch.int32)  # the u32 ids' bits
+
+        try:
+            with torch.cuda.stream(s):
+                counts = torch.empty((n,), dtype=torch.int64, device=dev)
+                for c0 in range(0, n, step):
+                    c1 = min(n, c0 + step)
+                    self.exact_range_count_device(ids_of(c0, c1), r, by_id=True, exclude_self=exclude_self,
+                                                  out=counts[c0:c1], stream=s)
+                offsets = torch.zeros((n + 1,), dtype=torch.int64, device=dev)
+                torch.cumsum(counts, 0, out=offsets[1:])
+                host_off = offsets.cpu()  # sizes the output: waits for the counts
+                total = int(host_off[-1])
+                ids = torch.empty((total,), dtype=torch.int32, device=dev)
+                dists = torch.empty((total,), dtype=torch.float32, device=dev)
+                for c0 in range(0, n, step):
+                    c1 = min(n, c0 + step)
+                    b, e = int(host_off[c0]), int(host_off[c1])
+                    self.exact_range_search_device(ids_of(c0, c1), r, offsets[c0:c1 + 1] - b, out=(ids[b:e], dists[b:e]),
+                                                   by_id=True, exclude_self=exclude_self, stream=s)
+            self.stream_status(s)  # synchronises s and raises what any chunk reported
+        finally:
+            self.release_stream(s)
+        if out == "device":
+            return offsets, ids, dists
+        return offsets.cpu().numpy().view(np.uint64), ids.cpu().numpy().view(np.uint32), dists.cpu().numpy()
+
     def search_batch_filtered(self, queries, filters, query_filter=None, max_search=DEFAULT_MAX_SEARCH,
                               num_elements=DEFAULT_NUM_ELEMENTS, already_element=False, with_stats=False, by_id=False,
                               exclude_self=False):
@@ -1002,6 +1141,28 @@ class MultiGranne:
         _check(load_library().granne_b200_multi_exact_search_within_batch(
             self._h, _ptr(q), nq, fmt, _ptr(offsets), _ptr(cand), k, _ptr(ids), _ptr(dists), _ptr(counts)))
         return ids, dists, counts
+
+    def exact_range_count(self, queries, radius, already_element=False, by_id=False, exclude_self=False):
+        """Granne.exact_range_count over all parts (granne_b200_multi_exact_range_count): a range-partitioned handle
+        sums the shards' counts.  GLOBAL uint64 ids as queries with by_id."""
+        q, fmt = self._host_queries(queries, already_element, by_id, exclude_self)
+        counts = np.empty(q.shape[0], dtype=np.uint64)
+        _check(load_library().granne_b200_multi_exact_range_count(self._h, _ptr(q), q.shape[0], fmt, _radius(radius),
+                                                                  _ptr(counts)))
+        return counts
+
+    def exact_range_search(self, queries, radius, already_element=False, by_id=False, exclude_self=False):
+        """Granne.exact_range_search over all parts (granne_b200_multi_exact_range_search): (offsets uint64 [nq + 1],
+        GLOBAL ids uint64, dists float32), each query's entries sorted by (distance, global id)."""
+        q, fmt = self._host_queries(queries, already_element, by_id, exclude_self)
+        r = _radius(radius)
+        offsets = _csr_offsets(self.exact_range_count(q, r, already_element=fmt == QUERY_ELEMENT, by_id=by_id,
+                                                      exclude_self=exclude_self))
+        ids = np.empty(int(offsets[-1]), dtype=np.uint64)
+        dists = np.empty(int(offsets[-1]), dtype=np.float32)
+        _check(load_library().granne_b200_multi_exact_range_search(self._h, _ptr(q), q.shape[0], fmt, r, _ptr(offsets),
+                                                                   _ptr(ids), _ptr(dists)))
+        return offsets, ids, dists
 
     def search_batch_filtered(self, queries, filters, query_filter=None, max_search=DEFAULT_MAX_SEARCH,
                               num_elements=DEFAULT_NUM_ELEMENTS, already_element=False, by_id=False,

@@ -30,6 +30,7 @@
 #include "rerank_kernels.cuh"
 #include "within_kernels.cuh"
 #include "ids_kernels.cuh"
+#include "range_kernels.cuh"
 
 namespace gb = granne_b200;
 
@@ -169,6 +170,8 @@ struct Workspace {
     Buffer<uint8_t> d_id_rows;
     Buffer<int> d_id_bad;
     Buffer<uint32_t> d_id_res;
+    // exact range fill: a chunk's per-query cursors into the caller's segments
+    Buffer<unsigned long long> d_range_cursor;
 };
 
 // The owners of the arrays a DeviceIndex points to, one slot per pointer: the memory and the bytes allocated for it.
@@ -839,15 +842,16 @@ void ws_release(Handle* h, std::unique_ptr<Workspace> w) {
     h->pool.push_back(std::move(w));
 }
 
-int ws_reserve(Workspace* w, size_t query_bytes, size_t nq, size_t k) {
+// A host call's buffers for nq queries and m result entries (ids | dists | counts: m, m and nq words).
+int ws_reserve(Workspace* w, size_t query_bytes, size_t nq, size_t m) {
     cudaStream_t s = w->stream.get();
     int rc;
-    if ((rc = w->d_queries.grow(query_bytes, s)) || (rc = w->d_ids.grow(2 * nq * k + nq, s)) ||
+    if ((rc = w->d_queries.grow(query_bytes, s)) || (rc = w->d_ids.grow(2 * m + nq, s)) ||
         (rc = w->d_stats.grow(nq * 4, s)))
         return rc;
-    w->d_dists = reinterpret_cast<float*>(w->d_ids.get() + nq * k);
-    w->d_counts = w->d_ids.get() + 2 * nq * k;
-    return w->h_pinned.grow(query_bytes + nq * k * 8 + nq * 4 + nq * 32 + 128, s);
+    w->d_dists = reinterpret_cast<float*>(w->d_ids.get() + m);
+    w->d_counts = w->d_ids.get() + 2 * m;
+    return w->h_pinned.grow(query_bytes + m * 8 + nq * 4 + nq * 32 + 128, s);
 }
 
 // One workspace per caller stream: calls on the same stream are serialised by the stream itself, so the status words /
@@ -1061,6 +1065,9 @@ int error_from_bits(int bits) {
         return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "a query_filter entry is >= num_filters");
     if (bits & gb::kStatusBadId)
         return fail(GRANNE_B200_ERR_OUT_OF_RANGE, "an element id is >= granne_b200_num_elements");
+    if (bits & gb::kStatusBadSegment)
+        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT,
+                    "a range search segment's length differs from its query's count (it is padded)");
     return GRANNE_B200_OK;
 }
 
@@ -1073,11 +1080,12 @@ size_t query_row_bytes(int kind, uint32_t dim, int fmt) {
 
 // The host-pointer form of a query call (arguments validated, nq > 0), on a pooled workspace and its stream: the
 // queries go up through pinned memory, the call's words are zeroed (Workspace::d_counters), `enqueue(w, stream, out)`
-// queues the call's kernels from w->d_queries into the workspace's result block (w->d_ids | w->d_dists | w->d_counts;
-// out.stats is null when the caller wants no stats), and one synchronise brings the results and the error word back.
+// queues the call's kernels from w->d_queries into the workspace's result block (w->d_ids | w->d_dists | w->d_counts:
+// m ids, m dists, nq counts; out.stats is null when the caller wants no stats), and one synchronise brings the results
+// and the error word back.  host_batch: the k columns of search_batch's layout, m = nq * k.
 template <class Enqueue>
-int host_batch(Handle* h, const void* queries, size_t nq, int fmt, size_t k, uint32_t* out_ids, float* out_dists,
-               uint32_t* out_counts, uint64_t* out_stats, Enqueue&& enqueue) {
+int host_batch_entries(Handle* h, const void* queries, size_t nq, int fmt, size_t m, uint32_t* out_ids,
+                       float* out_dists, uint32_t* out_counts, uint64_t* out_stats, Enqueue&& enqueue) {
     return guarded([&] {
         GB_DEVICE(h->device);
         std::unique_ptr<Workspace> ws;
@@ -1086,14 +1094,14 @@ int host_batch(Handle* h, const void* queries, size_t nq, int fmt, size_t k, uin
         Workspace* w = ws.get();
         const size_t qbytes = nq * query_row_bytes(h->dev.kind, h->dev.dim, fmt);
         const int status = [&] {
-            if ((rc = ws_reserve(w, qbytes, nq, k))) return rc;
+            if ((rc = ws_reserve(w, qbytes, nq, m))) return rc;
             cudaStream_t stream = w->stream.get();
             // pinned staging layout: queries | ids | dists | counts | error | stats, the blocks behind the queries and
             // behind the error word on 16-byte boundaries (ws_reserve sizes the buffer with slack for both)
             uint8_t* hp = w->h_pinned.get();
             uint32_t* hids = reinterpret_cast<uint32_t*>(hp + ((qbytes + 15) & ~size_t(15)));
-            float* hd = reinterpret_cast<float*>(hids + nq * k);
-            uint32_t* hc = reinterpret_cast<uint32_t*>(hd + nq * k);
+            float* hd = reinterpret_cast<float*>(hids + m);
+            uint32_t* hc = reinterpret_cast<uint32_t*>(hd + m);
             int* herr = reinterpret_cast<int*>(hc + nq);
             unsigned long long* hstats = reinterpret_cast<unsigned long long*>(
                 hp + ((reinterpret_cast<uint8_t*>(herr + 4) - hp + 15) & ~size_t(15)));
@@ -1103,14 +1111,14 @@ int host_batch(Handle* h, const void* queries, size_t nq, int fmt, size_t k, uin
             uint64_t* d_stats = out_stats ? reinterpret_cast<uint64_t*>(w->d_stats.get()) : nullptr;
             if ((rc = enqueue(w, stream, QueryOut{w->d_ids.get(), w->d_dists, w->d_counts, d_stats}))) return rc;
             // one packed copy: ids | dists | counts (device and pinned layouts match), then the 16-byte error word
-            GB_CUDA(cudaMemcpyAsync(hids, w->d_ids.get(), (2 * nq * k + nq) * 4, cudaMemcpyDeviceToHost, stream));
+            GB_CUDA(cudaMemcpyAsync(hids, w->d_ids.get(), (2 * m + nq) * 4, cudaMemcpyDeviceToHost, stream));
             GB_CUDA(cudaMemcpyAsync(herr, w->d_error, 4 * sizeof(int), cudaMemcpyDeviceToHost, stream));
             if (out_stats) GB_CUDA(cudaMemcpyAsync(hstats, w->d_stats.get(), nq * 32, cudaMemcpyDeviceToHost, stream));
             GB_CUDA(cudaStreamSynchronize(stream));
             if (out_stats) std::memcpy(out_stats, hstats, nq * 32);
-            if (k) {
-                std::memcpy(out_ids, hids, nq * k * 4);
-                std::memcpy(out_dists, hd, nq * k * 4);
+            if (m) {
+                std::memcpy(out_ids, hids, m * 4);
+                std::memcpy(out_dists, hd, m * 4);
             }
             if (out_counts) std::memcpy(out_counts, hc, nq * 4);
             return error_from_bits(herr[0]);
@@ -1118,6 +1126,12 @@ int host_batch(Handle* h, const void* queries, size_t nq, int fmt, size_t k, uin
         ws_release(h, std::move(ws));  // back to the pool on every path
         return status;
     });
+}
+template <class Enqueue>
+int host_batch(Handle* h, const void* queries, size_t nq, int fmt, size_t k, uint32_t* out_ids, float* out_dists,
+               uint32_t* out_counts, uint64_t* out_stats, Enqueue&& enqueue) {
+    return host_batch_entries(h, queries, nq, fmt, nq * k, out_ids, out_dists, out_counts, out_stats,
+                              std::forward<Enqueue>(enqueue));
 }
 
 // The device-pointer form of a query call (arguments validated, nq > 0): `enqueue(w, stream)` queues the call's
@@ -1172,13 +1186,9 @@ int with_call_inputs(cudaStream_t stream, const HostInput (&in)[N], Enqueue&& en
 // QUERY_ID runs the call into the caller's output; only a device call, whose ids no host has checked
 // (`host_checked`), needs the pass that blanks flagged queries.  QUERY_ID_EXCLUDING runs it with k + 1 columns into
 // the workspace (stats straight into the caller's: they do not depend on k) and drops each query's own id.
-template <class Call>
-int enqueue_query(Handle* h, Workspace* w, const void* d_q, size_t nq, int fmt, uint32_t k, const QueryOut& out,
-                  bool host_checked, cudaStream_t stream, Call&& call) {
-    if (!by_id(fmt)) return call(d_q, fmt, k, out);
+// The rows of nq ids (device memory) as ELEMENT queries in w->d_id_rows, their bad-id flags in w->d_id_bad.
+int enqueue_id_rows(Handle* h, Workspace* w, const uint32_t* ids, size_t nq, cudaStream_t stream) {
     const gb::DeviceIndex& d = h->dev;
-    const bool exclude = fmt == GRANNE_B200_QUERY_ID_EXCLUDING;
-    const uint32_t* ids = static_cast<const uint32_t*>(d_q);
     const size_t row = query_row_bytes(d.kind, d.dim, GRANNE_B200_QUERY_ELEMENT);
     int rc;
     if ((rc = w->d_id_rows.grow(std::max<size_t>(nq * row, 16), stream)) || (rc = w->d_id_bad.grow(nq, stream)))
@@ -1188,6 +1198,17 @@ int enqueue_query(Handle* h, Workspace* w, const void* d_q, size_t nq, int fmt, 
         d, ids, nq, d.num_elements, w->d_id_rows.get(), w->d_id_bad.get(), w->d_error);
     h->launches++;
     GB_CUDA(cudaGetLastError());
+    return GRANNE_B200_OK;
+}
+
+template <class Call>
+int enqueue_query(Handle* h, Workspace* w, const void* d_q, size_t nq, int fmt, uint32_t k, const QueryOut& out,
+                  bool host_checked, cudaStream_t stream, Call&& call) {
+    if (!by_id(fmt)) return call(d_q, fmt, k, out);
+    const bool exclude = fmt == GRANNE_B200_QUERY_ID_EXCLUDING;
+    const uint32_t* ids = static_cast<const uint32_t*>(d_q);
+    int rc = enqueue_id_rows(h, w, ids, nq, stream);
+    if (rc) return rc;
     QueryOut res = out;
     const uint32_t kk = exclude ? k + 1 : k;
     if (exclude) {
@@ -1211,10 +1232,12 @@ int enqueue_query(Handle* h, Workspace* w, const void* d_q, size_t nq, int fmt, 
 constexpr uint64_t kExactSlabFloats = 64ull << 20;
 constexpr uint64_t kExactMaxSlabRows = 1ull << 20;
 
-// Distances of the prepared query chunk (qc queries in w->d_exact_q) to `nrows` rows, slab by slab, each slab's keys
-// merged into the running lists.  Row r has id base + r.
-int exact_scan_rows(Handle* h, Workspace* w, uint32_t qc, uint32_t k, const void* rows, uint64_t nrows,
-                    uint32_t row_stride, uint32_t vec_group, uint64_t base, uint64_t slab, cudaStream_t stream) {
+// Distances of the prepared query chunk (qc queries in w->d_exact_q) to `nrows` rows, slab by slab into
+// w->d_exact_dists (qc rows of `slab` floats), each slab then handed to step(ns, id_base): the ns distances of row r
+// belong to element id_base + r.
+template <class Step>
+int exact_scan_rows(Handle* h, Workspace* w, uint32_t qc, const void* rows, uint64_t nrows, uint32_t row_stride,
+                    uint32_t vec_group, uint64_t base, uint64_t slab, cudaStream_t stream, Step& step) {
     const gb::DeviceIndex& d = h->dev;
     for (uint64_t s0 = 0; s0 < nrows; s0 += slab) {
         const uint64_t ns = std::min(slab, nrows - s0);
@@ -1241,24 +1264,24 @@ int exact_scan_rows(Handle* h, Workspace* w, uint32_t qc, uint32_t k, const void
         }
         h->launches++;
         GB_CUDA(cudaGetLastError());
-        gb::exact_select_kernel<<<qc, gb::kExactSelThreads, 0, stream>>>(w->d_exact_dists.get(), slab, ns,
-                                                                         (uint32_t)(base + s0), k,
-                                                                         w->d_exact_lists.get());
-        h->launches++;
-        GB_CUDA(cudaGetLastError());
+        const int rc = step(ns, base + s0);
+        if (rc) return rc;
     }
     return GRANNE_B200_OK;
 }
 
-// Enqueues one exact search on `stream`: nq queries (device memory, the caller's format) against [0, Index::len),
-// results in search_batch's layout.  A NaN distance or query sets kStatusNotFinite in w->d_error.
-int enqueue_exact(Handle* h, Workspace* w, const void* d_queries, size_t nq, int fmt, uint32_t k, const QueryOut& out,
-                  cudaStream_t stream) {
+// The exact scan of nq queries (device memory, the caller's format) against [0, Index::len), the loop the exact and
+// range calls share: query chunks of at most kExactMaxChunk, and per chunk begin(c0, qc), the queries prepared as
+// elements, every slab of rows (EMBEDDINGS: of every window of materialised rows) scanned and handed to
+// slab_step(c0, qc, ns, id_base, ld) with its distances in w->d_exact_dists (qc rows of ld floats), then end(c0, qc).
+// Without `scan` (no rows, or nothing to rank) only begin and end run.  A NaN distance or query sets kStatusNotFinite
+// in w->d_error.
+template <class Begin, class Slab, class End>
+int exact_scan(Handle* h, Workspace* w, const void* d_queries, size_t nq, int fmt, bool scan, cudaStream_t stream,
+               Begin&& begin, Slab&& slab_step, End&& end) {
     const gb::DeviceIndex& d = h->dev;
     const uint64_t n = h->index_len;
-    const uint32_t count = (uint32_t)std::min<uint64_t>(k, n);
     const bool i8 = d.kind == gb::kAngularI8, emb = d.kind == gb::kSumEmbeddings;
-    const bool scan = k > 0 && n > 0;
     const size_t in_row = query_row_bytes(d.kind, d.dim, fmt);
     const size_t qc_max = std::min<size_t>(nq, gb::kExactMaxChunk);
     uint64_t slab = 0;
@@ -1270,8 +1293,7 @@ int enqueue_exact(Handle* h, Workspace* w, const void* d_queries, size_t nq, int
         slab = std::min<uint64_t>(slab, (n + gb::kExactRB - 1) / gb::kExactRB * gb::kExactRB);
         const size_t qrow = i8 ? d.row_stride : (size_t)d.dim * 4;
         if ((rc = w->d_exact_q.grow(std::max<size_t>(qc_max * qrow, 16), stream)) ||
-            (rc = w->d_exact_qnorm.grow(qc_max, stream)) || (rc = w->d_exact_dists.grow(qc_max * slab, stream)) ||
-            (rc = w->d_exact_lists.grow(qc_max * gb::kExactMaxK, stream)))
+            (rc = w->d_exact_qnorm.grow(qc_max, stream)) || (rc = w->d_exact_dists.grow(qc_max * slab, stream)))
             return rc;
         if (emb) {
             // SumEmbeddings::get rows, window by window (compute_embeddings' ANGULAR rows, which search exactly like
@@ -1290,13 +1312,14 @@ int enqueue_exact(Handle* h, Workspace* w, const void* d_queries, size_t nq, int
     }
     for (size_t c0 = 0; c0 < nq; c0 += gb::kExactMaxChunk) {
         const uint32_t qc = (uint32_t)std::min<size_t>(gb::kExactMaxChunk, nq - c0);
+        if ((rc = begin(c0, qc))) return rc;
         if (scan) {
-            GB_CUDA(cudaMemsetAsync(w->d_exact_lists.get(), 0xFF, (size_t)qc * gb::kExactMaxK * 8, stream));
             gb::exact_prepare_kernel<<<(unsigned)std::min<uint64_t>(qc, (uint64_t)h->num_sms * 32), 32, 0, stream>>>(
                 d, static_cast<const uint8_t*>(d_queries) + c0 * in_row, fmt, qc, w->d_exact_q.get(),
                 w->d_exact_qnorm.get(), w->d_error);
             h->launches++;
             GB_CUDA(cudaGetLastError());
+            auto step = [&](uint64_t ns, uint64_t id_base) { return slab_step(c0, qc, ns, id_base, slab); };
             if (emb) {
                 EmbeddingsInput in;
                 in.dim = d.dim;
@@ -1307,22 +1330,144 @@ int enqueue_exact(Handle* h, Workspace* w, const void* d_queries, size_t nq, int
                                                 w->d_error, stream)))
                         return rc;
                     h->launches += 2;
-                    if ((rc = exact_scan_rows(h, w, qc, k, w->d_exact_rows.get(), nr, d.dim, 1, r0, slab, stream)))
+                    if ((rc = exact_scan_rows(h, w, qc, w->d_exact_rows.get(), nr, d.dim, 1, r0, slab, stream, step)))
                         return rc;
                 }
-            } else if ((rc = exact_scan_rows(h, w, qc, k, d.vectors, n, d.row_stride, d.vec_group, 0, slab, stream))) {
+            } else if ((rc = exact_scan_rows(h, w, qc, d.vectors, n, d.row_stride, d.vec_group, 0, slab, stream,
+                                             step))) {
                 return rc;
             }
         }
-        const uint64_t outs = std::max<uint64_t>((uint64_t)qc * k, out.counts ? qc : 0);
-        if (outs == 0) continue;
-        gb::exact_write_kernel<<<(unsigned)((outs + 255) / 256), 256, 0, stream>>>(
-            w->d_exact_lists.get(), qc, k, count, out.ids ? out.ids + c0 * k : nullptr,
-            out.dists ? out.dists + c0 * k : nullptr, out.counts ? out.counts + c0 : nullptr);
-        h->launches++;
-        GB_CUDA(cudaGetLastError());
+        if ((rc = end(c0, qc))) return rc;
     }
     return GRANNE_B200_OK;
+}
+
+// Enqueues one exact search on `stream`: nq queries (device memory, the caller's format) against [0, Index::len),
+// results in search_batch's layout.  A NaN distance or query sets kStatusNotFinite in w->d_error.
+int enqueue_exact(Handle* h, Workspace* w, const void* d_queries, size_t nq, int fmt, uint32_t k, const QueryOut& out,
+                  cudaStream_t stream) {
+    const uint64_t n = h->index_len;
+    const uint32_t count = (uint32_t)std::min<uint64_t>(k, n);
+    const bool scan = k > 0 && n > 0;
+    int rc;
+    if (scan && (rc = w->d_exact_lists.grow(std::min<size_t>(nq, gb::kExactMaxChunk) * gb::kExactMaxK, stream)))
+        return rc;
+    return exact_scan(
+        h, w, d_queries, nq, fmt, scan, stream,
+        [&](size_t, uint32_t qc) {
+            if (scan) GB_CUDA(cudaMemsetAsync(w->d_exact_lists.get(), 0xFF, (size_t)qc * gb::kExactMaxK * 8, stream));
+            return (int)GRANNE_B200_OK;
+        },
+        [&](size_t, uint32_t qc, uint64_t ns, uint64_t id_base, uint64_t ld) {
+            gb::exact_select_kernel<<<qc, gb::kExactSelThreads, 0, stream>>>(w->d_exact_dists.get(), ld, ns,
+                                                                             (uint32_t)id_base, k,
+                                                                             w->d_exact_lists.get());
+            h->launches++;
+            GB_CUDA(cudaGetLastError());
+            return (int)GRANNE_B200_OK;
+        },
+        [&](size_t c0, uint32_t qc) {
+            const uint64_t outs = std::max<uint64_t>((uint64_t)qc * k, out.counts ? qc : 0);
+            if (outs == 0) return (int)GRANNE_B200_OK;
+            gb::exact_write_kernel<<<(unsigned)((outs + 255) / 256), 256, 0, stream>>>(
+                w->d_exact_lists.get(), qc, k, count, out.ids ? out.ids + c0 * k : nullptr,
+                out.dists ? out.dists + c0 * k : nullptr, out.counts ? out.counts + c0 : nullptr);
+            h->launches++;
+            GB_CUDA(cudaGetLastError());
+            return (int)GRANNE_B200_OK;
+        });
+}
+
+// ---- exact range search (range_kernels.cuh) -----------------------------------------------------------------------
+// The per-query inputs of a range call by id: skip (QUERY_ID_EXCLUDING: the query's own id, removed from its range in
+// the count and the fill alike) and bad (a device call: the bad-id flags, whose queries count 0).
+struct RangeIds {
+    const uint32_t* skip;
+    const int* bad;
+};
+
+// Enqueues a range call whatever its format: `call(q, fmt, ids)` queues its kernels for device query rows q.  Ids are
+// read as elements first (enqueue_id_rows) and the call runs on those rows as ELEMENT queries; only a device call, whose
+// ids no host has checked (`host_checked`), passes the bad-id flags.
+template <class Call>
+int enqueue_range_query(Handle* h, Workspace* w, const void* d_q, size_t nq, int fmt, bool host_checked,
+                        cudaStream_t stream, Call&& call) {
+    if (!by_id(fmt)) return call(d_q, fmt, RangeIds{nullptr, nullptr});
+    const uint32_t* ids = static_cast<const uint32_t*>(d_q);
+    const int rc = enqueue_id_rows(h, w, ids, nq, stream);
+    if (rc) return rc;
+    return call(w->d_id_rows.get(), (int)GRANNE_B200_QUERY_ELEMENT,
+                RangeIds{fmt == GRANNE_B200_QUERY_ID_EXCLUDING ? ids : nullptr, host_checked ? nullptr : w->d_id_bad.get()});
+}
+
+gb::RangeArgs range_args(Workspace* w, size_t c0, uint64_t ns, uint64_t id_base, uint64_t ld, float radius,
+                         const RangeIds& ri) {
+    gb::RangeArgs a{};
+    a.dists = w->d_exact_dists.get();
+    a.ld = ld;
+    a.nrows = ns;
+    a.base = (uint32_t)id_base;
+    a.radius = radius;
+    a.skip = ri.skip ? ri.skip + c0 : nullptr;
+    a.bad = ri.bad ? ri.bad + c0 : nullptr;
+    return a;
+}
+
+dim3 range_grid(uint64_t ns, uint32_t qc) {
+    const uint64_t rows = (uint64_t)gb::kRangeThreads * gb::kRangeRowsPerThread;
+    return dim3((unsigned)((ns + rows - 1) / rows), qc);
+}
+
+// Enqueues the count of a range call: counts[q] = |R(q)| (u64, device memory) for nq queries (device memory, ELEMENT
+// or RAW_F32).  With n > 0 the scan always runs, so a NaN distance sets kStatusNotFinite whatever the radius.
+int enqueue_range_count(Handle* h, Workspace* w, const void* d_queries, size_t nq, int fmt, float radius,
+                        const RangeIds& ri, uint64_t* counts, cudaStream_t stream) {
+    GB_CUDA(cudaMemsetAsync(counts, 0, nq * 8, stream));
+    auto none = [](size_t, uint32_t) { return (int)GRANNE_B200_OK; };
+    return exact_scan(h, w, d_queries, nq, fmt, h->index_len > 0, stream, none,
+                      [&](size_t c0, uint32_t qc, uint64_t ns, uint64_t id_base, uint64_t ld) {
+                          gb::range_count_kernel<<<range_grid(ns, qc), gb::kRangeThreads, 0, stream>>>(
+                              range_args(w, c0, ns, id_base, ld, radius, ri),
+                              reinterpret_cast<unsigned long long*>(counts) + c0);
+                          h->launches++;
+                          GB_CUDA(cudaGetLastError());
+                          return (int)GRANNE_B200_OK;
+                      },
+                      none);
+}
+
+// Enqueues the fill of a range call: R(q) into the caller's segment [offsets[q], offsets[q + 1]) of ids / dists (device
+// memory), sorted by (distance, id).  Per chunk the cursors start at the chunk's offsets, every slab's entries in range
+// are emitted at them, and range_finish_kernel sorts each segment in place, or pads it and sets kStatusBadSegment when
+// its length is not the query's count.
+int enqueue_range_fill(Handle* h, Workspace* w, const void* d_queries, size_t nq, int fmt, float radius,
+                       const RangeIds& ri, const uint64_t* d_offsets, uint32_t* ids, float* dists,
+                       cudaStream_t stream) {
+    const unsigned long long* offsets = reinterpret_cast<const unsigned long long*>(d_offsets);
+    int rc = w->d_range_cursor.grow(std::min<size_t>(nq, gb::kExactMaxChunk), stream);
+    if (rc) return rc;
+    unsigned long long* cursor = w->d_range_cursor.get();
+    return exact_scan(
+        h, w, d_queries, nq, fmt, h->index_len > 0, stream,
+        [&](size_t c0, uint32_t qc) {
+            GB_CUDA(cudaMemcpyAsync(cursor, offsets + c0, (size_t)qc * 8, cudaMemcpyDeviceToDevice, stream));
+            return (int)GRANNE_B200_OK;
+        },
+        [&](size_t c0, uint32_t qc, uint64_t ns, uint64_t id_base, uint64_t ld) {
+            gb::range_emit_kernel<<<range_grid(ns, qc), gb::kRangeThreads, 0, stream>>>(
+                range_args(w, c0, ns, id_base, ld, radius, ri), cursor, offsets + c0, ids, dists);
+            h->launches++;
+            GB_CUDA(cudaGetLastError());
+            return (int)GRANNE_B200_OK;
+        },
+        [&](size_t c0, uint32_t qc) {
+            gb::range_finish_kernel<<<qc, gb::kRangeSortThreads, 0, stream>>>(offsets + c0, cursor, ids, dists,
+                                                                              w->d_error);
+            h->launches++;
+            GB_CUDA(cudaGetLastError());
+            return (int)GRANNE_B200_OK;
+        });
 }
 
 // ---- two-stage search: angular_int traversal, exact re-rank (rerank_kernels.cuh) ---------------------------------
@@ -1476,6 +1621,25 @@ template <class Id>
 int check_within_ids(const uint64_t* offsets, size_t nq, const Id* ids, uint64_t n) {
     for (uint64_t i = 0; i < offsets[nq]; ++i)
         if ((uint64_t)ids[i] >= n) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "candidate id >= Index::len");
+    return GRANNE_B200_OK;
+}
+
+// The argument rules of the range calls, in the order they are reported: validate_batch's (a NaN radius as the call's
+// own rule), then, when nq > 0, counts NULL (count) or offsets NULL (fill).  None reads the handle.
+int validate_range(const Handle* h, const void* q, size_t nq, int fmt, float radius, const void* counts,
+                   const uint64_t* offsets, bool fill) {
+    const int rc = validate_batch(h, q, nq, fmt, 0, nullptr, nullptr, radius != radius ? "radius is NaN" : nullptr);
+    if (rc) return rc;
+    if (nq > 0 && !fill && !counts) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "counts is null");
+    if (nq > 0 && fill && !offsets) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "offsets is null");
+    return GRANNE_B200_OK;
+}
+
+// The host checks of a host fill's offsets and outputs: their shape, then ids / dists NULL with offsets[nq] > 0.
+int check_range_outputs(const uint64_t* offsets, size_t nq, const void* ids, const void* dists) {
+    const int rc = check_within_offsets(offsets, nq);
+    if (rc) return rc;
+    if (offsets[nq] > 0 && (!ids || !dists)) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null buffer");
     return GRANNE_B200_OK;
 }
 
@@ -2146,6 +2310,74 @@ int granne_b200_exact_search_within_batch_device(granne_b200_index* h, const voi
                              [&](const void* q, int f, uint32_t kk, const QueryOut& o) {
                                  return enqueue_within(h, w, q, nq, f, d_offsets, d_ids, kk, o, stream);
                              });
+    });
+}
+
+int granne_b200_exact_range_count(granne_b200_index* h, const void* queries, size_t nq, int query_format, float radius,
+                                  uint64_t* counts) {
+    int rc = validate_range(h, queries, nq, query_format, radius, counts, nullptr, false);
+    if (rc || nq == 0) return rc;
+    if ((rc = check_host_query_ids(h, queries, nq, query_format))) return rc;
+    // the nq u64 counts fill the ids and dists columns of a result block of nq entries (2 nq words)
+    uint32_t* words = reinterpret_cast<uint32_t*>(counts);
+    return host_batch_entries(h, queries, nq, query_format, nq, words, reinterpret_cast<float*>(words + nq), nullptr,
+                              nullptr, [&](Workspace* w, cudaStream_t stream, const QueryOut& out) {
+                                  return enqueue_range_query(
+                                      h, w, w->d_queries.get(), nq, query_format, true, stream,
+                                      [&](const void* q, int f, const RangeIds& ri) {
+                                          return enqueue_range_count(h, w, q, nq, f, radius, ri,
+                                                                     reinterpret_cast<uint64_t*>(out.ids), stream);
+                                      });
+                              });
+}
+
+int granne_b200_exact_range_count_device(granne_b200_index* h, const void* d_queries, size_t nq, int query_format,
+                                         float radius, uint64_t* d_counts, void* cuda_stream) {
+    int rc = validate_range(h, d_queries, nq, query_format, radius, d_counts, nullptr, false);
+    if (rc || nq == 0) return rc;
+    return device_batch(h, cuda_stream, false, [&](Workspace* w, cudaStream_t stream) {
+        return enqueue_range_query(h, w, d_queries, nq, query_format, false, stream,
+                                   [&](const void* q, int f, const RangeIds& ri) {
+                                       return enqueue_range_count(h, w, q, nq, f, radius, ri, d_counts, stream);
+                                   });
+    });
+}
+
+int granne_b200_exact_range_search(granne_b200_index* h, const void* queries, size_t nq, int query_format,
+                                   float radius, const uint64_t* offsets, uint32_t* ids, float* dists) {
+    int rc = validate_range(h, queries, nq, query_format, radius, nullptr, offsets, true);
+    if (rc || nq == 0) return rc;
+    if ((rc = check_range_outputs(offsets, nq, ids, dists)) ||
+        (rc = check_host_query_ids(h, queries, nq, query_format)))
+        return rc;
+    return host_batch_entries(h, queries, nq, query_format, offsets[nq], ids, dists, nullptr, nullptr,
+                              [&](Workspace* w, cudaStream_t stream, const QueryOut& out) {
+                                  const HostInput in[] = {{offsets, (nq + 1) * 8}};
+                                  return with_call_inputs(stream, in, [&](const void* const* d) {
+                                      return enqueue_range_query(
+                                          h, w, w->d_queries.get(), nq, query_format, true, stream,
+                                          [&](const void* q, int f, const RangeIds& ri) {
+                                              return enqueue_range_fill(h, w, q, nq, f, radius, ri,
+                                                                        static_cast<const uint64_t*>(d[0]), out.ids,
+                                                                        out.dists, stream);
+                                          });
+                                  });
+                              });
+}
+
+int granne_b200_exact_range_search_device(granne_b200_index* h, const void* d_queries, size_t nq, int query_format,
+                                          float radius, const uint64_t* d_offsets, uint32_t* d_ids, float* d_dists,
+                                          void* cuda_stream) {
+    int rc = validate_range(h, d_queries, nq, query_format, radius, nullptr, d_offsets, true);
+    if (rc || nq == 0) return rc;
+    // without both outputs every segment must be empty (the kernels flag any other)
+    uint32_t* ids = d_ids && d_dists ? d_ids : nullptr;
+    return device_batch(h, cuda_stream, false, [&](Workspace* w, cudaStream_t stream) {
+        return enqueue_range_query(h, w, d_queries, nq, query_format, false, stream,
+                                   [&](const void* q, int f, const RangeIds& ri) {
+                                       return enqueue_range_fill(h, w, q, nq, f, radius, ri, d_offsets, ids,
+                                                                 ids ? d_dists : nullptr, stream);
+                                   });
     });
 }
 
@@ -3126,34 +3358,54 @@ int multi_batch(granne_b200_multi* m, const void* queries, size_t nq, int query_
 // Index::len) (checked on the host before any device call); their rows are read from the parts that own them
 // (granne_b200_get_elements), and the call runs on those rows as ELEMENT queries: into the caller's outputs for
 // QUERY_ID, with k + 1 columns for QUERY_ID_EXCLUDING, whose entry of the query's own global id is then removed.
+// nq u64 global ids by the part that owns them: local[s] the local ids of the queries rows_of[s] of part s.  An id in
+// no part's [shard_base, shard_base + Index::len) is ERR_OUT_OF_RANGE.
+struct MultiIds {
+    std::vector<std::vector<uint32_t>> local;
+    std::vector<std::vector<size_t>> rows_of;
+};
+int multi_ids(const granne_b200_multi* m, const uint64_t* gids, size_t nq, MultiIds* out) {
+    const size_t n = m->parts.size();
+    out->local.assign(n, {});
+    out->rows_of.assign(n, {});
+    for (size_t q = 0; q < nq; ++q) {
+        size_t s = 0;
+        if (m->mode == GRANNE_B200_MODE_RANGE_PARTITIONED)
+            s = std::upper_bound(m->base.begin(), m->base.end(), gids[q]) - m->base.begin() - 1;
+        if (gids[q] - m->base[s] >= m->parts[s]->index_len)
+            return fail(GRANNE_B200_ERR_OUT_OF_RANGE, "element id is in no part's Index::len range");
+        out->local[s].push_back((uint32_t)(gids[q] - m->base[s]));
+        out->rows_of[s].push_back(q);
+    }
+    return GRANNE_B200_OK;
+}
+
+// The ELEMENT rows of nq queries by global id, read from the parts that own them (granne_b200_get_elements).
+int multi_id_rows(granne_b200_multi* m, const MultiIds& ids, size_t nq, std::vector<uint8_t>* rows) {
+    const size_t row = query_row_bytes(m->kind, m->dim, GRANNE_B200_QUERY_ELEMENT);
+    std::vector<uint8_t> part;
+    rows->assign(nq * row, 0);
+    for (size_t s = 0; s < m->parts.size(); ++s) {
+        if (ids.local[s].empty()) continue;
+        part.resize(ids.local[s].size() * row);
+        const int rc = granne_b200_get_elements(m->parts[s], ids.local[s].data(), ids.local[s].size(), part.data());
+        if (rc) return rc;
+        for (size_t j = 0; j < ids.rows_of[s].size(); ++j)
+            std::memcpy(rows->data() + ids.rows_of[s][j] * row, part.data() + j * row, row);
+    }
+    return GRANNE_B200_OK;
+}
+
 template <class Call>
 int multi_query(granne_b200_multi* m, const void* queries, size_t nq, int fmt, uint32_t k, uint64_t* out_ids,
                 float* out_dists, uint32_t* out_counts, Call&& call) {
     if (!by_id(fmt)) return call(queries, fmt, k, out_ids, out_dists, out_counts);
     return guarded([&] {
         const uint64_t* gids = static_cast<const uint64_t*>(queries);
-        const size_t n = m->parts.size();
-        std::vector<std::vector<uint32_t>> local(n);
-        std::vector<std::vector<size_t>> rows_of(n);
-        for (size_t q = 0; q < nq; ++q) {
-            size_t s = 0;
-            if (m->mode == GRANNE_B200_MODE_RANGE_PARTITIONED)
-                s = std::upper_bound(m->base.begin(), m->base.end(), gids[q]) - m->base.begin() - 1;
-            if (gids[q] - m->base[s] >= m->parts[s]->index_len)
-                return fail(GRANNE_B200_ERR_OUT_OF_RANGE, "element id is in no part's Index::len range");
-            local[s].push_back((uint32_t)(gids[q] - m->base[s]));
-            rows_of[s].push_back(q);
-        }
-        const size_t row = query_row_bytes(m->kind, m->dim, GRANNE_B200_QUERY_ELEMENT);
-        std::vector<uint8_t> rows(nq * row), part;
-        for (size_t s = 0; s < n; ++s) {
-            if (local[s].empty()) continue;
-            part.resize(local[s].size() * row);
-            const int rc = granne_b200_get_elements(m->parts[s], local[s].data(), local[s].size(), part.data());
-            if (rc) return rc;
-            for (size_t j = 0; j < rows_of[s].size(); ++j)
-                std::memcpy(rows.data() + rows_of[s][j] * row, part.data() + j * row, row);
-        }
+        MultiIds mi;
+        std::vector<uint8_t> rows;
+        int rc0 = multi_ids(m, gids, nq, &mi);
+        if (rc0 || (rc0 = multi_id_rows(m, mi, nq, &rows))) return rc0;
         if (fmt == GRANNE_B200_QUERY_ID)
             return call(rows.data(), (int)GRANNE_B200_QUERY_ELEMENT, k, out_ids, out_dists, out_counts);
         const size_t kk = (size_t)k + 1;
@@ -3176,6 +3428,126 @@ int multi_query(granne_b200_multi* m, const void* queries, size_t nq, int fmt, u
                 out_dists[q * k + j] = std::numeric_limits<float>::infinity();
             }
         }
+        return (int)GRANNE_B200_OK;
+    });
+}
+
+// A range call on a multi handle (host buffers; arguments checked, nq > 0): counts when offsets is null, else the fill
+// of out_ids / out_dists.  REPLICATED: each device runs its slice of the queries (by id: the global ids are its local
+// ids), a fill with its slice's offsets rebased to the slice.  RANGE_PARTITIONED: every shard counts every query (by id:
+// on the rows the owning parts read); a fill then fills each shard's runs at offsets from those counts (a second scan)
+// and sorts each query's entries from all shards by (distance, global id) into its segment.  For QUERY_ID_EXCLUDING the
+// owning shard's distance of the query to itself (granne_b200_exact_search_within_batch on the one id) decides whether
+// the query's own global id is in its range, and it is removed from the count and the segment.
+int multi_range(granne_b200_multi* m, const void* queries, size_t nq, int fmt, float radius, const uint64_t* offsets,
+                uint64_t* out_ids, float* out_dists, uint64_t* counts) {
+    return guarded([&] {
+        const size_t n = m->parts.size();
+        const bool fill = offsets != nullptr;
+        const uint64_t* gids = static_cast<const uint64_t*>(queries);
+        MultiIds mi;
+        int rc;
+        if (by_id(fmt) && (rc = multi_ids(m, gids, nq, &mi))) return rc;
+        if (m->mode == GRANNE_B200_MODE_REPLICATED) {
+            std::vector<uint32_t> lids(by_id(fmt) ? nq : 0);
+            for (size_t q = 0; q < lids.size(); ++q) lids[q] = (uint32_t)gids[q];
+            const uint8_t* q0 = by_id(fmt) ? reinterpret_cast<const uint8_t*>(lids.data())
+                                           : static_cast<const uint8_t*>(queries);
+            const size_t qrow = query_row_bytes(m->kind, m->dim, fmt), per = nq / n, extra = nq % n;
+            return for_each_part(n, [&](size_t i) {
+                const size_t b = i * per + std::min(i, extra), cnt = per + (i < extra ? 1 : 0);
+                if (cnt == 0) return (int)GRANNE_B200_OK;
+                if (!fill) return granne_b200_exact_range_count(m->parts[i], q0 + b * qrow, cnt, fmt, radius, counts + b);
+                return guarded([&] {
+                    std::vector<uint64_t> off(cnt + 1);
+                    for (size_t j = 0; j <= cnt; ++j) off[j] = offsets[b + j] - offsets[b];
+                    std::vector<uint32_t> pids(off[cnt]);
+                    const int r = granne_b200_exact_range_search(m->parts[i], q0 + b * qrow, cnt, fmt, radius,
+                                                                 off.data(), pids.data(), out_dists + offsets[b]);
+                    for (size_t j = 0; j < pids.size(); ++j)
+                        out_ids[offsets[b] + j] = pids[j] == gb::kUnusedId ? ~0ull : (uint64_t)pids[j];
+                    return r;
+                });
+            });
+        }
+        // range-partitioned: by id, the rows the owners read, as ELEMENT queries on every shard
+        std::vector<uint8_t> rows;
+        const void* q = queries;
+        int f = fmt;
+        if (by_id(fmt)) {
+            if ((rc = multi_id_rows(m, mi, nq, &rows))) return rc;
+            q = rows.data();
+            f = GRANNE_B200_QUERY_ELEMENT;
+        }
+        std::vector<char> self_in(nq, 0);
+        if (fmt == GRANNE_B200_QUERY_ID_EXCLUDING) {
+            rc = for_each_part(n, [&](size_t s) {
+                const size_t c = mi.local[s].size();
+                if (c == 0) return (int)GRANNE_B200_OK;
+                return guarded([&] {
+                    std::vector<uint64_t> off(c + 1);
+                    for (size_t j = 0; j <= c; ++j) off[j] = j;
+                    std::vector<uint32_t> sid(c), scnt(c);
+                    std::vector<float> sd(c);
+                    const int r = granne_b200_exact_search_within_batch(m->parts[s], mi.local[s].data(), c,
+                                                                        GRANNE_B200_QUERY_ID, off.data(),
+                                                                        mi.local[s].data(), 1, sid.data(), sd.data(),
+                                                                        scnt.data());
+                    for (size_t j = 0; j < c && r == GRANNE_B200_OK; ++j)
+                        self_in[mi.rows_of[s][j]] = scnt[j] == 1 && sd[j] <= radius;
+                    return r;
+                });
+            });
+            if (rc) return rc;
+        }
+        std::vector<uint64_t> pc(n * nq);
+        if ((rc = for_each_part(n, [&](size_t i) {
+                 return granne_b200_exact_range_count(m->parts[i], q, nq, f, radius, pc.data() + i * nq);
+             })))
+            return rc;
+        if (!fill) {
+            for (size_t qi = 0; qi < nq; ++qi) {
+                uint64_t c = 0;
+                for (size_t i = 0; i < n; ++i) c += pc[i * nq + qi];
+                counts[qi] = c - (uint64_t)self_in[qi];
+            }
+            return (int)GRANNE_B200_OK;
+        }
+        std::vector<std::vector<uint64_t>> poff(n, std::vector<uint64_t>(nq + 1, 0));
+        std::vector<std::vector<uint32_t>> pid(n);
+        std::vector<std::vector<float>> pd(n);
+        for (size_t i = 0; i < n; ++i) {
+            for (size_t qi = 0; qi < nq; ++qi) poff[i][qi + 1] = poff[i][qi] + pc[i * nq + qi];
+            pid[i].resize(poff[i][nq]);
+            pd[i].resize(poff[i][nq]);
+        }
+        if ((rc = for_each_part(n, [&](size_t i) {
+                 return granne_b200_exact_range_search(m->parts[i], q, nq, f, radius, poff[i].data(), pid[i].data(),
+                                                       pd[i].data());
+             })))
+            return rc;
+        bool mismatch = false;
+        std::vector<std::pair<float, uint64_t>> all;
+        for (size_t qi = 0; qi < nq; ++qi) {
+            all.clear();
+            for (size_t i = 0; i < n; ++i)
+                for (uint64_t j = poff[i][qi]; j < poff[i][qi + 1]; ++j) {
+                    const uint64_t g = m->base[i] + pid[i][j];
+                    if (fmt == GRANNE_B200_QUERY_ID_EXCLUDING && g == gids[qi]) continue;
+                    all.emplace_back(pd[i][j], g);
+                }
+            std::sort(all.begin(), all.end());  // distances are never NaN here (a NaN fails the shard call)
+            const uint64_t b = offsets[qi], len = offsets[qi + 1] - b;
+            const bool ok = all.size() == len;
+            mismatch |= !ok;
+            for (uint64_t j = 0; j < len; ++j) {
+                out_ids[b + j] = ok ? all[j].second : ~0ull;
+                out_dists[b + j] = ok ? all[j].first : std::numeric_limits<float>::infinity();
+            }
+        }
+        if (mismatch)
+            return fail(GRANNE_B200_ERR_INVALID_ARGUMENT,
+                        "a range search segment's length differs from its query's count (it is padded)");
         return (int)GRANNE_B200_OK;
     });
 }
@@ -3326,6 +3698,22 @@ int granne_b200_multi_search_filtered_batch(granne_b200_multi* m, const void* qu
                                                                ids, ds, c, nullptr);
                                });
                        });
+}
+
+int granne_b200_multi_exact_range_count(granne_b200_multi* m, const void* queries, size_t nq, int query_format,
+                                        float radius, uint64_t* counts) {
+    if (!m) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "multi handle is null");
+    const int rc = validate_range(m->parts[0], queries, nq, query_format, radius, counts, nullptr, false);
+    if (rc || nq == 0) return rc;
+    return multi_range(m, queries, nq, query_format, radius, nullptr, nullptr, nullptr, counts);
+}
+
+int granne_b200_multi_exact_range_search(granne_b200_multi* m, const void* queries, size_t nq, int query_format,
+                                         float radius, const uint64_t* offsets, uint64_t* ids, float* dists) {
+    if (!m) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "multi handle is null");
+    int rc = validate_range(m->parts[0], queries, nq, query_format, radius, nullptr, offsets, true);
+    if (rc || nq == 0 || (rc = check_range_outputs(offsets, nq, ids, dists))) return rc;
+    return multi_range(m, queries, nq, query_format, radius, offsets, ids, dists, nullptr);
 }
 
 // Every image is checked on the host against its part before any part stages rows (multi_attach_rerank).

@@ -66,13 +66,16 @@ extern "C" {
                                        GRANNE_B200_ERR_OUT_OF_RANGE; in device calls a query with a bad id gets count 0,
                                        padding and zero stats, the others are unaffected, and granne_b200_stream_status
                                        reports ERR_OUT_OF_RANGE.  Accepted by search_batch, exact_search_batch,
-                                       exact_search_within_batch and search_filtered_batch (host and device forms, and
-                                       their multi-handle forms); search_batch_device_gather and the two-stage calls
-                                       reject it as an unknown format. */
+                                       exact_search_within_batch, search_filtered_batch, exact_range_count and
+                                       exact_range_search (host and device forms, and their multi-handle forms);
+                                       search_batch_device_gather and the two-stage calls reject it as an unknown
+                                       format. */
 #define GRANNE_B200_QUERY_ID_EXCLUDING 3 /* QUERY_ID without the element itself: the call's result for the same query
                                        with num_neighbors = k + 1, the entry whose id is ids[q] removed, cut to the first
                                        k.  Other elements at distance 0 (duplicates) stay.  Stats columns 0..2 are
-                                       QUERY_ID's.  The calls capped at GRANNE_B200_EXACT_MAX_K then take k <= 1023. */
+                                       QUERY_ID's.  The calls capped at GRANNE_B200_EXACT_MAX_K then take k <= 1023.
+                                       The range calls remove ids[q] from the query's range if it is there (its count
+                                       and segment shrink by one); other elements at distance 0 stay. */
 
 /* Per-query counters written to `out_stats` (4 x u64 per query).  n_dist / n_expand are exactly the number of
  * `dist_to_element` (src/index/mod.rs:1012,1027) and `get_neighbors` (:1025) calls the reference makes for the
@@ -291,6 +294,49 @@ int granne_b200_search_filtered_batch_device(granne_b200_index* h, const void* d
                                              const uint32_t* d_query_filter, uint32_t* d_out_ids, float* d_out_dists,
                                              uint32_t* d_out_counts, uint64_t* d_out_stats, void* cuda_stream);
 
+/* ---- exact range search: every element within a distance bound -------------------------------------------------------
+ * NOT a reference function: near-duplicate detection, threshold matching, density counts.  For n = granne_b200_len(h)
+ * (Index::len), d(q, i) the distance of granne_b200_exact_search_batch (the same bits) and a radius r (f32):
+ *     R(q) = { i : 0 <= i < n, d(q, i) <= r }
+ * with IEEE <=, so r = +-0.0 admits distance 0 and r = +inf admits every element.  The result of q is R(q) sorted
+ * ascending by (distance, id), the order of into_sorted_vec (src/index/mod.rs:1036), with no cap on its size; its first
+ * min(k, |R(q)|) entries are the entries of granne_b200_exact_search_batch(q, k) whose distance is <= r.
+ * Two phases, one radius per call:
+ *   granne_b200_exact_range_count   counts[q] = |R(q)| (nq u64)
+ *   granne_b200_exact_range_search  R(q) into ids[offsets[q], offsets[q + 1]) (u32) and dists[...] (f32), offsets being
+ *                                   nq + 1 u64, offsets[0] == 0, non-decreasing: normally the exclusive prefix sum of
+ *                                   the counts.  Distances are deterministic bit for bit, so both phases see the same
+ *                                   sets.  A segment whose length differs from its query's count is padded whole with
+ *                                   0xFFFFFFFF / +inf and the call reports ERR_INVALID_ARGUMENT (a device call through
+ *                                   granne_b200_stream_status); nothing is written outside a query's own segment.
+ * Queries are RAW_F32, ELEMENT, QUERY_ID or QUERY_ID_EXCLUDING (see GRANNE_B200_QUERY_ID).  With nq > 0 and n > 0 the
+ * scan runs whatever r is, so a NaN distance returns ERR_NOT_FINITE as in granne_b200_exact_search_batch.  nq == 0 and
+ * n == 0 are valid (all counts 0).  Argument checks run on the host before any device call; ERR_INVALID_ARGUMENT, in
+ * this order: the handle is NULL; an unknown query format; a NaN radius; nq above the batch limit; queries NULL with
+ * nq > 0; then, with nq > 0, counts NULL (count) or offsets NULL (search); and for the host search offsets that do not
+ * start at 0 or go backwards, then ids or dists NULL with offsets[nq] > 0.  Then (host calls) an id >= num_elements is
+ * ERR_OUT_OF_RANGE.
+ * The scan is granne_b200_exact_search_batch's (query chunks of 1024, bounded row slabs, embeddings windows), so a
+ * count costs about one exact scan and a search one more.  The search writes its entries straight into the caller's
+ * segments and sorts each segment there, so its workspace is bounded (8 bytes per query of a chunk besides the scan's)
+ * whatever the number of results; the host search stages its results in the handle's workspace, 8 bytes per result. */
+int granne_b200_exact_range_count(granne_b200_index* h, const void* queries, size_t nq, int query_format, float radius,
+                                  uint64_t* counts);
+/* Same with DEVICE pointers on cuda_stream (NULL = the default stream), asynchronous like
+ * granne_b200_exact_search_batch_device, with that stream's workspace and no host synchronisation.  A bad id gives its
+ * query count 0 and granne_b200_stream_status reports ERR_OUT_OF_RANGE. */
+int granne_b200_exact_range_count_device(granne_b200_index* h, const void* d_queries, size_t nq, int query_format,
+                                         float radius, uint64_t* d_counts, void* cuda_stream);
+int granne_b200_exact_range_search(granne_b200_index* h, const void* queries, size_t nq, int query_format,
+                                   float radius, const uint64_t* offsets, uint32_t* ids, float* dists);
+/* Same with DEVICE pointers (queries, offsets, outputs) on cuda_stream, asynchronous like
+ * granne_b200_exact_range_count_device.  The kernels check the segments: offsets that go backwards write nothing,
+ * NULL ids or dists take only empty segments, and either is reported as a length mismatch.  A bad id gives its query
+ * an empty range (its segment must be empty) and granne_b200_stream_status reports ERR_OUT_OF_RANGE. */
+int granne_b200_exact_range_search_device(granne_b200_index* h, const void* d_queries, size_t nq, int query_format,
+                                          float radius, const uint64_t* d_offsets, uint32_t* d_ids, float* d_dists,
+                                          void* cuda_stream);
+
 /* ---- two-stage search: traverse angular_int rows, re-rank by exact f32 angular distance ----------------------------
  * NOT a reference function: what a user of granne assembles by hand from two containers over one index.  For an
  * angular_int handle h with an attached container F (angular rows or SumEmbeddings) and a raw f32 query q:
@@ -342,7 +388,8 @@ int granne_b200_release_stream(granne_b200_index* h, void* cuda_stream);
 
 /* After synchronising a stream used with granne_b200_search_batch_device: GRANNE_B200_OK, or the first error
  * (ERR_NOT_FINITE / ERR_CAPACITY, or ERR_INVALID_ARGUMENT for a bad candidate list of
- * granne_b200_exact_search_within_batch_device, or ERR_OUT_OF_RANGE for an element id >= num_elements of a
+ * granne_b200_exact_search_within_batch_device or a range search segment whose length is not its count, or
+ * ERR_OUT_OF_RANGE for an element id >= num_elements of a
  * GRANNE_B200_QUERY_ID* call or of granne_b200_get_elements_device) any query of the calls issued since the previous
  * check raised. */
 int granne_b200_stream_status(granne_b200_index* h);
@@ -414,6 +461,17 @@ int granne_b200_multi_exact_search_within_batch(granne_b200_multi* m, const void
                                                 int query_format, const uint64_t* offsets, const uint64_t* ids,
                                                 uint32_t num_neighbors, uint64_t* out_ids, float* out_dists,
                                                 uint32_t* out_counts);
+/* granne_b200_exact_range_count / granne_b200_exact_range_search over a multi handle (HOST buffers), with u64 GLOBAL
+ * ids in QUERY_ID* queries (as granne_b200_multi_search_batch) and in the results.  Argument rules as the single-device
+ * calls.  REPLICATED slices the queries over the devices (a search with each slice's offsets rebased into the caller's
+ * arrays).  RANGE_PARTITIONED counts every query on every shard and sums the counts; a search counts every shard first
+ * (so it scans each shard twice), fills each shard's runs and merges them per query by (distance, global id) into the
+ * caller's segment on the host.  QUERY_ID_EXCLUDING on a range-partitioned handle also asks the owning shard for the
+ * query's distance to itself (one exact within-list call). */
+int granne_b200_multi_exact_range_count(granne_b200_multi* m, const void* queries, size_t nq, int query_format,
+                                        float radius, uint64_t* counts);
+int granne_b200_multi_exact_range_search(granne_b200_multi* m, const void* queries, size_t nq, int query_format,
+                                         float radius, const uint64_t* offsets, uint64_t* ids, float* dists);
 /* granne_b200_search_filtered_batch over a multi handle: the bitmaps are over GLOBAL ids, results are u64 GLOBAL ids.
  * REPLICATED slices the queries together with their query_filter entries over the devices; RANGE_PARTITIONED runs
  * every query on every shard, shard s reading bit shard_base[s] + local id of the same bitmaps, and merges the shard

@@ -70,6 +70,29 @@ std::vector<uint8_t> sized_bytes(Call&& call) {
 }
 
 // One result list per query from the C ABI's (ids, dists, counts) with k slots per query: its first counts[q] pairs.
+// Range results in CSR form (offsets [nq + 1], ids, dists) as one list per query.
+template <class Result, class Id>
+std::vector<Result> csr_lists(const std::vector<uint64_t>& offsets, const std::vector<Id>& ids,
+                              const std::vector<float>& dists) {
+    std::vector<Result> out(offsets.empty() ? 0 : offsets.size() - 1);
+    for (size_t q = 0; q < out.size(); ++q)
+        for (uint64_t j = offsets[q]; j < offsets[q + 1]; ++j) out[q].emplace_back(ids[j], dists[j]);
+    return out;
+}
+
+// Count, prefix sum, fill: the two phases of a range search into CSR arrays.
+template <class Id, class Count, class Fill>
+void range_csr(size_t nq, Count&& count, Fill&& fill, std::vector<uint64_t>* offsets, std::vector<Id>* ids,
+               std::vector<float>* dists) {
+    std::vector<uint64_t> counts(nq);
+    count(counts.data());
+    offsets->assign(nq + 1, 0);
+    for (size_t q = 0; q < nq; ++q) (*offsets)[q + 1] = (*offsets)[q] + counts[q];
+    ids->resize(offsets->back());
+    dists->resize(offsets->back());
+    fill(offsets->data(), ids->data(), dists->data());
+}
+
 template <class Result, class Id>
 std::vector<Result> result_lists(const std::vector<Id>& ids, const std::vector<float>& dists,
                                  const std::vector<uint32_t>& counts, size_t k) {
@@ -275,6 +298,21 @@ public:
                                              ids.data(), dists.data(), counts.data()));
         return detail::result_lists<SearchResult>(ids, dists, counts, num_neighbors);
     }
+    // Exact range search (granne_b200_exact_range_count, then granne_b200_exact_range_search): every element of
+    // [0, len()) whose distance to the query is <= radius, sorted by (distance, id), the reference's distance bit for
+    // bit.  Not a reference function.  Queries in any format, ids included.
+    std::vector<SearchResult> exact_range_search(const void* queries, size_t nq, int query_format, float radius) const {
+        std::vector<uint64_t> offsets;
+        std::vector<uint32_t> ids;
+        std::vector<float> dists;
+        detail::range_csr(
+            nq, [&](uint64_t* c) { check(granne_b200_exact_range_count(h_, queries, nq, query_format, radius, c)); },
+            [&](const uint64_t* o, uint32_t* i, float* d) {
+                check(granne_b200_exact_range_search(h_, queries, nq, query_format, radius, o, i, d));
+            },
+            &offsets, &ids, &dists);
+        return detail::csr_lists<SearchResult>(offsets, ids, dists);
+    }
     // Exact k nearest neighbours of each query within its own candidate list (granne_b200_exact_search_within_batch):
     // lists[q] holds query q's ids (< len(); duplicates count once); the first min(k, |set(lists[q])|) by (distance,
     // id), the reference's distance bit for bit.  Not a reference function.
@@ -462,6 +500,20 @@ public:
                                                    static_cast<uint32_t>(num_neighbors), ids.data(), d.data(),
                                                    c.data()));
         return detail::result_lists<Result>(ids, d, c, num_neighbors);
+    }
+    // Granne::exact_range_search over every part (granne_b200_multi_exact_range_count, then _search): GLOBAL ids in
+    // the results, and as queries of the QUERY_ID* formats (u64)
+    std::vector<Result> exact_range_search(const void* queries, size_t nq, int query_format, float radius) const {
+        std::vector<uint64_t> offsets, ids;
+        std::vector<float> dists;
+        detail::range_csr(
+            nq,
+            [&](uint64_t* c) { check(granne_b200_multi_exact_range_count(h_, queries, nq, query_format, radius, c)); },
+            [&](const uint64_t* o, uint64_t* i, float* d) {
+                check(granne_b200_multi_exact_range_search(h_, queries, nq, query_format, radius, o, i, d));
+            },
+            &offsets, &ids, &dists);
+        return detail::csr_lists<Result>(offsets, ids, dists);
     }
     // Granne::exact_search_within over every part for nq raw f32 queries (nq x dim, row-major, as the *_raw calls
     // take them), GLOBAL ids in the lists and the results (granne_b200_multi_exact_search_within_batch)
