@@ -142,6 +142,16 @@ extern "C" {
         filters: *const u32, num_filters: u32, filter_words: u64, query_filter: *const u32, out_ids: *mut u64,
         out_dists: *mut f32, out_counts: *mut u32,
     ) -> c_int;
+    fn granne_b200_exact_search_filtered_batch(
+        h: *mut RawIndex, queries: *const c_void, nq: usize, query_format: c_int, filters: *const u32,
+        num_filters: u32, filter_words: u64, query_filter: *const u32, num_neighbors: u32, out_ids: *mut u32,
+        out_dists: *mut f32, out_counts: *mut u32,
+    ) -> c_int;
+    fn granne_b200_multi_exact_search_filtered_batch(
+        m: *mut RawMulti, queries: *const c_void, nq: usize, query_format: c_int, filters: *const u32,
+        num_filters: u32, filter_words: u64, query_filter: *const u32, num_neighbors: u32, out_ids: *mut u64,
+        out_dists: *mut f32, out_counts: *mut u32,
+    ) -> c_int;
     fn granne_b200_set_rerank_elements(h: *mut RawIndex, elements: *const c_void, elements_len: usize) -> c_int;
     fn granne_b200_search_rerank_batch(
         h: *mut RawIndex, queries: *const f32, nq: usize, query_format: c_int, max_search: u32, num_candidates: u32,
@@ -411,6 +421,37 @@ impl GpuGranne {
             .collect()
     }
 
+    /// Exact filtered k-NN (not a reference function): the first min(k, |A|) of the ids < len() the query's filter
+    /// admits, by (distance, id), with `exact_search`'s distances.  Filters as in `search_filtered`; no max_search.
+    pub fn exact_search_filtered(
+        &self, queries: &[f32], nq: usize, query_format: c_int, num_neighbors: usize, filters: &[u32],
+        filter_words: usize, query_filter: Option<&[u32]>,
+    ) -> Vec<Vec<(usize, f32)>> {
+        assert_eq!(queries.len(), nq * self.dim);
+        assert!(filter_words > 0 && filters.len() % filter_words == 0);
+        if let Some(f) = query_filter {
+            assert_eq!(f.len(), nq);
+        }
+        let mut ids = vec![0u32; nq * num_neighbors];
+        let mut dists = vec![0f32; nq * num_neighbors];
+        let mut counts = vec![0u32; nq];
+        check(unsafe {
+            granne_b200_exact_search_filtered_batch(
+                self.h, queries.as_ptr() as *const c_void, nq, query_format, filters.as_ptr(),
+                (filters.len() / filter_words) as u32, filter_words as u64,
+                query_filter.map_or(std::ptr::null(), |f| f.as_ptr()), num_neighbors as u32, ids.as_mut_ptr(),
+                dists.as_mut_ptr(), counts.as_mut_ptr(),
+            )
+        });
+        (0..nq)
+            .map(|q| {
+                (0..counts[q] as usize)
+                    .map(|j| (ids[q * num_neighbors + j] as usize, dists[q * num_neighbors + j]))
+                    .collect()
+            })
+            .collect()
+    }
+
     /// The ordering half of `Granne::reorder` (`src/index/reorder.rs:126-174`); apply it with
     /// `granne_b200_apply_order` (or granne's own `reorder_layers` + `Permutable::permute`).
     pub fn compute_order(&mut self) -> Vec<usize> {
@@ -669,6 +710,30 @@ impl GpuMultiGranne {
                                                     (filters.len() / filter_words) as u32, filter_words as u64,
                                                     query_filter.map_or(std::ptr::null(), |f| f.as_ptr()),
                                                     ids.as_mut_ptr(), d.as_mut_ptr(), c.as_mut_ptr())
+        });
+        (0..nq)
+            .map(|i| (0..c[i] as usize).map(|j| (ids[i * num_neighbors + j] as usize, d[i * num_neighbors + j])).collect())
+            .collect()
+    }
+
+    /// `exact_search_filtered` over every part: the bitmaps are over GLOBAL ids, and so are the results.
+    pub fn exact_search_filtered(
+        &self, elements: &[f32], num_neighbors: usize, filters: &[u32], filter_words: usize,
+        query_filter: Option<&[u32]>,
+    ) -> Vec<Vec<(usize, f32)>> {
+        let nq = elements.len() / self.dim;
+        assert!(filter_words > 0 && filters.len() % filter_words == 0);
+        if let Some(f) = query_filter {
+            assert_eq!(f.len(), nq);
+        }
+        let (mut ids, mut d, mut c) = (vec![0u64; nq * num_neighbors], vec![0f32; nq * num_neighbors], vec![0u32; nq]);
+        check(unsafe {
+            granne_b200_multi_exact_search_filtered_batch(self.m, elements.as_ptr() as *const c_void, nq, QUERY_ELEMENT,
+                                                          filters.as_ptr(), (filters.len() / filter_words) as u32,
+                                                          filter_words as u64,
+                                                          query_filter.map_or(std::ptr::null(), |f| f.as_ptr()),
+                                                          num_neighbors as u32, ids.as_mut_ptr(), d.as_mut_ptr(),
+                                                          c.as_mut_ptr())
         });
         (0..nq)
             .map(|i| (0..c[i] as usize).map(|j| (ids[i * num_neighbors + j] as usize, d[i * num_neighbors + j])).collect())

@@ -119,6 +119,10 @@ def load_library():
         "granne_b200_search_filtered_batch_device": (i32, [vp, vp, sz, i32, u32, u32, vp, u32, u64, vp, vp, vp, vp, vp,
                                                            vp]),
         "granne_b200_multi_search_filtered_batch": (i32, [vp, vp, sz, i32, u32, u32, vp, u32, u64, vp, vp, vp, vp]),
+        "granne_b200_exact_search_filtered_batch": (i32, [vp, vp, sz, i32, vp, u32, u64, vp, u32, vp, vp, vp]),
+        "granne_b200_exact_search_filtered_batch_device": (i32, [vp, vp, sz, i32, vp, u32, u64, vp, u32, vp, vp, vp,
+                                                                 vp]),
+        "granne_b200_multi_exact_search_filtered_batch": (i32, [vp, vp, sz, i32, vp, u32, u64, vp, u32, vp, vp, vp]),
         "granne_b200_set_rerank_elements": (i32, [vp, vp, sz]),
         "granne_b200_set_rerank_elements_device": (i32, [vp, vp, u64, u32]),
         "granne_b200_search_rerank_batch": (i32, [vp, vp, sz, i32, u32, u32, u32, vp, vp, vp, vp]),
@@ -272,6 +276,21 @@ def _query_filter(query_filter, nq):
     if qf.size and (qf.min() < 0 or int(qf.max()) > 0xFFFFFFFF):
         raise ValueError("query_filter entries must be non-negative and fit uint32")
     return np.ascontiguousarray(qf, dtype=np.uint32)
+
+
+def _check_device_filters(filters, query_filter, q):
+    """The filters (int32 [F, W]) and query_filter (int32 [nq] or None) of a device call for the queries q: contiguous
+    CUDA tensors on the queries' device, since the kernels index them directly."""
+    import torch
+
+    for t, shape, what in ((filters, None, "filters"), (query_filter, (q.shape[0],), "query_filter")):
+        if t is None and what == "query_filter":
+            continue
+        if (not isinstance(t, torch.Tensor) or not t.is_cuda or t.device != q.device or t.dtype != torch.int32
+                or not t.is_contiguous() or (shape is None and t.dim() != 2)
+                or (shape is not None and tuple(t.shape) != shape)):
+            raise ValueError("%s must be a contiguous int32 CUDA tensor of shape %s on the queries' device"
+                             % (what, "(F, W)" if shape is None else "(nq,)"))
 
 
 def _radius(radius):
@@ -781,7 +800,8 @@ class Granne:
         k admitted elements among those it scores in the bottom layer, by (distance, id).  Not a reference function.
         `filters`: a bool mask of shape (len,) or (F, len), or packed uint32 words (F, W), W >= ceil(len / 32) (id i
         is bit i % 32 of word i // 32); query_filter: one filter index per query (None: filter 0 for all).  k <=
-        EXACT_MAX_K and may exceed max_search; no exact fallback, so a selective filter may return fewer than k.
+        EXACT_MAX_K and may exceed max_search; no exact fallback, so a selective filter may return fewer than k
+        (exact_search_filtered returns the exact answer over the same filters).
         Returns search_batch's (ids, dists, counts[, stats]); stats columns 0..2 equal search_batch's."""
         q, fmt = self._host_queries(queries, already_element, by_id, exclude_self)
         nq, k = q.shape[0], int(num_elements)
@@ -802,18 +822,9 @@ class Granne:
         """Device-resident search_batch_filtered: CUDA tensors in (queries; filters int32 [F, W] holding the uint32
         words; query_filter int32 [nq] or None) and out, asynchronous on `stream` like search_batch_device.  The kernel
         checks query_filter: an entry >= F gives its query count 0 and padding, and stream_status() raises."""
-        import torch
-
         q, fmt = self._device_queries(queries, already_element, by_id, exclude_self)
         nq, k = q.shape[0], int(num_elements)
-        for t, shape, what in ((filters, None, "filters"), (query_filter, (nq,), "query_filter")):
-            if t is None and what == "query_filter":
-                continue
-            if (not isinstance(t, torch.Tensor) or not t.is_cuda or t.device != q.device or t.dtype != torch.int32
-                    or not t.is_contiguous() or (shape is None and t.dim() != 2)
-                    or (shape is not None and tuple(t.shape) != shape)):
-                raise ValueError("%s must be a contiguous int32 CUDA tensor of shape %s on the queries' device"
-                                 % (what, "(F, W)" if shape is None else "(nq,)"))
+        _check_device_filters(filters, query_filter, q)
         ids, dists, counts = _device_outputs(q, k, out)
         _check_stats(stats, q)
         _check(load_library().granne_b200_search_filtered_batch_device(
@@ -822,6 +833,42 @@ class Granne:
             C.c_void_p(query_filter.data_ptr()) if query_filter is not None else None, C.c_void_p(ids.data_ptr()),
             C.c_void_p(dists.data_ptr()), C.c_void_p(counts.data_ptr()),
             C.c_void_p(stats.data_ptr()) if stats is not None else None, C.c_void_p(_raw_stream(stream, q.device))))
+        return ids, dists, counts
+
+    def exact_search_filtered(self, queries, filters, query_filter=None, num_elements=DEFAULT_NUM_ELEMENTS,
+                              already_element=False, by_id=False, exclude_self=False):
+        """Exact filtered k nearest neighbours (granne_b200_exact_search_filtered_batch): for each query the first
+        min(k, |A|) of the elements i < len(self) its filter admits, by (distance, id), with exact_search_batch's
+        distances bit for bit.  Not a reference function.  `filters` and `query_filter` as in search_batch_filtered;
+        queries as in exact_search_batch (exclude_self drops the query's own id when its filter admits it); k <=
+        EXACT_MAX_K.  Only admitted rows are scanned: a chunk of 1024 queries costs the rows its filters' union admits,
+        so queries that share a filter are best passed next to each other.  Returns (ids, dists, counts) in
+        search_batch's layout."""
+        q, fmt = self._host_queries(queries, already_element, by_id, exclude_self)
+        nq, k = q.shape[0], int(num_elements)
+        words = _filter_words(filters, len(self))
+        qf = _query_filter(query_filter, nq)
+        ids, dists, counts, _ = _host_outputs(nq, k, np.uint32)
+        _check(load_library().granne_b200_exact_search_filtered_batch(
+            self._h, _ptr(q), nq, fmt, _ptr(words), words.shape[0], words.shape[1],
+            _ptr(qf) if qf is not None else None, k, _ptr(ids), _ptr(dists), _ptr(counts)))
+        return ids, dists, counts
+
+    def exact_search_filtered_device(self, queries, filters, query_filter=None, num_elements=DEFAULT_NUM_ELEMENTS,
+                                     already_element=False, out=None, stream=None, by_id=False, exclude_self=False):
+        """Device-resident exact_search_filtered: CUDA tensors in (queries; filters int32 [F, W] holding the uint32
+        words; query_filter int32 [nq] or None) and out, asynchronous on `stream` like exact_search_batch_device and
+        without waiting for the device.  The kernels check query_filter: an entry >= F gives its query count 0 and
+        padding, and stream_status() raises; so does a NaN distance to an admitted element."""
+        q, fmt = self._device_queries(queries, already_element, by_id, exclude_self)
+        nq, k = q.shape[0], int(num_elements)
+        _check_device_filters(filters, query_filter, q)
+        ids, dists, counts = _device_outputs(q, k, out)
+        _check(load_library().granne_b200_exact_search_filtered_batch_device(
+            self._h, C.c_void_p(q.data_ptr()), nq, fmt, C.c_void_p(filters.data_ptr()), filters.shape[0],
+            filters.shape[1], C.c_void_p(query_filter.data_ptr()) if query_filter is not None else None, k,
+            C.c_void_p(ids.data_ptr()), C.c_void_p(dists.data_ptr()), C.c_void_p(counts.data_ptr()),
+            C.c_void_p(_raw_stream(stream, q.device))))
         return ids, dists, counts
 
     def set_rerank_elements(self, elements):
@@ -1177,6 +1224,20 @@ class MultiGranne:
         _check(load_library().granne_b200_multi_search_filtered_batch(
             self._h, _ptr(q), nq, fmt, int(max_search), k, _ptr(words), words.shape[0], words.shape[1],
             _ptr(qf) if qf is not None else None, _ptr(ids), _ptr(dists), _ptr(counts)))
+        return ids, dists, counts
+
+    def exact_search_filtered(self, queries, filters, query_filter=None, num_elements=DEFAULT_NUM_ELEMENTS,
+                              already_element=False, by_id=False, exclude_self=False):
+        """Granne.exact_search_filtered over all parts (granne_b200_multi_exact_search_filtered_batch): the filters
+        are over GLOBAL ids, as in search_batch_filtered, and the results are GLOBAL uint64 ids."""
+        q, fmt = self._host_queries(queries, already_element, by_id, exclude_self)
+        nq, k = q.shape[0], int(num_elements)
+        words = _filter_words(filters, len(self))
+        qf = _query_filter(query_filter, nq)
+        ids, dists, counts, _ = _host_outputs(nq, k, np.uint64)
+        _check(load_library().granne_b200_multi_exact_search_filtered_batch(
+            self._h, _ptr(q), nq, fmt, _ptr(words), words.shape[0], words.shape[1],
+            _ptr(qf) if qf is not None else None, k, _ptr(ids), _ptr(dists), _ptr(counts)))
         return ids, dists, counts
 
     def set_rerank_elements(self, elements):

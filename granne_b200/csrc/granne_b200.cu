@@ -160,6 +160,10 @@ struct Workspace {
     Buffer<unsigned long long> d_exact_lists;
     Buffer<float> d_exact_rows;
     Buffer<float> d_exact_table;
+    // exact filtered search: a list of admitted ids | the chunk's filters | the counts [ids, filters, list cursor];
+    // the queries' prepare statuses
+    Buffer<uint32_t> d_exact_ids;
+    Buffer<int> d_exact_qstat;
     // two-stage search: stage 1's candidates, one block ids | dists | counts for the current call's nq x C
     Buffer<uint32_t> d_rerank;
     // exact search within lists: a chunk's running lists | segment prefix; its locks | query flags
@@ -1257,10 +1261,10 @@ int exact_scan_rows(Handle* h, Workspace* w, uint32_t qc, const void* rows, uint
         const dim3 grid((unsigned)((ns + gb::kExactRB - 1) / gb::kExactRB), (qc + gb::kExactQB - 1) / gb::kExactQB);
         if (d.kind == gb::kAngularI8) {
             a.rows = static_cast<const int8_t*>(rows) + s0 * row_stride;
-            gb::exact_scan_i8_kernel<<<grid, 256, 0, stream>>>(a);
+            gb::exact_scan_i8_kernel<false><<<grid, 256, 0, stream>>>(a);
         } else {
             a.rows = static_cast<const float*>(rows) + s0 * row_stride;
-            gb::exact_scan_f32_kernel<<<grid, 256, 0, stream>>>(a);
+            gb::exact_scan_f32_kernel<false><<<grid, 256, 0, stream>>>(a);
         }
         h->launches++;
         GB_CUDA(cudaGetLastError());
@@ -1270,15 +1274,80 @@ int exact_scan_rows(Handle* h, Workspace* w, uint32_t qc, const void* rows, uint
     return GRANNE_B200_OK;
 }
 
+// Distances of the prepared query chunk to the rows of a list (LISTED): row r of w->d_exact_dists is element ids[r] of
+// `rows` (ids null: row r), for r < count[0] (device memory; at most `cap`).  The host does not know the count, so the
+// grid is one wave of the scan's blocks (at most the list's capacity in row tiles) and the blocks stride over the
+// tiles: a short list costs a small launch, not the slab grid, and an empty one a launch whose blocks return.  (The
+// slab-shaped grid, its blocks past the count returning, measured 0.9 ms slower at 0.1 % and 15 % slower on full f32
+// lists over 10M x 128 on an H100, though 6 % faster on i8 rows.)
+int exact_scan_listed(Handle* h, Workspace* w, uint32_t qc, const void* rows, uint32_t row_stride, uint32_t vec_group,
+                      const uint32_t* ids, const uint32_t* count, uint64_t cap, uint64_t ld, cudaStream_t stream) {
+    const gb::DeviceIndex& d = h->dev;
+    gb::ExactScanArgs a{};
+    a.rows = rows;
+    a.row_stride = row_stride;
+    a.vec_group = vec_group;
+    a.dim = d.dim;
+    a.full = d.full;
+    a.tail = d.tail;
+    a.queries = w->d_exact_q.get();
+    a.qnorm = w->d_exact_qnorm.get();
+    a.nq = qc;
+    a.dists = w->d_exact_dists.get();
+    a.ld = ld;
+    a.row_ids = ids;
+    a.row_count = count;
+    const unsigned gy = (qc + gb::kExactQB - 1) / gb::kExactQB;
+    // two 256-thread blocks per SM are resident: no more than fit, so that no block waits for a whole list's tiles
+    const uint64_t wave = std::max<uint64_t>(1, (uint64_t)h->num_sms * 2 / gy);
+    const dim3 grid((unsigned)std::max<uint64_t>(1, std::min(wave, (cap + gb::kExactRB - 1) / gb::kExactRB)), gy);
+    if (d.kind == gb::kAngularI8)
+        gb::exact_scan_i8_kernel<true><<<grid, 256, 0, stream>>>(a);
+    else
+        gb::exact_scan_f32_kernel<true><<<grid, 256, 0, stream>>>(a);
+    h->launches++;
+    GB_CUDA(cudaGetLastError());
+    return GRANNE_B200_OK;
+}
+
+// Ids per list of a filtered scan: a slab, and for EMBEDDINGS at most a window of materialised rows; at least 32, so
+// that a word of the bitmaps always fits (exact_list_ids_kernel).
+uint64_t list_cap(uint64_t slab, uint64_t wrows, bool emb) {
+    return emb ? std::min(slab, std::max<uint64_t>(wrows, 32)) : slab;
+}
+
+// The ExactList of query chunk c0 of a filtered scan (exact_scan with filters): its id buffer holds `slab` ids, the
+// chunk's filters, then the three counts (exact_list_ids_kernel).
+gb::ExactList exact_list(Workspace* w, const DeviceFilters& f, size_t c0, uint64_t slab) {
+    gb::ExactList l{};
+    l.ids = w->d_exact_ids.get();
+    l.count = l.ids + slab + gb::kExactMaxChunk;
+    l.filters = f.words;
+    l.query_filter = f.query_filter ? f.query_filter + c0 : nullptr;
+    l.filter_words = f.filter_words;
+    l.bit_base = f.bit_base;
+    l.num_filters = f.num_filters;
+    l.qstatus = w->d_exact_qstat.get();
+    l.error = w->d_error;
+    return l;
+}
+
 // The exact scan of nq queries (device memory, the caller's format) against [0, Index::len), the loop the exact and
 // range calls share: query chunks of at most kExactMaxChunk, and per chunk begin(c0, qc), the queries prepared as
 // elements, every slab of rows (EMBEDDINGS: of every window of materialised rows) scanned and handed to
 // slab_step(c0, qc, ns, id_base, ld) with its distances in w->d_exact_dists (qc rows of ld floats), then end(c0, qc).
 // Without `scan` (no rows, or nothing to rank) only begin and end run.  A NaN distance or query sets kStatusNotFinite
 // in w->d_error.
+//
+// With `filt` (the exact filtered call) the rows scanned are the ids the chunk's filters admit (exact_list): they are
+// listed on the device, up to list_cap ids at a time from a cursor that stays on the device, only their rows are
+// scanned (exact_scan_listed), and slab_step(c0, qc, slab, 0, slab) finds the ids and their count in the chunk's
+// ExactList.  The host issues as many lists as the densest filter could need; those past the end are empty.  A NaN is
+// left for that step to flag (exact_select_kernel<true>), with each query's prepare status in w->d_exact_qstat.  No
+// host synchronisation: the counts stay on the device.
 template <class Begin, class Slab, class End>
 int exact_scan(Handle* h, Workspace* w, const void* d_queries, size_t nq, int fmt, bool scan, cudaStream_t stream,
-               Begin&& begin, Slab&& slab_step, End&& end) {
+               Begin&& begin, Slab&& slab_step, End&& end, const DeviceFilters* filt = nullptr) {
     const gb::DeviceIndex& d = h->dev;
     const uint64_t n = h->index_len;
     const bool i8 = d.kind == gb::kAngularI8, emb = d.kind == gb::kSumEmbeddings;
@@ -1300,7 +1369,8 @@ int exact_scan(Handle* h, Workspace* w, const void* d_queries, size_t nq, int fm
             // the container); the staged table's rows are padded to a multiple of 4 floats, the sum kernel reads
             // dense rows
             wrows = std::min<uint64_t>(n, emb_window_rows(std::max<uint32_t>(d.dim, 1)));
-            if ((rc = w->d_exact_rows.grow(std::max<size_t>(wrows * d.dim, 16), stream))) return rc;
+            const uint64_t rows_cap = filt ? std::max(wrows, list_cap(slab, wrows, emb)) : wrows;
+            if ((rc = w->d_exact_rows.grow(std::max<size_t>(rows_cap * d.dim, 16), stream))) return rc;
             if (d.row_stride != d.dim && d.num_vectors) {
                 if ((rc = w->d_exact_table.grow((size_t)d.num_vectors * d.dim, stream))) return rc;
                 GB_CUDA(cudaMemcpy2DAsync(w->d_exact_table.get(), (size_t)d.dim * 4, d.vectors,
@@ -1309,6 +1379,9 @@ int exact_scan(Handle* h, Workspace* w, const void* d_queries, size_t nq, int fm
                 table = w->d_exact_table.get();
             }
         }
+        if (filt && ((rc = w->d_exact_ids.grow(slab + gb::kExactMaxChunk + 3, stream)) ||
+                     (rc = w->d_exact_qstat.grow(qc_max, stream))))
+            return rc;
     }
     for (size_t c0 = 0; c0 < nq; c0 += gb::kExactMaxChunk) {
         const uint32_t qc = (uint32_t)std::min<size_t>(gb::kExactMaxChunk, nq - c0);
@@ -1316,11 +1389,41 @@ int exact_scan(Handle* h, Workspace* w, const void* d_queries, size_t nq, int fm
         if (scan) {
             gb::exact_prepare_kernel<<<(unsigned)std::min<uint64_t>(qc, (uint64_t)h->num_sms * 32), 32, 0, stream>>>(
                 d, static_cast<const uint8_t*>(d_queries) + c0 * in_row, fmt, qc, w->d_exact_q.get(),
-                w->d_exact_qnorm.get(), w->d_error);
+                w->d_exact_qnorm.get(), w->d_error, filt ? w->d_exact_qstat.get() : nullptr);
             h->launches++;
             GB_CUDA(cudaGetLastError());
             auto step = [&](uint64_t ns, uint64_t id_base) { return slab_step(c0, qc, ns, id_base, slab); };
-            if (emb) {
+            if (filt) {
+                const gb::ExactList l = exact_list(w, *filt, c0, slab);
+                uint32_t* count = const_cast<uint32_t*>(l.count);
+                uint32_t* ids = w->d_exact_ids.get();
+                gb::exact_chunk_filters_kernel<<<1, gb::kExactListThreads, 0, stream>>>(
+                    l.query_filter, qc, filt->num_filters, ids + slab, count);
+                h->launches++;
+                GB_CUDA(cudaGetLastError());
+                // lists of at most `cap` ids, each but the last fuller than cap - 32 (exact_list_ids_kernel)
+                const uint64_t cap = list_cap(slab, wrows, emb);
+                const uint64_t lists = (n + cap - 32) / (cap - 31);
+                for (uint64_t li = 0; li < lists; ++li) {
+                    gb::exact_list_ids_kernel<<<1, gb::kExactListThreads, 0, stream>>>(
+                        filt->words, filt->filter_words, filt->bit_base, ids + slab, count, n, (uint32_t)cap, ids);
+                    h->launches++;
+                    GB_CUDA(cudaGetLastError());
+                    if (emb) {
+                        gb::exact_listed_rows_kernel<<<(unsigned)std::min<uint64_t>(cap, (uint64_t)h->num_sms * 32), 32,
+                                                       (size_t)d.dim * 4, stream>>>(d, ids, count,
+                                                                                    w->d_exact_rows.get());
+                        h->launches++;
+                        GB_CUDA(cudaGetLastError());
+                        rc = exact_scan_listed(h, w, qc, w->d_exact_rows.get(), d.dim, 1, nullptr, count, cap, slab,
+                                               stream);
+                    } else {
+                        rc = exact_scan_listed(h, w, qc, d.vectors, d.row_stride, d.vec_group, ids, count, cap, slab,
+                                               stream);
+                    }
+                    if (rc || (rc = step(slab, 0))) return rc;
+                }
+            } else if (emb) {
                 EmbeddingsInput in;
                 in.dim = d.dim;
                 for (uint64_t r0 = 0; r0 < n; r0 += wrows) {
@@ -1344,9 +1447,11 @@ int exact_scan(Handle* h, Workspace* w, const void* d_queries, size_t nq, int fm
 }
 
 // Enqueues one exact search on `stream`: nq queries (device memory, the caller's format) against [0, Index::len),
-// results in search_batch's layout.  A NaN distance or query sets kStatusNotFinite in w->d_error.
+// results in search_batch's layout.  A NaN distance or query sets kStatusNotFinite in w->d_error.  With `filt` (the
+// exact filtered call) query q ranks the ids its filter admits only: the LISTED scan, select and write (exact_scan);
+// a query whose query_filter entry is >= num_filters gets count 0 and padding and sets kStatusBadFilter.
 int enqueue_exact(Handle* h, Workspace* w, const void* d_queries, size_t nq, int fmt, uint32_t k, const QueryOut& out,
-                  cudaStream_t stream) {
+                  cudaStream_t stream, const DeviceFilters* filt = nullptr) {
     const uint64_t n = h->index_len;
     const uint32_t count = (uint32_t)std::min<uint64_t>(k, n);
     const bool scan = k > 0 && n > 0;
@@ -1359,24 +1464,40 @@ int enqueue_exact(Handle* h, Workspace* w, const void* d_queries, size_t nq, int
             if (scan) GB_CUDA(cudaMemsetAsync(w->d_exact_lists.get(), 0xFF, (size_t)qc * gb::kExactMaxK * 8, stream));
             return (int)GRANNE_B200_OK;
         },
-        [&](size_t, uint32_t qc, uint64_t ns, uint64_t id_base, uint64_t ld) {
-            gb::exact_select_kernel<<<qc, gb::kExactSelThreads, 0, stream>>>(w->d_exact_dists.get(), ld, ns,
-                                                                             (uint32_t)id_base, k,
-                                                                             w->d_exact_lists.get());
+        [&](size_t c0, uint32_t qc, uint64_t ns, uint64_t id_base, uint64_t ld) {
+            if (filt)
+                gb::exact_select_kernel<true><<<qc, gb::kExactSelThreads, 0, stream>>>(
+                    w->d_exact_dists.get(), ld, ns, 0, k, w->d_exact_lists.get(), exact_list(w, *filt, c0, ld));
+            else
+                gb::exact_select_kernel<false><<<qc, gb::kExactSelThreads, 0, stream>>>(
+                    w->d_exact_dists.get(), ld, ns, (uint32_t)id_base, k, w->d_exact_lists.get(), gb::ExactList{});
             h->launches++;
             GB_CUDA(cudaGetLastError());
             return (int)GRANNE_B200_OK;
         },
         [&](size_t c0, uint32_t qc) {
-            const uint64_t outs = std::max<uint64_t>((uint64_t)qc * k, out.counts ? qc : 0);
+            // a filtered call always writes: its kernel also checks the chunk's query_filter entries
+            const uint64_t outs = std::max<uint64_t>((uint64_t)qc * k, out.counts || filt ? qc : 0);
             if (outs == 0) return (int)GRANNE_B200_OK;
-            gb::exact_write_kernel<<<(unsigned)((outs + 255) / 256), 256, 0, stream>>>(
-                w->d_exact_lists.get(), qc, k, count, out.ids ? out.ids + c0 * k : nullptr,
-                out.dists ? out.dists + c0 * k : nullptr, out.counts ? out.counts + c0 : nullptr);
+            uint32_t* ids = out.ids ? out.ids + c0 * k : nullptr;
+            float* dists = out.dists ? out.dists + c0 * k : nullptr;
+            uint32_t* counts = out.counts ? out.counts + c0 : nullptr;
+            if (filt) {
+                gb::ExactList l{};
+                l.query_filter = filt->query_filter ? filt->query_filter + c0 : nullptr;
+                l.num_filters = filt->num_filters;
+                l.error = w->d_error;
+                gb::exact_write_kernel<true><<<(unsigned)((outs + 255) / 256), 256, 0, stream>>>(
+                    scan ? w->d_exact_lists.get() : nullptr, qc, k, 0, ids, dists, counts, l);
+            } else {
+                gb::exact_write_kernel<false><<<(unsigned)((outs + 255) / 256), 256, 0, stream>>>(
+                    w->d_exact_lists.get(), qc, k, count, ids, dists, counts, gb::ExactList{});
+            }
             h->launches++;
             GB_CUDA(cudaGetLastError());
             return (int)GRANNE_B200_OK;
-        });
+        },
+        filt);
 }
 
 // ---- exact range search (range_kernels.cuh) -----------------------------------------------------------------------
@@ -1707,15 +1828,24 @@ int enqueue_within(Handle* h, Workspace* w, const void* d_queries, size_t nq, in
 
 // ---- filtered search (search_kernel<Dist, R, true>) -----------------------------------------------------------------
 // The rules of a filtered call that read no handle, in the order they are reported: validate_batch's, with
-// max_search >= 1 and k <= GRANNE_B200_EXACT_MAX_K as the call's own; then, when nq > 0, the filters' pointer and count.
+// max_search >= 1 and k <= GRANNE_B200_EXACT_MAX_K as the call's own (the exact filtered call: k only); then, when
+// nq > 0, the filters' pointer and count, and QUERY_ID_EXCLUDING's k (check_filter_args).
+int check_filter_args(size_t nq, int fmt, uint32_t k, const void* filters, uint32_t num_filters) {
+    if (nq > 0 && (!filters || num_filters == 0))
+        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "filters is null or num_filters is 0");
+    return check_exclude_k(fmt, k, GRANNE_B200_EXACT_MAX_K);
+}
 int validate_filtered(const Handle* h, const void* q, size_t nq, int fmt, uint32_t max_search, uint32_t k,
                       const void* ids, const void* dists, const void* filters, uint32_t num_filters) {
     const int rc = validate_batch(h, q, nq, fmt, k, ids, dists,
                                   max_search == 0 ? kMaxSearchRule : k > GRANNE_B200_EXACT_MAX_K ? kExactKRule : nullptr);
-    if (rc) return rc;
-    if (nq > 0 && (!filters || num_filters == 0))
-        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "filters is null or num_filters is 0");
-    return check_exclude_k(fmt, k, GRANNE_B200_EXACT_MAX_K);
+    return rc ? rc : check_filter_args(nq, fmt, k, filters, num_filters);
+}
+// The exact filtered call's: exact_search_batch's, then the filters' (there is no max_search).
+int validate_exact_filtered(const Handle* h, const void* q, size_t nq, int fmt, uint32_t k, const void* ids,
+                            const void* dists, const void* filters, uint32_t num_filters) {
+    const int rc = validate_exact(h, q, nq, fmt, k, ids, dists);
+    return rc ? rc : check_filter_args(nq, fmt, k, filters, num_filters);
 }
 
 // A bitmap of filter_words words must hold a bit for every id in [0, span).
@@ -1752,6 +1882,27 @@ int search_filtered_host(Handle* h, const void* queries, size_t nq, int fmt, uin
                                                    [&](const void* q, int f2, uint32_t kk, const QueryOut& o) {
                                                        return enqueue_search(h, w, q, nq, f2, max_search, kk, o,
                                                                              stream, nullptr, nullptr, &f);
+                                                   });
+                          });
+                      });
+}
+
+// An exact filtered search from host buffers (arguments checked, nq > 0), its inputs copied up like
+// search_filtered_host's.
+int exact_filtered_host(Handle* h, const void* queries, size_t nq, int fmt, uint32_t k, const uint32_t* filters,
+                        uint32_t num_filters, uint64_t filter_words, const uint32_t* query_filter, uint64_t bit_base,
+                        uint32_t* out_ids, float* out_dists, uint32_t* out_counts) {
+    return host_batch(h, queries, nq, fmt, k, out_ids, out_dists, out_counts, nullptr,
+                      [&](Workspace* w, cudaStream_t stream, const QueryOut& out) {
+                          const HostInput in[] = {{filters, (size_t)num_filters * filter_words * 4},
+                                                  {query_filter, query_filter ? nq * 4 : 0}};
+                          return with_call_inputs(stream, in, [&](const void* const* d) {
+                              const DeviceFilters f{static_cast<const uint32_t*>(d[0]),
+                                                    query_filter ? static_cast<const uint32_t*>(d[1]) : nullptr,
+                                                    filter_words, num_filters, bit_base};
+                              return enqueue_query(h, w, w->d_queries.get(), nq, fmt, k, out, true, stream,
+                                                   [&](const void* q, int f2, uint32_t kk, const QueryOut& o) {
+                                                       return enqueue_exact(h, w, q, nq, f2, kk, o, stream, &f);
                                                    });
                           });
                       });
@@ -2412,6 +2563,40 @@ int granne_b200_search_filtered_batch_device(granne_b200_index* h, const void* d
                              [&](const void* q, int f2, uint32_t kk, const QueryOut& o) {
                                  return enqueue_search(h, w, q, nq, f2, max_search, kk, o, stream, nullptr, nullptr,
                                                        &f);
+                             });
+    });
+}
+
+int granne_b200_exact_search_filtered_batch(granne_b200_index* h, const void* queries, size_t nq, int query_format,
+                                            const uint32_t* filters, uint32_t num_filters, uint64_t filter_words,
+                                            const uint32_t* query_filter, uint32_t num_neighbors, uint32_t* out_ids,
+                                            float* out_dists, uint32_t* out_counts) {
+    int rc = validate_exact_filtered(h, queries, nq, query_format, num_neighbors, out_ids, out_dists, filters,
+                                     num_filters);
+    if (rc || nq == 0) return rc;
+    if ((rc = check_filter_words(filter_words, h->index_len)) ||
+        (rc = check_query_filter(query_filter, nq, num_filters)) ||
+        (rc = check_host_query_ids(h, queries, nq, query_format)))
+        return rc;
+    return exact_filtered_host(h, queries, nq, query_format, num_neighbors, filters, num_filters, filter_words,
+                               query_filter, 0, out_ids, out_dists, out_counts);
+}
+
+int granne_b200_exact_search_filtered_batch_device(granne_b200_index* h, const void* d_queries, size_t nq,
+                                                   int query_format, const uint32_t* d_filters, uint32_t num_filters,
+                                                   uint64_t filter_words, const uint32_t* d_query_filter,
+                                                   uint32_t num_neighbors, uint32_t* d_out_ids, float* d_out_dists,
+                                                   uint32_t* d_out_counts, void* cuda_stream) {
+    int rc = validate_exact_filtered(h, d_queries, nq, query_format, num_neighbors, d_out_ids, d_out_dists, d_filters,
+                                     num_filters);
+    if (rc || nq == 0) return rc;
+    if ((rc = check_filter_words(filter_words, h->index_len))) return rc;
+    return device_batch(h, cuda_stream, false, [&](Workspace* w, cudaStream_t stream) {
+        const DeviceFilters f{d_filters, d_query_filter, filter_words, num_filters, 0};
+        return enqueue_query(h, w, d_queries, nq, query_format, num_neighbors,
+                             {d_out_ids, d_out_dists, d_out_counts, nullptr}, false, stream,
+                             [&](const void* q, int f2, uint32_t kk, const QueryOut& o) {
+                                 return enqueue_exact(h, w, q, nq, f2, kk, o, stream, &f);
                              });
     });
 }
@@ -3432,6 +3617,14 @@ int multi_query(granne_b200_multi* m, const void* queries, size_t nq, int fmt, u
     });
 }
 
+// The ids a multi handle's bitmaps must cover: [0, span) holds the global id of every part's elements.
+uint64_t multi_filter_span(const granne_b200_multi* m) {
+    uint64_t span = m->total_len;
+    for (size_t s = 0; m->mode == GRANNE_B200_MODE_RANGE_PARTITIONED && s < m->parts.size(); ++s)
+        span = std::max(span, m->base[s] + m->parts[s]->index_len);
+    return span;
+}
+
 // A range call on a multi handle (host buffers; arguments checked, nq > 0): counts when offsets is null, else the fill
 // of out_ids / out_dists.  REPLICATED: each device runs its slice of the queries (by id: the global ids are its local
 // ids), a fill with its slice's offsets rebased to the slice.  RANGE_PARTITIONED: every shard counts every query (by id:
@@ -3682,10 +3875,8 @@ int granne_b200_multi_search_filtered_batch(granne_b200_multi* m, const void* qu
     int rc = validate_filtered(m->parts[0], queries, nq, query_format, max_search, num_neighbors, out_ids, out_dists,
                                filters, num_filters);
     if (rc || nq == 0) return rc;
-    const bool range = m->mode == GRANNE_B200_MODE_RANGE_PARTITIONED;
-    uint64_t span = m->total_len;  // ids [0, span) are global ids of some part
-    for (size_t s = 0; range && s < m->parts.size(); ++s) span = std::max(span, m->base[s] + m->parts[s]->index_len);
-    if ((rc = check_filter_words(filter_words, span)) || (rc = check_query_filter(query_filter, nq, num_filters)))
+    if ((rc = check_filter_words(filter_words, multi_filter_span(m))) ||
+        (rc = check_query_filter(query_filter, nq, num_filters)))
         return rc;
     return multi_query(m, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts,
                        [&](const void* rows, int fmt, uint32_t k, uint64_t* oi, float* od, uint32_t* oc) {
@@ -3696,6 +3887,34 @@ int granne_b200_multi_search_filtered_batch(granne_b200_multi* m, const void* qu
                                                                num_filters, filter_words,
                                                                query_filter ? query_filter + b : nullptr, m->base[i],
                                                                ids, ds, c, nullptr);
+                               });
+                       });
+}
+
+// As granne_b200_multi_search_filtered_batch: REPLICATED slices the queries with their query_filter entries;
+// RANGE_PARTITIONED runs every query on every shard over the global bitmaps (bit shard_base[s] + local id), and
+// multi_batch merges the shards' exact filtered lists by (distance, global id), which is the exact filtered answer over
+// the union of the shards.
+int granne_b200_multi_exact_search_filtered_batch(granne_b200_multi* m, const void* queries, size_t nq,
+                                                  int query_format, const uint32_t* filters, uint32_t num_filters,
+                                                  uint64_t filter_words, const uint32_t* query_filter,
+                                                  uint32_t num_neighbors, uint64_t* out_ids, float* out_dists,
+                                                  uint32_t* out_counts) {
+    if (!m) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "multi handle is null");
+    int rc = validate_exact_filtered(m->parts[0], queries, nq, query_format, num_neighbors, out_ids, out_dists,
+                                     filters, num_filters);
+    if (rc || nq == 0) return rc;
+    if ((rc = check_filter_words(filter_words, multi_filter_span(m))) ||
+        (rc = check_query_filter(query_filter, nq, num_filters)))
+        return rc;
+    return multi_query(m, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts,
+                       [&](const void* rows, int fmt, uint32_t k, uint64_t* oi, float* od, uint32_t* oc) {
+                           return multi_batch(
+                               m, rows, nq, fmt, k, oi, od, oc,
+                               [&](size_t i, size_t b, const void* q, size_t cnt, uint32_t* ids, float* ds, uint32_t* c) {
+                                   return exact_filtered_host(m->parts[i], q, cnt, fmt, k, filters, num_filters,
+                                                              filter_words, query_filter ? query_filter + b : nullptr,
+                                                              m->base[i], ids, ds, c);
                                });
                        });
 }

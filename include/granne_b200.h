@@ -66,8 +66,9 @@ extern "C" {
                                        GRANNE_B200_ERR_OUT_OF_RANGE; in device calls a query with a bad id gets count 0,
                                        padding and zero stats, the others are unaffected, and granne_b200_stream_status
                                        reports ERR_OUT_OF_RANGE.  Accepted by search_batch, exact_search_batch,
-                                       exact_search_within_batch, search_filtered_batch, exact_range_count and
-                                       exact_range_search (host and device forms, and their multi-handle forms);
+                                       exact_search_within_batch, search_filtered_batch,
+                                       exact_search_filtered_batch, exact_range_count and exact_range_search (host
+                                       and device forms, and their multi-handle forms);
                                        search_batch_device_gather and the two-stage calls reject it as an unknown
                                        format. */
 #define GRANNE_B200_QUERY_ID_EXCLUDING 3 /* QUERY_ID without the element itself: the call's result for the same query
@@ -265,8 +266,8 @@ int granne_b200_exact_search_within_batch_device(granne_b200_index* h, const voi
  * Every element of S(q) strictly closer than the last of search_batch(q, max_search, max_search) is among its results,
  * so an all-admitting filter returns search_batch(q, max_search, k) (k <= max_search) whenever that call's k-th
  * distance is strictly below its max_search-th, or it returns fewer than max_search results.  There
- * is no exact fallback: a selective filter may return fewer than k (granne_b200_exact_search_within_batch ranks a
- * list of ids exactly).
+ * is no exact fallback: a selective filter may return fewer than k (granne_b200_exact_search_filtered_batch returns
+ * the exact answer over the same bitmaps).
  *   filters        num_filters bitmaps of filter_words u32 words each, bitmap f at filters + f * filter_words; id i is
  *                  admitted by filter f iff bit i % 32 (LSB first) of word i / 32 of bitmap f is set.  Bits at or
  *                  beyond Index::len are ignored.
@@ -293,6 +294,51 @@ int granne_b200_search_filtered_batch_device(granne_b200_index* h, const void* d
                                              uint32_t num_filters, uint64_t filter_words,
                                              const uint32_t* d_query_filter, uint32_t* d_out_ids, float* d_out_dists,
                                              uint32_t* d_out_counts, uint64_t* d_out_stats, void* cuda_stream);
+
+/* ---- exact filtered k-nearest neighbours: the k nearest elements an id bitmap admits --------------------------------
+ * NOT a reference function: the exact answer of a filtered search — a small tenant's, a rare category's or an ACL's
+ * nearest elements, and the ground truth filtered search is measured against.  For n = granne_b200_len(h)
+ * (Index::len), a query q with filter f(q) (query_filter[q], or 0 when query_filter is NULL) and
+ *     A_f = { i < n : bit i of bitmap f is set }
+ * (filtered search's bitmaps, bit order and layout; bits at or beyond n are ignored) the result of q is the first
+ * min(k, |A_f(q)|) entries of
+ *     sort ascending { (dist_to_element(q, i), i) : i in A_f(q) }
+ * with granne_b200_exact_search_batch's distance bits and (distance, id) order.  An all-admitting filter gives
+ * granne_b200_exact_search_batch(q, k); the bitmap of a list L gives granne_b200_exact_search_within_batch(q, L, k).
+ * Ids in [n, num_elements) of a container larger than its index are never returned.
+ *   queries        as granne_b200_exact_search_batch (RAW_F32, ELEMENT, QUERY_ID or QUERY_ID_EXCLUDING; the last runs
+ *                  k + 1 and drops the query's own id, which is there only when its filter admits it)
+ *   filters, num_filters, filter_words, query_filter   as granne_b200_search_filtered_batch
+ *   num_neighbors  k, 0..GRANNE_B200_EXACT_MAX_K; there is no max_search
+ *   out_*          as granne_b200_exact_search_batch; out_counts[q] = min(k, |A_f(q)|)
+ * nq == 0, k == 0 and empty filters are valid.  Only rows admitted by a filter some query of the call uses are read.
+ * ERR_NOT_FINITE when some query q has a NaN distance to an element of A_f(q) (for angular_int: a NaN raw query with a
+ * non-empty A_f(q)); a NaN element no query's filter admits, or a NaN query whose A_f(q) is empty, does not fail the
+ * call.  ERR_INVALID_ARGUMENT, in this order: the handle is NULL; an unknown query format; k >
+ * GRANNE_B200_EXACT_MAX_K; nq above the batch limit; a NULL queries or output buffer; then, when nq > 0: filters NULL
+ * or num_filters == 0; QUERY_ID_EXCLUDING with k > 1023; filter_words < ceil(n / 32); and (host call) a query_filter
+ * entry >= num_filters.  The host call checks them all before any device call and copies filters and query_filter up
+ * in its one round trip, into memory held only until its kernels have run.
+ * Cost: per query chunk (1024 queries) the rows of U, the union of the filters the chunk's queries name, plus 2F x n /
+ * 32 bitmap words (F = the distinct filters the chunk names) and three small launches per list of up to a slab of ids
+ * (65536 for a chunk of 1024 queries; ceil(n / (slab - 31)) lists, of which those past U's last id are empty) — not
+ * the n rows of granne_b200_exact_search_batch.  A chunk whose queries share one filter scans exactly its admitted
+ * rows, so callers with many distinct filters get the best grouping by ordering their queries by filter.  Workspace
+ * is exact_search_batch's plus one list of ids per chunk, whatever n and the density. */
+int granne_b200_exact_search_filtered_batch(granne_b200_index* h, const void* queries, size_t nq, int query_format,
+                                            const uint32_t* filters, uint32_t num_filters, uint64_t filter_words,
+                                            const uint32_t* query_filter, uint32_t num_neighbors, uint32_t* out_ids,
+                                            float* out_dists, uint32_t* out_counts);
+/* Same with DEVICE pointers (queries, filters, query_filter, outputs) on cuda_stream (NULL = the default stream),
+ * asynchronous like granne_b200_exact_search_batch_device and without a host synchronisation (the admitted counts stay
+ * on the device).  The host checks the rules up to filter_words; the kernels check query_filter: a query whose entry
+ * is >= num_filters gets count 0 and padding (its entry is never used as an index), the other queries are answered,
+ * and granne_b200_stream_status reports ERR_INVALID_ARGUMENT. */
+int granne_b200_exact_search_filtered_batch_device(granne_b200_index* h, const void* d_queries, size_t nq,
+                                                   int query_format, const uint32_t* d_filters, uint32_t num_filters,
+                                                   uint64_t filter_words, const uint32_t* d_query_filter,
+                                                   uint32_t num_neighbors, uint32_t* d_out_ids, float* d_out_dists,
+                                                   uint32_t* d_out_counts, void* cuda_stream);
 
 /* ---- exact range search: every element within a distance bound -------------------------------------------------------
  * NOT a reference function: near-duplicate detection, threshold matching, density counts.  For n = granne_b200_len(h)
@@ -482,6 +528,15 @@ int granne_b200_multi_search_filtered_batch(granne_b200_multi* m, const void* qu
                                             uint32_t max_search, uint32_t num_neighbors, const uint32_t* filters,
                                             uint32_t num_filters, uint64_t filter_words, const uint32_t* query_filter,
                                             uint64_t* out_ids, float* out_dists, uint32_t* out_counts);
+/* granne_b200_exact_search_filtered_batch over a multi handle, with granne_b200_multi_search_filtered_batch's bitmaps
+ * over GLOBAL ids, filter_words rule and split: REPLICATED slices the queries with their query_filter entries;
+ * RANGE_PARTITIONED runs every query on every shard, shard s reading bit shard_base[s] + local id (shard bases need not
+ * be multiples of 32), and merges the shards' exact lists by (distance, global id).  Results are u64 GLOBAL ids. */
+int granne_b200_multi_exact_search_filtered_batch(granne_b200_multi* m, const void* queries, size_t nq,
+                                                  int query_format, const uint32_t* filters, uint32_t num_filters,
+                                                  uint64_t filter_words, const uint32_t* query_filter,
+                                                  uint32_t num_neighbors, uint64_t* out_ids, float* out_dists,
+                                                  uint32_t* out_counts);
 /* granne_b200_set_rerank_elements on every part: REPLICATED takes one image (elements_bytes[0]) and stages it on every
  * device; RANGE_PARTITIONED takes one image per shard.  Every image is checked before any is staged; if a part then fails to
  * stage its rows (a device error), the parts this call attached release theirs again, so the call can be repeated. */

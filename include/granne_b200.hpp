@@ -349,6 +349,21 @@ public:
                                                 nullptr));
         return detail::result_lists<SearchResult>(ids, dists, counts, num_neighbors);
     }
+    // Exact filtered k-NN (granne_b200_exact_search_filtered_batch): the first min(k, |A|) of the ids < len() the
+    // query's filter admits, by (distance, id), with exact_search's distances.  Filters as in search_filtered; there is
+    // no max_search.  k <= GRANNE_B200_EXACT_MAX_K.  Not a reference function.
+    std::vector<SearchResult> exact_search_filtered(const void* queries, size_t nq, int query_format,
+                                                    size_t num_neighbors, const uint32_t* filters,
+                                                    uint32_t num_filters, uint64_t filter_words,
+                                                    const uint32_t* query_filter = nullptr) const {
+        std::vector<uint32_t> ids(nq * num_neighbors), counts(nq);
+        std::vector<float> dists(nq * num_neighbors);
+        check(granne_b200_exact_search_filtered_batch(h_, queries, nq, query_format, filters, num_filters,
+                                                      filter_words, query_filter,
+                                                      static_cast<uint32_t>(num_neighbors), ids.data(), dists.data(),
+                                                      counts.data()));
+        return detail::result_lists<SearchResult>(ids, dists, counts, num_neighbors);
+    }
 
     // Two-stage search (granne_b200_search_rerank_batch): attach the container of this angular_int index's elements
     // once (angular f32 rows, or the SumEmbeddings container the rows were computed from), then search_rerank
@@ -549,6 +564,21 @@ public:
                                                       static_cast<uint32_t>(max_search),
                                                       static_cast<uint32_t>(num_neighbors), filters, num_filters,
                                                       filter_words, query_filter, ids.data(), d.data(), c.data()));
+        return detail::result_lists<Result>(ids, d, c, num_neighbors);
+    }
+    // Granne::exact_search_filtered over every part for nq raw f32 queries: bitmaps over GLOBAL ids, GLOBAL ids in the
+    // results (granne_b200_multi_exact_search_filtered_batch)
+    std::vector<Result> exact_search_filtered(const std::vector<float>& queries, size_t num_neighbors,
+                                              const uint32_t* filters, uint32_t num_filters, uint64_t filter_words,
+                                              const uint32_t* query_filter = nullptr) const {
+        const size_t nq = dim_ ? queries.size() / dim_ : 0;
+        std::vector<uint64_t> ids(nq * num_neighbors);
+        std::vector<float> d(nq * num_neighbors);
+        std::vector<uint32_t> c(nq);
+        check(granne_b200_multi_exact_search_filtered_batch(h_, queries.data(), nq, GRANNE_B200_QUERY_RAW_F32, filters,
+                                                            num_filters, filter_words, query_filter,
+                                                            static_cast<uint32_t>(num_neighbors), ids.data(),
+                                                            d.data(), c.data()));
         return detail::result_lists<Result>(ids, d, c, num_neighbors);
     }
 

@@ -1,19 +1,19 @@
-"""Measures filtered search (Granne.search_batch_filtered_device) against unfiltered search and exact search within the
-admitted ids, on one H100.
+"""Measures filtered search (Granne.search_batch_filtered_device) against unfiltered search and the exact filtered
+search over the same bitmap, on one H100.
 
 Data: bench.py's clustered 10M x 128 f32 rows (rerank_bench.generate) with a GPU-built index (M = 30, max_search 200);
 1024 raw queries in one device batch, k = 10, max_search 200 and 800.  Filters: one random filter admitting 100 %, 50 %,
 10 % and 1 % of n.  Per (max_search, share):
   * QPS of search_batch_device and search_batch_filtered_device, timed by CUDA events over --windows windows of
     --calls calls each, the two calls alternating window by window; median, min and max of the windows;
-  * recall@10 of the filtered search against the exact filtered answer (exact_search_within_device over the admitted
-    ids, one call per query of a --sample query sample; exact_search_batch_device at 100 %), and the share of the 1024
-    queries that returned fewer than k;
-  * exact_search_within_device time on --sample queries that all list the admitted ids (exact_search_batch_device at
-    100 %), as queries per second: where the exact path and the graph path cross over.
+  * recall@10 of the filtered search over the whole batch against the exact filtered answer (one
+    exact_search_filtered_device call over the same bitmap), also over its first 64 queries, and the share of the
+    1024 queries that returned fewer than k;
+  * the time of that exact_search_filtered_device call on the 1024 queries, as queries per second: where the exact
+    path and the graph path cross over.
 Prints the card name and power limit read in the same run, then one JSON line per (max_search, share).
 
-    python tools/filtered_bench.py [--elements 10000000] [--windows 7] [--calls 5] [--sample 64]
+    python tools/filtered_bench.py [--elements 10000000] [--windows 7] [--calls 5]
 """
 import argparse
 import json
@@ -47,7 +47,6 @@ def main():
     ap.add_argument("--elements", type=int, default=10_000_000)
     ap.add_argument("--windows", type=int, default=7)
     ap.add_argument("--calls", type=int, default=5)
-    ap.add_argument("--sample", type=int, default=64)
     a = ap.parse_args()
     import torch
 
@@ -69,28 +68,21 @@ def main():
     g = granne_b200.Granne.from_device_elements(index, "angular", rows["angular"])
     rng = np.random.default_rng(7)
     s = torch.cuda.Stream()
-    qs = q[:a.sample].contiguous()
     for share in (1.0, 0.5, 0.1, 0.01):
         mask = np.ones(n, bool) if share == 1.0 else rng.random(n) < share
-        admitted = np.nonzero(mask)[0].astype(np.uint32)
+        admitted = int(mask.sum())
         words = granne_b200.api._filter_words(mask, n)
         dw = torch.from_numpy(words.view(np.int32)).to(dev)
-        # the exact filtered answer for the sample, and the exact path's time on it
-        d_ids = torch.from_numpy(admitted.view(np.int32)).to(dev)
-        d_off = torch.tensor([0, admitted.size], dtype=torch.int64, device=dev)
+        # the exact filtered answer for the whole batch, and the exact path's time on it
         with torch.cuda.stream(s):
-            if share == 1.0:
-                def exact(st):
-                    return g.exact_search_batch_device(qs, k, stream=st)
-            else:
-                def exact(st):
-                    return [g.exact_search_within_device(qs[i:i + 1], d_off, d_ids, k, stream=st)
-                            for i in range(a.sample)]
+            def exact(st):
+                return g.exact_search_filtered_device(q, dw, None, k, stream=st)
+
             exact(s)
             ex_t = [window(torch, s, exact, 1) for _ in range(3)]
-            res = exact(s)
+            truth = exact(s)[0]
             s.synchronize()
-            truth = (res[0] if share == 1.0 else torch.cat([r[0] for r in res])).cpu().numpy().view(np.uint32)
+            truth = truth.cpu().numpy().view(np.uint32)
         g.stream_status()
         for ef in (200, 800):
             with torch.cuda.stream(s):
@@ -113,22 +105,22 @@ def main():
             g.stream_status()
             fi, fc = fi.cpu().numpy().view(np.uint32), fc.cpu().numpy()
             hits = [len(set(fi[i, :fc[i]].tolist()) & set(truth[i][truth[i] != 0xFFFFFFFF].tolist()))
-                    for i in range(a.sample)]
-            want = [min(k, int((truth[i] != 0xFFFFFFFF).sum())) for i in range(a.sample)]
+                    for i in range(nq)]
+            want = [min(k, int((truth[i] != 0xFFFFFFFF).sum())) for i in range(nq)]
             qps_p = [nq * a.calls / t for t in tp]
             qps_f = [nq * a.calls / t for t in tf]
             print(json.dumps({
-                "max_search": ef, "admitted_share": share, "admitted": int(admitted.size), "nq": nq, "k": k,
+                "max_search": ef, "admitted_share": share, "admitted": admitted, "nq": nq, "k": k,
                 "search_qps": float(np.median(qps_p)), "search_qps_min": min(qps_p), "search_qps_max": max(qps_p),
                 "filtered_qps": float(np.median(qps_f)), "filtered_qps_min": min(qps_f),
                 "filtered_qps_max": max(qps_f), "filtered_over_search": float(np.median(qps_f) / np.median(qps_p)),
-                "recall_at_10": float(sum(hits) / max(1, sum(want))), "recall_sample": a.sample,
+                "recall_at_10": float(sum(hits) / max(1, sum(want))), "recall_queries": nq,
+                "recall_at_10_first_64": float(sum(hits[:64]) / max(1, sum(want[:64]))),
                 "share_fewer_than_k": float((fc < k).mean()),
-                "exact_qps": a.sample / float(np.median(ex_t)), "exact_qps_min": a.sample / max(ex_t),
-                "exact_qps_max": a.sample / min(ex_t),
-                "exact_path": "exact_search_batch" if share == 1.0 else "exact_search_within",
+                "exact_qps": nq / float(np.median(ex_t)), "exact_qps_min": nq / max(ex_t),
+                "exact_qps_max": nq / min(ex_t), "exact_path": "exact_search_filtered",
             }), flush=True)
-        del dw, d_ids
+        del dw
         torch.cuda.empty_cache()
     g.close()
 
