@@ -10,14 +10,16 @@
 //   exact_prepare_kernel    the queries as elements (prepare_query: normalise or quantise)
 //   exact_scan_f32_kernel   distances of a chunk x slab into the slab buffer, CUDA-core FMAs in the reference order
 //   exact_scan_i8_kernel    the same for i8 rows: exact integer dot products, then finish_angular_i8
-//   exact_select_kernel     per query: keys of the slab below the running k-th key join the running top-k list
-//   exact_write_kernel      the lists into the search_batch output layout
+//   exact_select_kernel     per query: keys of the slab below the running k-th key join the running top-k list (the
+//                           block's key_sort, keys.cuh)
+//   exact_write_kernel      the lists into the search_batch output layout (store_key)
 // EMBEDDINGS rows are materialised window by window by sum_embeddings_kernel + make_elements_kernel and scanned as
 // natural-layout f32 rows.
 //
 // The exact filtered call (granne_b200_exact_search_filtered_batch*) scans lists of ids instead of slabs of rows
 // (LISTED = true): per query chunk
-//   exact_chunk_filters_kernel  the distinct filters the chunk's queries name
+//   exact_chunk_filters_kernel  the distinct filters the chunk's queries name (key_sort of their ids, then
+//                               block_exclusive_scan)
 // then per list of at most a slab of ids
 //   exact_list_ids_kernel       the next ids their union admits, ascending, from a cursor in device memory
 //   exact_listed_rows_kernel    (EMBEDDINGS) the rows of those ids only
@@ -27,7 +29,7 @@
 //   exact_write_kernel<true>    per-query counts (the admitted keys the list holds)
 #pragma once
 
-#include "search_kernels.cuh"
+#include "keys.cuh"
 
 namespace granne_b200 {
 
@@ -342,29 +344,11 @@ __global__ void __launch_bounds__(256, 2) exact_scan_i8_kernel(const ExactScanAr
     }
 }
 
-// Bitonic sort of the kExactSelSlots keys in S, ascending (all threads of the block).
-__device__ __forceinline__ void exact_sort_slots(unsigned long long* S) {
-    for (uint32_t k2 = 2; k2 <= (uint32_t)kExactSelSlots; k2 <<= 1) {
-        for (uint32_t j = k2 >> 1; j > 0; j >>= 1) {
-            for (uint32_t t = threadIdx.x; t < (uint32_t)kExactSelSlots / 2; t += blockDim.x) {
-                const uint32_t i = 2 * t - (t & (j - 1)), ixj = i + j;
-                const unsigned long long x = S[i], y = S[ixj];
-                const bool up = (i & k2) == 0;
-                if ((x > y) == up) {
-                    S[i] = y;
-                    S[ixj] = x;
-                }
-            }
-            __syncthreads();
-        }
-    }
-}
-
 // The candidates S[kExactMaxK, kExactMaxK + *cnt) join the running list S[0, k): sort, keep the first k.
 __device__ __forceinline__ void exact_flush(unsigned long long* S, int* cnt, uint32_t k) {
     for (uint32_t i = kExactMaxK + *cnt + threadIdx.x; i < (uint32_t)kExactSelSlots; i += blockDim.x) S[i] = ~0ull;
     __syncthreads();
-    exact_sort_slots(S);
+    key_sort(BlockGroup{}, S, kExactSelSlots);
     for (uint32_t i = k + threadIdx.x; i < kExactMaxK; i += blockDim.x) S[i] = ~0ull;
     if (threadIdx.x == 0) *cnt = 0;
     __syncthreads();
@@ -449,16 +433,8 @@ __global__ void exact_write_kernel(const unsigned long long* __restrict__ lists,
     const unsigned long long t = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x;
     if (t < (unsigned long long)nq * k) {
         const uint32_t q = (uint32_t)(t / k), r = (uint32_t)(t % k);
-        uint32_t id = kUnusedId;
-        float d = __int_as_float(0x7f800000);
-        const unsigned long long key = LISTED ? (lists ? lists[(size_t)q * kExactMaxK + r] : ~0ull) : 0ull;
-        if (LISTED ? key != ~0ull : r < count) {
-            const unsigned long long kk = LISTED ? key : lists[(size_t)q * kExactMaxK + r];
-            id = key_id(kk);
-            d = __uint_as_float(key_dbits(kk));
-        }
-        out_ids[t] = id;
-        out_dists[t] = d;
+        const bool used = LISTED ? lists && lists[(size_t)q * kExactMaxK + r] != ~0ull : r < count;
+        store_key(out_ids, out_dists, t, used ? lists[(size_t)q * kExactMaxK + r] : ~0ull, used);
     }
     if constexpr (LISTED) {
         if (t < nq) {
@@ -481,34 +457,6 @@ __global__ void exact_write_kernel(const unsigned long long* __restrict__ lists,
 }
 
 // ---- exact filtered search: lists of admitted ids ----------------------------------------------------------------------
-// Exclusive prefix sum over the block (blockDim.x a multiple of 32, at most 1024) of v; *total the sum of all.
-__device__ __forceinline__ uint32_t block_exclusive_scan(uint32_t v, uint32_t* total) {
-    __shared__ uint32_t warp_sums[32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-    uint32_t x = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t y = __shfl_up_sync(kFullMask, x, o);
-        if (lane >= o) x += y;
-    }
-    if (lane == 31) warp_sums[warp] = x;
-    __syncthreads();
-    if (warp == 0) {
-        uint32_t w = lane < nw ? warp_sums[lane] : 0u;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t y = __shfl_up_sync(kFullMask, w, o);
-            if (lane >= o) w += y;
-        }
-        warp_sums[lane] = w;  // inclusive over warps
-    }
-    __syncthreads();
-    const uint32_t before = (warp ? warp_sums[warp - 1] : 0u) + x - v;
-    *total = warp_sums[nw - 1];
-    __syncthreads();  // warp_sums may be reused by the caller's next scan
-    return before;
-}
-
 constexpr int kExactListThreads = 1024;
 
 // The distinct valid filters the chunk's qc <= kExactMaxChunk queries name (query_filter null: filter 0), ascending,
@@ -523,19 +471,7 @@ __global__ void __launch_bounds__(kExactListThreads) exact_chunk_filters_kernel(
     uint32_t f = t < qc ? (query_filter ? query_filter[t] : 0u) : ~0u;
     s[t] = f < num_filters ? f : ~0u;
     __syncthreads();
-    for (uint32_t k2 = 2; k2 <= (uint32_t)kExactListThreads; k2 <<= 1) {
-        for (uint32_t j = k2 >> 1; j > 0; j >>= 1) {
-            const uint32_t ixj = t ^ j;
-            if (ixj > t) {
-                const uint32_t x = s[t], y = s[ixj];
-                if ((x > y) == ((t & k2) == 0)) {
-                    s[t] = y;
-                    s[ixj] = x;
-                }
-            }
-            __syncthreads();
-        }
-    }
+    key_sort(BlockGroup{}, s, kExactListThreads);
     f = s[t];
     const bool keep = f != ~0u && (t == 0 || s[t - 1] != f);
     uint32_t total;

@@ -62,6 +62,17 @@ int guarded(F&& body) {
         }                                                                                               \
     } while (0)
 
+// Launches Kern over (grid, block) with `smem` bytes of dynamic shared memory on `stream`, adds it to `launches` (null
+// for a call without a handle) and returns the launch's error, so that a failed launch is reported by the call that made
+// it rather than left behind as the thread's last error.
+template <auto Kern, class... Args>
+int launch(dim3 grid, dim3 block, size_t smem, cudaStream_t stream, std::atomic<uint64_t>* launches, Args&&... args) {
+    Kern<<<grid, block, smem, stream>>>(std::forward<Args>(args)...);
+    if (launches) ++*launches;
+    GB_CUDA(cudaGetLastError());
+    return GRANNE_B200_OK;
+}
+
 // Every entry point runs on its handle's device and leaves the caller's current device as it found it (a host
 // application — e.g. one torch process per GPU — must not see its default device change under it).  A guard is
 // declared before anything that owns device memory, so that the memory is also freed on that device.
@@ -330,15 +341,13 @@ int upload_rows(Handle* h, const gb::DeviceIndex& d, const uint8_t* src, uint64_
             from = tmp.get();
         }
         uint8_t* to = dst + r0 * d.row_stride * esz;
-        if (i8)
-            gb::pad_rows_i8_kernel<<<h->num_sms * 8, 256>>>(reinterpret_cast<const int8_t*>(from),
-                                                            reinterpret_cast<int8_t*>(to), nr, d.dim, d.row_stride);
-        else
-            gb::permute_rows_f32_kernel<<<h->num_sms * 8, 256>>>(reinterpret_cast<const float*>(from),
-                                                                 reinterpret_cast<float*>(to), nr, d.dim, d.full,
-                                                                 d.vec_group, d.row_stride);
-        h->launches++;
-        GB_CUDA(cudaGetLastError());
+        rc = i8 ? launch<gb::pad_rows_i8_kernel>(h->num_sms * 8, 256, 0, nullptr, &h->launches,
+                                                 reinterpret_cast<const int8_t*>(from), reinterpret_cast<int8_t*>(to),
+                                                 nr, d.dim, d.row_stride)
+                : launch<gb::permute_rows_f32_kernel>(h->num_sms * 8, 256, 0, nullptr, &h->launches,
+                                                      reinterpret_cast<const float*>(from), reinterpret_cast<float*>(to),
+                                                      nr, d.dim, d.full, d.vec_group, d.row_stride);
+        if (rc) return rc;
     }
     GB_CUDA(cudaDeviceSynchronize());
     return GRANNE_B200_OK;
@@ -470,17 +479,17 @@ uint64_t emb_window_end(const EmbeddingsInput& in, uint64_t r0) {
 }
 
 // The two kernels for `nr` elements on `stream`: raw rows into d_raw, then Vector::from per row into d_out.  d_out may
-// be d_raw (ANGULAR): make_elements_kernel holds a row in shared memory before it writes the row back.
+// be d_raw (ANGULAR): make_elements_kernel holds a row in shared memory before it writes the row back.  Both are
+// counted on `launches` (null: not counted).
 int launch_embeddings(const EmbeddingsInput& in, int kind, int num_sms, const float* d_table,
                       const unsigned long long* d_off, uint64_t term_base, const uint32_t* d_terms, uint64_t nr,
-                      float* d_raw, void* d_out, int* d_status, cudaStream_t stream) {
+                      float* d_raw, void* d_out, int* d_status, cudaStream_t stream, std::atomic<uint64_t>* launches) {
     const gb::SumRowsArgs a{d_table, d_off, term_base, d_terms, nr, in.dim, kind, d_raw, d_status};
-    gb::sum_embeddings_kernel<<<(unsigned)std::min<uint64_t>((nr + 7) / 8, (uint64_t)num_sms * 4), 256, 0, stream>>>(a);
-    GB_CUDA(cudaGetLastError());
-    gb::make_elements_kernel<<<(unsigned)std::min<uint64_t>(nr, (uint64_t)num_sms * 32), 32, (size_t)in.dim * 4,
-                               stream>>>(d_raw, nr, in.dim, kind, d_out);
-    GB_CUDA(cudaGetLastError());
-    return GRANNE_B200_OK;
+    const int rc = launch<gb::sum_embeddings_kernel>((unsigned)std::min<uint64_t>((nr + 7) / 8, (uint64_t)num_sms * 4),
+                                                     256, 0, stream, launches, a);
+    return rc ? rc
+              : launch<gb::make_elements_kernel>((unsigned)std::min<uint64_t>(nr, (uint64_t)num_sms * 32), 32,
+                                                 (size_t)in.dim * 4, stream, launches, d_raw, nr, in.dim, kind, d_out);
 }
 
 int embeddings_status(int* d_status) {
@@ -727,15 +736,12 @@ int raise_smem_limit(const Handle* h) {
     return GRANNE_B200_OK;
 }
 
-// Launches the one-warp kernel Kern<<<grid, 32, smem, stream>>>(d, a) over the staged container d and counts it.
+// Launches the one-warp kernel Kern(d, a) over the staged container d, grid CTAs of 32 threads with `smem` bytes of
+// dynamic shared memory, and counts it.
 template <auto Kern, class Args>
 int launch_warps(Handle* h, unsigned grid, size_t smem, cudaStream_t stream, const gb::DeviceIndex& d, const Args& a) {
     const int rc = raise_smem_limit<Kern>(h);
-    if (rc) return rc;
-    Kern<<<grid, 32, smem, stream>>>(d, a);
-    h->launches++;
-    GB_CUDA(cudaGetLastError());
-    return GRANNE_B200_OK;
+    return rc ? rc : launch<Kern>(grid, 32, smem, stream, &h->launches, d, a);
 }
 
 // Resident one-warp CTAs per SM of Kern with `smem` bytes of dynamic shared memory, queried once per (kernel, smem).
@@ -1198,11 +1204,9 @@ int enqueue_id_rows(Handle* h, Workspace* w, const uint32_t* ids, size_t nq, cud
     if ((rc = w->d_id_rows.grow(std::max<size_t>(nq * row, 16), stream)) || (rc = w->d_id_bad.grow(nq, stream)))
         return rc;
     const size_t smem = d.kind == gb::kSumEmbeddings ? (size_t)d.dim * 4 : 0;
-    gb::get_elements_kernel<<<(unsigned)std::min<uint64_t>(nq, (uint64_t)h->num_sms * 32), 32, smem, stream>>>(
-        d, ids, nq, d.num_elements, w->d_id_rows.get(), w->d_id_bad.get(), w->d_error);
-    h->launches++;
-    GB_CUDA(cudaGetLastError());
-    return GRANNE_B200_OK;
+    return launch<gb::get_elements_kernel>((unsigned)std::min<uint64_t>(nq, (uint64_t)h->num_sms * 32), 32, smem, stream,
+                                           &h->launches, d, ids, nq, d.num_elements, w->d_id_rows.get(),
+                                           w->d_id_bad.get(), w->d_error);
 }
 
 template <class Call>
@@ -1222,12 +1226,10 @@ int enqueue_query(Handle* h, Workspace* w, const void* d_q, size_t nq, int fmt, 
     }
     if ((rc = call(w->d_id_rows.get(), (int)GRANNE_B200_QUERY_ELEMENT, kk, res))) return rc;
     if (!exclude && host_checked) return GRANNE_B200_OK;
-    gb::id_results_kernel<<<(unsigned)std::min<uint64_t>((nq + 3) / 4, (uint64_t)h->num_sms * 16), 128, 0, stream>>>(
-        res.ids, res.dists, res.counts, kk, ids, w->d_id_bad.get(), exclude, nq, k, out.ids, out.dists, out.counts,
-        reinterpret_cast<unsigned long long*>(out.stats));
-    h->launches++;
-    GB_CUDA(cudaGetLastError());
-    return GRANNE_B200_OK;
+    return launch<gb::id_results_kernel>((unsigned)std::min<uint64_t>((nq + 3) / 4, (uint64_t)h->num_sms * 16), 128, 0,
+                                         stream, &h->launches, res.ids, res.dists, res.counts, kk, ids,
+                                         w->d_id_bad.get(), exclude, nq, k, out.ids, out.dists, out.counts,
+                                         reinterpret_cast<unsigned long long*>(out.stats));
 }
 
 // ---- exact k-NN (exact_kernels.cuh) -------------------------------------------------------------------------------
@@ -1259,17 +1261,15 @@ int exact_scan_rows(Handle* h, Workspace* w, uint32_t qc, const void* rows, uint
         a.ld = slab;
         a.error = w->d_error;
         const dim3 grid((unsigned)((ns + gb::kExactRB - 1) / gb::kExactRB), (qc + gb::kExactQB - 1) / gb::kExactQB);
+        int rc;
         if (d.kind == gb::kAngularI8) {
             a.rows = static_cast<const int8_t*>(rows) + s0 * row_stride;
-            gb::exact_scan_i8_kernel<false><<<grid, 256, 0, stream>>>(a);
+            rc = launch<gb::exact_scan_i8_kernel<false>>(grid, 256, 0, stream, &h->launches, a);
         } else {
             a.rows = static_cast<const float*>(rows) + s0 * row_stride;
-            gb::exact_scan_f32_kernel<false><<<grid, 256, 0, stream>>>(a);
+            rc = launch<gb::exact_scan_f32_kernel<false>>(grid, 256, 0, stream, &h->launches, a);
         }
-        h->launches++;
-        GB_CUDA(cudaGetLastError());
-        const int rc = step(ns, base + s0);
-        if (rc) return rc;
+        if (rc || (rc = step(ns, base + s0))) return rc;
     }
     return GRANNE_B200_OK;
 }
@@ -1301,13 +1301,8 @@ int exact_scan_listed(Handle* h, Workspace* w, uint32_t qc, const void* rows, ui
     // two 256-thread blocks per SM are resident: no more than fit, so that no block waits for a whole list's tiles
     const uint64_t wave = std::max<uint64_t>(1, (uint64_t)h->num_sms * 2 / gy);
     const dim3 grid((unsigned)std::max<uint64_t>(1, std::min(wave, (cap + gb::kExactRB - 1) / gb::kExactRB)), gy);
-    if (d.kind == gb::kAngularI8)
-        gb::exact_scan_i8_kernel<true><<<grid, 256, 0, stream>>>(a);
-    else
-        gb::exact_scan_f32_kernel<true><<<grid, 256, 0, stream>>>(a);
-    h->launches++;
-    GB_CUDA(cudaGetLastError());
-    return GRANNE_B200_OK;
+    return d.kind == gb::kAngularI8 ? launch<gb::exact_scan_i8_kernel<true>>(grid, 256, 0, stream, &h->launches, a)
+                                    : launch<gb::exact_scan_f32_kernel<true>>(grid, 256, 0, stream, &h->launches, a);
 }
 
 // Ids per list of a filtered scan: a slab, and for EMBEDDINGS at most a window of materialised rows; at least 32, so
@@ -1387,34 +1382,34 @@ int exact_scan(Handle* h, Workspace* w, const void* d_queries, size_t nq, int fm
         const uint32_t qc = (uint32_t)std::min<size_t>(gb::kExactMaxChunk, nq - c0);
         if ((rc = begin(c0, qc))) return rc;
         if (scan) {
-            gb::exact_prepare_kernel<<<(unsigned)std::min<uint64_t>(qc, (uint64_t)h->num_sms * 32), 32, 0, stream>>>(
-                d, static_cast<const uint8_t*>(d_queries) + c0 * in_row, fmt, qc, w->d_exact_q.get(),
-                w->d_exact_qnorm.get(), w->d_error, filt ? w->d_exact_qstat.get() : nullptr);
-            h->launches++;
-            GB_CUDA(cudaGetLastError());
+            if ((rc = launch<gb::exact_prepare_kernel>((unsigned)std::min<uint64_t>(qc, (uint64_t)h->num_sms * 32), 32, 0,
+                                                       stream, &h->launches, d,
+                                                       static_cast<const uint8_t*>(d_queries) + c0 * in_row, fmt, qc,
+                                                       w->d_exact_q.get(), w->d_exact_qnorm.get(), w->d_error,
+                                                       filt ? w->d_exact_qstat.get() : nullptr)))
+                return rc;
             auto step = [&](uint64_t ns, uint64_t id_base) { return slab_step(c0, qc, ns, id_base, slab); };
             if (filt) {
                 const gb::ExactList l = exact_list(w, *filt, c0, slab);
                 uint32_t* count = const_cast<uint32_t*>(l.count);
                 uint32_t* ids = w->d_exact_ids.get();
-                gb::exact_chunk_filters_kernel<<<1, gb::kExactListThreads, 0, stream>>>(
-                    l.query_filter, qc, filt->num_filters, ids + slab, count);
-                h->launches++;
-                GB_CUDA(cudaGetLastError());
+                if ((rc = launch<gb::exact_chunk_filters_kernel>(1, gb::kExactListThreads, 0, stream, &h->launches,
+                                                                 l.query_filter, qc, filt->num_filters, ids + slab,
+                                                                 count)))
+                    return rc;
                 // lists of at most `cap` ids, each but the last fuller than cap - 32 (exact_list_ids_kernel)
                 const uint64_t cap = list_cap(slab, wrows, emb);
                 const uint64_t lists = (n + cap - 32) / (cap - 31);
                 for (uint64_t li = 0; li < lists; ++li) {
-                    gb::exact_list_ids_kernel<<<1, gb::kExactListThreads, 0, stream>>>(
-                        filt->words, filt->filter_words, filt->bit_base, ids + slab, count, n, (uint32_t)cap, ids);
-                    h->launches++;
-                    GB_CUDA(cudaGetLastError());
+                    if ((rc = launch<gb::exact_list_ids_kernel>(1, gb::kExactListThreads, 0, stream, &h->launches,
+                                                                filt->words, filt->filter_words, filt->bit_base,
+                                                                ids + slab, count, n, (uint32_t)cap, ids)))
+                        return rc;
                     if (emb) {
-                        gb::exact_listed_rows_kernel<<<(unsigned)std::min<uint64_t>(cap, (uint64_t)h->num_sms * 32), 32,
-                                                       (size_t)d.dim * 4, stream>>>(d, ids, count,
-                                                                                    w->d_exact_rows.get());
-                        h->launches++;
-                        GB_CUDA(cudaGetLastError());
+                        if ((rc = launch<gb::exact_listed_rows_kernel>(
+                                 (unsigned)std::min<uint64_t>(cap, (uint64_t)h->num_sms * 32), 32, (size_t)d.dim * 4,
+                                 stream, &h->launches, d, ids, count, w->d_exact_rows.get())))
+                            return rc;
                         rc = exact_scan_listed(h, w, qc, w->d_exact_rows.get(), d.dim, 1, nullptr, count, cap, slab,
                                                stream);
                     } else {
@@ -1430,9 +1425,8 @@ int exact_scan(Handle* h, Workspace* w, const void* d_queries, size_t nq, int fm
                     const uint64_t nr = std::min(wrows, n - r0);
                     if ((rc = launch_embeddings(in, gb::kAngularF32, h->num_sms, table, d.sum_offsets + r0, 0,
                                                 d.sum_terms, nr, w->d_exact_rows.get(), w->d_exact_rows.get(),
-                                                w->d_error, stream)))
+                                                w->d_error, stream, &h->launches)))
                         return rc;
-                    h->launches += 2;
                     if ((rc = exact_scan_rows(h, w, qc, w->d_exact_rows.get(), nr, d.dim, 1, r0, slab, stream, step)))
                         return rc;
                 }
@@ -1466,14 +1460,12 @@ int enqueue_exact(Handle* h, Workspace* w, const void* d_queries, size_t nq, int
         },
         [&](size_t c0, uint32_t qc, uint64_t ns, uint64_t id_base, uint64_t ld) {
             if (filt)
-                gb::exact_select_kernel<true><<<qc, gb::kExactSelThreads, 0, stream>>>(
-                    w->d_exact_dists.get(), ld, ns, 0, k, w->d_exact_lists.get(), exact_list(w, *filt, c0, ld));
-            else
-                gb::exact_select_kernel<false><<<qc, gb::kExactSelThreads, 0, stream>>>(
-                    w->d_exact_dists.get(), ld, ns, (uint32_t)id_base, k, w->d_exact_lists.get(), gb::ExactList{});
-            h->launches++;
-            GB_CUDA(cudaGetLastError());
-            return (int)GRANNE_B200_OK;
+                return launch<gb::exact_select_kernel<true>>(qc, gb::kExactSelThreads, 0, stream, &h->launches,
+                                                             w->d_exact_dists.get(), ld, ns, 0, k,
+                                                             w->d_exact_lists.get(), exact_list(w, *filt, c0, ld));
+            return launch<gb::exact_select_kernel<false>>(qc, gb::kExactSelThreads, 0, stream, &h->launches,
+                                                          w->d_exact_dists.get(), ld, ns, (uint32_t)id_base, k,
+                                                          w->d_exact_lists.get(), gb::ExactList{});
         },
         [&](size_t c0, uint32_t qc) {
             // a filtered call always writes: its kernel also checks the chunk's query_filter entries
@@ -1482,20 +1474,18 @@ int enqueue_exact(Handle* h, Workspace* w, const void* d_queries, size_t nq, int
             uint32_t* ids = out.ids ? out.ids + c0 * k : nullptr;
             float* dists = out.dists ? out.dists + c0 * k : nullptr;
             uint32_t* counts = out.counts ? out.counts + c0 : nullptr;
+            const unsigned grid = (unsigned)((outs + 255) / 256);
             if (filt) {
                 gb::ExactList l{};
                 l.query_filter = filt->query_filter ? filt->query_filter + c0 : nullptr;
                 l.num_filters = filt->num_filters;
                 l.error = w->d_error;
-                gb::exact_write_kernel<true><<<(unsigned)((outs + 255) / 256), 256, 0, stream>>>(
-                    scan ? w->d_exact_lists.get() : nullptr, qc, k, 0, ids, dists, counts, l);
-            } else {
-                gb::exact_write_kernel<false><<<(unsigned)((outs + 255) / 256), 256, 0, stream>>>(
-                    w->d_exact_lists.get(), qc, k, count, ids, dists, counts, gb::ExactList{});
+                return launch<gb::exact_write_kernel<true>>(grid, 256, 0, stream, &h->launches,
+                                                            scan ? w->d_exact_lists.get() : nullptr, qc, k, 0, ids,
+                                                            dists, counts, l);
             }
-            h->launches++;
-            GB_CUDA(cudaGetLastError());
-            return (int)GRANNE_B200_OK;
+            return launch<gb::exact_write_kernel<false>>(grid, 256, 0, stream, &h->launches, w->d_exact_lists.get(), qc,
+                                                         k, count, ids, dists, counts, gb::ExactList{});
         },
         filt);
 }
@@ -1548,12 +1538,10 @@ int enqueue_range_count(Handle* h, Workspace* w, const void* d_queries, size_t n
     auto none = [](size_t, uint32_t) { return (int)GRANNE_B200_OK; };
     return exact_scan(h, w, d_queries, nq, fmt, h->index_len > 0, stream, none,
                       [&](size_t c0, uint32_t qc, uint64_t ns, uint64_t id_base, uint64_t ld) {
-                          gb::range_count_kernel<<<range_grid(ns, qc), gb::kRangeThreads, 0, stream>>>(
-                              range_args(w, c0, ns, id_base, ld, radius, ri),
-                              reinterpret_cast<unsigned long long*>(counts) + c0);
-                          h->launches++;
-                          GB_CUDA(cudaGetLastError());
-                          return (int)GRANNE_B200_OK;
+                          return launch<gb::range_count_kernel>(range_grid(ns, qc), gb::kRangeThreads, 0, stream,
+                                                                &h->launches,
+                                                                range_args(w, c0, ns, id_base, ld, radius, ri),
+                                                                reinterpret_cast<unsigned long long*>(counts) + c0);
                       },
                       none);
 }
@@ -1576,18 +1564,13 @@ int enqueue_range_fill(Handle* h, Workspace* w, const void* d_queries, size_t nq
             return (int)GRANNE_B200_OK;
         },
         [&](size_t c0, uint32_t qc, uint64_t ns, uint64_t id_base, uint64_t ld) {
-            gb::range_emit_kernel<<<range_grid(ns, qc), gb::kRangeThreads, 0, stream>>>(
-                range_args(w, c0, ns, id_base, ld, radius, ri), cursor, offsets + c0, ids, dists);
-            h->launches++;
-            GB_CUDA(cudaGetLastError());
-            return (int)GRANNE_B200_OK;
+            return launch<gb::range_emit_kernel>(range_grid(ns, qc), gb::kRangeThreads, 0, stream, &h->launches,
+                                                 range_args(w, c0, ns, id_base, ld, radius, ri), cursor, offsets + c0,
+                                                 ids, dists);
         },
         [&](size_t c0, uint32_t qc) {
-            gb::range_finish_kernel<<<qc, gb::kRangeSortThreads, 0, stream>>>(offsets + c0, cursor, ids, dists,
-                                                                              w->d_error);
-            h->launches++;
-            GB_CUDA(cudaGetLastError());
-            return (int)GRANNE_B200_OK;
+            return launch<gb::range_finish_kernel>(qc, gb::kRangeSortThreads, 0, stream, &h->launches, offsets + c0,
+                                                   cursor, ids, dists, w->d_error);
         });
 }
 
@@ -1793,10 +1776,9 @@ int enqueue_within(Handle* h, Workspace* w, const void* d_queries, size_t nq, in
         for (size_t c0 = 0; c0 < nq; c0 += gb::kExactMaxChunk) {
             const uint32_t qc = (uint32_t)std::min<size_t>(gb::kExactMaxChunk, nq - c0);
             const unsigned long long* offs = reinterpret_cast<const unsigned long long*>(d_offsets) + c0;
-            gb::within_segments_kernel<<<1, gb::kExactMaxChunk, 0, stream>>>(offs, qc, c0 == 0, d_ids, prefix, locks,
-                                                                            qflags, counter, w->d_error);
-            h->launches++;
-            GB_CUDA(cudaGetLastError());
+            if ((err = launch<gb::within_segments_kernel>(1, gb::kExactMaxChunk, 0, stream, &h->launches, offs, qc,
+                                                          c0 == 0, d_ids, prefix, locks, qflags, counter, w->d_error)))
+                return err;
             if (k) GB_CUDA(cudaMemsetAsync(lists, 0xFF, (size_t)qc * k * 8, stream));
             gb::WithinArgs a{};
             a.queries = static_cast<const uint8_t*>(d_queries) + c0 * in_row;
@@ -1816,11 +1798,10 @@ int enqueue_within(Handle* h, Workspace* w, const void* d_queries, size_t nq, in
             a.out_counts = out.counts ? out.counts + c0 : nullptr;
             a.error_flag = w->d_error;
             a.tiles = eng.tiles;
-            if ((err = launch_warps<kern>(h, (unsigned)occ * h->num_sms, smem, stream, d, a))) return err;
-            gb::within_write_kernel<<<qc, 128, 0, stream>>>(lists, prefix, qflags, k, a.out_ids, a.out_dists,
-                                                            a.out_counts);
-            h->launches++;
-            GB_CUDA(cudaGetLastError());
+            if ((err = launch_warps<kern>(h, (unsigned)occ * h->num_sms, smem, stream, d, a)) ||
+                (err = launch<gb::within_write_kernel>(qc, 128, 0, stream, &h->launches, lists, prefix, qflags, k,
+                                                       a.out_ids, a.out_dists, a.out_counts)))
+                return err;
         }
         return (int)GRANNE_B200_OK;
     });
@@ -1981,9 +1962,9 @@ int builder_index_elements(Builder* b, uint32_t layer_m, uint32_t ef, uint64_t a
         const uint64_t present = reinsert ? num : first + pos;
         const uint64_t bsz = std::min<uint64_t>(std::min<uint64_t>(max_batch, std::max<uint64_t>(1, present / 16)), total - pos);
         const uint32_t start = reinsert ? (uint32_t)(num - 1 - pos) : (uint32_t)(first + pos);
-        gb::iota_kernel<<<(unsigned)((bsz + 255) / 256), 256, 0, stream>>>(b->d_ids.get(), (uint32_t)bsz, start,
-                                                                            reinsert ? -1 : 1);
-        h->launches++;
+        if ((rc = launch<gb::iota_kernel>((unsigned)((bsz + 255) / 256), 256, 0, stream, &h->launches, b->d_ids.get(),
+                                          (uint32_t)bsz, start, reinsert ? -1 : 1)))
+            return rc;
         // candidates = search_for_neighbors(layer, prev_layers.search(e,1,1), e, max_search) (:819-820)
         GB_CUDA(cudaMemsetAsync(b->ws->d_counters.get(), 0, kSearchCounterBytes, stream));
         rc = enqueue_search(h, b->ws.get(), b->d_ids.get(), bsz, gb::kQueryById, ef, ef,
@@ -2031,8 +2012,9 @@ int builder_index_last_layer(Builder* b, uint64_t max_num_elements) {
     if (rc) return rc;
     uint32_t* grown = mem.get();
     cudaStream_t stream = b->ws->stream.get();
-    gb::fill_u32_kernel<<<h->num_sms * 4, 256, 0, stream>>>(grown, (unsigned long long)num * b->stride, gb::kUnusedId);
-    h->launches++;
+    if ((rc = launch<gb::fill_u32_kernel>(h->num_sms * 4, 256, 0, stream, &h->launches, grown,
+                                          (unsigned long long)num * b->stride, gb::kUnusedId)))
+        return rc;
     if (have) GB_CUDA(cudaMemcpyAsync(grown, d.layer_rows[cur], (size_t)have * b->stride * 4, cudaMemcpyDeviceToDevice, stream));
     // the replaced rows stay alive until the copy out of them has completed: the first pass below synchronises the
     // stream before it returns OK, and a failed pass is synchronised here
@@ -2219,8 +2201,7 @@ int granne_b200_get_element(const granne_b200_index* hc, uint64_t idx, void* out
         Buffer<uint8_t> d;
         int rc = d.grow(bytes, nullptr);
         if (rc) return rc;
-        gb::get_element_kernel<<<1, 32>>>(h->dev, idx, d.get());
-        h->launches++;
+        if ((rc = launch<gb::get_element_kernel>(1, 32, 0, nullptr, &h->launches, h->dev, idx, d.get()))) return rc;
         GB_CUDA(cudaMemcpy(out, d.get(), bytes, cudaMemcpyDeviceToHost));
         return GRANNE_B200_OK;
     });
@@ -2244,11 +2225,11 @@ int granne_b200_get_elements(granne_b200_index* h, const uint32_t* ids, size_t n
                 return rc;
             GB_CUDA(cudaMemcpyAsync(w->d_queries.get(), ids, n * 4, cudaMemcpyHostToDevice, stream));
             const size_t smem = h->dev.kind == gb::kSumEmbeddings ? (size_t)h->dev.dim * 4 : 0;
-            gb::get_elements_kernel<<<(unsigned)std::min<uint64_t>(n, (uint64_t)h->num_sms * 32), 32, smem, stream>>>(
-                h->dev, reinterpret_cast<const uint32_t*>(w->d_queries.get()), n, h->dev.num_elements,
-                w->d_id_rows.get(), nullptr, w->d_error);
-            h->launches++;
-            GB_CUDA(cudaGetLastError());
+            if ((rc = launch<gb::get_elements_kernel>((unsigned)std::min<uint64_t>(n, (uint64_t)h->num_sms * 32), 32, smem,
+                                                      stream, &h->launches, h->dev,
+                                                      reinterpret_cast<const uint32_t*>(w->d_queries.get()), n,
+                                                      h->dev.num_elements, w->d_id_rows.get(), nullptr, w->d_error)))
+                return rc;
             GB_CUDA(cudaMemcpyAsync(out, w->d_id_rows.get(), bytes, cudaMemcpyDeviceToHost, stream));
             GB_CUDA(cudaStreamSynchronize(stream));
             return (int)GRANNE_B200_OK;
@@ -2264,11 +2245,9 @@ int granne_b200_get_elements_device(granne_b200_index* h, const uint32_t* d_ids,
     if (n == 0) return GRANNE_B200_OK;
     return device_batch(h, cuda_stream, false, [&](Workspace* w, cudaStream_t stream) {
         const size_t smem = h->dev.kind == gb::kSumEmbeddings ? (size_t)h->dev.dim * 4 : 0;
-        gb::get_elements_kernel<<<(unsigned)std::min<uint64_t>(n, (uint64_t)h->num_sms * 32), 32, smem, stream>>>(
-            h->dev, d_ids, n, h->dev.num_elements, d_out, nullptr, w->d_error);
-        h->launches++;
-        GB_CUDA(cudaGetLastError());
-        return GRANNE_B200_OK;
+        return launch<gb::get_elements_kernel>((unsigned)std::min<uint64_t>(n, (uint64_t)h->num_sms * 32), 32, smem,
+                                               stream, &h->launches, h->dev, d_ids, n, h->dev.num_elements, d_out,
+                                               nullptr, w->d_error);
     });
 }
 
@@ -2290,10 +2269,8 @@ static int search_device_impl(granne_b200_index* h, const void* d_queries, size_
     if (nq == 0)  // nothing to store, but the peers wait for this call's sequence number all the same
         return guarded([&] {
             GB_DEVICE(h->device);
-            gb::publish_seq_kernel<<<1, 1, 0, static_cast<cudaStream_t>(cuda_stream)>>>(device_gather(*pg, nullptr));
-            h->launches++;
-            GB_CUDA(cudaGetLastError());
-            return GRANNE_B200_OK;
+            return launch<gb::publish_seq_kernel>(1, 1, 0, static_cast<cudaStream_t>(cuda_stream), &h->launches,
+                                                  device_gather(*pg, nullptr));
         });
     return device_batch(h, cuda_stream, true, [&](Workspace* w, cudaStream_t stream) {
         return enqueue_query(h, w, d_queries, nq, query_format, num_neighbors,
@@ -2960,9 +2937,10 @@ int granne_b200_elements_from_raw(int element_kind, const float* raw, uint64_t n
     for (uint64_t r0 = 0; r0 < n; r0 += slab) {
         const uint64_t nr = std::min(slab, n - r0);
         GB_CUDA(cudaMemcpy(d_raw.get(), raw + r0 * dim, (size_t)nr * dim * 4, cudaMemcpyHostToDevice));
-        gb::make_elements_kernel<<<(unsigned)std::min<uint64_t>(nr, (uint64_t)sms * 32), 32, (size_t)dim * 4>>>(
-            d_raw.get(), nr, dim, element_kind, d_out.get());
-        GB_CUDA(cudaGetLastError());
+        if ((rc = launch<gb::make_elements_kernel>((unsigned)std::min<uint64_t>(nr, (uint64_t)sms * 32), 32,
+                                                   (size_t)dim * 4, nullptr, nullptr, d_raw.get(), nr, dim,
+                                                   element_kind, d_out.get())))
+            return rc;
         GB_CUDA(cudaMemcpy(o + 8 + (size_t)r0 * dim * esz, d_out.get(), (size_t)nr * dim * esz,
                            cudaMemcpyDeviceToHost));
     }
@@ -2983,10 +2961,9 @@ int granne_b200_elements_from_raw_device(int element_kind, const float* d_raw, u
     int rc = check_device(device, &sms, &optin);
     if (rc) return rc;
     GB_DEVICE(device);
-    gb::make_elements_kernel<<<(unsigned)std::min<uint64_t>(n, (uint64_t)sms * 32), 32, (size_t)dim * 4,
-                               static_cast<cudaStream_t>(cuda_stream)>>>(d_raw, n, dim, element_kind, d_out);
-    GB_CUDA(cudaGetLastError());
-    return GRANNE_B200_OK;
+    return launch<gb::make_elements_kernel>((unsigned)std::min<uint64_t>(n, (uint64_t)sms * 32), 32, (size_t)dim * 4,
+                                            static_cast<cudaStream_t>(cuda_stream), nullptr, d_raw, n, dim,
+                                            element_kind, d_out);
 }
 
 // compute_embeddings_and_save_to_disk (embeddings/parsing.rs:102-152) into a caller buffer.  Two windows are in
@@ -3064,7 +3041,7 @@ int granne_b200_compute_embeddings(int element_kind, const void* elements_bytes,
             if (nt) GB_CUDA(cudaMemcpyAsync(w.d_terms.get(), w.h_terms.get(), nt * 4, cudaMemcpyHostToDevice, s));
             void* rows_out = element_kind == GRANNE_B200_ANGULAR ? static_cast<void*>(w.d_raw.get()) : w.d_i8.get();
             if ((rc = launch_embeddings(in, element_kind, sms, d_table.get(), w.d_off.get(), t0, w.d_terms.get(), nr,
-                                        w.d_raw.get(), rows_out, d_status.get(), s)))
+                                        w.d_raw.get(), rows_out, d_status.get(), s, nullptr)))
                 return rc;
             GB_CUDA(cudaMemcpyAsync(w.h_out.get(), rows_out, nr * row_bytes, cudaMemcpyDeviceToHost, s));
             w.r0 = r0;
@@ -3117,7 +3094,7 @@ int granne_b200_compute_embeddings_device(int element_kind, const void* elements
             void* rows_out = element_kind == GRANNE_B200_ANGULAR ? static_cast<void*>(raw)
                                                                   : static_cast<int8_t*>(d_out) + r0 * in.dim;
             if ((rc = launch_embeddings(in, element_kind, sms, d_table.get(), d_off.get() + r0, 0, d_terms.get(), nr,
-                                        raw, rows_out, d_status.get(), s)))
+                                        raw, rows_out, d_status.get(), s, nullptr)))
                 return rc;
             r0 = r1;
         }
@@ -3232,9 +3209,9 @@ int granne_b200_compute_order(granne_b200_index* h, uint64_t* order_out, uint64_
                 view.layer_len[0] = h->dev.layer_len[j];
                 for (uint64_t base = layer_lens[j]; base < n; base += batch) {
                     const uint64_t bsz = std::min<uint64_t>(batch, n - base);
-                    gb::iota_kernel<<<(unsigned)((bsz + 255) / 256), 256, 0, stream>>>(d_q.get(), (uint32_t)bsz,
-                                                                                        (uint32_t)base, 1);
-                    h->launches++;
+                    if ((rc = launch<gb::iota_kernel>((unsigned)((bsz + 255) / 256), 256, 0, stream, &h->launches,
+                                                      d_q.get(), (uint32_t)bsz, (uint32_t)base, 1)))
+                        return rc;
                     GB_CUDA(cudaMemsetAsync(w->d_counters.get(), 0, kHostCallBytes, stream));
                     rc = enqueue_search(h, w, d_q.get(), bsz, gb::kQueryById, 1, 1,
                                         {d_ids.get(), d_d.get(), d_cnt.get(), nullptr}, stream, nullptr, &view);
@@ -3354,9 +3331,10 @@ int granne_b200_merge_topk_device(int device, const uint32_t* d_part_ids, const 
     GB_CUDA(cudaMallocAsync(&d_base, num_parts * 8, stream));
     GB_CUDA(cudaMemcpyAsync(d_base, part_base, num_parts * 8, cudaMemcpyHostToDevice, stream));
     const unsigned block = 128, grid = (unsigned)((nq + block - 1) / block);
-    gb::merge_topk_kernel<<<grid, block, 0, stream>>>(d_part_ids, d_part_dists, d_base, (uint32_t)num_parts, nq, k,
-                                                      reinterpret_cast<unsigned long long*>(d_out_ids), d_out_dists);
-    GB_CUDA(cudaGetLastError());
+    const int rc = launch<gb::merge_topk_kernel>(grid, block, 0, stream, nullptr, d_part_ids, d_part_dists, d_base,
+                                                 (uint32_t)num_parts, nq, k,
+                                                 reinterpret_cast<unsigned long long*>(d_out_ids), d_out_dists);
+    if (rc) return rc;
     GB_CUDA(cudaFreeAsync(d_base, stream));
     return GRANNE_B200_OK;
 }

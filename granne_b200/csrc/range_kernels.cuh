@@ -7,12 +7,14 @@
 //   range_emit_kernel    the same entries appended, as (id, distance) pairs, to the caller's segment of the query at a
 //                        per-query cursor; a cursor past the segment's end counts on but writes nothing
 //   range_finish_kernel  per query: a segment whose length equals its cursor's count is sorted in place by make_key
-//                        (a bitonic network over shared-memory tiles and, for longer segments, global compare-exchange
-//                        steps); any other segment is padded (0xFFFFFFFF / +inf) and kStatusBadSegment is raised
+//                        (keys.cuh's bitonic network on shared-memory tiles and, for longer segments, the same network's
+//                        wider stages as global compare-exchange steps); any other segment is padded (0xFFFFFFFF / +inf)
+//                        and kStatusBadSegment is raised
 // The output is written in place, so a fill needs no buffer of its results whatever their number.
 #pragma once
 
 #include "exact_kernels.cuh"
+#include "keys.cuh"
 
 namespace granne_b200 {
 
@@ -84,46 +86,6 @@ __global__ void __launch_bounds__(kRangeThreads) range_emit_kernel(const RangeAr
     }
 }
 
-// One compare-exchange of the ascending network: the smaller key to position i (i < j).
-__device__ __forceinline__ void range_cmpswap(unsigned long long* S, uint32_t i, uint32_t j) {
-    const unsigned long long x = S[i], y = S[j];
-    if (x > y) {
-        S[i] = y;
-        S[j] = x;
-    }
-}
-
-// The bitonic network on the p keys of S (shared memory, p a power of two <= kRangeTile), all threads of the block:
-// stages k2 = 2 .. p, each a flip step (i against its mirror i ^ (k2 - 1)) and then half-cleaners (i against i + j)
-// for j = k2 / 4 .. 1.  Every comparator puts the smaller key first, so keys of ~0 at the end stay there: a segment of
-// any length sorts as if padded with ~0 to a power of two.  range_tile_clean: the half-cleaners j = kRangeTile / 2 .. 1
-// that end a stage wider than a tile.
-__device__ void range_tile_sort(unsigned long long* S, uint32_t p) {
-    for (uint32_t k2 = 2; k2 <= p; k2 <<= 1) {
-        for (uint32_t t = threadIdx.x; t < p / 2; t += blockDim.x) {
-            const uint32_t i = 2 * t - (t & (k2 / 2 - 1));
-            range_cmpswap(S, i, i ^ (k2 - 1));
-        }
-        __syncthreads();
-        for (uint32_t j = k2 / 4; j > 0; j >>= 1) {
-            for (uint32_t t = threadIdx.x; t < p / 2; t += blockDim.x) {
-                const uint32_t i = 2 * t - (t & (j - 1));
-                range_cmpswap(S, i, i + j);
-            }
-            __syncthreads();
-        }
-    }
-}
-__device__ void range_tile_clean(unsigned long long* S) {
-    for (uint32_t j = kRangeTile / 2; j > 0; j >>= 1) {
-        for (uint32_t t = threadIdx.x; t < kRangeTile / 2; t += blockDim.x) {
-            const uint32_t i = 2 * t - (t & (j - 1));
-            range_cmpswap(S, i, i + j);
-        }
-        __syncthreads();
-    }
-}
-
 // The keys [t0, t0 + p) of a segment of len entries into S (~0 past len), and back.
 __device__ __forceinline__ void range_load(unsigned long long* S, const uint32_t* ids, const float* dists,
                                            unsigned long long t0, uint32_t p, unsigned long long len) {
@@ -133,12 +95,8 @@ __device__ __forceinline__ void range_load(unsigned long long* S, const uint32_t
 }
 __device__ __forceinline__ void range_store(const unsigned long long* S, uint32_t* ids, float* dists,
                                             unsigned long long t0, uint32_t p, unsigned long long len) {
-    for (uint32_t i = threadIdx.x; i < p; i += blockDim.x) {
-        if (t0 + i < len) {
-            ids[t0 + i] = key_id(S[i]);
-            dists[t0 + i] = __uint_as_float(key_dbits(S[i]));
-        }
-    }
+    for (uint32_t i = threadIdx.x; i < p; i += blockDim.x)
+        if (t0 + i < len) store_key(ids, dists, t0 + i, S[i], true);
     __syncthreads();
 }
 
@@ -148,10 +106,8 @@ __device__ __forceinline__ void range_global_cmpswap(uint32_t* ids, float* dists
     if (j >= len) return;
     const unsigned long long x = make_key(dists[i], ids[i]), y = make_key(dists[j], ids[j]);
     if (x > y) {
-        ids[i] = key_id(y);
-        dists[i] = __uint_as_float(key_dbits(y));
-        ids[j] = key_id(x);
-        dists[j] = __uint_as_float(key_dbits(x));
+        store_key(ids, dists, i, y, true);
+        store_key(ids, dists, j, x, true);
     }
 }
 
@@ -170,10 +126,8 @@ __global__ void __launch_bounds__(kRangeSortThreads) range_finish_kernel(const u
     if (stop < start || (stop > start && !out_ids) || count != stop - start) {
         if (threadIdx.x == 0) atomicOr(error, kStatusBadSegment);
         if (stop > start && out_ids)
-            for (unsigned long long i = start + threadIdx.x; i < stop; i += blockDim.x) {
-                out_ids[i] = kUnusedId;
-                out_dists[i] = __int_as_float(0x7f800000);
-            }
+            for (unsigned long long i = start + threadIdx.x; i < stop; i += blockDim.x)
+                store_key(out_ids, out_dists, i, ~0ull, false);
         return;
     }
     const unsigned long long len = count;
@@ -184,13 +138,13 @@ __global__ void __launch_bounds__(kRangeSortThreads) range_finish_kernel(const u
     while (p < len) p <<= 1;
     if (p <= kRangeTile) {
         range_load(S, ids, dists, 0, (uint32_t)p, len);
-        range_tile_sort(S, (uint32_t)p);
+        key_sort(BlockGroup{}, S, (uint32_t)p);
         range_store(S, ids, dists, 0, (uint32_t)p, len);
         return;
     }
     for (unsigned long long t0 = 0; t0 < len; t0 += kRangeTile) {
         range_load(S, ids, dists, t0, kRangeTile, len);
-        range_tile_sort(S, kRangeTile);
+        key_sort(BlockGroup{}, S, kRangeTile);
         range_store(S, ids, dists, t0, kRangeTile, len);
     }
     for (unsigned long long k2 = 2ull * kRangeTile; k2 <= p; k2 <<= 1) {
@@ -208,7 +162,7 @@ __global__ void __launch_bounds__(kRangeSortThreads) range_finish_kernel(const u
         }
         for (unsigned long long t0 = 0; t0 < len; t0 += kRangeTile) {
             range_load(S, ids, dists, t0, kRangeTile, len);
-            range_tile_clean(S);
+            key_clean(BlockGroup{}, S, kRangeTile, kRangeTile / 2);
             range_store(S, ids, dists, t0, kRangeTile, len);
         }
     }

@@ -11,11 +11,11 @@
 // The result depends only on the set of candidates, not on the order stage 1 wrote them in.
 //
 // One warp per query, persistent over a work counter: normalise the query (prepare_query), distances of the candidates
-// 32 at a time through Dist::dists, their make_key(d, id) keys into shared memory padded with ~0 to a power of two, a
-// warp bitonic sort, the first k keys out.
+// 32 at a time through Dist::dists, their make_key(d, id) keys into shared memory padded with ~0 to a power of two,
+// key_sort by the warp, the first k keys out through warp_store_row (keys.cuh).
 #pragma once
 
-#include "search_kernels.cuh"
+#include "keys.cuh"
 
 namespace granne_b200 {
 
@@ -45,26 +45,6 @@ struct RerankArgs {
     int* error_flag;             // kStatusNotFinite is or-ed in on a NaN distance
     WarpTiles tiles;
 };
-
-// Ascending sort of keys[0, p) (p a power of two) by the warp.  The pairs (i, i ^ j) of one step are disjoint, so a
-// lane exchanges its pairs without waiting for another lane until the step ends.
-__device__ __forceinline__ void warp_bitonic_sort(unsigned long long* keys, uint32_t p, int lane) {
-    for (uint32_t size = 2; size <= p; size <<= 1) {
-        for (uint32_t j = size >> 1; j > 0; j >>= 1) {
-            for (uint32_t i = lane; i < p; i += 32) {
-                const uint32_t l = i ^ j;
-                if (l > i) {
-                    const unsigned long long x = keys[i], y = keys[l];
-                    if ((x > y) == ((i & size) == 0)) {
-                        keys[i] = y;
-                        keys[l] = x;
-                    }
-                }
-            }
-            __syncwarp();
-        }
-    }
-}
 
 template <class Dist>
 __global__ void __launch_bounds__(32) rerank_kernel(const DeviceIndex ix, const RerankArgs a) {
@@ -98,18 +78,13 @@ __global__ void __launch_bounds__(32) rerank_kernel(const DeviceIndex ix, const 
         const uint32_t p = rerank_key_slots(n);
         for (uint32_t i = n + c.lane; i < p; i += 32) keys[i] = ~0ull;
         __syncwarp();
-        warp_bitonic_sort(keys, p, c.lane);
+        key_sort(WarpGroup{c.lane}, keys, p);
         uint32_t found = n < k ? n : k;
         if (__any_sync(kFullMask, c.status & kStatusNotFinite)) {
             found = 0;
             if (c.lane == 0) atomicOr(a.error_flag, kStatusNotFinite);
         }
-        for (uint32_t r = c.lane; r < k; r += 32) {
-            const unsigned long long key = keys[r];
-            a.out_ids[qi * k + r] = r < found ? key_id(key) : kUnusedId;
-            a.out_dists[qi * k + r] = r < found ? __uint_as_float(key_dbits(key)) : __int_as_float(0x7f800000);
-        }
-        if (c.lane == 0 && a.out_counts) a.out_counts[qi] = found;
+        warp_store_row(keys, found, k, qi, a.out_ids, a.out_dists, a.out_counts, c.lane);
         __syncwarp();  // the next query rewrites the keys
     }
 }

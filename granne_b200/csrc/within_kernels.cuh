@@ -8,11 +8,13 @@
 // The lists are CSR (offsets: nq + 1 u64, ids: offsets[nq] u32).  A call runs in query chunks of at most
 // kExactMaxChunk queries:
 //   within_segments_kernel  per query the segments of at most kWithinSegment candidates its list splits into, their
-//                           prefix over the chunk, and the offsets check; resets the chunk's locks, flags and counter
+//                           prefix over the chunk (block_exclusive_scan), and the offsets check; resets the chunk's
+//                           locks, flags and counter
 //   within_kernel           persistent warps over the chunk's segments: ids checked against Index::len, distances 32 at
-//                           a time through Dist::dists, make_key keys sorted in shared memory, duplicates dropped.  A
-//                           query of one segment writes its output row directly; the segments of a longer list merge
-//                           their keys below the query's running k-th key into its running list, under a per-query lock
+//                           a time through Dist::dists, make_key keys sorted in shared memory (key_sort by the warp),
+//                           duplicates dropped.  A query of one segment writes its output row directly (warp_store_row);
+//                           the segments of a longer list merge their keys below the query's running k-th key into its
+//                           running list (key_merge), under a per-query lock
 //   within_write_kernel     the running lists (and the empty or rejected lists) into the search_batch output layout
 // The result is the first k keys of the union of the segments' keys, and keys are unique per id, so it does not depend
 // on the order segments finish in, nor on the order or multiplicity of the ids in a list.
@@ -20,6 +22,7 @@
 
 #include "build_kernels.cuh"
 #include "exact_kernels.cuh"
+#include "keys.cuh"
 #include "rerank_kernels.cuh"
 
 namespace granne_b200 {
@@ -64,8 +67,7 @@ __global__ void __launch_bounds__(kExactMaxChunk) within_segments_kernel(const u
                                                                         int* __restrict__ qflags,
                                                                         unsigned long long* __restrict__ work_counter,
                                                                         int* __restrict__ error) {
-    __shared__ unsigned long long warp_sums[kExactMaxChunk / 32];
-    const uint32_t q = threadIdx.x, lane = q & 31, wid = q >> 5;
+    const uint32_t q = threadIdx.x;
     unsigned long long segs = 0;
     if (q < nq) {
         const unsigned long long lo = offsets[q], hi = offsets[q + 1];
@@ -75,27 +77,9 @@ __global__ void __launch_bounds__(kExactMaxChunk) within_segments_kernel(const u
         qflags[q] = bad ? kStatusBadList : 0;
         if (bad) atomicOr(error, kStatusBadList);
     }
-    // inclusive scan in the warp, then over the warp totals
-    unsigned long long v = segs;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const unsigned long long t = __shfl_up_sync(kFullMask, v, o);
-        if (lane >= (uint32_t)o) v += t;
-    }
-    if (lane == 31) warp_sums[wid] = v;
-    __syncthreads();
-    if (wid == 0) {
-        unsigned long long w = warp_sums[lane];
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const unsigned long long t = __shfl_up_sync(kFullMask, w, o);
-            if (lane >= (uint32_t)o) w += t;
-        }
-        warp_sums[lane] = w;
-    }
-    __syncthreads();
-    const unsigned long long incl = v + (wid ? warp_sums[wid - 1] : 0ull);
-    if (q < nq) seg_prefix[q + 1] = incl;
+    unsigned long long total;
+    const unsigned long long before = block_exclusive_scan(segs, &total);
+    if (q < nq) seg_prefix[q + 1] = before + segs;
     if (q == 0) {
         seg_prefix[0] = 0;
         *work_counter = 0;
@@ -120,18 +104,6 @@ __device__ __forceinline__ uint32_t warp_unique_keys(unsigned long long* keys, u
         __syncwarp();
     }
     return u;
-}
-
-// Row qi of the output: the first `found` of keys (ascending), then padding.
-__device__ __forceinline__ void within_store_row(const WithinArgs& a, uint32_t qi, const unsigned long long* keys,
-                                                 uint32_t found, int lane) {
-    const uint32_t k = a.num_neighbors;
-    for (uint32_t r = lane; r < k; r += 32) {
-        const unsigned long long key = r < found ? keys[r] : ~0ull;
-        a.out_ids[(size_t)qi * k + r] = r < found ? key_id(key) : kUnusedId;
-        a.out_dists[(size_t)qi * k + r] = r < found ? __uint_as_float(key_dbits(key)) : __int_as_float(0x7f800000);
-    }
-    if (lane == 0 && a.out_counts) a.out_counts[qi] = found;
 }
 
 template <class Dist>
@@ -175,7 +147,7 @@ __global__ void __launch_bounds__(32, 16) within_kernel(const DeviceIndex ix, co
                 atomicOr(a.error_flag, kStatusBadList);
                 if (nseg > 1) atomicOr(a.qflags + q, kStatusBadList);
             }
-            if (nseg == 1) within_store_row(a, q, keys, 0, c.lane);
+            if (nseg == 1) warp_store_row(keys, 0, k, q, a.out_ids, a.out_dists, a.out_counts, c.lane);
             continue;
         }
         if (k == 0) {  // nothing to rank: the ids are checked, no distance is computed
@@ -195,7 +167,7 @@ __global__ void __launch_bounds__(32, 16) within_kernel(const DeviceIndex ix, co
         const uint32_t p = rerank_key_slots(n);
         for (uint32_t i = n + c.lane; i < p; i += 32) keys[i] = ~0ull;
         __syncwarp();
-        warp_bitonic_sort(keys, p, c.lane);
+        key_sort(WarpGroup{c.lane}, keys, p);
         const bool nan = __any_sync(kFullMask, c.status & kStatusNotFinite);
         if (nan && c.lane == 0) {
             atomicOr(a.error_flag, kStatusNotFinite);
@@ -204,7 +176,7 @@ __global__ void __launch_bounds__(32, 16) within_kernel(const DeviceIndex ix, co
         const uint32_t u = nan ? 0u : warp_unique_keys(keys, n, c.lane);
         const uint32_t m = u < k ? u : k;
         if (nseg == 1) {
-            within_store_row(a, q, keys, m, c.lane);
+            warp_store_row(keys, m, k, q, a.out_ids, a.out_dists, a.out_counts, c.lane);
             __syncwarp();  // the next segment rewrites the keys
             continue;
         }
@@ -215,8 +187,7 @@ __global__ void __launch_bounds__(32, 16) within_kernel(const DeviceIndex ix, co
         for (uint32_t b = 0; b < m; b += 32)
             mp += __popc(__ballot_sync(kFullMask, b + c.lane < m && keys[b + c.lane] < thr));
         if (mp > 0) {
-            // keys[0, P): this segment's mp keys ascending, then ~0; keys[P, 2P): the running list descending, so that
-            // keys[0, 2P) is bitonic and log2(2P) half-cleaner steps sort it
+            // keys[0, P): this segment's mp keys ascending, then ~0; keys[P, 2P): the running list, ascending
             node_lock(a.locks, q, c.lane);
             uint32_t listed = 0;
             for (uint32_t j0 = 0; j0 < P; j0 += 32) {
@@ -224,24 +195,12 @@ __global__ void __launch_bounds__(32, 16) within_kernel(const DeviceIndex ix, co
                 const unsigned long long x = j < k ? __ldcg(list + j) : ~0ull;
                 listed += __popc(__ballot_sync(kFullMask, x != ~0ull));
                 if (j < P) {
-                    keys[2 * P - 1 - j] = x;
+                    keys[P + j] = x;
                     if (j >= mp) keys[j] = ~0ull;
                 }
             }
             __syncwarp();
-            for (uint32_t j = P; j > 0; j >>= 1) {
-                for (uint32_t i = c.lane; i < 2 * P; i += 32) {
-                    const uint32_t l = i ^ j;
-                    if (l > i) {
-                        const unsigned long long x = keys[i], y = keys[l];
-                        if (x > y) {
-                            keys[i] = y;
-                            keys[l] = x;
-                        }
-                    }
-                }
-                __syncwarp();
-            }
+            key_merge(WarpGroup{c.lane}, keys, 2 * P);
             const uint32_t merged = warp_unique_keys(keys, mp + listed, c.lane);
             for (uint32_t r = c.lane; r < k; r += 32) __stcg(list + r, r < merged ? keys[r] : ~0ull);
             __threadfence();
@@ -265,10 +224,7 @@ __global__ void within_write_kernel(const unsigned long long* __restrict__ lists
     for (uint32_t r0 = 0; r0 < k; r0 += blockDim.x) {
         const uint32_t r = r0 + threadIdx.x;
         const unsigned long long key = (ok && r < k) ? lists[(size_t)q * k + r] : ~0ull;
-        if (r < k) {
-            out_ids[(size_t)q * k + r] = key != ~0ull ? key_id(key) : kUnusedId;
-            out_dists[(size_t)q * k + r] = key != ~0ull ? __uint_as_float(key_dbits(key)) : __int_as_float(0x7f800000);
-        }
+        if (r < k) store_key(out_ids, out_dists, (size_t)q * k + r, key, key != ~0ull);
         found += __syncthreads_count(key != ~0ull);
     }
     if (threadIdx.x == 0 && out_counts) out_counts[q] = found;
