@@ -18,6 +18,19 @@ def random_sum_embeddings(go, dim, num_embeddings, num_elements, seed):
     return go.Elements.sum_embeddings(emb, elements)
 
 
+def varied_sum_embeddings(go, dim, num_embeddings, num_elements, seed, special=((7, 0), (13, 1), (19, 33), (24, 70))):
+    """Sum-of-embeddings elements whose term lists are drawn at random with repetition (a term can occur more than
+    once), 2 to 9 terms each, except that element i has exactly m terms when (i % 25, m) is in `special`: by default
+    elements without terms (zero vectors), of one term, and of more than 32 and 64 terms (more than one and two warp
+    widths of term ids)."""
+    rng = np.random.default_rng(seed)
+    emb = random_vectors(num_embeddings, dim, seed)
+    lengths = dict(special)
+    lists = [rng.integers(0, num_embeddings, size=lengths.get(i % 25, int(rng.integers(2, 10)))).tolist()
+             for i in range(num_elements)]
+    return go.Elements.sum_embeddings(emb, lists)
+
+
 def clustered_vectors(n, dim, seed, n_centers=None, sub_dim=16, spread=0.3):
     """Measurement distribution (SURVEY.md §8d): Gaussian mixture on a random low-dimensional subspace."""
     rng = np.random.default_rng(seed)
