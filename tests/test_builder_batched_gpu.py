@@ -18,20 +18,13 @@ import pytest
 
 import granne_b200
 from helpers.data import clustered_vectors, random_sum_embeddings, random_vectors
+from helpers.fixtures import library  # noqa: F401  (autouse)
 from helpers.index_image import assert_same_index
 
 pytestmark = pytest.mark.gpu
 
 DEFAULT_MAX_BATCH = 4096  # the builder's largest insertion batch when GRANNE_B200_BUILD_MAX_BATCH is unset
 THREADS = max(1, min(16, os.cpu_count() or 1))  # the model's searches of one batch; its image does not depend on it
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _lib():
-    from granne_b200 import build
-
-    build.build()
-    granne_b200.load_library()
 
 
 @pytest.fixture(autouse=True)

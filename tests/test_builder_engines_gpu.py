@@ -24,6 +24,7 @@ import pytest
 
 import granne_b200
 from helpers.data import (clustered_vectors, edge_i8_rows, edge_raw_f32, random_vectors, varied_sum_embeddings)
+from helpers.fixtures import library  # noqa: F401  (autouse)
 from helpers.index_image import assert_same_index
 
 pytestmark = pytest.mark.gpu
@@ -60,14 +61,6 @@ SEQUENTIAL = [
     ("embeddings", 300, 1000, NARROW, ("DistSum", "several passes")),
     ("embeddings", 4096, 300, WIDE, ("DistSum", "several passes")),       # 32 passes of 128 floats
 ]
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _lib():
-    from granne_b200 import build
-
-    build.build()
-    granne_b200.load_library()
 
 
 @pytest.fixture(autouse=True)

@@ -10,17 +10,10 @@ import pytest
 
 import granne_b200
 from helpers.data import random_sum_embeddings, random_vectors
+from helpers.fixtures import library  # noqa: F401  (autouse)
 from helpers.index_image import assert_same_index
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _lib():
-    from granne_b200 import build
-
-    build.build()
-    granne_b200.load_library()
 
 
 @pytest.fixture(autouse=True)

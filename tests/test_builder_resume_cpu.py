@@ -12,21 +12,15 @@ import pytest
 import granne_b200
 from granne_b200 import api
 from helpers.data import build_fixture, index_from_lists
+from helpers.fixtures import compile_cxx_client
+from helpers.fixtures import library  # noqa: F401  (autouse)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 OK, INVALID, FORMAT, NO_DEVICE = 0, -1, -2, -5
 
 
 @pytest.fixture(scope="module")
-def lib():
-    from granne_b200 import build
-
-    build.build()
-    return granne_b200.load_library()
-
-
-@pytest.fixture(scope="module")
-def fixture(lib, oracle):
+def fixture(library, oracle):
     el, g, index_bytes, elements_bytes, _ = build_fixture(oracle, "angular", 300, 8, seed=21, num_neighbors=10,
                                                           max_search=20)
     assert g.num_layers() >= 2
@@ -52,51 +46,52 @@ def from_index(lib, index_bytes, elements_bytes, kind=api.ANGULAR, **cfg):
     return rc, h
 
 
-def test_truncated_or_corrupted_images_are_format_errors(lib, fixture):
+def test_truncated_or_corrupted_images_are_format_errors(library, fixture):
     index_bytes, elements_bytes = fixture
     garbled = bytearray(index_bytes)
     garbled[1024 + 8:1024 + 40] = b"\xff" * 32  # the first layer's offset chunk
     for bad in [b"", b"granne", index_bytes[:1024], index_bytes[:-7], index_bytes[:len(index_bytes) // 2],
                 b"grannf" + index_bytes[6:], b"granne{not json".ljust(1024, b" ") + index_bytes[1024:],
                 bytes(garbled)]:
-        rc, h = from_index(lib, bad, elements_bytes)
+        rc, h = from_index(library, bad, elements_bytes)
         assert rc == FORMAT and not h.value, (bad[:16], len(bad), rc)
-        assert lib.granne_b200_last_error()
+        assert library.granne_b200_last_error()
 
 
-def test_too_many_layers_is_a_format_error(lib, oracle, fixture):
+def test_too_many_layers_is_a_format_error(library, oracle, fixture):
     _, elements_bytes = fixture
     image = index_from_lists(oracle, [[[]]] * 25)  # 25 one-node layers; the builder holds at most 24
     assert len(api.inspect_index(image)) == 25
-    rc, h = from_index(lib, image, elements_bytes)
+    rc, h = from_index(library, image, elements_bytes)
     assert rc == FORMAT and not h.value
-    assert "layers" in lib.granne_b200_last_error().decode()
+    assert "layers" in library.granne_b200_last_error().decode()
 
 
 @pytest.mark.parametrize("m", [0, 256])
-def test_num_neighbors_outside_the_format_is_rejected(lib, fixture, m):
+def test_num_neighbors_outside_the_format_is_rejected(library, fixture, m):
     index_bytes, elements_bytes = fixture
-    rc, h = from_index(lib, index_bytes, elements_bytes, num_neighbors=m)
+    rc, h = from_index(library, index_bytes, elements_bytes, num_neighbors=m)
     assert rc == INVALID and not h.value
-    assert "num_neighbors" in lib.granne_b200_last_error().decode()
+    assert "num_neighbors" in library.granne_b200_last_error().decode()
 
 
-def test_null_arguments_are_rejected(lib, fixture):
+def test_null_arguments_are_rejected(library, fixture):
     index_bytes, elements_bytes = fixture
     c = api._build_config(30, 200, 15.0, True, None)
     h = C.c_void_p()
-    assert lib.granne_b200_builder_from_index(C.byref(c), None, 0, 0, None, 0, None, 0, 0, C.byref(h)) == INVALID
+    assert library.granne_b200_builder_from_index(C.byref(c), None, 0, 0, None, 0, None, 0, 0, C.byref(h)) == INVALID
     ib = np.frombuffer(index_bytes, dtype=np.uint8)
-    assert lib.granne_b200_builder_from_index(None, api._ptr(ib), ib.size, 0, None, 0, None, 0, 0, C.byref(h)) == INVALID
-    assert lib.granne_b200_builder_from_index_device_elements(C.byref(c), api._ptr(ib), ib.size, 0, None, 10, 8, 0,
-                                                              C.byref(h)) == INVALID
+    assert library.granne_b200_builder_from_index(None, api._ptr(ib), ib.size, 0, None, 0, None, 0, 0,
+                                                  C.byref(h)) == INVALID
+    assert library.granne_b200_builder_from_index_device_elements(C.byref(c), api._ptr(ib), ib.size, 0, None, 10, 8, 0,
+                                                                  C.byref(h)) == INVALID
     assert not h.value
 
 
-def test_a_valid_image_reaches_the_device_check(lib, fixture):
+def test_a_valid_image_reaches_the_device_check(library, fixture):
     _no_gpu()
     index_bytes, elements_bytes = fixture
-    rc, h = from_index(lib, index_bytes, elements_bytes, num_neighbors=5)
+    rc, h = from_index(library, index_bytes, elements_bytes, num_neighbors=5)
     assert rc == NO_DEVICE and not h.value
     with pytest.raises(granne_b200.GranneError) as ei:
         granne_b200.GranneBuilder("angular", elements_bytes, index_bytes=index_bytes)
@@ -121,7 +116,7 @@ def test_from_files_rejects_incomplete_arguments(tmp_path, fixture, monkeypatch)
         granne_b200.GranneBuilder.from_files("bogus", str(tmp_path / "elements"))
 
 
-def test_from_files_reaches_the_library(lib, tmp_path, fixture):
+def test_from_files_reaches_the_library(library, tmp_path, fixture):
     _no_gpu()
     index_bytes, elements_bytes = fixture
     (tmp_path / "index").write_bytes(index_bytes)
@@ -136,26 +131,9 @@ def test_from_files_reaches_the_library(lib, tmp_path, fixture):
     assert ei.value.code == FORMAT
 
 
-def build_resume_client(out_dir):
-    """Compiles tests/helpers/cxx_resume_client.cpp against include/granne_b200.hpp and the library."""
-    import shutil
-
-    from granne_b200 import build
-
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    build.build()
-    libdir = os.path.dirname(granne_b200.library_path())
-    exe = os.path.join(str(out_dir), "cxx_resume_client")
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-Wall", "-Wextra", "-Werror", "-I" + os.path.join(ROOT, "include"),
-                           os.path.join(ROOT, "tests", "helpers", "cxx_resume_client.cpp"), "-o", exe,
-                           "-L" + libdir, "-lgranne_b200", "-Wl,-rpath," + libdir])
-    return exe
-
-
-def test_cxx_from_bytes_reports_statuses_without_a_device(lib, tmp_path, fixture):
+def test_cxx_from_bytes_reports_statuses_without_a_device(library, tmp_path, fixture):
     _no_gpu()
-    exe = build_resume_client(tmp_path)
+    exe = compile_cxx_client("cxx_resume_client.cpp", tmp_path)
     index_bytes, elements_bytes = fixture
     (tmp_path / "index").write_bytes(index_bytes)
     (tmp_path / "elements").write_bytes(elements_bytes)

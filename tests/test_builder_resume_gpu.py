@@ -22,20 +22,14 @@ import pytest
 
 import granne_b200
 from helpers.data import random_sum_embeddings, random_vectors
+from helpers.fixtures import compile_cxx_client
+from helpers.fixtures import library  # noqa: F401  (autouse)
 from helpers.index_image import assert_same_index
 
 pytestmark = pytest.mark.gpu
 
 THREADS = max(1, min(16, os.cpu_count() or 1))  # the oracle's searches of one batch; its image does not depend on it
 INVALID, FORMAT = -1, -2
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _lib():
-    from granne_b200 import build
-
-    build.build()
-    granne_b200.load_library()
 
 
 @pytest.fixture(autouse=True)
@@ -400,9 +394,7 @@ def test_errors_are_statuses_and_leave_the_device_usable(oracle):
 
 # ---- the C++ mirror: read_index_reduce_num_neighbors (tests.rs:243-290) ------------------------------------------
 def test_cxx_read_index_reduce_num_neighbors(oracle, tmp_path):
-    from test_builder_resume_cpu import build_resume_client
-
-    exe = build_resume_client(tmp_path)
+    exe = compile_cxx_client("cxx_resume_client.cpp", tmp_path)
     el = oracle.Elements.angular(random_vectors(1000, 5, seed=11))
     (tmp_path / "elements").write_bytes(el.to_bytes(0))
     env = dict(os.environ, GRANNE_B200_BUILD_MAX_BATCH="1")

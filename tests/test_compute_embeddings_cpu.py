@@ -8,27 +8,20 @@ import pytest
 
 import granne_b200
 from granne_b200 import api
-from helpers import embeddings_oracle as eo
+from helpers import composed_oracle as co
+from helpers.fixtures import library  # noqa: F401  (autouse)
 
 OK, INVALID, FORMAT, NO_DEVICE = 0, -1, -2, -5
 
 
-@pytest.fixture(scope="module")
-def lib():
-    from granne_b200 import build
-
-    build.build()
-    return granne_b200.load_library()
-
-
 def test_oracle_known_answer():
-    table = eo.table_image([[1, 2, -3], [0.5, 0, 1]])
-    el = eo.elements_image([[0, 1], [], [1]])
-    img = eo.compute_embeddings("angular_int", el, table)
+    table = co.table_image([[1, 2, -3], [0.5, 0, 1]])
+    el = co.elements_image([[0, 1], [], [1]])
+    img = co.compute_embeddings("angular_int", el, table)
     # [1.5, 2, -2] * 127 / 2 -> 95.25, 127, -127;  [] -> zeros;  [0.5, 0, 1] * 127 / 1 -> 63.5, 0, 127
     want = np.uint64(3).tobytes() + np.array([95, 127, -127, 0, 0, 0, 63, 0, 127], dtype=np.int8).tobytes()
     assert img.tobytes() == want
-    ang = np.frombuffer(eo.compute_embeddings("angular", el, table)[8:].tobytes(), dtype=np.float32).reshape(3, 3)
+    ang = np.frombuffer(co.compute_embeddings("angular", el, table)[8:].tobytes(), dtype=np.float32).reshape(3, 3)
     assert np.array_equal(ang[1], np.zeros(3, np.float32))
 
 
@@ -75,26 +68,26 @@ def test_oracle_matches_numpy(oracle, seed):
         elements.append([int(t) for t in rng.integers(0, m, c)])
     if n > 3 and m > 3:
         elements[1], elements[2], elements[3] = [0], [1, 2], [3, 3]
-    ti, ei = eo.table_image(table), eo.elements_image(elements)
+    ti, ei = co.table_image(table), co.elements_image(elements)
     for kind in ("angular_int", "angular"):
-        img = eo.compute_embeddings(kind, ei, ti, threads=3)
+        img = co.compute_embeddings(kind, ei, ti, threads=3)
         assert img.tobytes() == _numpy_image(kind, table, elements, oracle.normalize_f32), (kind, seed)
     if n > 3 and m > 3:
-        row = np.frombuffer(eo.compute_embeddings("angular", ei, ti)[8 + 4 * dim: 8 + 8 * dim].tobytes(), np.float32)
+        row = np.frombuffer(co.compute_embeddings("angular", ei, ti)[8 + 4 * dim: 8 + 8 * dim].tobytes(), np.float32)
         assert np.array_equal(np.signbit(row), np.ones(dim, bool))  # -0.0 / 0 norm: the row is kept
 
 
 def test_oracle_empty_cases():
-    table = eo.table_image(np.ones((4, 5), np.float32))
-    assert eo.compute_embeddings("angular_int", eo.elements_image([]), table).tobytes() == bytes(8)
+    table = co.table_image(np.ones((4, 5), np.float32))
+    assert co.compute_embeddings("angular_int", co.elements_image([]), table).tobytes() == bytes(8)
     empty_table = np.uint64(5).tobytes()  # width 5, no rows
-    assert eo.compute_embeddings("angular", eo.elements_image([[], []]), empty_table).tobytes() == bytes(8)
-    with pytest.raises(eo.NotFinite):
-        eo.compute_embeddings("angular_int", eo.elements_image([[0]]), eo.table_image([[np.nan, 1.0]]))
-    with pytest.raises(eo.NotFinite):
-        eo.compute_embeddings("angular", eo.elements_image([[0, 0]]), eo.table_image([[3e38, 1.0]]))
+    assert co.compute_embeddings("angular", co.elements_image([[], []]), empty_table).tobytes() == bytes(8)
+    with pytest.raises(co.NotFinite):
+        co.compute_embeddings("angular_int", co.elements_image([[0]]), co.table_image([[np.nan, 1.0]]))
+    with pytest.raises(co.NotFinite):
+        co.compute_embeddings("angular", co.elements_image([[0, 0]]), co.table_image([[3e38, 1.0]]))
     # +inf in an angular_int sum quantises like the reference: inf/inf and finite/inf give 0
-    img = eo.compute_embeddings("angular_int", eo.elements_image([[0, 0]]), eo.table_image([[3e38, 1.0]]))
+    img = co.compute_embeddings("angular_int", co.elements_image([[0, 0]]), co.table_image([[3e38, 1.0]]))
     assert img.tobytes() == np.uint64(2).tobytes() + bytes(2)
 
 
@@ -117,75 +110,75 @@ def _call_device(lib, kind, el, emb, d_out=None):
     return rc, n.value, dim.value
 
 
-TABLE = eo.table_image(np.arange(12, dtype=np.float32).reshape(4, 3))
-ELEMENTS = eo.elements_image([[0, 1], [], [3, 3, 2]])
+TABLE = co.table_image(np.arange(12, dtype=np.float32).reshape(4, 3))
+ELEMENTS = co.elements_image([[0, 1], [], [3, 3, 2]])
 
 
 @pytest.mark.parametrize("cut", [0, 4, 7, 8, 12, 20, 23])
-def test_truncated_images_are_format_errors(lib, cut):
-    assert _call(lib, 1, ELEMENTS[:cut], TABLE)[0] == FORMAT
-    assert _call_device(lib, 0, ELEMENTS[:cut], TABLE)[0] == FORMAT
+def test_truncated_images_are_format_errors(library, cut):
+    assert _call(library, 1, ELEMENTS[:cut], TABLE)[0] == FORMAT
+    assert _call_device(library, 0, ELEMENTS[:cut], TABLE)[0] == FORMAT
     if cut < len(TABLE) and (cut < 8 or (cut - 8) % 12):
-        assert _call(lib, 0, ELEMENTS, TABLE[:max(cut, 3)])[0] == FORMAT
+        assert _call(library, 0, ELEMENTS, TABLE[:max(cut, 3)])[0] == FORMAT
 
 
-def test_format_errors(lib):
+def test_format_errors(library):
     width0 = np.uint64(0).tobytes() + bytes(12)
-    assert _call(lib, 1, ELEMENTS, width0)[0] == FORMAT
-    assert _call(lib, 1, eo.elements_image([[0], [4]]), TABLE)[0] == FORMAT  # id 4 >= 4 rows
-    assert _call(lib, 0, eo.elements_image([[0xFFFFFF]]), TABLE)[0] == FORMAT
-    assert _call_device(lib, 1, eo.elements_image([[0xFFFFFF]]), TABLE)[0] == FORMAT
-    assert _call(lib, 1, eo.elements_image([[0]]), np.uint64(1).tobytes())[0] == FORMAT  # a table without rows
-    assert "missing embedding id" in lib.granne_b200_last_error().decode()
+    assert _call(library, 1, ELEMENTS, width0)[0] == FORMAT
+    assert _call(library, 1, co.elements_image([[0], [4]]), TABLE)[0] == FORMAT  # id 4 >= 4 rows
+    assert _call(library, 0, co.elements_image([[0xFFFFFF]]), TABLE)[0] == FORMAT
+    assert _call_device(library, 1, co.elements_image([[0xFFFFFF]]), TABLE)[0] == FORMAT
+    assert _call(library, 1, co.elements_image([[0]]), np.uint64(1).tobytes())[0] == FORMAT  # a table without rows
+    assert "missing embedding id" in library.granne_b200_last_error().decode()
     # the table loader's rule: a width wider than the payload is malformed, so only width 1 can have no rows
-    assert _call(lib, 1, eo.elements_image([[]]), np.uint64(3).tobytes())[0] == FORMAT
+    assert _call(library, 1, co.elements_image([[]]), np.uint64(3).tobytes())[0] == FORMAT
 
 
-def test_invalid_arguments(lib):
+def test_invalid_arguments(library):
     for kind in (2, -1, 3):
-        assert _call(lib, kind, ELEMENTS, TABLE)[0] == INVALID
-        assert _call_device(lib, kind, ELEMENTS, TABLE)[0] == INVALID
-    assert _call(lib, 1, None, TABLE)[0] == INVALID
-    assert _call(lib, 1, ELEMENTS, None)[0] == INVALID
-    assert _call(lib, 1, ELEMENTS, TABLE, use_len=False)[0] == INVALID
+        assert _call(library, kind, ELEMENTS, TABLE)[0] == INVALID
+        assert _call_device(library, kind, ELEMENTS, TABLE)[0] == INVALID
+    assert _call(library, 1, None, TABLE)[0] == INVALID
+    assert _call(library, 1, ELEMENTS, None)[0] == INVALID
+    assert _call(library, 1, ELEMENTS, TABLE, use_len=False)[0] == INVALID
     eb, mb = np.frombuffer(ELEMENTS, np.uint8), np.frombuffer(TABLE, np.uint8)
-    assert lib.granne_b200_compute_embeddings_device(1, api._ptr(eb), eb.size, api._ptr(mb), mb.size, 0, None, None,
-                                                     None, None) == INVALID
-    wide = eo.table_image(np.zeros((2, 4097), np.float32))
-    assert _call(lib, 1, eo.elements_image([[1]]), wide)[0] == INVALID
-    assert _call_device(lib, 0, eo.elements_image([[1]]), wide)[0] == INVALID
+    assert library.granne_b200_compute_embeddings_device(1, api._ptr(eb), eb.size, api._ptr(mb), mb.size, 0, None, None,
+                                                         None, None) == INVALID
+    wide = co.table_image(np.zeros((2, 4097), np.float32))
+    assert _call(library, 1, co.elements_image([[1]]), wide)[0] == INVALID
+    assert _call_device(library, 0, co.elements_image([[1]]), wide)[0] == INVALID
     buf = np.zeros(64, np.uint8)
-    rc, need = _call(lib, 1, ELEMENTS, TABLE, out=api._ptr(buf), cap=8 + 9 - 1)
+    rc, need = _call(library, 1, ELEMENTS, TABLE, out=api._ptr(buf), cap=8 + 9 - 1)
     assert rc == INVALID and need == 8 + 9
-    assert _call(lib, 1, ELEMENTS, TABLE, out=api._ptr(buf), cap=0)[0] == INVALID
+    assert _call(library, 1, ELEMENTS, TABLE, out=api._ptr(buf), cap=0)[0] == INVALID
 
 
-def test_size_queries_need_no_device(lib):
-    assert _call(lib, 1, ELEMENTS, TABLE) == (OK, 8 + 3 * 3)
-    assert _call(lib, 0, ELEMENTS, TABLE) == (OK, 8 + 3 * 3 * 4)
-    assert _call_device(lib, 0, ELEMENTS, TABLE) == (OK, 3, 3)
-    big = eo.elements_image([[i % 4] for i in range(1000)])
-    assert _call(lib, 0, big, TABLE) == (OK, 8 + 1000 * 3 * 4)
-    assert _call(lib, 1, eo.elements_image([]), TABLE) == (OK, 8)
-    assert _call(lib, 1, eo.elements_image([[], []]), np.uint64(1).tobytes()) == (OK, 8)
-    assert _call_device(lib, 1, eo.elements_image([[], []]), np.uint64(1).tobytes()) == (OK, 2, 0)
+def test_size_queries_need_no_device(library):
+    assert _call(library, 1, ELEMENTS, TABLE) == (OK, 8 + 3 * 3)
+    assert _call(library, 0, ELEMENTS, TABLE) == (OK, 8 + 3 * 3 * 4)
+    assert _call_device(library, 0, ELEMENTS, TABLE) == (OK, 3, 3)
+    big = co.elements_image([[i % 4] for i in range(1000)])
+    assert _call(library, 0, big, TABLE) == (OK, 8 + 1000 * 3 * 4)
+    assert _call(library, 1, co.elements_image([]), TABLE) == (OK, 8)
+    assert _call(library, 1, co.elements_image([[], []]), np.uint64(1).tobytes()) == (OK, 8)
+    assert _call_device(library, 1, co.elements_image([[], []]), np.uint64(1).tobytes()) == (OK, 2, 0)
 
 
-def test_valid_input_without_a_device(lib):
+def test_valid_input_without_a_device(library):
     import torch
 
     if torch.cuda.is_available():
         pytest.skip("a device is present")
     buf = np.zeros(64, np.uint8)
-    assert _call(lib, 1, ELEMENTS, TABLE, out=api._ptr(buf), cap=buf.size)[0] == NO_DEVICE
-    assert _call(lib, 0, eo.elements_image([]), TABLE, out=api._ptr(buf), cap=buf.size)[0] == NO_DEVICE
-    assert _call_device(lib, 1, ELEMENTS, TABLE, d_out=api._ptr(buf))[0] == NO_DEVICE
+    assert _call(library, 1, ELEMENTS, TABLE, out=api._ptr(buf), cap=buf.size)[0] == NO_DEVICE
+    assert _call(library, 0, co.elements_image([]), TABLE, out=api._ptr(buf), cap=buf.size)[0] == NO_DEVICE
+    assert _call_device(library, 1, ELEMENTS, TABLE, d_out=api._ptr(buf))[0] == NO_DEVICE
     with pytest.raises(granne_b200.GranneError) as e:
         granne_b200.compute_embeddings("angular_int", ELEMENTS, TABLE)
     assert e.value.code == NO_DEVICE
 
 
-def test_python_argument_checks(lib, tmp_path):
+def test_python_argument_checks(library, tmp_path):
     for bad in ("embeddings", "nope"):
         with pytest.raises(ValueError):
             granne_b200.compute_embeddings(bad, ELEMENTS, TABLE)
@@ -202,7 +195,7 @@ def test_python_argument_checks(lib, tmp_path):
     with pytest.raises(granne_b200.GranneError) as e:
         granne_b200.compute_embeddings("angular", ELEMENTS[:9], TABLE)
     assert e.value.code == FORMAT
-    (tmp_path / "el").write_bytes(eo.elements_image([[9]]))
+    (tmp_path / "el").write_bytes(co.elements_image([[9]]))
     (tmp_path / "emb").write_bytes(TABLE)
     with pytest.raises(granne_b200.GranneError) as e:
         granne_b200.compute_embeddings_and_save_to_disk(str(tmp_path / "el"), str(tmp_path / "emb"),

@@ -1,33 +1,17 @@
 """include/granne_b200.hpp (the C++ mirror of granne's Rust API) compiles warning-free, links against the C ABI
 library and, without a GPU, fails loudly with GRANNE_B200_ERR_NO_DEVICE instead of falling back to the CPU."""
-import os
-import shutil
 import subprocess
 
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def build_client(out_dir):
-    import granne_b200
-    from granne_b200 import build
-
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    build.build()
-    libdir = os.path.dirname(granne_b200.library_path())
-    exe = os.path.join(str(out_dir), "cxx_client")
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-Wall", "-Wextra", "-Werror", "-I" + os.path.join(ROOT, "include"),
-                           os.path.join(ROOT, "tests", "helpers", "cxx_client.cpp"), "-o", exe, "-L" + libdir,
-                           "-lgranne_b200", "-Wl,-rpath," + libdir])
-    return exe
+from helpers.fixtures import compile_cxx_client
+from helpers.fixtures import library  # noqa: F401  (autouse)
 
 
 def test_cxx_header_compiles_and_has_no_cpu_fallback(tmp_path):
     import torch
 
-    exe = build_client(tmp_path)
+    exe = compile_cxx_client("cxx_client.cpp", tmp_path)
     if torch.cuda.is_available():
         pytest.skip("GPU present: the no-device path cannot be exercised")
     r = subprocess.run([exe, "nodevice"], capture_output=True, text=True, timeout=120)

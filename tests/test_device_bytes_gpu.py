@@ -11,19 +11,12 @@ import pytest
 
 import granne_b200
 from granne_b200 import words
+from helpers.fixtures import library  # noqa: F401  (autouse)
 
 pytestmark = pytest.mark.gpu
 
 GOLDEN = sorted(glob.glob(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "*.npz")))
 M = 12  # the builders' num_neighbors: stride 16, wider than the rows the builder keeps
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _lib():
-    from granne_b200 import build
-
-    build.build()
-    granne_b200.load_library()
 
 
 def _alloc(nbytes):

@@ -11,22 +11,10 @@ import pytest
 
 import granne_b200
 from helpers.data import random_vectors
+from helpers.fixtures import assert_same
+from helpers.fixtures import library  # noqa: F401  (autouse)
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _lib():
-    from granne_b200 import build
-
-    build.build()
-    granne_b200.load_library()
-
-
-def _same(a, b, what):
-    for x, y, name in zip(a[:3], b[:3], ("ids", "dists", "counts")):
-        assert np.array_equal(np.asarray(x).view(np.uint32), np.asarray(y).view(np.uint32)), what + " " + name
-    assert np.array_equal(a[3][:, :3], b[3][:, :3]), what + " counters"
 
 
 @pytest.mark.parametrize("kind,n,dim", [("angular", 6000, 64), ("angular_int", 4000, 100), ("angular", 3000, 28)])
@@ -51,12 +39,12 @@ def test_device_resident_elements_equal_the_file_image_path(oracle, kind, n, dim
     got_dev = from_dev.search_batch(q, 50, 10, with_stats=True)
     got_img = from_img.search_batch(q, 50, 10, with_stats=True)
     got_built = built.search_batch(q, 50, 10, with_stats=True)
-    _same(got_dev, got_img, "device vs image")
-    _same(got_dev, got_built, "device vs builder snapshot")
+    assert_same(got_dev, got_img, "device vs image", stats=True)
+    assert_same(got_dev, got_built, "device vs builder snapshot", stats=True)
     # and against the oracle on the very same files
     g = oracle.Granne.from_bytes(index_bytes, oracle.Elements.from_bytes(kind, image))
     ref = g.search_batch(q, 50, 10, with_stats=True)
-    _same(ref, got_dev, "oracle vs device")
+    assert_same(ref, got_dev, "oracle vs device", stats=True)
     assert np.array_equal(from_dev.get_element(17), from_img.get_element(17))
     for h in (from_dev, from_img, built):
         h.close()
@@ -132,11 +120,11 @@ def test_retry_pass_serves_heavy_queries_exactly(oracle):
     q = random_vectors(3000, 48, seed=42)
     ref = ref_index.search_batch(q, 60, 10, with_stats=True)
     got = p.search_batch(q, 60, 10, with_stats=True)
-    _same(ref, got, "first batch")
+    assert_same(ref, got, "first batch", stats=True)
     first = int((got[3][:, 3] != 0).sum())
     for _ in range(4):  # the scale adapts between calls (the counter is read back without synchronising)
         got = p.search_batch(q, 60, 10, with_stats=True)
-        _same(ref, got, "later batch")
+        assert_same(ref, got, "later batch", stats=True)
     later = int((got[3][:, 3] != 0).sum())
     assert (got[3][:, 3] <= 1).all(), "nobody should need the 4-CTA slow pass here"
     if first > 30:

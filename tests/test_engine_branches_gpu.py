@@ -9,21 +9,13 @@ embeddings use DistSum (128 floats per pass, 32 terms per id load)."""
 import numpy as np
 import pytest
 
-import granne_b200
 from helpers.data import random_vectors
+from helpers.fixtures import library  # noqa: F401  (autouse)
 from test_parity_gpu import assert_parity, open_product, run_both
 
 pytestmark = pytest.mark.gpu
 
 GENERIC_STAGED_MAX_CHUNKS = 64  # DistF32Generic stages rows of <= 64 32-float chunks; wider rows load directly
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _lib():
-    from granne_b200 import build
-
-    build.build()
-    granne_b200.load_library()
 
 
 def _index(oracle, el, m=20, ef=30):

@@ -4,14 +4,14 @@ C++ header and the Rust shim, and the Python checks that run before any library 
 handle's Index::len (filter_words) and the host check of query_filter are checked in test_exact_filtered_gpu.py."""
 import ctypes as C
 import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
 import granne_b200
 from granne_b200 import api
+from helpers.fixtures import compile_cxx_client
+from helpers.fixtures import library  # noqa: F401  (autouse)
 
 INVALID = -1
 FAKE = C.c_void_p(1)  # never dereferenced by a call whose arguments break a rule
@@ -27,14 +27,6 @@ FILTERS = "filters is null or num_filters is 0"
 EXCLUDE_K = "num_neighbors exceeds 1023 with GRANNE_B200_QUERY_ID_EXCLUDING (the call runs k + 1)"
 NAMES = ["granne_b200_exact_search_filtered_batch", "granne_b200_exact_search_filtered_batch_device",
          "granne_b200_multi_exact_search_filtered_batch"]
-
-
-@pytest.fixture(scope="module")
-def lib():
-    from granne_b200 import build
-
-    build.build()
-    return granne_b200.load_library()
 
 
 def _call(lib, which="host", handle=FAKE, q=True, nq=2, fmt=api.QUERY_RAW_F32, k=10, out=True, filters=True,
@@ -60,60 +52,60 @@ def _call(lib, which="host", handle=FAKE, q=True, nq=2, fmt=api.QUERY_RAW_F32, k
 
 
 @pytest.mark.parametrize("which", ["host", "device"])
-def test_each_rule(lib, which):
-    assert _call(lib, which, handle=None) == (INVALID, HANDLE)
-    assert _call(lib, which, fmt=7) == (INVALID, FORMAT)
-    assert _call(lib, which, k=1025) == (INVALID, EXACT_K)
-    assert _call(lib, which, nq=TOO_MANY) == (INVALID, NQ)
-    assert _call(lib, which, q=False) == (INVALID, NULL)
-    assert _call(lib, which, out=False) == (INVALID, NULL)
-    assert _call(lib, which, filters=False) == (INVALID, FILTERS)
-    assert _call(lib, which, num_filters=0) == (INVALID, FILTERS)
-    assert _call(lib, which, fmt=api.QUERY_ID_EXCLUDING, k=1024, filters=False) == (INVALID, FILTERS)
-    assert _call(lib, which, fmt=api.QUERY_ID_EXCLUDING, k=1024) == (INVALID, EXCLUDE_K)
+def test_each_rule(library, which):
+    assert _call(library, which, handle=None) == (INVALID, HANDLE)
+    assert _call(library, which, fmt=7) == (INVALID, FORMAT)
+    assert _call(library, which, k=1025) == (INVALID, EXACT_K)
+    assert _call(library, which, nq=TOO_MANY) == (INVALID, NQ)
+    assert _call(library, which, q=False) == (INVALID, NULL)
+    assert _call(library, which, out=False) == (INVALID, NULL)
+    assert _call(library, which, filters=False) == (INVALID, FILTERS)
+    assert _call(library, which, num_filters=0) == (INVALID, FILTERS)
+    assert _call(library, which, fmt=api.QUERY_ID_EXCLUDING, k=1024, filters=False) == (INVALID, FILTERS)
+    assert _call(library, which, fmt=api.QUERY_ID_EXCLUDING, k=1024) == (INVALID, EXCLUDE_K)
 
 
 @pytest.mark.parametrize("which", ["host", "device"])
-def test_rule_order(lib, which):
+def test_rule_order(library, which):
     everything = dict(handle=None, fmt=7, k=1025, nq=TOO_MANY, q=False, out=False, filters=False)
     order = [("handle", HANDLE), ("fmt", FORMAT), ("k", EXACT_K), ("nq", NQ), ("q", NULL), ("out", NULL),
              ("filters", FILTERS)]
     for i, (_, msg) in enumerate(order):
         broken = {name: everything[name] for name, _ in order[i:]}
-        assert _call(lib, which, **broken) == (INVALID, msg), broken
+        assert _call(library, which, **broken) == (INVALID, msg), broken
 
 
 @pytest.mark.parametrize("which", ["host", "device"])
-def test_every_query_format_passes_the_format_rule(lib, which):
+def test_every_query_format_passes_the_format_rule(library, which):
     for fmt in (api.QUERY_RAW_F32, api.QUERY_ELEMENT, api.QUERY_ID, api.QUERY_ID_EXCLUDING):
-        assert _call(lib, which, fmt=fmt, filters=False) == (INVALID, FILTERS)
+        assert _call(library, which, fmt=fmt, filters=False) == (INVALID, FILTERS)
 
 
 @pytest.mark.parametrize("which", ["host", "device"])
-def test_no_queries_is_ok_before_the_filters_and_the_handle_are_read(lib, which):
-    assert _call(lib, which, nq=0, q=False, out=False, filters=False, num_filters=0)[0] == 0
-    assert _call(lib, which, nq=0, k=0, q=False, out=False, filters=False)[0] == 0
+def test_no_queries_is_ok_before_the_filters_and_the_handle_are_read(library, which):
+    assert _call(library, which, nq=0, q=False, out=False, filters=False, num_filters=0)[0] == 0
+    assert _call(library, which, nq=0, k=0, q=False, out=False, filters=False)[0] == 0
 
 
-def test_k_zero_needs_no_output_buffers(lib):
+def test_k_zero_needs_no_output_buffers(library):
     # k == 0 writes no entry: null ids / dists break no rule, the call goes on to the filters' rule
-    assert _call(lib, "host", k=0, out=False, filters=False) == (INVALID, FILTERS)
+    assert _call(library, "host", k=0, out=False, filters=False) == (INVALID, FILTERS)
 
 
-def test_multi_null_handle_first(lib):
+def test_multi_null_handle_first(library):
     # before every single-device rule (those follow on a real handle: test_exact_filtered_gpu.py)
-    assert _call(lib, "multi", handle=None, fmt=7, k=1025, filters=False) == (INVALID, "multi handle is null")
-    assert _call(lib, "multi", handle=None, nq=0) == (INVALID, "multi handle is null")
+    assert _call(library, "multi", handle=None, fmt=7, k=1025, filters=False) == (INVALID, "multi handle is null")
+    assert _call(library, "multi", handle=None, nq=0) == (INVALID, "multi handle is null")
 
 
-def test_symbols_in_the_headers_and_the_shim(lib):
+def test_symbols_in_the_headers_and_the_shim(library):
     header = open(os.path.join(ROOT, "include", "granne_b200.h")).read()
     raw = C.CDLL(granne_b200.library_path())
     for name in NAMES:
         assert "int %s(" % name in header
         assert hasattr(raw, name)
     assert "#define GRANNE_B200_ABI_VERSION 2 " in header
-    assert lib.granne_b200_abi_version() == 2
+    assert library.granne_b200_abi_version() == 2
     cxx = open(os.path.join(ROOT, "include", "granne_b200.hpp")).read()
     assert cxx.count("exact_search_filtered(") == 2
     shim = open(os.path.join(ROOT, "bindings", "rust", "src", "lib.rs")).read()
@@ -122,13 +114,8 @@ def test_symbols_in_the_headers_and_the_shim(lib):
     assert shim.count("pub fn exact_search_filtered(") == 2
 
 
-def test_cxx_exact_filtered_client_compiles(lib, tmp_path):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    libdir = os.path.dirname(granne_b200.library_path())
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-Wall", "-Wextra", "-Werror", "-I" + os.path.join(ROOT, "include"),
-                           os.path.join(ROOT, "tests", "helpers", "cxx_exact_filtered_client.cpp"), "-o",
-                           str(tmp_path / "client"), "-L" + libdir, "-lgranne_b200", "-Wl,-rpath," + libdir])
+def test_cxx_exact_filtered_client_compiles(library, tmp_path):
+    compile_cxx_client("cxx_exact_filtered_client.cpp", tmp_path)
 
 
 class _Fake(api.Granne):

@@ -1,4 +1,4 @@
-"""Exact k nearest neighbours without a device: the brute-force checker (tests/helpers/exact_oracle.cpp) against a
+"""Exact k nearest neighbours without a device: the brute-force checker (tests/helpers/composed_oracle.cpp) against a
 per-pair restatement with the oracle's own distances, and the host-side statuses of the new C entry points."""
 import ctypes as C
 
@@ -7,18 +7,11 @@ import pytest
 
 import granne_b200
 from granne_b200 import api
-from helpers import exact_oracle as xo
+from helpers import composed_oracle as co
 from helpers.data import random_vectors
+from helpers.fixtures import library  # noqa: F401  (autouse)
 
 INVALID = -1
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _lib():
-    from granne_b200 import build
-
-    build.build()
-    granne_b200.load_library()
 
 
 def _restated(oracle, kind, rows, queries, k, n):
@@ -45,7 +38,7 @@ def test_checker_equals_a_per_pair_restatement(oracle, kind, k, n):
     raw[20] = 0.0      # an all-zero row
     el = oracle.Elements.angular(raw) if kind == "angular" else oracle.Elements.angular_int(raw)
     rows = el.rows()
-    c = xo.Container(kind, el.to_bytes(0))
+    c = co.Container(kind, el.to_bytes(0))
     q = np.concatenate([random_vectors(4, 37, 4), raw[10:11]])
     got = c.exact_search(q, k, index_len=n)
     want = _restated(oracle, kind, rows, q, k, n)
@@ -58,8 +51,8 @@ def test_checker_raises_on_nan(oracle):
     el = oracle.Elements.angular(raw, as_is=True)
     bad = raw.copy()
     bad[7, 2] = np.nan
-    c = xo.Container("angular", np.uint64(16).tobytes() + bad.tobytes())
-    with pytest.raises(xo.NotFinite):
+    c = co.Container("angular", np.uint64(16).tobytes() + bad.tobytes())
+    with pytest.raises(co.NotFinite):
         c.exact_search(random_vectors(2, 16, 2), 5)
     assert len(el) == 30
 

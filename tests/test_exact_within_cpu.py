@@ -6,8 +6,8 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import granne_b200
 from granne_b200 import api
+from helpers.fixtures import library  # noqa: F401  (autouse)
 
 INVALID = -1
 FAKE = C.c_void_p(1)  # never dereferenced by a call whose arguments break a rule
@@ -20,14 +20,6 @@ NULL = "null buffer"
 OFFSETS_NULL = "offsets is null"
 IDS_NULL = "ids is null"
 SHAPE = "offsets must start at 0 and not decrease"
-
-
-@pytest.fixture(scope="module")
-def lib():
-    from granne_b200 import build
-
-    build.build()
-    return granne_b200.load_library()
 
 
 def _call(lib, device=False, q=True, nq=2, fmt=api.QUERY_RAW_F32, k=10, out=True, offsets=(0, 2, 3), ids=True):
@@ -51,45 +43,45 @@ def _call(lib, device=False, q=True, nq=2, fmt=api.QUERY_RAW_F32, k=10, out=True
 
 
 @pytest.mark.parametrize("device", [False, True])
-def test_shared_rules(lib, device):
-    assert _call(lib, device, fmt=7) == (INVALID, FORMAT)
-    assert _call(lib, device, k=1025) == (INVALID, EXACT_K)
-    assert _call(lib, device, nq=TOO_MANY) == (INVALID, NQ)
-    assert _call(lib, device, q=False) == (INVALID, NULL)
-    assert _call(lib, device, out=False) == (INVALID, NULL)
+def test_shared_rules(library, device):
+    assert _call(library, device, fmt=7) == (INVALID, FORMAT)
+    assert _call(library, device, k=1025) == (INVALID, EXACT_K)
+    assert _call(library, device, nq=TOO_MANY) == (INVALID, NQ)
+    assert _call(library, device, q=False) == (INVALID, NULL)
+    assert _call(library, device, out=False) == (INVALID, NULL)
     # reported in that order, before the lists' rules
-    assert _call(lib, device, fmt=7, k=1025, offsets=None) == (INVALID, FORMAT)
-    assert _call(lib, device, k=1025, nq=TOO_MANY, q=False, offsets=None) == (INVALID, EXACT_K)
-    assert _call(lib, device, q=False, offsets=None) == (INVALID, NULL)
+    assert _call(library, device, fmt=7, k=1025, offsets=None) == (INVALID, FORMAT)
+    assert _call(library, device, k=1025, nq=TOO_MANY, q=False, offsets=None) == (INVALID, EXACT_K)
+    assert _call(library, device, q=False, offsets=None) == (INVALID, NULL)
 
 
 @pytest.mark.parametrize("device", [False, True])
-def test_offsets_null(lib, device):
-    assert _call(lib, device, offsets=None) == (INVALID, OFFSETS_NULL)
-    assert _call(lib, device, offsets=None, ids=False) == (INVALID, OFFSETS_NULL)
+def test_offsets_null(library, device):
+    assert _call(library, device, offsets=None) == (INVALID, OFFSETS_NULL)
+    assert _call(library, device, offsets=None, ids=False) == (INVALID, OFFSETS_NULL)
 
 
-def test_ids_null_when_the_lists_name_ids(lib):
-    assert _call(lib, ids=False) == (INVALID, IDS_NULL)
+def test_ids_null_when_the_lists_name_ids(library):
+    assert _call(library, ids=False) == (INVALID, IDS_NULL)
     # before the shape of the offsets
-    assert _call(lib, ids=False, offsets=(1, 0, 3)) == (INVALID, IDS_NULL)
+    assert _call(library, ids=False, offsets=(1, 0, 3)) == (INVALID, IDS_NULL)
 
 
 @pytest.mark.parametrize("offsets", [(1, 2, 3), (0, 3, 2), (0, 2, 1), (5, 5, 5)])
-def test_offsets_shape(lib, offsets):
-    assert _call(lib, offsets=offsets) == (INVALID, SHAPE)
-    assert _call(lib, offsets=offsets, ids=False) == (INVALID, IDS_NULL)
+def test_offsets_shape(library, offsets):
+    assert _call(library, offsets=offsets) == (INVALID, SHAPE)
+    assert _call(library, offsets=offsets, ids=False) == (INVALID, IDS_NULL)
 
 
-def test_no_queries_is_ok_before_the_handle_is_read(lib):
-    assert _call(lib, nq=0, q=False, out=False, offsets=None, ids=False)[0] == 0
-    assert _call(lib, device=True, nq=0, q=False, out=False, offsets=None, ids=False)[0] == 0
+def test_no_queries_is_ok_before_the_handle_is_read(library):
+    assert _call(library, nq=0, q=False, out=False, offsets=None, ids=False)[0] == 0
+    assert _call(library, device=True, nq=0, q=False, out=False, offsets=None, ids=False)[0] == 0
 
 
-def test_multi_null_handle(lib):
+def test_multi_null_handle(library):
     q = np.zeros((1, 8), np.float32)
-    rc = lib.granne_b200_multi_exact_search_within_batch(None, api._ptr(q), 1, 0, None, None, 10, None, None, None)
-    assert (rc, lib.granne_b200_last_error().decode()) == (INVALID, "multi handle is null")
+    rc = library.granne_b200_multi_exact_search_within_batch(None, api._ptr(q), 1, 0, None, None, 10, None, None, None)
+    assert (rc, library.granne_b200_last_error().decode()) == (INVALID, "multi handle is null")
 
 
 def test_lists_pack_into_csr():

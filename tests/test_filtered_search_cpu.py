@@ -6,9 +6,9 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import granne_b200
 from granne_b200 import api
-from helpers.filtered_oracle import pack
+from helpers.composed_oracle import pack
+from helpers.fixtures import library  # noqa: F401  (autouse)
 
 INVALID = -1
 FAKE = C.c_void_p(1)  # never dereferenced by a call whose arguments break a rule
@@ -21,14 +21,6 @@ EXACT_K = "num_neighbors exceeds GRANNE_B200_EXACT_MAX_K (1024)"
 NQ = "too many queries in one batch"
 NULL = "null buffer"
 FILTERS = "filters is null or num_filters is 0"
-
-
-@pytest.fixture(scope="module")
-def lib():
-    from granne_b200 import build
-
-    build.build()
-    return granne_b200.load_library()
 
 
 def _call(lib, which="host", handle=FAKE, q=True, nq=2, fmt=api.QUERY_RAW_F32, ef=50, k=10, out=True, filters=True,
@@ -54,42 +46,42 @@ def _call(lib, which="host", handle=FAKE, q=True, nq=2, fmt=api.QUERY_RAW_F32, e
 
 
 @pytest.mark.parametrize("which", ["host", "device"])
-def test_each_rule(lib, which):
-    assert _call(lib, which, handle=None) == (INVALID, HANDLE)
-    assert _call(lib, which, fmt=7) == (INVALID, FORMAT)
-    assert _call(lib, which, ef=0) == (INVALID, MAX_SEARCH)
-    assert _call(lib, which, k=1025) == (INVALID, EXACT_K)
-    assert _call(lib, which, nq=TOO_MANY) == (INVALID, NQ)
-    assert _call(lib, which, q=False) == (INVALID, NULL)
-    assert _call(lib, which, out=False) == (INVALID, NULL)
-    assert _call(lib, which, filters=False) == (INVALID, FILTERS)
-    assert _call(lib, which, num_filters=0) == (INVALID, FILTERS)
+def test_each_rule(library, which):
+    assert _call(library, which, handle=None) == (INVALID, HANDLE)
+    assert _call(library, which, fmt=7) == (INVALID, FORMAT)
+    assert _call(library, which, ef=0) == (INVALID, MAX_SEARCH)
+    assert _call(library, which, k=1025) == (INVALID, EXACT_K)
+    assert _call(library, which, nq=TOO_MANY) == (INVALID, NQ)
+    assert _call(library, which, q=False) == (INVALID, NULL)
+    assert _call(library, which, out=False) == (INVALID, NULL)
+    assert _call(library, which, filters=False) == (INVALID, FILTERS)
+    assert _call(library, which, num_filters=0) == (INVALID, FILTERS)
 
 
 @pytest.mark.parametrize("which", ["host", "device"])
-def test_rule_order(lib, which):
+def test_rule_order(library, which):
     everything = dict(handle=None, fmt=7, ef=0, k=1025, nq=TOO_MANY, q=False, out=False, filters=False)
     order = [("handle", HANDLE), ("fmt", FORMAT), ("ef", MAX_SEARCH), ("k", EXACT_K), ("nq", NQ), ("q", NULL),
              ("out", NULL), ("filters", FILTERS)]
     for i, (_, msg) in enumerate(order):
         broken = {name: everything[name] for name, _ in order[i:]}
-        assert _call(lib, which, **broken) == (INVALID, msg), broken
+        assert _call(library, which, **broken) == (INVALID, msg), broken
 
 
 @pytest.mark.parametrize("which", ["host", "device"])
-def test_k_may_exceed_max_search(lib, which):
+def test_k_may_exceed_max_search(library, which):
     # k > max_search breaks no rule: the call goes on to the filters' rule
-    assert _call(lib, which, ef=5, k=1024, filters=False) == (INVALID, FILTERS)
+    assert _call(library, which, ef=5, k=1024, filters=False) == (INVALID, FILTERS)
 
 
 @pytest.mark.parametrize("which", ["host", "device"])
-def test_no_queries_is_ok_before_the_filters_and_the_handle_are_read(lib, which):
-    assert _call(lib, which, nq=0, q=False, out=False, filters=False, num_filters=0)[0] == 0
+def test_no_queries_is_ok_before_the_filters_and_the_handle_are_read(library, which):
+    assert _call(library, which, nq=0, q=False, out=False, filters=False, num_filters=0)[0] == 0
 
 
-def test_multi_null_handle_first(lib):
+def test_multi_null_handle_first(library):
     # before every single-device rule (those follow on a real handle: test_filtered_search_gpu.py)
-    assert _call(lib, "multi", handle=None, fmt=7, ef=0, filters=False) == (INVALID, "multi handle is null")
+    assert _call(library, "multi", handle=None, fmt=7, ef=0, filters=False) == (INVALID, "multi handle is null")
 
 
 def test_bool_mask_packs_lsb_first():

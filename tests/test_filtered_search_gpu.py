@@ -1,35 +1,25 @@
 """Filtered search on the GPU (granne_b200_search_filtered_batch*).  Ids, distance bits, counts and stats[:, :3] equal an
-oracle composed from the CPU oracle's own pieces (tests/helpers/filtered_oracle.cpp: its descent, its bottom-layer
+oracle composed from the CPU oracle's own pieces (tests/helpers/composed_oracle.cpp: its descent, its bottom-layer
 search recording the scored ids, the filter, dist_to_element, a sort by (distance, id)).  Also: every engine, every
 list variant and the slow pass, many queries per warp through the pass ladder, per-query filters, stray bits beyond
 len, ties and NaN, the identities with search_batch, the rejections, the device variant under concurrency, every
 handle source, both multi modes and a C++ client."""
-import os
-import shutil
-import subprocess
 import threading
 
 import numpy as np
 import pytest
 
 import granne_b200
-from helpers import filtered_oracle as fo
+from helpers import composed_oracle as co
 from helpers.data import build_fixture, index_from_lists, random_vectors
+from helpers.fixtures import assert_same, cxx_client
+from helpers.fixtures import library  # noqa: F401  (autouse)
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 INVALID, NOT_FINITE = -1, -6
 UNUSED = 0xFFFFFFFF
 MAX_CTAS_PER_SM = 32
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _lib():
-    from granne_b200 import build
-
-    build.build()
-    granne_b200.load_library()
 
 
 class Case:
@@ -38,7 +28,7 @@ class Case:
     def __init__(self, index_bytes, kind, eb, mb=None, g=None):
         self.ib, self.kind, self.eb, self.mb = index_bytes, kind, eb, mb
         self.g = g if g is not None else granne_b200.Granne.from_bytes(index_bytes, kind, eb, mb)
-        self.o = fo.Filtered(index_bytes, kind, eb, mb)
+        self.o = co.Filtered(index_bytes, kind, eb, mb)
         self.n = len(self.g)
         assert len(self.o) == self.n
 
@@ -64,21 +54,11 @@ def _masks(n, densities, seed):
 DENSITIES = [0, "one", 0.01, 0.1, 0.5, 1.0]
 
 
-def _same(got, want, what=""):
-    gi, gd, gc, gs = got
-    wi, wd, wc, ws = want
-    assert np.array_equal(gc, wc), what + " counts"
-    bad = np.nonzero((gi != wi).any(axis=1))[0]
-    assert bad.size == 0, "%s ids differ for queries %s: want %s got %s" % (what, bad[:5], wi[bad[:1]], gi[bad[:1]])
-    assert np.array_equal(gd.view(np.uint32), wd.view(np.uint32)), what + " dists"
-    assert np.array_equal(gs[:, :3], ws), what + " n_dist/n_expand/n_neighbors"
-
-
 def check(c, q, masks, ef, k, query_filter=None, already_element=False, what=""):
-    words = fo.pack(masks)
+    words = co.pack(masks)
     want = c.o.search(q, words, ef, k, query_filter, already_element=already_element)
     got = c.g.search_batch_filtered(q, masks, query_filter, ef, k, already_element=already_element, with_stats=True)
-    _same(got, want, what)
+    assert_same(got, want, what, stats=True)
     # every returned id is admitted by its query's filter
     qf = np.zeros(len(q), np.int64) if query_filter is None else np.asarray(query_filter)
     m = np.atleast_2d(masks)
@@ -183,14 +163,14 @@ def test_len_not_a_multiple_of_32_with_stray_bits(oracle):
     c = _case(oracle, "angular", 1000, 32, seed=12)
     assert c.n % 32 != 0
     masks = _masks(c.n, [0.2, 0.6], 13)
-    words = fo.pack(masks)
+    words = co.pack(masks)
     stray = np.concatenate([words, np.full((2, 3), 0xFFFFFFFF, np.uint32)], axis=1)
     stray[:, c.n // 32] |= np.uint32(0xFFFFFFFF) << np.uint32(c.n % 32)
     q = random_vectors(40, 32, 14)
     qf = _per_query(40, 2)
     want = c.o.search(q, words, 40, 10, qf)
-    _same(c.g.search_batch_filtered(q, stray, qf, 40, 10, with_stats=True), want, "stray bits")
-    _same(c.g.search_batch_filtered(q, masks, qf, 40, 10, with_stats=True), want, "bool masks")
+    assert_same(c.g.search_batch_filtered(q, stray, qf, 40, 10, with_stats=True), want, "stray bits", stats=True)
+    assert_same(c.g.search_batch_filtered(q, masks, qf, 40, 10, with_stats=True), want, "bool masks", stats=True)
 
 
 def test_nan_as_search_batch(shared):
@@ -233,7 +213,7 @@ def test_host_rejections(shared):
     c = shared
     q = random_vectors(3, 32, 18)
     lib = granne_b200.load_library()
-    words = fo.pack(np.ones(c.n, bool))
+    words = co.pack(np.ones(c.n, bool))
     ids = np.zeros((3, 10), np.uint32)
     d = np.zeros((3, 10), np.float32)
 
@@ -261,7 +241,7 @@ def _device(c, q, masks, ef, k, qf=None, stream=None):
 
     dev = torch.device("cuda", 0)
     tq = torch.from_numpy(q).to(dev)
-    tw = torch.from_numpy(fo.pack(masks).view(np.int32)).to(dev)
+    tw = torch.from_numpy(co.pack(masks).view(np.int32)).to(dev)
     tqf = None if qf is None else torch.from_numpy(np.asarray(qf, np.uint32).view(np.int32)).to(dev)
     stats = torch.empty((q.shape[0], 4), dtype=torch.int64, device=dev)
     ids, d, cnt = c.g.search_batch_filtered_device(tq, tw, tqf, ef, k, stats=stats, stream=stream)
@@ -289,8 +269,8 @@ def test_device_bad_query_filter(shared):
     bad = np.array([2, 4])
     assert (gc[bad] == 0).all() and (gi[bad] == UNUSED).all() and np.isinf(gd[bad]).all()
     good = np.array([0, 1, 3, 5])
-    want = c.o.search(q[good], fo.pack(masks), 40, 10, qf[good])
-    _same((gi[good], gd[good], gc[good], gs[good]), want, "device, good queries")
+    want = c.o.search(q[good], co.pack(masks), 40, 10, qf[good])
+    assert_same((gi[good], gd[good], gc[good], gs[good]), want, "device, good queries", stats=True)
     c.g.stream_status()  # the error was reported once
 
 
@@ -307,10 +287,10 @@ def test_device_streams_and_threads(shared):
         qf = _per_query(nq, 3)
         with torch.cuda.stream(streams[s]):
             outs.append(_device(c, q, masks, ef, k, qf, stream=streams[s]))
-        wants.append(c.o.search(q, fo.pack(masks), ef, k, qf))
+        wants.append(c.o.search(q, co.pack(masks), ef, k, qf))
     torch.cuda.synchronize()
     for s in range(len(plans)):
-        _same(_host(outs[s]), wants[s], "stream %d" % s)
+        assert_same(_host(outs[s]), wants[s], "stream %d" % s, stats=True)
     c.g.stream_status()
     for st in streams:
         c.g.release_stream(st)
@@ -341,15 +321,15 @@ def test_handle_sources(oracle, tmp_path):
     q = random_vectors(24, 64, 33)
     masks = _masks(c.n, DENSITIES, 34)
     qf = _per_query(24, len(DENSITIES))
-    want = c.o.search(q, fo.pack(masks), 60, 10, qf)
+    want = c.o.search(q, co.pack(masks), 60, 10, qf)
     idx, el = tmp_path / "index.bin", tmp_path / "elements.bin"
     idx.write_bytes(c.ib)
     el.write_bytes(c.eb)
     f = granne_b200.Granne(str(idx), "angular", str(el))
-    _same(f.search_batch_filtered(q, masks, qf, 60, 10, with_stats=True), want, "file images")
+    assert_same(f.search_batch_filtered(q, masks, qf, 60, 10, with_stats=True), want, "file images", stats=True)
     rows = np.frombuffer(bytes(c.eb[8:]), np.float32).reshape(-1, 64)
     d = granne_b200.Granne.from_device_elements(c.ib, "angular", torch.from_numpy(rows.copy()).to("cuda:0"))
-    _same(d.search_batch_filtered(q, masks, qf, 60, 10, with_stats=True), want, "device elements")
+    assert_same(d.search_batch_filtered(q, masks, qf, 60, 10, with_stats=True), want, "device elements", stats=True)
     # a builder's get_index: checked against the oracle over the builder's own index image
     raw = random_vectors(2500, 64, 35)
     b = granne_b200.GranneBuilder("angular", granne_b200.elements_from_raw("angular", raw), num_neighbors=12,
@@ -369,7 +349,7 @@ def test_multi_handle(oracle, mode):
     raw = random_vectors(2500, dim, 38)
     masks = _masks(2500, [0.02, 0.3, 1.0], 39)
     qf = _per_query(30, 3)
-    words = fo.pack(masks)
+    words = co.pack(masks)
     k = 10
     if mode == "replicated":
         c = _case(oracle, "angular", 2500, dim, seed=38)
@@ -382,7 +362,7 @@ def test_multi_handle(oracle, mode):
             el = oracle.Elements.angular(raw[a:b])
             ib = oracle.GranneBuilder(el, num_neighbors=16, max_search=40).build(threads=8).to_bytes()
             shards.append((ib, el.to_bytes()))
-            parts.append((a, fo.Filtered(ib, "angular", el.to_bytes())))
+            parts.append((a, co.Filtered(ib, "angular", el.to_bytes())))
         m = granne_b200.MultiGranne.partitioned(shards, "angular", [0, 0])
         assert m.shard_base(1) == 1000
         res = [(base, o.search(q, words, 50, k, qf, bit_base=base)) for base, o in parts]
@@ -414,22 +394,14 @@ def test_multi_handle(oracle, mode):
 
 
 def test_cxx_client(oracle, tmp_path):
-    cxx = shutil.which("g++")
-    if cxx is None:
-        pytest.skip("no C++ compiler")
     c = _case(oracle, "angular", 2000, 64, seed=44)
     idx, el = tmp_path / "index.bin", tmp_path / "elements.bin"
     idx.write_bytes(c.ib)
     el.write_bytes(c.eb)
-    exe = tmp_path / "client"
-    libdir = os.path.dirname(granne_b200.library_path())
-    subprocess.check_call([cxx, "-std=c++17", "-O1", "-Wall", "-Wextra", "-Werror", "-I" + os.path.join(ROOT, "include"),
-                           os.path.join(ROOT, "tests", "helpers", "cxx_filtered_client.cpp"), "-o", str(exe),
-                           "-L" + libdir, "-lgranne_b200", "-Wl,-rpath," + libdir])
-    out = subprocess.run([str(exe), str(idx), str(el)], capture_output=True, text=True, timeout=120)
+    out = cxx_client("cxx_filtered_client.cpp", [idx, el], tmp_path)
     assert out.returncode == 0, out.stdout + out.stderr
     odd = (np.arange(c.n) % 2 == 1)
-    wi, wd, wc, _ = c.o.search(c.g.get_element(7)[None, :], fo.pack(odd), 40, 5, already_element=True)
+    wi, wd, wc, _ = c.o.search(c.g.get_element(7)[None, :], co.pack(odd), 40, 5, already_element=True)
     lines = out.stdout.split()
     assert [int(x) for x in lines[0::2]] == wi[0, :wc[0]].tolist()
     assert [np.float32(x).view(np.uint32) for x in lines[1::2]] == wd[0, :wc[0]].view(np.uint32).tolist()

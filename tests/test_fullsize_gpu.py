@@ -5,6 +5,7 @@ import numpy as np
 import pytest
 
 import granne_b200
+from helpers.fixtures import library  # noqa: F401  (autouse)
 
 pytestmark = pytest.mark.gpu
 
@@ -16,9 +17,7 @@ def big():
     import sys, os
     sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
     from bench import clustered
-    from granne_b200 import build
 
-    build.build()
     nc = 4096
     eb = granne_b200.elements_from_raw("angular", clustered(N, DIM, 1234, nc))
     b = granne_b200.GranneBuilder("angular", eb, num_neighbors=30, max_search=200)

@@ -12,26 +12,19 @@ import pytest
 import granne_b200
 from granne_b200 import api
 from helpers.data import build_fixture
+from helpers.fixtures import library  # noqa: F401  (autouse)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-@pytest.fixture(scope="module")
-def lib():
-    from granne_b200 import build
-
-    build.build()
-    return granne_b200.load_library()
-
-
-def test_library_exports_every_declared_symbol(lib):
+def test_library_exports_every_declared_symbol(library):
     header = open(os.path.join(ROOT, "include", "granne_b200.h")).read()
     names = set(re.findall(r"\b(granne_b200_[a-z0-9_]+)\s*\(", header))
     assert len(names) >= 20
     raw = ctypes.CDLL(granne_b200.library_path())
     for n in sorted(names):
         assert hasattr(raw, n), n
-    assert lib.granne_b200_abi_version() == 2
+    assert library.granne_b200_abi_version() == 2
 
 
 def test_no_torch_or_cxx_types_in_the_header():
@@ -41,7 +34,7 @@ def test_no_torch_or_cxx_types_in_the_header():
 
 
 @pytest.mark.parametrize("n,dim,m", [(1, 8, 5), (59, 8, 5), (60, 8, 5), (61, 8, 5), (1500, 16, 20), (3000, 8, 30)])
-def test_loader_decodes_layers_like_the_oracle(lib, oracle, n, dim, m):
+def test_loader_decodes_layers_like_the_oracle(library, oracle, n, dim, m):
     # sizes around the 60-offsets-per-chunk boundary (offsets.rs:7,249-259)
     el, g, index_bytes, _, _ = build_fixture(oracle, "angular", n, dim, seed=n, num_neighbors=m, max_search=30)
     shape = api.inspect_index(index_bytes)
@@ -59,7 +52,7 @@ def test_loader_decodes_layers_like_the_oracle(lib, oracle, n, dim, m):
         assert seen_max == maxdeg
 
 
-def test_loader_handles_raw_and_vbyte_lists(lib, oracle):
+def test_loader_handles_raw_and_vbyte_lists(library, oracle):
     # hand-made index: lists that exercise the raw-u32 rule (set_vector.rs:275-283), empty lists, <4 entries
     import json
 
@@ -99,7 +92,7 @@ def test_loader_handles_raw_and_vbyte_lists(lib, oracle):
     assert [oracle.set_decode(e) for e in enc] == [sorted(l) for l in small]
 
 
-def test_format_errors_are_statuses_not_crashes(lib, oracle):
+def test_format_errors_are_statuses_not_crashes(library, oracle):
     el, g, index_bytes, elements_bytes, _ = build_fixture(oracle, "angular", 200, 8, seed=3, num_neighbors=8,
                                                           max_search=20)
     for bad in [b"", b"granne", b"grannf" + index_bytes[6:], index_bytes[:1024], index_bytes[:-7],
@@ -110,7 +103,7 @@ def test_format_errors_are_statuses_not_crashes(lib, oracle):
     assert "granne" in str(ei.value) or "metadata" in str(ei.value) or "layer" in str(ei.value)
 
 
-def test_open_without_a_gpu_fails_loudly(lib, oracle):
+def test_open_without_a_gpu_fails_loudly(library, oracle):
     import torch
 
     if torch.cuda.is_available():
@@ -125,14 +118,14 @@ def test_open_without_a_gpu_fails_loudly(lib, oracle):
 
 
 @pytest.mark.parametrize("n,dim,m", [(1, 8, 5), (60, 8, 5), (61, 8, 5), (1500, 16, 20), (4000, 8, 30)])
-def test_writer_is_byte_identical_to_the_oracle_writer(lib, oracle, n, dim, m):
+def test_writer_is_byte_identical_to_the_oracle_writer(library, oracle, n, dim, m):
     # Index::write_index (src/index/io.rs:11-70, set_vector.rs:117-148,169-221, offsets.rs:233-241): the product's
     # writer re-encodes an oracle-written image byte for byte (header JSON, offset chunks, raw-vs-vbyte rule)
     el, g, index_bytes, _, _ = build_fixture(oracle, "angular", n, dim, seed=n + 1, num_neighbors=m, max_search=30)
     assert api.reencode_index(index_bytes) == index_bytes
 
 
-def test_writer_round_trips_the_golden_images(lib):
+def test_writer_round_trips_the_golden_images(library):
     import glob
 
     for path in glob.glob(os.path.join(ROOT, "tests", "golden", "*.npz")):
@@ -140,7 +133,7 @@ def test_writer_round_trips_the_golden_images(lib):
         assert api.reencode_index(image) == image
 
 
-def test_header_is_plain_c_and_links_from_c(lib, tmp_path):
+def test_header_is_plain_c_and_links_from_c(library, tmp_path):
     # the boundary is a C ABI: the header compiles as strict C99 and a C program links against the shared library
     import shutil
     import subprocess
@@ -195,7 +188,7 @@ def test_rust_shim_declarations_match_the_header():
 
 
 @pytest.mark.parametrize("seed", range(12))
-def test_random_graphs_decode_and_reencode_like_the_oracle(lib, oracle, seed):
+def test_random_graphs_decode_and_reencode_like_the_oracle(library, oracle, seed):
     # differential check on random adjacency lists: empty / short / long lists, small and large id gaps (raw-vs-vbyte
     # rule, set_vector.rs:130-141), layer sizes around the 60-offsets-per-chunk boundary (offsets.rs:7)
     from helpers.data import index_from_lists

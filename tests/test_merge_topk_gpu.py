@@ -10,19 +10,12 @@ import pytest
 
 import granne_b200
 from helpers.data import build_fixture, random_vectors
+from helpers.fixtures import library  # noqa: F401  (autouse)
 from helpers.topk_tiles import PAD_GID, make_tiles, reference_merge, tie_bases
 from test_multi_capi_gpu import _devices
 from test_parity_gpu import open_product
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _lib():
-    from granne_b200 import build
-
-    build.build()
-    granne_b200.load_library()
 
 
 def device_tiles(ids, dists):

@@ -12,17 +12,10 @@ import pytest
 import granne_b200
 from granne_b200.distributed import merge_topk_host
 from helpers.data import build_fixture, random_vectors
+from helpers.fixtures import library  # noqa: F401  (autouse)
 
 pytestmark = pytest.mark.gpu
 INVALID = -1  # GRANNE_B200_ERR_INVALID_ARGUMENT
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _lib():
-    from granne_b200 import build
-
-    build.build()
-    granne_b200.load_library()
 
 
 def _devices(minimum):

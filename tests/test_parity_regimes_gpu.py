@@ -10,21 +10,13 @@ import sys
 import numpy as np
 import pytest
 
-import granne_b200
 from helpers.data import build_fixture, index_from_lists, random_vectors
+from helpers.fixtures import library  # noqa: F401  (autouse)
 from test_parity_gpu import assert_parity, open_product
 
 pytestmark = pytest.mark.gpu
 
 MAX_CTAS_PER_SM = 32  # the most resident CTAs an H100 SM holds: the fast pass's grid never exceeds this x SMs
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _lib():
-    from granne_b200 import build
-
-    build.build()
-    granne_b200.load_library()
 
 
 def queries_for_four_per_warp():

@@ -13,6 +13,7 @@ import pytest
 
 import granne_b200
 from helpers.data import build_fixture, index_from_lists, random_vectors
+from helpers.fixtures import library  # noqa: F401  (autouse)
 from test_parity_gpu import assert_parity, open_product
 from test_parity_regimes_gpu import queries_for_four_per_warp
 
@@ -23,14 +24,6 @@ PAD_ID = 0xFFFFFFFF
 INF_BITS = 0x7F800000
 SPARE_FLAGS = 2  # flag entries past n_peers, which must stay untouched too
 INVALID_ARGUMENT = -1
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _lib():
-    from granne_b200 import build
-
-    build.build()
-    granne_b200.load_library()
 
 
 class Peers:

@@ -7,8 +7,8 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import granne_b200
 from granne_b200 import api
+from helpers.fixtures import library  # noqa: F401  (autouse)
 
 INVALID = -1
 FAKE = C.c_void_p(1)  # never dereferenced by a call whose arguments break a rule
@@ -23,14 +23,6 @@ OFFSETS_NULL = "offsets is null"
 IDS_NULL = "ids is null"
 FILTERS = "filters is null or num_filters is 0"
 ALL_CALLS = ["search", "exact", "rerank", "within", "filtered"]
-
-
-@pytest.fixture(scope="module")
-def lib():
-    from granne_b200 import build
-
-    build.build()
-    return granne_b200.load_library()
 
 
 def _call(lib, call, q=True, nq=2, fmt=api.QUERY_RAW_F32, max_search=50, k=10, ids=True, offsets=(0, 2, 3),
@@ -61,48 +53,48 @@ def _call(lib, call, q=True, nq=2, fmt=api.QUERY_RAW_F32, max_search=50, k=10, i
 
 
 @pytest.mark.parametrize("call", ALL_CALLS)
-def test_shared_rules(lib, call):
-    assert _call(lib, call, fmt=7) == (INVALID, FORMAT)
-    assert _call(lib, call, nq=TOO_MANY) == (INVALID, NQ)
-    assert _call(lib, call, q=False) == (INVALID, NULL)
-    assert _call(lib, call, ids=False) == (INVALID, NULL)
+def test_shared_rules(library, call):
+    assert _call(library, call, fmt=7) == (INVALID, FORMAT)
+    assert _call(library, call, nq=TOO_MANY) == (INVALID, NQ)
+    assert _call(library, call, q=False) == (INVALID, NULL)
+    assert _call(library, call, ids=False) == (INVALID, NULL)
 
 
 @pytest.mark.parametrize("call", ["search", "rerank", "filtered"])
-def test_max_search_rule(lib, call):
-    assert _call(lib, call, max_search=0) == (INVALID, MAX_SEARCH)
+def test_max_search_rule(library, call):
+    assert _call(library, call, max_search=0) == (INVALID, MAX_SEARCH)
     # reported after the format, before the batch size and the buffers
-    assert _call(lib, call, max_search=0, fmt=7) == (INVALID, FORMAT)
-    assert _call(lib, call, max_search=0, nq=TOO_MANY, q=False) == (INVALID, MAX_SEARCH)
+    assert _call(library, call, max_search=0, fmt=7) == (INVALID, FORMAT)
+    assert _call(library, call, max_search=0, nq=TOO_MANY, q=False) == (INVALID, MAX_SEARCH)
 
 
-def test_exact_k_rule(lib):
+def test_exact_k_rule(library):
     for call in ("exact", "within", "filtered"):
-        assert _call(lib, call, k=1025) == (INVALID, EXACT_K)
-        assert _call(lib, call, k=1025, fmt=7) == (INVALID, FORMAT)
-        assert _call(lib, call, k=1025, nq=TOO_MANY, q=False) == (INVALID, EXACT_K)
+        assert _call(library, call, k=1025) == (INVALID, EXACT_K)
+        assert _call(library, call, k=1025, fmt=7) == (INVALID, FORMAT)
+        assert _call(library, call, k=1025, nq=TOO_MANY, q=False) == (INVALID, EXACT_K)
 
 
-def test_within_rules_in_order(lib):
+def test_within_rules_in_order(library):
     # the exact-k rule, then a null offsets with nq > 0, then null ids when offsets[nq] > 0
-    assert _call(lib, "within", k=1025, offsets=None, cand=False) == (INVALID, EXACT_K)
-    assert _call(lib, "within", q=False, offsets=None, cand=False) == (INVALID, NULL)
-    assert _call(lib, "within", offsets=None, cand=False) == (INVALID, OFFSETS_NULL)
-    assert _call(lib, "within", cand=False) == (INVALID, IDS_NULL)
+    assert _call(library, "within", k=1025, offsets=None, cand=False) == (INVALID, EXACT_K)
+    assert _call(library, "within", q=False, offsets=None, cand=False) == (INVALID, NULL)
+    assert _call(library, "within", offsets=None, cand=False) == (INVALID, OFFSETS_NULL)
+    assert _call(library, "within", cand=False) == (INVALID, IDS_NULL)
 
 
-def test_filtered_rules_in_order(lib):
+def test_filtered_rules_in_order(library):
     # max_search, then the exact-k rule, then null or zero filters
-    assert _call(lib, "filtered", max_search=0, k=1025, filters=False) == (INVALID, MAX_SEARCH)
-    assert _call(lib, "filtered", k=1025, filters=False, num_filters=0) == (INVALID, EXACT_K)
-    assert _call(lib, "filtered", q=False, filters=False) == (INVALID, NULL)
-    assert _call(lib, "filtered", filters=False) == (INVALID, FILTERS)
-    assert _call(lib, "filtered", num_filters=0) == (INVALID, FILTERS)
+    assert _call(library, "filtered", max_search=0, k=1025, filters=False) == (INVALID, MAX_SEARCH)
+    assert _call(library, "filtered", k=1025, filters=False, num_filters=0) == (INVALID, EXACT_K)
+    assert _call(library, "filtered", q=False, filters=False) == (INVALID, NULL)
+    assert _call(library, "filtered", filters=False) == (INVALID, FILTERS)
+    assert _call(library, "filtered", num_filters=0) == (INVALID, FILTERS)
 
 
-def test_no_queries_is_ok_before_the_handle_is_read(lib):
+def test_no_queries_is_ok_before_the_handle_is_read(library):
     for call in ("search", "exact", "within", "filtered"):
-        assert _call(lib, call, nq=0, q=False, ids=False, offsets=None, cand=False, filters=False)[0] == 0
+        assert _call(library, call, nq=0, q=False, ids=False, offsets=None, cand=False, filters=False)[0] == 0
 
 
 def test_raw_stream():

@@ -5,14 +5,14 @@ so a handle that is never dereferenced serves."""
 import ctypes as C
 import os
 import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
 import granne_b200
 from granne_b200 import api
+from helpers.fixtures import compile_cxx_client
+from helpers.fixtures import library  # noqa: F401  (autouse)
 
 INVALID = -1
 FAKE = C.c_void_p(1)
@@ -23,14 +23,6 @@ EXCL_K = "num_neighbors exceeds 1023 with GRANNE_B200_QUERY_ID_EXCLUDING (the ca
 EXACT_K = "num_neighbors exceeds GRANNE_B200_EXACT_MAX_K (1024)"
 OFFSETS_NULL = "offsets is null"
 FILTERS = "filters is null or num_filters is 0"
-
-
-@pytest.fixture(scope="module")
-def lib():
-    from granne_b200 import build
-
-    build.build()
-    return granne_b200.load_library()
 
 
 def _call(lib, call, fmt, k=10, nq=2, q=True, offsets=True, filters=True):
@@ -76,48 +68,48 @@ ACCEPTING = ["search", "search_device", "exact", "exact_device", "within", "with
 
 
 @pytest.mark.parametrize("call", ACCEPTING)
-def test_id_formats_pass_the_shared_rules(lib, call):
+def test_id_formats_pass_the_shared_rules(library, call):
     # with nq = 0 a call that takes the format returns OK before it reads the handle
     for fmt in (api.QUERY_ID, api.QUERY_ID_EXCLUDING):
-        assert _call(lib, call, fmt, nq=0, q=False)[0] == 0
-        assert _call(lib, call, fmt, q=False) == (INVALID, NULL)  # null ids
-    assert _call(lib, call, 4) == (INVALID, FORMAT)
+        assert _call(library, call, fmt, nq=0, q=False)[0] == 0
+        assert _call(library, call, fmt, q=False) == (INVALID, NULL)  # null ids
+    assert _call(library, call, 4) == (INVALID, FORMAT)
 
 
 @pytest.mark.parametrize("call", ["gather", "rerank", "rerank_device"])
-def test_gather_and_rerank_reject_id_formats(lib, call):
+def test_gather_and_rerank_reject_id_formats(library, call):
     for fmt in (api.QUERY_ID, api.QUERY_ID_EXCLUDING):
-        assert _call(lib, call, fmt, nq=0, q=False) == (INVALID, FORMAT)
+        assert _call(library, call, fmt, nq=0, q=False) == (INVALID, FORMAT)
 
 
 @pytest.mark.parametrize("call", ["exact", "exact_device", "within", "within_device", "filtered", "filtered_device"])
-def test_exclusion_k_rule_and_order(lib, call):
+def test_exclusion_k_rule_and_order(library, call):
     X = api.QUERY_ID_EXCLUDING
-    assert _call(lib, call, X, k=1024, nq=0, q=False) == (INVALID, EXCL_K)
-    assert _call(lib, call, X, k=1023, nq=0, q=False)[0] == 0
-    assert _call(lib, call, api.QUERY_ID, k=1024, nq=0, q=False)[0] == 0
+    assert _call(library, call, X, k=1024, nq=0, q=False) == (INVALID, EXCL_K)
+    assert _call(library, call, X, k=1023, nq=0, q=False)[0] == 0
+    assert _call(library, call, api.QUERY_ID, k=1024, nq=0, q=False)[0] == 0
     # after the existing rules: the cap itself, null buffers, null offsets / filters
-    assert _call(lib, call, X, k=1025) == (INVALID, EXACT_K)
-    assert _call(lib, call, X, k=1024, q=False) == (INVALID, NULL)
+    assert _call(library, call, X, k=1025) == (INVALID, EXACT_K)
+    assert _call(library, call, X, k=1024, q=False) == (INVALID, NULL)
     if call.startswith("within"):
-        assert _call(lib, call, X, k=1024, offsets=False) == (INVALID, OFFSETS_NULL)
+        assert _call(library, call, X, k=1024, offsets=False) == (INVALID, OFFSETS_NULL)
     if call.startswith("filtered"):
-        assert _call(lib, call, X, k=1024, filters=False) == (INVALID, FILTERS)
+        assert _call(library, call, X, k=1024, filters=False) == (INVALID, FILTERS)
 
 
-def test_search_has_no_exclusion_cap_below_u32(lib):
-    assert _call(lib, "search", api.QUERY_ID_EXCLUDING, k=5000, nq=0, q=False)[0] == 0
-    assert _call(lib, "search", api.QUERY_ID_EXCLUDING, k=0xFFFFFFFF, nq=0, q=False)[0] == INVALID
+def test_search_has_no_exclusion_cap_below_u32(library):
+    assert _call(library, "search", api.QUERY_ID_EXCLUDING, k=5000, nq=0, q=False)[0] == 0
+    assert _call(library, "search", api.QUERY_ID_EXCLUDING, k=0xFFFFFFFF, nq=0, q=False)[0] == INVALID
 
 
-def test_get_elements_null_and_empty(lib):
-    assert lib.granne_b200_get_elements(None, None, 0, None) == INVALID
-    assert lib.granne_b200_get_elements(FAKE, None, 3, None) == INVALID
-    assert lib.granne_b200_get_elements_device(None, None, 0, None, None) == INVALID
-    assert lib.granne_b200_get_elements_device(FAKE, None, 0, None, None) == 0
+def test_get_elements_null_and_empty(library):
+    assert library.granne_b200_get_elements(None, None, 0, None) == INVALID
+    assert library.granne_b200_get_elements(FAKE, None, 3, None) == INVALID
+    assert library.granne_b200_get_elements_device(None, None, 0, None, None) == INVALID
+    assert library.granne_b200_get_elements_device(FAKE, None, 0, None, None) == 0
 
 
-def test_abi_symbols_and_constants(lib):
+def test_abi_symbols_and_constants(library):
     header = open(os.path.join(ROOT, "include", "granne_b200.h")).read()
     assert re.search(r"#define GRANNE_B200_QUERY_ID 2\b", header)
     assert re.search(r"#define GRANNE_B200_QUERY_ID_EXCLUDING 3\b", header)
@@ -130,13 +122,8 @@ def test_abi_symbols_and_constants(lib):
     assert (api.QUERY_ID, api.QUERY_ID_EXCLUDING) == (2, 3)
 
 
-def test_cxx_ids_client_compiles(lib, tmp_path):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    libdir = os.path.dirname(granne_b200.library_path())
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-Wall", "-Wextra", "-Werror", "-I" + os.path.join(ROOT, "include"),
-                           os.path.join(ROOT, "tests", "helpers", "cxx_ids_client.cpp"), "-o",
-                           str(tmp_path / "client"), "-L" + libdir, "-lgranne_b200", "-Wl,-rpath," + libdir])
+def test_cxx_ids_client_compiles(library, tmp_path):
+    compile_cxx_client("cxx_ids_client.cpp", tmp_path)
 
 
 class _Fake(api.Granne):
@@ -182,9 +169,9 @@ def test_python_device_ids_must_be_int32_cuda():
         g.get_elements_device(np.array([1, 2], np.int32))
 
 
-def test_stream_status_of_and_part_len(lib):
-    assert lib.granne_b200_stream_status_of(None, None) == INVALID
-    assert lib.granne_b200_multi_part_len(None, 0) == 0
+def test_stream_status_of_and_part_len(library):
+    assert library.granne_b200_stream_status_of(None, None) == INVALID
+    assert library.granne_b200_multi_part_len(None, 0) == 0
     header = open(os.path.join(ROOT, "include", "granne_b200.h")).read()
     assert "int granne_b200_stream_status_of(granne_b200_index* h, void* cuda_stream);" in header
     assert "fn granne_b200_multi_part_len(" in open(os.path.join(ROOT, "bindings", "rust", "src", "lib.rs")).read()

@@ -10,22 +10,16 @@ import numpy as np
 import pytest
 
 import granne_b200
-from helpers import exact_oracle as xo
+from helpers import composed_oracle as co
 from helpers.data import build_fixture, index_from_lists, random_vectors
+from helpers.fixtures import assert_same, cxx_client
+from helpers.fixtures import library  # noqa: F401  (autouse)
 
 pytestmark = pytest.mark.gpu
 
 UNUSED = 0xFFFFFFFF
 OUT_OF_RANGE = -8
 CALLS = ["search", "exact", "within", "filtered"]
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _lib():
-    from granne_b200 import build
-
-    build.build()
-    granne_b200.load_library()
 
 
 _CACHE = {}
@@ -92,14 +86,6 @@ def _device(g, call, q, k, lists=None, words=None, **kw):
             stats.cpu().numpy().view(np.uint64) if stats is not None else None)
 
 
-def _same(a, b, stats=True):
-    assert np.array_equal(a[2], b[2])
-    assert np.array_equal(a[0], b[0])
-    assert np.array_equal(np.asarray(a[1]).view(np.uint32), np.asarray(b[1]).view(np.uint32))
-    if stats and a[3] is not None and b[3] is not None:
-        assert np.array_equal(a[3][:, :3], b[3][:, :3])
-
-
 def _exclude_model(res, ids, k):
     """QUERY_ID_EXCLUDING from the QUERY_ID result with k + 1 columns: self removed, cut to k (ids of the result's
     own dtype: u32, or u64 global ids, padded with its maximum)."""
@@ -144,13 +130,13 @@ def test_id_call_equals_element_call(oracle, kind, dim, call):
     rows = g.get_elements(ids)
     for k in (0, 1, 10, 45):
         want = _host(g, call, rows, k, lists, words, already_element=True)
-        _same(_host(g, call, ids, k, lists, words, by_id=True), want)
+        assert_same(_host(g, call, ids, k, lists, words, by_id=True), want, stats=True)
         d_ids = torch.from_numpy(ids.view(np.int32)).cuda(g.device)
-        _same(_device(g, call, d_ids, k, lists, words, by_id=True), want)
+        assert_same(_device(g, call, d_ids, k, lists, words, by_id=True), want, stats=True)
         kk = min(k + 1, 1024)
         model = _exclude_model(_host(g, call, ids, kk, lists, words, by_id=True), ids, k)
-        _same(_host(g, call, ids, k, lists, words, exclude_self=True), model)
-        _same(_device(g, call, d_ids, k, lists, words, exclude_self=True), model)
+        assert_same(_host(g, call, ids, k, lists, words, exclude_self=True), model, stats=True)
+        assert_same(_device(g, call, d_ids, k, lists, words, exclude_self=True), model, stats=True)
     g.stream_status()
 
 
@@ -161,10 +147,10 @@ def test_search_by_id_equals_the_oracle(oracle, kind, dim):
     rows = np.stack([el.get(int(i)) for i in ids])
     wi, wd, wc, ws = og.search_batch(rows, 40, 12, already_element=True, with_stats=True)
     gi, gd, gc, gs = g.search_batch(ids, 40, 12, by_id=True, with_stats=True)
-    _same((gi, gd, gc, gs), (wi, wd, wc, np.c_[ws, np.zeros(len(ids), np.uint64)]))
-    c = xo.Container(kind, el.to_bytes(0), el.to_bytes(1) if kind == "embeddings" else None)
-    _same((*g.exact_search_batch(ids, 12, by_id=True), None),
-          (*c.exact_search(rows, 12, index_len=len(g), already_element=True), None))
+    assert_same((gi, gd, gc, gs), (wi, wd, wc, np.c_[ws, np.zeros(len(ids), np.uint64)]), stats=True)
+    c = co.Container(kind, el.to_bytes(0), el.to_bytes(1) if kind == "embeddings" else None)
+    assert_same((*g.exact_search_batch(ids, 12, by_id=True), None),
+                (*c.exact_search(rows, 12, index_len=len(g), already_element=True), None), stats=True)
 
 
 def test_exclusion_edges(oracle):
@@ -182,7 +168,7 @@ def test_exclusion_edges(oracle):
     assert np.array_equal(wi[0], g.exact_search_within(ids, lists, 2, by_id=True)[0])
     # k > max_search: at most max_search results exist; without self one fewer when self is found
     got = g.search_batch(ids, 5, 20, exclude_self=True, with_stats=True)
-    _same(got, _exclude_model(g.search_batch(ids, 5, 21, by_id=True, with_stats=True), ids, 20))
+    assert_same(got, _exclude_model(g.search_batch(ids, 5, 21, by_id=True, with_stats=True), ids, 20), stats=True)
     assert (got[2] <= 5).all()
     # k = 1023 on the capped calls
     words = np.full((1, 19), 0xFFFFFFFF, np.uint32)
@@ -190,7 +176,7 @@ def test_exclusion_edges(oracle):
         res = _host(g, call, ids, 1023, [np.arange(600, dtype=np.uint32)] * len(ids), words, exclude_self=True)
         model = _exclude_model(_host(g, call, ids, 1024, [np.arange(600, dtype=np.uint32)] * len(ids), words,
                                      by_id=True), ids, 1023)
-        _same(res, model)
+        assert_same(res, model, stats=True)
         with pytest.raises(granne_b200.GranneError):
             _host(g, call, ids, 1024, [np.arange(600, dtype=np.uint32)] * len(ids), words, exclude_self=True)
     # nq = 0 in every call, host and device
@@ -229,7 +215,7 @@ def test_bad_ids(oracle, kind, dim):
             assert got[2][1] == 0 and (got[0][1] == UNUSED).all() and np.isinf(got[1][1]).all()
             if got[3] is not None:
                 assert (got[3][1] == 0).all()
-            _same(tuple(None if x is None else x[[0, 2]] for x in got), want)
+            assert_same(tuple(None if x is None else x[[0, 2]] for x in got), want, stats=True)
             with pytest.raises(granne_b200.GranneError) as ei:
                 g.stream_status()
             assert ei.value.code == OUT_OF_RANGE
@@ -252,9 +238,9 @@ def test_builder_snapshot_ids_past_len():
     assert len(g) == 1000 and g.num_elements() == 1500
     ids = np.array([999, 1000, 1499, 1200], np.uint32)
     rows = g.get_elements(ids)
-    _same(_host(g, "search", ids, 8, by_id=True), _host(g, "search", rows, 8, already_element=True))
-    _same(_host(g, "exact", ids, 8, exclude_self=True),
-          _exclude_model(_host(g, "exact", ids, 9, by_id=True), ids, 8))
+    assert_same(_host(g, "search", ids, 8, by_id=True), _host(g, "search", rows, 8, already_element=True), stats=True)
+    assert_same(_host(g, "exact", ids, 8, exclude_self=True),
+                _exclude_model(_host(g, "exact", ids, 9, by_id=True), ids, 8), stats=True)
     with pytest.raises(granne_b200.GranneError):
         g.search_batch(np.array([1500], np.uint32), 40, 8, by_id=True)
 
@@ -270,9 +256,9 @@ def test_retry_and_slow_passes(oracle):
     got = g.search_batch(ids, ef, 10, by_id=True, with_stats=True)
     flags = got[3][:, 3]
     assert (flags == 0).any() and (flags >= 1).any(), np.bincount(flags.astype(np.int64))
-    _same(got, g.search_batch(g.get_elements(ids), ef, 10, already_element=True, with_stats=True))
-    _same(g.search_batch(ids, ef, 10, exclude_self=True, with_stats=True),
-          _exclude_model(g.search_batch(ids, ef, 11, by_id=True, with_stats=True), ids, 10))
+    assert_same(got, g.search_batch(g.get_elements(ids), ef, 10, already_element=True, with_stats=True), stats=True)
+    assert_same(g.search_batch(ids, ef, 10, exclude_self=True, with_stats=True),
+                _exclude_model(g.search_batch(ids, ef, 11, by_id=True, with_stats=True), ids, 10), stats=True)
     g.close()
     # the all-identical plateau (test_parity_regimes_gpu): every query is answered by the slow pass
     n, dim = 400, 8
@@ -286,11 +272,11 @@ def test_retry_and_slow_passes(oracle):
     assert (got[3][:, 3] == 2).all()
     wi, wd, wc, ws = og.search_batch(np.stack([el.get(int(i)) for i in ids]), 20, 10, already_element=True,
                                      with_stats=True)
-    _same(got, (wi, wd, wc, ws))
+    assert_same(got, (wi, wd, wc, ws), stats=True)
     got = g.search_batch(ids, 20, 10, exclude_self=True, with_stats=True)
     assert (got[3][:, 3] == 2).all()
-    _same(got, _exclude_model((*og.search_batch(np.stack([el.get(int(i)) for i in ids]), 20, 11,
-                                                  already_element=True), None), ids, 10))
+    assert_same(got, _exclude_model((*og.search_batch(np.stack([el.get(int(i)) for i in ids]), 20, 11,
+                                                      already_element=True), None), ids, 10), stats=True)
     g.close()
 
 
@@ -359,10 +345,10 @@ def test_multi_handle(oracle, mode):
         return (*m.search_batch_filtered(q, words, max_search=40, num_elements=k, **kw), None)
 
     for call in CALLS:
-        _same(run(call, gids, 10, by_id=True), run(call, rows, 10, already_element=True))
+        assert_same(run(call, gids, 10, by_id=True), run(call, rows, 10, already_element=True), stats=True)
         ri, rd, rc, _ = run(call, rows, 11, already_element=True)
         want = _exclude_model((ri, rd, rc, None), gids, 10)
-        _same(run(call, gids, 10, exclude_self=True), want)
+        assert_same(run(call, gids, 10, exclude_self=True), want, stats=True)
     with pytest.raises(granne_b200.GranneError) as ei:
         m.search_batch(np.array([10**9], np.uint64), 40, 10, by_id=True)
     assert ei.value.code == OUT_OF_RANGE
@@ -380,7 +366,7 @@ def test_knn_graph(oracle):
         emb = z["embeddings"].tobytes() if z["embeddings"].size else None
         kind, eb = str(z["kind"]), z["elements"].tobytes()
         handles.append((granne_b200.Granne.from_bytes(z["index"].tobytes(), kind, eb, emb),
-                        (oracle.Elements.from_bytes(kind, eb, emb), xo.Container(kind, eb, emb))))
+                        (oracle.Elements.from_bytes(kind, eb, emb), co.Container(kind, eb, emb))))
     raw = random_vectors(20000, 32, seed=11)
     b = granne_b200.GranneBuilder("angular", granne_b200.elements_from_raw("angular", raw), num_neighbors=16,
                                   max_search=60)
@@ -390,17 +376,17 @@ def test_knn_graph(oracle):
         n = len(g)
         ids = np.arange(n, dtype=np.uint32)
         gi, gd, gc = g.knn_graph(max_search=60, num_elements=8, chunk=777)
-        _same((gi, gd, gc, None), (*g.search_batch(ids, 60, 8, exclude_self=True), None))
+        assert_same((gi, gd, gc, None), (*g.search_batch(ids, 60, 8, exclude_self=True), None), stats=True)
         assert not (gi == ids[:, None]).any()
         xi, xd, xc = g.knn_graph(num_elements=8, exact=True, chunk=4096)
-        _same((xi, xd, xc, None), (*g.exact_search_batch(ids, 8, exclude_self=True), None))
+        assert_same((xi, xd, xc, None), (*g.exact_search_batch(ids, 8, exclude_self=True), None), stats=True)
         if el is not None:
             rows = np.stack([el[0].get(int(i)) for i in ids])
             wi, wd, wc = el[1].exact_search(rows, 9, index_len=n, already_element=True)
-            _same((xi, xd, xc, None), _exclude_model((wi, wd, wc, None), ids, 8))
+            assert_same((xi, xd, xc, None), _exclude_model((wi, wd, wc, None), ids, 8), stats=True)
         di, dd, dc = g.knn_graph(max_search=60, num_elements=8, exclude_self=False, out="device")
-        _same((di.cpu().numpy().view(np.uint32), dd.cpu().numpy(), dc.cpu().numpy().view(np.uint32), None),
-              (*g.search_batch(ids, 60, 8, by_id=True), None))
+        assert_same((di.cpu().numpy().view(np.uint32), dd.cpu().numpy(), dc.cpu().numpy().view(np.uint32), None),
+                    (*g.search_batch(ids, 60, 8, by_id=True), None), stats=True)
 
 
 @pytest.mark.parametrize("mode", ["replicated", "partitioned"])
@@ -425,7 +411,7 @@ def test_multi_knn_graph(oracle, mode):
     k = 6
     per = []
     for (_, eb, el), b in zip(shards, bases):
-        li, ld, lc = xo.Container("angular", eb).exact_search(rows, k + 1, index_len=len(el), already_element=True)
+        li, ld, lc = co.Container("angular", eb).exact_search(rows, k + 1, index_len=len(el), already_element=True)
         per.append((np.where(li == UNUSED, np.uint64(2**64 - 1), li.astype(np.uint64) + np.uint64(b)), ld, lc))
     wi = np.full((len(gids), k + 1), np.uint64(2**64 - 1))
     wd = np.full((len(gids), k + 1), np.inf, np.float32)
@@ -439,10 +425,10 @@ def test_multi_knn_graph(oracle, mode):
         wd[q, :len(cand)] = [d for d, _ in cand]
     want = _exclude_model((wi, wd, wc, None), gids, k)
     xi, xd, xc = m.knn_graph(num_elements=k, exact=True, chunk=97)
-    _same((xi, xd, xc, None), want)
+    assert_same((xi, xd, xc, None), want, stats=True)
     assert not (xi == gids[:, None]).any()
     gi, gd, gc = m.knn_graph(max_search=40, num_elements=k, chunk=128)
-    _same((gi, gd, gc, None), (*m.search_batch(gids, 40, k, exclude_self=True), None))
+    assert_same((gi, gd, gc, None), (*m.search_batch(gids, 40, k, exclude_self=True), None), stats=True)
     assert not (gi == gids[:, None]).any()
     m.close()
 
@@ -460,22 +446,9 @@ def test_knn_graph_reports_only_its_own_stream(oracle):
 
 
 def test_cxx_ids_client(oracle, tmp_path):
-    import os
-    import shutil
-    import subprocess
-
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     el, _, ib, eb, _ = build_fixture(oracle, "angular", 1500, 32, seed=21, num_neighbors=12, max_search=50)
     (tmp_path / "index").write_bytes(ib)
     (tmp_path / "elements").write_bytes(eb)
-    libdir = os.path.dirname(granne_b200.library_path())
-    exe = tmp_path / "cxx_ids_client"
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-Wall", "-Wextra", "-Werror", "-I" + os.path.join(root, "include"),
-                           os.path.join(root, "tests", "helpers", "cxx_ids_client.cpp"), "-o", str(exe),
-                           "-L" + libdir, "-lgranne_b200", "-Wl,-rpath," + libdir])
-    out = subprocess.run([str(exe), str(tmp_path / "index"), str(tmp_path / "elements")], capture_output=True,
-                         text=True, timeout=300)
+    out = cxx_client("cxx_ids_client.cpp", [tmp_path / "index", tmp_path / "elements"], tmp_path, timeout=300)
     assert out.returncode == 0 and "ok" in out.stdout, out.stdout + out.stderr
     assert float(out.stdout.split()[1]) > 0.95  # verify_search's bar (src/index/tests.rs:50-62)

@@ -4,14 +4,14 @@ and the Rust shim, and the Python packing and rejections.  The rules are checked
 handle that is never dereferenced serves."""
 import ctypes as C
 import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
 import granne_b200
 from granne_b200 import api
+from helpers.fixtures import compile_cxx_client
+from helpers.fixtures import library  # noqa: F401  (autouse)
 
 INVALID = -1
 FAKE = C.c_void_p(1)  # never dereferenced by a call whose arguments break a rule
@@ -26,14 +26,6 @@ COUNTS_NULL = "counts is null"
 OFFSETS_NULL = "offsets is null"
 OFFSETS_SHAPE = "offsets must start at 0 and not decrease"
 CALLS = ["count", "count_device", "search", "search_device"]
-
-
-@pytest.fixture(scope="module")
-def lib():
-    from granne_b200 import build
-
-    build.build()
-    return granne_b200.load_library()
 
 
 def _call(lib, call, h=FAKE, q=True, nq=2, fmt=api.QUERY_RAW_F32, radius=0.5, counts=True, offsets=(0, 2, 3),
@@ -59,47 +51,47 @@ def _call(lib, call, h=FAKE, q=True, nq=2, fmt=api.QUERY_RAW_F32, radius=0.5, co
 
 
 @pytest.mark.parametrize("call", CALLS)
-def test_rules_in_order(lib, call):
+def test_rules_in_order(library, call):
     nan = float("nan")
     # validate_batch's order: handle, format, the NaN radius (the call's own rule), batch size, queries
-    assert _call(lib, call, h=None, fmt=7, radius=nan) == (INVALID, HANDLE)
-    assert _call(lib, call, fmt=7, radius=nan, nq=TOO_MANY) == (INVALID, FORMAT)
-    assert _call(lib, call, radius=nan, nq=TOO_MANY, q=False) == (INVALID, RADIUS)
-    assert _call(lib, call, nq=TOO_MANY, q=False) == (INVALID, NQ)
-    assert _call(lib, call, q=False, counts=False, offsets=None) == (INVALID, NULL)
+    assert _call(library, call, h=None, fmt=7, radius=nan) == (INVALID, HANDLE)
+    assert _call(library, call, fmt=7, radius=nan, nq=TOO_MANY) == (INVALID, FORMAT)
+    assert _call(library, call, radius=nan, nq=TOO_MANY, q=False) == (INVALID, RADIUS)
+    assert _call(library, call, nq=TOO_MANY, q=False) == (INVALID, NQ)
+    assert _call(library, call, q=False, counts=False, offsets=None) == (INVALID, NULL)
     # then the call's own output: counts, or offsets
     if call.startswith("count"):
-        assert _call(lib, call, counts=False) == (INVALID, COUNTS_NULL)
+        assert _call(library, call, counts=False) == (INVALID, COUNTS_NULL)
     else:
-        assert _call(lib, call, offsets=None, outs=False) == (INVALID, OFFSETS_NULL)
+        assert _call(library, call, offsets=None, outs=False) == (INVALID, OFFSETS_NULL)
 
 
 @pytest.mark.parametrize("call", CALLS)
-def test_nan_radius_is_rejected_even_without_queries(lib, call):
-    assert _call(lib, call, radius=float("nan"), nq=0, q=False) == (INVALID, RADIUS)
+def test_nan_radius_is_rejected_even_without_queries(library, call):
+    assert _call(library, call, radius=float("nan"), nq=0, q=False) == (INVALID, RADIUS)
 
 
 @pytest.mark.parametrize("call", CALLS)
-def test_no_queries_is_ok_before_the_handle_is_read(lib, call):
+def test_no_queries_is_ok_before_the_handle_is_read(library, call):
     for fmt in (api.QUERY_RAW_F32, api.QUERY_ELEMENT, api.QUERY_ID, api.QUERY_ID_EXCLUDING):
-        assert _call(lib, call, fmt=fmt, nq=0, q=False, counts=False, offsets=None, outs=False)[0] == 0
+        assert _call(library, call, fmt=fmt, nq=0, q=False, counts=False, offsets=None, outs=False)[0] == 0
     for radius in (float("inf"), float("-inf"), -0.0, 0.0, -1.0):
-        assert _call(lib, call, radius=radius, nq=0, q=False, counts=False, offsets=None, outs=False)[0] == 0
+        assert _call(library, call, radius=radius, nq=0, q=False, counts=False, offsets=None, outs=False)[0] == 0
 
 
-def test_host_search_checks_offsets_then_outputs(lib):
-    assert _call(lib, "search", offsets=(1, 2, 3)) == (INVALID, OFFSETS_SHAPE)
-    assert _call(lib, "search", offsets=(0, 2, 1)) == (INVALID, OFFSETS_SHAPE)
-    assert _call(lib, "search", offsets=(0, 2, 1), outs=False) == (INVALID, OFFSETS_SHAPE)
-    assert _call(lib, "search", outs=False) == (INVALID, NULL)  # offsets[nq] > 0
+def test_host_search_checks_offsets_then_outputs(library):
+    assert _call(library, "search", offsets=(1, 2, 3)) == (INVALID, OFFSETS_SHAPE)
+    assert _call(library, "search", offsets=(0, 2, 1)) == (INVALID, OFFSETS_SHAPE)
+    assert _call(library, "search", offsets=(0, 2, 1), outs=False) == (INVALID, OFFSETS_SHAPE)
+    assert _call(library, "search", outs=False) == (INVALID, NULL)  # offsets[nq] > 0
 
 
-def test_multi_null_handle(lib):
+def test_multi_null_handle(library):
     cnt = np.zeros(1, np.uint64)
     offs = np.zeros(2, np.uint64)
-    assert lib.granne_b200_multi_exact_range_count(None, None, 0, 0, 0.5, api._ptr(cnt)) == INVALID
-    assert lib.granne_b200_multi_exact_range_search(None, None, 0, 0, 0.5, api._ptr(offs), None, None) == INVALID
-    assert lib.granne_b200_last_error().decode() == "multi handle is null"
+    assert library.granne_b200_multi_exact_range_count(None, None, 0, 0, 0.5, api._ptr(cnt)) == INVALID
+    assert library.granne_b200_multi_exact_range_search(None, None, 0, 0, 0.5, api._ptr(offs), None, None) == INVALID
+    assert library.granne_b200_last_error().decode() == "multi handle is null"
 
 
 NAMES = ["granne_b200_exact_range_count", "granne_b200_exact_range_count_device", "granne_b200_exact_range_search",
@@ -107,14 +99,14 @@ NAMES = ["granne_b200_exact_range_count", "granne_b200_exact_range_count_device"
          "granne_b200_multi_exact_range_search"]
 
 
-def test_symbols_in_the_headers_and_the_shim(lib):
+def test_symbols_in_the_headers_and_the_shim(library):
     header = open(os.path.join(ROOT, "include", "granne_b200.h")).read()
     raw = C.CDLL(granne_b200.library_path())
     for name in NAMES:
         assert "int %s(" % name in header
         assert hasattr(raw, name)
     assert "#define GRANNE_B200_ABI_VERSION 2 " in header
-    assert lib.granne_b200_abi_version() == 2
+    assert library.granne_b200_abi_version() == 2
     cxx = open(os.path.join(ROOT, "include", "granne_b200.hpp")).read()
     assert cxx.count("exact_range_search(const void* queries, size_t nq, int query_format, float radius) const") == 2
     shim = open(os.path.join(ROOT, "bindings", "rust", "src", "lib.rs")).read()
@@ -124,13 +116,8 @@ def test_symbols_in_the_headers_and_the_shim(lib):
     assert shim.count("pub fn exact_range_search(") == 2
 
 
-def test_cxx_range_client_compiles(lib, tmp_path):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    libdir = os.path.dirname(granne_b200.library_path())
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-Wall", "-Wextra", "-Werror", "-I" + os.path.join(ROOT, "include"),
-                           os.path.join(ROOT, "tests", "helpers", "cxx_range_client.cpp"), "-o",
-                           str(tmp_path / "client"), "-L" + libdir, "-lgranne_b200", "-Wl,-rpath," + libdir])
+def test_cxx_range_client_compiles(library, tmp_path):
+    compile_cxx_client("cxx_range_client.cpp", tmp_path)
 
 
 class _Fake(api.Granne):

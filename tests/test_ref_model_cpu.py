@@ -9,9 +9,10 @@ from fractions import Fraction
 import numpy as np
 import pytest
 
-from helpers import exact_oracle as xo
+from helpers import composed_oracle as co
 from helpers import ref_model as M
 from helpers.data import edge_i8_rows, edge_raw_f32, index_from_lists, random_sum_embeddings, random_vectors
+from helpers.fixtures import elements_image
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 U32 = np.uint32
@@ -162,10 +163,6 @@ def test_f32_distance_within_float64_bound(dim):
 
 
 # ---- exact ranking ---------------------------------------------------------------------------------------------------
-def _image(rows):
-    return np.uint64(rows.shape[1]).tobytes() + np.ascontiguousarray(rows).tobytes()
-
-
 @pytest.mark.parametrize("kind", ["angular", "angular_int"])
 def test_exact_ranking(kind):
     raw = edge_raw_f32(300, 33, 5)
@@ -173,7 +170,7 @@ def test_exact_ranking(kind):
     rows[40:60] = rows[10]  # ties broken by id
     q = M.element_rows(kind, random_vectors(12, 33, 6))
     q[0] = rows[10]
-    c = xo.Container(kind, _image(rows))
+    c = co.Container(kind, elements_image(rows))
     d = M.distances(kind, rows, q)
     for k in (1, 10, 64, 400):
         want = c.exact_search(q, k, already_element=True)

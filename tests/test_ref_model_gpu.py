@@ -10,6 +10,8 @@ import pytest
 import granne_b200
 from helpers import ref_model as M
 from helpers.data import edge_i8_rows, edge_raw_f32, index_from_lists, random_vectors
+from helpers.fixtures import elements_image
+from helpers.fixtures import library  # noqa: F401  (autouse)
 from helpers.index_image import assert_same_index
 from helpers.model_checks import assert_same, assert_within_f64_bound
 
@@ -19,21 +21,8 @@ F32_WIDTHS = [1, 33, 2101, 4096, 8192, 16384]
 I8_WIDTHS = [1041, 4096, 16384]
 
 
-@pytest.fixture(scope="module", autouse=True)
-def _lib():
-    from granne_b200 import build
-
-    build.build()
-    granne_b200.load_library()
-
-
 def _bits(a):
     return np.asarray(a, dtype=np.float32).view(np.uint32)
-
-
-def _image(rows):
-    rows = np.ascontiguousarray(rows)
-    return np.uint64(rows.shape[1]).tobytes() + rows.tobytes()
 
 
 def _host(t):
@@ -81,7 +70,7 @@ def _case(kind, dim):
 
 
 def _open(oracle, kind, rows, layers):
-    return granne_b200.Granne.from_bytes(index_from_lists(oracle, layers), kind, _image(rows))
+    return granne_b200.Granne.from_bytes(index_from_lists(oracle, layers), kind, elements_image(rows))
 
 
 # ---- every query call on dense indexes at every width -------------------------------------------------------------------
@@ -175,7 +164,7 @@ def test_elements_from_raw_and_compute_distances(dim):
     for kind in ("angular", "angular_int"):
         img = granne_b200.elements_from_raw(kind, raw)
         want = M.element_rows(kind, raw)
-        assert bytes(img) == _image(want), kind
+        assert bytes(img) == elements_image(want), kind
     a, b = raw, np.roll(raw, 1, axis=0)
     b[:4] = a[:4]
     a[9] = a[9] * np.float32(-3)
@@ -192,7 +181,7 @@ def test_elements_from_raw_at_its_width_limit():
     raw = edge_raw_f32(12, 12000, 5)
     for kind in ("angular", "angular_int"):
         want = M.element_rows(kind, raw)
-        assert bytes(granne_b200.elements_from_raw(kind, raw)) == _image(want), kind
+        assert bytes(granne_b200.elements_from_raw(kind, raw)) == elements_image(want), kind
         got = granne_b200.api.elements_from_raw_device(kind, torch.from_numpy(raw).cuda())
         assert np.array_equal(_host(got).view(np.uint8), want.view(np.uint8)), kind
         with pytest.raises(granne_b200.GranneError):
@@ -217,7 +206,7 @@ def test_compute_embeddings_at_the_table_limit(oracle):
     sums = np.stack([M.sum_embedding(table, t) for t in terms])
     for kind in ("angular", "angular_int"):
         img = granne_b200.api.compute_embeddings(kind, eb, mb)
-        assert bytes(img) == _image(M.element_rows(kind, sums)), kind
+        assert bytes(img) == elements_image(M.element_rows(kind, sums)), kind
 
 
 def test_embeddings_search_and_rerank_at_the_table_limit(oracle):
@@ -241,7 +230,7 @@ def test_embeddings_search_and_rerank_at_the_table_limit(oracle):
 
     # two-stage: an angular_int index over the quantised sums, re-ranked by the SumEmbeddings container
     q8 = M.quantize(np.stack([M.sum_embedding(table, t) for t in terms]))
-    p = granne_b200.Granne.from_bytes(ib, "angular_int", _image(q8))
+    p = granne_b200.Granne.from_bytes(ib, "angular_int", elements_image(q8))
     p.set_rerank_embeddings(eb, mb)
     d8 = M.distances("angular_int", q8, M.quantize(raw))
     want = [M.rerank(layers, d8[q], d[q], 40, 25, 10) for q in range(len(raw))]
@@ -256,8 +245,8 @@ def test_rerank_over_attached_f32_rows(oracle, dim):
     raw_rows = edge_raw_f32(n, dim, dim)
     f, q8 = M.normalize_f32(raw_rows), M.quantize(raw_rows)
     layers = graph(n, dim + 1)
-    p = granne_b200.Granne.from_bytes(index_from_lists(oracle, layers), "angular_int", _image(q8))
-    p.set_rerank_elements(_image(f))
+    p = granne_b200.Granne.from_bytes(index_from_lists(oracle, layers), "angular_int", elements_image(q8))
+    p.set_rerank_elements(elements_image(f))
     raw = random_vectors(10, dim, 4)
     d8, df = M.distances("angular_int", q8, M.quantize(raw)), M.distances("angular", f, M.normalize_f32(raw))
     for ef, c, k in ((20, 20, 10), (60, 50, 50)):
@@ -287,7 +276,7 @@ def test_multi_handle_one_gpu(oracle, kind, dim):
     raw = raw[:10]
     q = M.element_rows(kind, raw)
     ib = index_from_lists(oracle, layers)
-    m = granne_b200.MultiGranne.replicated(ib, kind, _image(rows), [0])
+    m = granne_b200.MultiGranne.replicated(ib, kind, elements_image(rows), [0])
     d = M.distances(kind, rows, q)
     want = [M.search(layers, d[i], 20, 10)[0] for i in range(len(q))]
     assert_same(m.search_batch(raw, 20, 10), want, 10, "replicated search", np.uint64)
@@ -297,7 +286,8 @@ def test_multi_handle_one_gpu(oracle, kind, dim):
 
     cut = n // 2 + 3
     parts = [(rows[:cut], graph(cut, 1)), (rows[cut:], graph(n - cut, 2))]
-    m = granne_b200.MultiGranne.partitioned([(index_from_lists(oracle, l), _image(r)) for r, l in parts], kind, [0, 0])
+    m = granne_b200.MultiGranne.partitioned([(index_from_lists(oracle, l), elements_image(r)) for r, l in parts], kind,
+                                            [0, 0])
     bases = [m.shard_base(s) for s in range(2)]
     assert bases == [0, cut]
     ds = [M.distances(kind, r, q) for r, _ in parts]
@@ -329,7 +319,7 @@ def test_every_pass_of_the_ladder_against_the_model(oracle):
     n, dim = 400, 8
     rows = M.normalize_f32(np.tile(random_vectors(1, dim, seed=5), (n, 1)))
     layers = [[sorted({(i * 30 + j) % n for j in range(1, 31)} - {i}) for i in range(n)]]
-    p = granne_b200.Granne.from_bytes(index_from_lists(oracle, layers), "angular", _image(rows))
+    p = granne_b200.Granne.from_bytes(index_from_lists(oracle, layers), "angular", elements_image(rows))
     raw = random_vectors(256, dim, seed=6)
     d = M.distances("angular", rows, M.normalize_f32(raw))
     got = p.search_batch(raw, 20, 10, with_stats=True)

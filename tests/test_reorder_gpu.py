@@ -5,16 +5,9 @@ import pytest
 
 import granne_b200
 from helpers.data import build_fixture, random_vectors
+from helpers.fixtures import library  # noqa: F401  (autouse)
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _lib():
-    from granne_b200 import build
-
-    build.build()
-    granne_b200.load_library()
 
 
 def _assert_same_results(ref, got):

@@ -4,9 +4,6 @@ oracle's own pieces: its angular_int search gives the candidate set S, angular::
 distance, and (distance, id) order picks the first k.  Also: every f32 engine layout, the edges of C and k, the
 rejections, the stage-1 and recall identities, concurrent use, every handle source, the multi handle and a C++ client."""
 import ctypes as C
-import os
-import shutil
-import subprocess
 import threading
 
 import numpy as np
@@ -15,25 +12,13 @@ import pytest
 import granne_b200
 from granne_b200 import api
 from helpers.data import clustered_vectors, random_vectors
+from helpers.fixtures import assert_same, cxx_client, elements_image
+from helpers.fixtures import library  # noqa: F401  (autouse)
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 INVALID, FORMAT, NOT_FINITE = -1, -2, -6
 UNUSED = 0xFFFFFFFF
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _lib():
-    from granne_b200 import build
-
-    build.build()
-    granne_b200.load_library()
-
-
-def _image(rows):
-    rows = np.ascontiguousarray(rows)
-    return np.uint64(rows.shape[1]).tobytes() + rows.tobytes()
 
 
 class Composed:
@@ -69,14 +54,6 @@ class Composed:
         return g
 
 
-def _same(got, want):
-    gi, gd, gc = got
-    wi, wd, wc = want
-    assert np.array_equal(np.asarray(gc).view(np.uint32), wc)
-    assert np.array_equal(np.asarray(gi).view(np.uint32), wi)
-    assert np.array_equal(np.asarray(gd).view(np.uint32), wd.view(np.uint32))
-
-
 def _oracle_case(go, n, dim, seed, m=10, ef=40):
     raw = random_vectors(n, dim, seed)
     el = go.Elements.angular_int(raw)
@@ -92,7 +69,7 @@ def test_every_f32_engine_layout(oracle, dim):
     g = c.gpu()
     q = random_vectors(24, dim, dim + 7)
     got = g.search_batch_rerank(q, 30, max_search=50, num_elements=10)
-    _same(got, c.rerank(q, 50, 30, 10))
+    assert_same(got, c.rerank(q, 50, 30, 10))
     # stage 1 is search_batch(q, max_search, C) on the same handle: with k = C the result is that set, re-ordered
     si, _, sc = g.search_batch(q, 50, 30)
     ai, ad, ac = g.search_batch_rerank(q, 30, max_search=50, num_elements=30)
@@ -116,10 +93,10 @@ def test_gpu_built_index_and_get_index_handle(oracle, dim):
     c = Composed(oracle, b.index_bytes().tobytes(), raw)
     q = random_vectors(40, dim, 3)
     want = c.rerank(q, 60, 40, 10)
-    _same(c.gpu().search_batch_rerank(q, 40, max_search=60), want)
+    assert_same(c.gpu().search_batch_rerank(q, 40, max_search=60), want)
     snap = b.get_index()
     snap.set_rerank_elements(c.f32.to_bytes())
-    _same(snap.search_batch_rerank(q, 40, max_search=60), want)
+    assert_same(snap.search_batch_rerank(q, 40, max_search=60), want)
 
 
 @pytest.mark.parametrize("max_search,cands,k", [(50, 1, 1), (50, 10, 10), (50, 50, 10), (20, 100, 10),
@@ -130,7 +107,7 @@ def test_candidate_and_neighbour_edges(oracle, max_search, cands, k):
     q = random_vectors(12, 32, 6)
     got = g.search_batch_rerank(q, cands, max_search=max_search, num_elements=k)
     want = c.rerank(q, max_search, cands, k)
-    _same(got, want)
+    assert_same(got, want)
     assert (want[2] <= min(k, cands, max_search)).all()
 
 
@@ -149,15 +126,15 @@ def test_index_shorter_than_its_containers(oracle):
     g = c.gpu()
     assert len(g) == 400 and g.num_elements() == 600
     got = g.search_batch_rerank(q, 50, max_search=80)
-    _same(got, c.rerank(q, 80, 50, 10))
+    assert_same(got, c.rerank(q, 80, 50, 10))
     assert (got[0] < 400).all()
     # exactly Index::len f32 rows are enough, one fewer is not
     g2 = c.gpu(with_f32=False)
-    g2.set_rerank_elements(_image(c.f32.rows()[:400]))
-    _same(g2.search_batch_rerank(q, 50, max_search=80), got)
+    g2.set_rerank_elements(elements_image(c.f32.rows()[:400]))
+    assert_same(g2.search_batch_rerank(q, 50, max_search=80), got)
     g3 = c.gpu(with_f32=False)
     with pytest.raises(granne_b200.GranneError) as e:
-        g3.set_rerank_elements(_image(c.f32.rows()[:399]))
+        g3.set_rerank_elements(elements_image(c.f32.rows()[:399]))
     assert e.value.code == INVALID
 
 
@@ -168,7 +145,7 @@ def test_duplicate_rows_order_ties_by_id(oracle):
                                               max_search=60).build().to_bytes(), raw)
     q = np.concatenate([base[:8], random_vectors(4, 48, 5)])
     got = c.gpu().search_batch_rerank(q, 100, max_search=150, num_elements=40)
-    _same(got, c.rerank(q, 150, 100, 40))
+    assert_same(got, c.rerank(q, 150, 100, 40))
     d = got[1]
     assert any((d[i, 1:] == d[i, :-1]).any() for i in range(len(q)))  # ties occur, and were ordered by id
 
@@ -188,12 +165,12 @@ def test_rejections(oracle):
     q = random_vectors(3, 32, 8)
     bare = c.gpu(with_f32=False)
     assert _raw_rerank(bare, q) == INVALID  # nothing attached
-    for bad in (b"\x20\x00", _image(c.f32.rows())[:-3]):
+    for bad in (b"\x20\x00", elements_image(c.f32.rows())[:-3]):
         with pytest.raises(granne_b200.GranneError) as e:
             bare.set_rerank_elements(bad)
         assert e.value.code == FORMAT
     with pytest.raises(granne_b200.GranneError) as e:
-        bare.set_rerank_elements(_image(random_vectors(300, 33, 1)))
+        bare.set_rerank_elements(elements_image(random_vectors(300, 33, 1)))
     assert e.value.code == INVALID  # wrong width
     g = c.gpu()
     with pytest.raises(granne_b200.GranneError) as e:
@@ -239,7 +216,7 @@ def test_nan_row_is_not_finite(oracle):
     rows = c.f32.rows().copy()
     rows[only_late[0], 5] = np.nan
     g = c.gpu(with_f32=False)
-    g.set_rerank_elements(_image(rows))
+    g.set_rerank_elements(elements_image(rows))
     with pytest.raises(granne_b200.GranneError) as e:
         g.search_batch_rerank(q, 10, max_search=50)
     assert e.value.code == NOT_FINITE
@@ -287,7 +264,7 @@ def test_device_variant_on_two_streams_and_host_threads(oracle):
     g = c.gpu()
     q = random_vectors(300, 64, 13)
     want = c.rerank(q, 60, 30, 10)
-    _same(g.search_batch_rerank(q, 30, max_search=60), want)
+    assert_same(g.search_batch_rerank(q, 30, max_search=60), want)
     dq = torch.from_numpy(q).cuda()
     streams = [torch.cuda.Stream(), torch.cuda.Stream()]
     outs = []
@@ -310,7 +287,7 @@ def test_device_variant_on_two_streams_and_host_threads(oracle):
     g.stream_status()
     assert len(outs) == 20
     for i, d, cnt in outs:
-        _same((i.view(np.uint32), d, cnt.view(np.uint32)), want)
+        assert_same((i.view(np.uint32), d, cnt.view(np.uint32)), want)
 
 
 def test_device_elements_handle_and_device_attach(oracle):
@@ -325,12 +302,12 @@ def test_device_elements_handle_and_device_attach(oracle):
     assert g.device_bytes() >= before + 800 * 96 * 4
     q = random_vectors(30, 96, 15)
     want = c.rerank(q, 50, 40, 10)
-    _same(g.search_batch_rerank(q, 40, max_search=50), want)
+    assert_same(g.search_batch_rerank(q, 40, max_search=50), want)
     stats = torch.zeros((30, api.STATS_PER_QUERY), dtype=torch.int64, device="cuda")
     got = g.search_batch_rerank_device(torch.from_numpy(q).cuda(), 40, max_search=50, stats=stats)
     torch.cuda.synchronize()
     g.stream_status()
-    _same([t.cpu().numpy() for t in got], want)
+    assert_same([t.cpu().numpy() for t in got], want)
     _, _, _, s1 = g.search_batch(q, 50, 40, with_stats=True)
     _, _, _, hs = g.search_batch_rerank(q, 40, max_search=50, with_stats=True)
     assert np.array_equal(stats.cpu().numpy().view(np.uint64)[:, :3], s1[:, :3])
@@ -370,9 +347,6 @@ def test_multi_replicated_and_partitioned(oracle):
 
 
 def test_cxx_client(tmp_path, oracle):
-    cxx = shutil.which("g++")
-    if cxx is None:
-        pytest.skip("no C++ compiler")
     c = _oracle_case(oracle, 500, 64, 18)
     idx, i8, f32 = tmp_path / "index.bin", tmp_path / "i8.bin", tmp_path / "f32.bin"
     idx.write_bytes(c.index_bytes)
@@ -381,12 +355,7 @@ def test_cxx_client(tmp_path, oracle):
     q = random_vectors(4, 64, 19)
     qf = tmp_path / "q.bin"
     qf.write_bytes(q.tobytes())
-    exe = tmp_path / "client"
-    libdir = os.path.dirname(granne_b200.library_path())
-    subprocess.check_call([cxx, "-std=c++17", "-O1", "-Wall", "-Wextra", "-Werror", "-I" + os.path.join(ROOT, "include"),
-                           os.path.join(ROOT, "tests", "helpers", "cxx_rerank_client.cpp"), "-o", str(exe),
-                           "-L" + libdir, "-lgranne_b200", "-Wl,-rpath," + libdir])
-    out = subprocess.run([str(exe), str(idx), str(i8), str(f32), str(qf)], capture_output=True, text=True, timeout=120)
+    out = cxx_client("cxx_rerank_client.cpp", [idx, i8, f32, qf], tmp_path)
     assert out.returncode == 0, out.stdout + out.stderr
     wi, wd, wc = c.rerank(q, 50, 20, 5)
     lines = out.stdout.split()

@@ -4,51 +4,42 @@ import os
 import re
 
 import numpy as np
-import pytest
 
-import granne_b200
 from granne_b200 import api
+from helpers.fixtures import library  # noqa: F401  (autouse)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 INVALID = -1
 NEW_SYMBOLS = ("granne_b200_set_rerank_embeddings", "granne_b200_multi_set_rerank_embeddings")
 
 
-@pytest.fixture(scope="module")
-def lib():
-    from granne_b200 import build
-
-    build.build()
-    return granne_b200.load_library()
-
-
 def _images():
-    from helpers import embeddings_oracle as eo
+    from helpers import composed_oracle as co
 
     table = np.ones((3, 4), np.float32)
-    return (np.frombuffer(eo.elements_image([[0, 1], [2]]), np.uint8),
-            np.frombuffer(eo.table_image(table), np.uint8))
+    return (np.frombuffer(co.elements_image([[0, 1], [2]]), np.uint8),
+            np.frombuffer(co.table_image(table), np.uint8))
 
 
-def test_calls_without_a_handle_are_invalid(lib):
+def test_calls_without_a_handle_are_invalid(library):
     el, emb = _images()
-    assert lib.granne_b200_set_rerank_embeddings(None, api._ptr(el), el.size, api._ptr(emb), emb.size) == INVALID
-    assert b"null" in lib.granne_b200_last_error()
-    assert lib.granne_b200_set_rerank_embeddings(None, None, 0, None, 0) == INVALID
-    assert b"null" in lib.granne_b200_last_error()
+    assert library.granne_b200_set_rerank_embeddings(None, api._ptr(el), el.size, api._ptr(emb), emb.size) == INVALID
+    assert b"null" in library.granne_b200_last_error()
+    assert library.granne_b200_set_rerank_embeddings(None, None, 0, None, 0) == INVALID
+    assert b"null" in library.granne_b200_last_error()
     import ctypes as C
 
     ptrs = (C.c_void_p * 1)(el.ctypes.data)
     lens = (C.c_size_t * 1)(el.size)
-    assert lib.granne_b200_multi_set_rerank_embeddings(None, ptrs, lens, api._ptr(emb), emb.size) == INVALID
-    assert b"null" in lib.granne_b200_last_error()
-    assert lib.granne_b200_multi_set_rerank_embeddings(None, None, None, None, 0) == INVALID
-    assert b"null" in lib.granne_b200_last_error()
+    assert library.granne_b200_multi_set_rerank_embeddings(None, ptrs, lens, api._ptr(emb), emb.size) == INVALID
+    assert b"null" in library.granne_b200_last_error()
+    assert library.granne_b200_multi_set_rerank_embeddings(None, None, None, None, 0) == INVALID
+    assert b"null" in library.granne_b200_last_error()
 
 
-def test_symbols_exported(lib):
+def test_symbols_exported(library):
     for name in NEW_SYMBOLS:
-        assert hasattr(lib, name), name
+        assert hasattr(library, name), name
 
 
 def test_rust_shim_and_cxx_header_declare_them():

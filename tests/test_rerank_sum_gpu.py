@@ -7,9 +7,6 @@ with the f32 re-rank and the "embeddings" handle, the edges of C and k, NaN tabl
 device memory, every handle source, the multi handle, string queries and a C++ client."""
 import ctypes as C
 import json
-import os
-import shutil
-import subprocess
 import threading
 
 import numpy as np
@@ -17,23 +14,16 @@ import pytest
 
 import granne_b200
 from granne_b200 import api
-from helpers import embeddings_oracle as eo
+from helpers import composed_oracle as co
 from helpers.data import random_vectors
+from helpers.fixtures import assert_same, cxx_client
+from helpers.fixtures import library  # noqa: F401  (autouse)
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 INVALID, FORMAT, NOT_FINITE = -1, -2, -6
 UNUSED = 0xFFFFFFFF
 COUNTS = [0, 1, 2, 9, 32, 33, 300]  # term counts that reach every DistSum branch (none, one, 32-term groups)
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _lib():
-    from granne_b200 import build
-
-    build.build()
-    granne_b200.load_library()
 
 
 def _container(n, dim, num_rows, seed, counts=COUNTS):
@@ -57,8 +47,8 @@ class Composed:
 
     def __init__(self, go, table, elements, index_bytes=None, m=10, ef=40):
         self.table, self.elements = table, elements
-        self.ei, self.ti = eo.elements_image(elements), eo.table_image(table)
-        self.i8_image = eo.compute_embeddings("angular_int", self.ei, self.ti, threads=8).tobytes()
+        self.ei, self.ti = co.elements_image(elements), co.table_image(table)
+        self.i8_image = co.compute_embeddings("angular_int", self.ei, self.ti, threads=8).tobytes()
         self.i8 = go.Elements.from_bytes("angular_int", self.i8_image)
         if index_bytes is None:
             index_bytes = go.GranneBuilder(self.i8, num_neighbors=m, max_search=ef).build().to_bytes()
@@ -90,14 +80,6 @@ class Composed:
         return g
 
 
-def _same(got, want):
-    gi, gd, gc = got
-    wi, wd, wc = want
-    assert np.array_equal(np.asarray(gc).view(np.uint32), wc)
-    assert np.array_equal(np.asarray(gi).view(np.uint32), wi)
-    assert np.array_equal(np.asarray(gd).view(np.uint32), wd.view(np.uint32))
-
-
 def _queries(nq, dim, seed):
     return (random_vectors(nq, dim, seed) * 3).astype(np.float32)
 
@@ -109,13 +91,13 @@ def test_composed_oracle_and_identities(oracle, dim):
     g = c.gpu()
     q = _queries(16, dim, dim + 1)
     got = g.search_batch_rerank(q, 30, max_search=50, num_elements=10)
-    _same(got, c.rerank(q, 50, 30, 10))
+    assert_same(got, c.rerank(q, 50, 30, 10))
 
     # the f32 two-stage search over compute_embeddings("angular") rows on a second handle: the same result
     f32_image = granne_b200.compute_embeddings("angular", c.ei, c.ti).tobytes()
     f = c.gpu(attach=False)
     f.set_rerank_elements(f32_image)
-    _same(f.search_batch_rerank(q, 30, max_search=50, num_elements=10), got)
+    assert_same(f.search_batch_rerank(q, 30, max_search=50, num_elements=10), got)
 
     # with k = C the id set is search_batch(q, max_search, C) on the same handle
     si, _, sc = g.search_batch(q, 50, 30)
@@ -138,7 +120,7 @@ def test_composed_oracle_and_identities(oracle, dim):
 
     # every candidate that is an empty element has distance exactly 1.0; a wide candidate set reaches them
     wi, wd, wc = g.search_batch_rerank(q[:4], 1024, max_search=1024, num_elements=1024)
-    _same((wi, wd, wc), c.rerank(q[:4], 1024, 1024, 1024))
+    assert_same((wi, wd, wc), c.rerank(q[:4], 1024, 1024, 1024))
     empty = [j for j, el in enumerate(c.elements) if not el]
     seen = 0
     for i in range(4):
@@ -156,7 +138,7 @@ def test_candidate_and_neighbour_edges(oracle, max_search, cands, k):
     g = c.gpu()
     q = _queries(12, 48, 6)
     want = c.rerank(q, max_search, cands, k)
-    _same(g.search_batch_rerank(q, cands, max_search=max_search, num_elements=k), want)
+    assert_same(g.search_batch_rerank(q, cands, max_search=max_search, num_elements=k), want)
     assert (want[2] <= min(k, cands, max_search)).all()
 
 
@@ -181,7 +163,7 @@ def test_nan_table_row_is_not_finite(oracle):
     bad = table.copy()
     bad[row, 5] = np.nan
     g = c.gpu(attach=False)
-    g.set_rerank_embeddings(c.ei, eo.table_image(bad))
+    g.set_rerank_embeddings(c.ei, co.table_image(bad))
     with pytest.raises(granne_b200.GranneError) as e:
         g.search_batch_rerank(q, 10, max_search=50)
     assert e.value.code == NOT_FINITE
@@ -195,7 +177,7 @@ def test_nan_table_row_is_not_finite(oracle):
     with pytest.raises(granne_b200.GranneError) as e:
         g.stream_status()
     assert e.value.code == NOT_FINITE
-    _same(g.search_batch_rerank(q[:2], 10, max_search=50), c.rerank(q[:2], 50, 10, 10))
+    assert_same(g.search_batch_rerank(q[:2], 10, max_search=50), c.rerank(q[:2], 50, 10, 10))
     g.stream_status()
 
 
@@ -211,23 +193,23 @@ def test_rejections(oracle):
     want = c.rerank(q, 50, 10, 10)
     bare = c.gpu(attach=False)
     cases = [
-        (eo.elements_image(elements), eo.table_image(table[:, :31]), INVALID),  # width mismatch
-        (eo.elements_image(elements[:299]), c.ti, INVALID),  # fewer elements than the index
+        (co.elements_image(elements), co.table_image(table[:, :31]), INVALID),  # width mismatch
+        (co.elements_image(elements[:299]), c.ti, INVALID),  # fewer elements than the index
         (c.ei[:-2], c.ti, FORMAT),  # truncated term lists
         (c.ei, c.ti[:-3], FORMAT),  # truncated table
         (c.ei[:5], c.ti, FORMAT),
-        (eo.elements_image(elements[:-1] + [[100]]), c.ti, FORMAT),  # a term id past the table
+        (co.elements_image(elements[:-1] + [[100]]), c.ti, FORMAT),  # a term id past the table
     ]
     for ei, ti, code in cases:
         assert _raw_attach(bare, ei, ti) == code
-        _same(bare.search_batch(q, 50, 10), c.g.search_batch(q, 50, 10))  # the handle still searches
+        assert_same(bare.search_batch(q, 50, 10), c.g.search_batch(q, 50, 10))  # the handle still searches
     # a table wider than 4096 (with an index of that width)
     wide_t, wide_e = _container(40, 4100, 20, 9, counts=[1, 2])
     w = Composed(oracle, wide_t, wide_e)
     assert _raw_attach(w.gpu(attach=False), w.ei, w.ti) == INVALID
     # a correct attach still succeeds after every rejection
     bare.set_rerank_embeddings(c.ei, c.ti)
-    _same(bare.search_batch_rerank(q, 10, max_search=50), want)
+    assert_same(bare.search_batch_rerank(q, 10, max_search=50), want)
     # second attach of either kind, in both orders
     f32_image = granne_b200.compute_embeddings("angular", c.ei, c.ti).tobytes()
     assert _raw_attach(bare, c.ei, c.ti) == INVALID
@@ -237,8 +219,8 @@ def test_rejections(oracle):
     rows_first = c.gpu(attach=False)
     rows_first.set_rerank_elements(f32_image)
     assert _raw_attach(rows_first, c.ei, c.ti) == INVALID
-    _same(rows_first.search_batch_rerank(q, 10, max_search=50), want)
-    _same(bare.search_batch_rerank(q, 10, max_search=50), want)
+    assert_same(rows_first.search_batch_rerank(q, 10, max_search=50), want)
+    assert_same(bare.search_batch_rerank(q, 10, max_search=50), want)
     # not an angular_int index
     e_handle = granne_b200.Granne.from_bytes(c.index_bytes, "embeddings", c.ei, c.ti)
     assert _raw_attach(e_handle, c.ei, c.ti) == INVALID
@@ -266,7 +248,7 @@ def test_concurrent_attaches_and_searches(oracle):
     [t.join() for t in ts]
     assert len(outs) == 12
     for o in outs:
-        _same(o, want)
+        assert_same(o, want)
 
 
 def _sum_bytes(c):
@@ -297,7 +279,7 @@ def test_device_bytes(oracle):
               for s in (200, 150, 250)]
     m = granne_b200.MultiGranne.partitioned([(s.index_bytes, s.i8_image) for s in shards], "angular_int", [0])
     with pytest.raises(granne_b200.GranneError) as e:
-        m.set_rerank_embeddings([shards[0].ei, shards[1].ei, eo.elements_image(shards[2].elements[:10])], c.ti)
+        m.set_rerank_embeddings([shards[0].ei, shards[1].ei, co.elements_image(shards[2].elements[:10])], c.ti)
     assert e.value.code == INVALID
     m.set_rerank_embeddings([s.ei for s in shards], c.ti)
     q = _queries(5, 30, 42)
@@ -315,26 +297,26 @@ def test_device_elements_handle(oracle):
     g.set_rerank_embeddings(c.ei, c.ti)
     q = _queries(30, 96, 16)
     want = c.rerank(q, 50, 40, 10)
-    _same(g.search_batch_rerank(q, 40, max_search=50), want)
+    assert_same(g.search_batch_rerank(q, 40, max_search=50), want)
     got = g.search_batch_rerank_device(torch.from_numpy(q).cuda(), 40, max_search=50)
     torch.cuda.synchronize()
     g.stream_status()
-    _same([t.cpu().numpy() for t in got], want)
+    assert_same([t.cpu().numpy() for t in got], want)
 
 
 @pytest.mark.parametrize("dim", [100, 300])
 def test_gpu_built_index_and_get_index_handle(oracle, dim):
     table, elements = _container(1500, dim, 700, dim)
-    i8_image = eo.compute_embeddings("angular_int", eo.elements_image(elements), eo.table_image(table)).tobytes()
+    i8_image = co.compute_embeddings("angular_int", co.elements_image(elements), co.table_image(table)).tobytes()
     b = granne_b200.GranneBuilder("angular_int", i8_image, num_neighbors=12, max_search=40)
     b.build()
     c = Composed(oracle, table, elements, index_bytes=b.index_bytes().tobytes())
     q = _queries(40, dim, 3)
     want = c.rerank(q, 60, 40, 10)
-    _same(c.gpu().search_batch_rerank(q, 40, max_search=60), want)
+    assert_same(c.gpu().search_batch_rerank(q, 40, max_search=60), want)
     snap = b.get_index()
     snap.set_rerank_embeddings(c.ei, c.ti)
-    _same(snap.search_batch_rerank(q, 40, max_search=60), want)
+    assert_same(snap.search_batch_rerank(q, 40, max_search=60), want)
 
 
 def test_multi_replicated_and_partitioned(oracle):
@@ -395,9 +377,6 @@ def test_string_queries(oracle, tmp_path):
 
 
 def test_cxx_client(tmp_path, oracle):
-    cxx = shutil.which("g++")
-    if cxx is None:
-        pytest.skip("no C++ compiler")
     c = Composed(oracle, *_container(500, 64, 300, 20))
     idx, i8, el, emb = (tmp_path / f for f in ("index.bin", "i8.bin", "el.bin", "emb.bin"))
     idx.write_bytes(c.index_bytes)
@@ -407,13 +386,7 @@ def test_cxx_client(tmp_path, oracle):
     q = _queries(4, 64, 21)
     qf = tmp_path / "q.bin"
     qf.write_bytes(q.tobytes())
-    exe = tmp_path / "client"
-    libdir = os.path.dirname(granne_b200.library_path())
-    subprocess.check_call([cxx, "-std=c++17", "-O1", "-Wall", "-Wextra", "-Werror", "-I" + os.path.join(ROOT, "include"),
-                           os.path.join(ROOT, "tests", "helpers", "cxx_rerank_sum_client.cpp"), "-o", str(exe),
-                           "-L" + libdir, "-lgranne_b200", "-Wl,-rpath," + libdir])
-    out = subprocess.run([str(exe), str(idx), str(i8), str(el), str(emb), str(qf)], capture_output=True, text=True,
-                         timeout=120)
+    out = cxx_client("cxx_rerank_sum_client.cpp", [idx, i8, el, emb, qf], tmp_path)
     assert out.returncode == 0, out.stdout + out.stderr
     wi, wd, wc = c.rerank(q, 50, 20, 5)
     assert (wc == 5).all()

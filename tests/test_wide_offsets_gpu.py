@@ -22,6 +22,7 @@ import pytest
 
 import granne_b200
 from helpers import ref_model as M
+from helpers.fixtures import library  # noqa: F401  (autouse)
 from helpers.model_checks import assert_same, assert_within_f64_bound, bits
 from helpers.wide_fixture import (NUM_QUERIES, Bits, Wide, first_id_at, rank, row_bytes, sparse_graph, sparse_index,
                                   words_of)
@@ -42,14 +43,6 @@ RERANK = [("angular_int", 128, ("DistI8", "sub-warp groups"), (1 << 31, 1 << 32)
 EF, K = 64, 10             # graph search
 KW, KF = 100, 64           # within lists, filtered
 MARGIN = 3 * GB            # layers, workspaces and the model's device tensors
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _lib():
-    from granne_b200 import build
-
-    build.build()
-    granne_b200.load_library()
 
 
 def _host(t):

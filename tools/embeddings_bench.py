@@ -49,7 +49,7 @@ def container(torch, gb, dev, n, seed):
 
 
 def materialise(torch, gb, c, calls):
-    from helpers import embeddings_oracle as eo
+    from helpers import composed_oracle as co
 
     el, emb = c.elements_image, c.embeddings_image
     n, dim, terms = c.n, 100, int(c.offsets[-1])
@@ -79,7 +79,7 @@ def materialise(torch, gb, c, calls):
         gb.compute_embeddings(kind, el, emb, out=host_img)
         host_s = time.perf_counter() - t0
         t0 = time.perf_counter()
-        ref = eo.compute_embeddings(kind, el.tobytes(), emb.tobytes(), threads=os.cpu_count())
+        ref = co.compute_embeddings(kind, el.tobytes(), emb.tobytes(), threads=os.cpu_count())
         oracle_s = time.perf_counter() - t0
         assert np.array_equal(ref, host_img), kind + ": the host variant's image differs from the oracle's"
         del ref, host_img

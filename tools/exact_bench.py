@@ -42,7 +42,7 @@ def make(kind, n, dim, seed):
     import torch
     import granne_b200
     from oracle import granne_oracle as go
-    from helpers import exact_oracle as xo
+    from helpers import composed_oracle as co
 
     g = torch.Generator(device="cuda").manual_seed(seed)
     dt = torch.float32 if kind == "angular" else torch.int8
@@ -54,13 +54,13 @@ def make(kind, n, dim, seed):
             rows[r0:r1] = x / x.norm(dim=1, keepdim=True)
         else:
             rows[r0:r1] = (x * 255).to(torch.int8)
-    h = granne_b200.Granne.from_device_elements(xo.single_layer_index(go, n), kind, rows)
+    h = granne_b200.Granne.from_device_elements(co.single_layer_index(go, n), kind, rows)
     return h, rows
 
 
 def run(name, kind, n, dim, reps, oracle_q, nq=1024, k=10):
     import torch
-    from helpers import exact_oracle as xo
+    from helpers import composed_oracle as co
 
     h, rows = make(kind, n, dim, 1)
     q = (torch.rand((nq, dim), generator=torch.Generator(device="cuda").manual_seed(2), device="cuda") - 0.5)
@@ -99,7 +99,7 @@ def run(name, kind, n, dim, reps, oracle_q, nq=1024, k=10):
         res["torch_top10_differs"] = float((top.cpu().numpy() != ids.astype(np.int64)).any(axis=1).mean())
     if oracle_q and n <= 10_000_000:
         host = rows.cpu().numpy()
-        c = xo.Container(kind, np.uint64(dim).tobytes() + host.tobytes())
+        c = co.Container(kind, np.uint64(dim).tobytes() + host.tobytes())
         t0 = time.perf_counter()
         wi, wd, _ = c.exact_search(qh[:oracle_q] if kind == "angular" else qh[:oracle_q], k, threads=16)
         res["oracle_16t_s"] = time.perf_counter() - t0

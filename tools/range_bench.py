@@ -99,7 +99,7 @@ def main():
     build.build()
     from oracle import granne_oracle as go
     from helpers.data import clustered_vectors
-    from helpers.exact_oracle import single_layer_index
+    from helpers.composed_oracle import single_layer_index
 
     go.build_lib()
     targets = [int(t) for t in args.targets.split(",") if t]

@@ -183,11 +183,11 @@ def main():
 
     if "i8" not in skip:
         from oracle import granne_oracle as go
-        from helpers import exact_oracle as xo
+        from helpers import composed_oracle as co
 
         dim = 100
         rows, q = generate(torch, granne_b200, n, dim, 4321, ("angular_int",), nq)
-        h = granne_b200.Granne.from_device_elements(xo.single_layer_index(go, n), "angular_int", rows["angular_int"])
+        h = granne_b200.Granne.from_device_elements(co.single_layer_index(go, n), "angular_int", rows["angular_int"])
         run(h, "i8_hybrid_1000", q, [rng.integers(0, n, 1000) for _ in range(nq)], (dim + 15) // 16 * 16)
         h.close()
         rows = None
@@ -196,11 +196,11 @@ def main():
     if "emb" not in skip:
         from bench import DATA_SEED, QUERY_SEED, SumContainer
         from oracle import granne_oracle as go
-        from helpers import exact_oracle as xo
+        from helpers import composed_oracle as co
 
         ne, dim = a.emb_elements, 100
         cont = SumContainer(torch, granne_b200, dev, types.SimpleNamespace(dim=dim, num_neighbors=30), ne, DATA_SEED)
-        e = granne_b200.Granne.from_bytes(xo.single_layer_index(go, ne), "embeddings",
+        e = granne_b200.Granne.from_bytes(co.single_layer_index(go, ne), "embeddings",
                                           cont.elements_image.tobytes(), cont.embeddings_image.tobytes())
         q = torch.from_numpy(np.ascontiguousarray(cont.queries(nq, QUERY_SEED), dtype=np.float32)).to(dev)
         # row bytes: the element's terms (mean terms_per_element table rows of dim f32) and its 5-byte offset
