@@ -172,6 +172,28 @@ extern "C" {
         m: *mut RawMulti, queries: *const f32, nq: usize, query_format: c_int, max_search: u32, num_candidates: u32,
         num_neighbors: u32, out_ids: *mut u64, out_dists: *mut f32, out_counts: *mut u32,
     ) -> c_int;
+    fn granne_b200_search_diverse_batch(
+        h: *mut RawIndex, queries: *const c_void, nq: usize, query_format: c_int, max_search: u32, num_neighbors: u32,
+        out_ids: *mut u32, out_dists: *mut f32, out_counts: *mut u32, out_stats: *mut u64,
+    ) -> c_int;
+    fn granne_b200_search_diverse_batch_device(
+        h: *mut RawIndex, d_queries: *const c_void, nq: usize, query_format: c_int, max_search: u32,
+        num_neighbors: u32, d_out_ids: *mut u32, d_out_dists: *mut f32, d_out_counts: *mut u32, d_out_stats: *mut u64,
+        cuda_stream: *mut c_void,
+    ) -> c_int;
+    fn granne_b200_select_neighbors_batch(
+        h: *mut RawIndex, cand_ids: *const u32, cand_dists: *const f32, cand_counts: *const u32, nq: usize,
+        stride: u32, num_neighbors: u32, out_ids: *mut u32, out_dists: *mut f32, out_counts: *mut u32,
+    ) -> c_int;
+    fn granne_b200_multi_search_diverse_batch(
+        m: *mut RawMulti, queries: *const c_void, nq: usize, query_format: c_int, max_search: u32, num_neighbors: u32,
+        out_ids: *mut u64, out_dists: *mut f32, out_counts: *mut u32,
+    ) -> c_int;
+    fn granne_b200_select_neighbors_batch_device(
+        h: *mut RawIndex, d_cand_ids: *const u32, d_cand_dists: *const f32, d_cand_counts: *const u32, nq: usize,
+        stride: u32, num_neighbors: u32, d_out_ids: *mut u32, d_out_dists: *mut f32, d_out_counts: *mut u32,
+        cuda_stream: *mut c_void,
+    ) -> c_int;
 }
 
 pub const ANGULAR: c_int = 0; // angular::Vectors

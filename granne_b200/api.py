@@ -14,6 +14,7 @@ _ELEMENT_TYPES = {"angular": ANGULAR, "angular_int": ANGULAR_INT, "embeddings": 
 STATS_PER_QUERY = 4
 EXACT_MAX_K = 1024  # GRANNE_B200_EXACT_MAX_K
 RERANK_MAX_CANDIDATES = 1024  # GRANNE_B200_RERANK_MAX_CANDIDATES
+DIVERSE_MAX_CANDIDATES = 1024  # GRANNE_B200_DIVERSE_MAX_CANDIDATES
 DEFAULT_MAX_SEARCH = 200   # py/src/lib.rs:14
 DEFAULT_NUM_ELEMENTS = 10  # py/src/lib.rs:15
 
@@ -131,6 +132,11 @@ def load_library():
         "granne_b200_set_rerank_embeddings": (i32, [vp, vp, sz, vp, sz]),
         "granne_b200_multi_set_rerank_embeddings": (i32, [vp, vp, vp, vp, sz]),
         "granne_b200_multi_search_rerank_batch": (i32, [vp, vp, sz, i32, u32, u32, u32, vp, vp, vp]),
+        "granne_b200_search_diverse_batch": (i32, [vp, vp, sz, i32, u32, u32, vp, vp, vp, vp]),
+        "granne_b200_search_diverse_batch_device": (i32, [vp, vp, sz, i32, u32, u32, vp, vp, vp, vp, vp]),
+        "granne_b200_multi_search_diverse_batch": (i32, [vp, vp, sz, i32, u32, u32, vp, vp, vp]),
+        "granne_b200_select_neighbors_batch": (i32, [vp, vp, vp, vp, sz, u32, u32, vp, vp, vp]),
+        "granne_b200_select_neighbors_batch_device": (i32, [vp, vp, vp, vp, sz, u32, u32, vp, vp, vp, vp]),
         "granne_b200_device_bytes": (u64, [vp]),
     }
     for name, (res, args) in sig.items():
@@ -951,6 +957,82 @@ class Granne:
             C.c_void_p(stats.data_ptr()) if stats is not None else None, C.c_void_p(_raw_stream(stream, q.device))))
         return ids, dists, counts
 
+    # ---- diverse search (granne_b200_search_diverse_batch*, granne_b200_select_neighbors_batch*) ----
+    def search_batch_diverse(self, queries, max_search=DEFAULT_MAX_SEARCH, num_elements=DEFAULT_NUM_ELEMENTS,
+                             already_element=False, with_stats=False, by_id=False, exclude_self=False):
+        """The neighbours granne would link each query to if it were inserted: search_batch(q, max_search,
+        max_search) (without the element itself for exclude_self), then GranneBuilder::select_neighbors
+        (src/index/mod.rs:849-883) keeps a candidate only if it is at least as close to the query as to every
+        candidate kept before it, up to num_elements.  Not a reference function.  max_search <=
+        DIVERSE_MAX_CANDIDATES; queries and keywords as in search_batch.  Returns (ids, dists, counts) in
+        search_batch's layout, in candidate order with the search's distances; with_stats adds the search's
+        counters."""
+        q, fmt = self._host_queries(queries, already_element, by_id, exclude_self)
+        nq, k = q.shape[0], int(num_elements)
+        ids, dists, counts, stats = _host_outputs(nq, k, np.uint32, with_stats)
+        _check(load_library().granne_b200_search_diverse_batch(self._h, _ptr(q), nq, fmt, int(max_search), k,
+                                                               _ptr(ids), _ptr(dists), _ptr(counts),
+                                                               _ptr(stats) if with_stats else None))
+        if with_stats:
+            return ids, dists, counts, stats
+        return ids, dists, counts
+
+    def search_batch_diverse_device(self, queries, max_search=DEFAULT_MAX_SEARCH, num_elements=DEFAULT_NUM_ELEMENTS,
+                                    already_element=False, out=None, stats=None, stream=None, by_id=False,
+                                    exclude_self=False):
+        """Device-resident search_batch_diverse: CUDA tensors in and out as in search_batch_device, asynchronous on
+        `stream`; errors are raised by stream_status()."""
+        q, fmt = self._device_queries(queries, already_element, by_id, exclude_self)
+        nq, k = q.shape[0], int(num_elements)
+        ids, dists, counts = _device_outputs(q, k, out)
+        _check_stats(stats, q)
+        _check(load_library().granne_b200_search_diverse_batch_device(
+            self._h, C.c_void_p(q.data_ptr()), nq, fmt, int(max_search), k, C.c_void_p(ids.data_ptr()),
+            C.c_void_p(dists.data_ptr()), C.c_void_p(counts.data_ptr()),
+            C.c_void_p(stats.data_ptr()) if stats is not None else None, C.c_void_p(_raw_stream(stream, q.device))))
+        return ids, dists, counts
+
+    def select_neighbors(self, ids, dists, counts, num_elements=DEFAULT_NUM_ELEMENTS):
+        """select_neighbors(list_q, num_elements) over caller lists, search_batch_diverse's selection: it composes with
+        every query call's (ids, dists, counts) as they are (exact_search_batch(q, C) gives the exact diverse answer).
+        ids uint32 [nq, C] (< len(self)), dists float32 [nq, C] ascending within each list's first counts[q] entries,
+        counts [nq] <= C; C <= DIVERSE_MAX_CANDIDATES.  Returns (ids, dists, counts) in search_batch's layout."""
+        ci = np.asarray(ids)
+        if ci.ndim != 2:
+            raise ValueError("ids must have shape (nq, C)")
+        nq, stride = ci.shape
+        ci = np.ascontiguousarray(ci, dtype=np.uint32)
+        cd = np.ascontiguousarray(dists, dtype=np.float32)
+        cc = np.ascontiguousarray(counts, dtype=np.uint32)
+        if cd.shape != ci.shape or cc.shape != (nq,):
+            raise ValueError("dists must have the shape of ids (nq, C), counts (nq,)")
+        k = int(num_elements)
+        out_ids, out_dists, out_counts, _ = _host_outputs(nq, k, np.uint32)
+        _check(load_library().granne_b200_select_neighbors_batch(
+            self._h, _ptr(ci), _ptr(cd), _ptr(cc), nq, stride, k, _ptr(out_ids), _ptr(out_dists), _ptr(out_counts)))
+        return out_ids, out_dists, out_counts
+
+    def select_neighbors_device(self, ids, dists, counts, num_elements=DEFAULT_NUM_ELEMENTS, out=None, stream=None):
+        """Device-resident select_neighbors: the (ids int32 [nq, C], dists float32 [nq, C], counts int32 [nq]) CUDA
+        tensors of any *_device call as they are, asynchronous on `stream`.  The kernel checks the lists: a bad list
+        gets count 0 and padding, and stream_status() raises."""
+        import torch
+
+        for t, dt, what in ((ids, torch.int32, "ids"), (dists, torch.float32, "dists"), (counts, torch.int32, "counts")):
+            if (not isinstance(t, torch.Tensor) or not t.is_cuda or t.device.index != self.device or t.dtype != dt
+                    or not t.is_contiguous()):
+                raise ValueError("%s must be a contiguous %s CUDA tensor on cuda:%d" % (what, dt, self.device))
+        if ids.dim() != 2 or tuple(dists.shape) != tuple(ids.shape) or tuple(counts.shape) != (ids.shape[0],):
+            raise ValueError("ids and dists must have shape (nq, C), counts (nq,)")
+        nq, stride = ids.shape
+        k = int(num_elements)
+        out_ids, out_dists, out_counts = _device_outputs(ids, k, out)
+        _check(load_library().granne_b200_select_neighbors_batch_device(
+            self._h, C.c_void_p(ids.data_ptr()), C.c_void_p(dists.data_ptr()), C.c_void_p(counts.data_ptr()), nq,
+            stride, k, C.c_void_p(out_ids.data_ptr()), C.c_void_p(out_dists.data_ptr()),
+            C.c_void_p(out_counts.data_ptr()), C.c_void_p(_raw_stream(stream, ids.device))))
+        return out_ids, out_dists, out_counts
+
     def _word_tables(self):
         """(WordDict, embeddings table, per-element id lists) for an "embeddings" index opened with words_path."""
         if getattr(self, "_words", None) is None:
@@ -1165,6 +1247,18 @@ class MultiGranne:
         ids, dists, counts, _ = _host_outputs(nq, k, np.uint64)
         _check(load_library().granne_b200_multi_search_batch(self._h, _ptr(q), nq, fmt, int(max_search), k, _ptr(ids),
                                                              _ptr(dists), _ptr(counts)))
+        return ids, dists, counts
+
+    def search_batch_diverse(self, queries, max_search=DEFAULT_MAX_SEARCH, num_elements=DEFAULT_NUM_ELEMENTS,
+                             already_element=False, by_id=False, exclude_self=False):
+        """Granne.search_batch_diverse over all parts (granne_b200_multi_search_diverse_batch): GLOBAL uint64 ids.
+        Partitioned, the shards' max_search lists are merged by (distance, global id) and select_neighbors runs over
+        the global container."""
+        q, fmt = self._host_queries(queries, already_element, by_id, exclude_self)
+        nq, k = q.shape[0], int(num_elements)
+        ids, dists, counts, _ = _host_outputs(nq, k, np.uint64)
+        _check(load_library().granne_b200_multi_search_diverse_batch(self._h, _ptr(q), nq, fmt, int(max_search), k,
+                                                                     _ptr(ids), _ptr(dists), _ptr(counts)))
         return ids, dists, counts
 
     def exact_search_batch(self, queries, num_elements=DEFAULT_NUM_ELEMENTS, already_element=False, by_id=False,

@@ -35,13 +35,6 @@ struct BuildArgs {
 
 constexpr float kHundredEps = 100.0f * 1.1920929e-07f;  // NotNan::new(100.0 * f32::EPSILON) (:813,829)
 
-// ElementContainer::get(id) -> the query slot (c.qs / q registers) of the distance engine.
-template <class Dist>
-__device__ __forceinline__ void set_query_from_element(const DeviceIndex& ix, WarpCtx& c, Dist& dist, uint32_t id) {
-    load_element_to_qs(ix, c, id);
-    dist.load_query(ix, c);
-}
-
 __device__ __forceinline__ void node_lock(int* locks, uint32_t i, int lane) {
     if (lane == 0) {
         while (atomicCAS(locks + i, 0, 1) != 0) {

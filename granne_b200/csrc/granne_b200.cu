@@ -28,6 +28,7 @@
 #include "search_kernels.cuh"
 #include "exact_kernels.cuh"
 #include "rerank_kernels.cuh"
+#include "diverse_kernels.cuh"
 #include "within_kernels.cuh"
 #include "ids_kernels.cuh"
 #include "range_kernels.cuh"
@@ -146,10 +147,11 @@ struct Workspace {
     Buffer<unsigned long long> d_stats;
     Buffer<int> d_status;  // nq ints
     // one 64-byte block: [0..2] work counters of the three passes, [3] fast pass flagged something, [4] retry pass
-    // flagged something, [5] done counter (fused gather), [6] work counter of the re-rank kernel; d_error = words
-    // [8..11].  A call zeroes its words with one memset before its kernels: a host call the whole block, since it
-    // reports the errors of its own kernels only (kHostCallBytes, host_batch); a device call or a builder batch the
-    // counters when it searches, leaving the error word sticky (kSearchCounterBytes).
+    // flagged something, [5] done counter (fused gather), [6] work counter of the re-rank kernel, [7] work counter of
+    // the diverse selection; d_error = words [8..11].  A call zeroes its words with one memset before its kernels: a
+    // host call the whole block, since it reports the errors of its own kernels only (kHostCallBytes, host_batch); a
+    // device call or a builder batch the counters when it searches, leaving the error word sticky
+    // (kSearchCounterBytes).
     Buffer<unsigned int> d_counters;
     int* d_error = nullptr;              // [0]=sticky error bits of this call (inside the counters block)
     Buffer<unsigned long long> d_retried;  // cumulative: queries that needed more than the fast pass
@@ -175,7 +177,7 @@ struct Workspace {
     // the queries' prepare statuses
     Buffer<uint32_t> d_exact_ids;
     Buffer<int> d_exact_qstat;
-    // two-stage search: stage 1's candidates, one block ids | dists | counts for the current call's nq x C
+    // two-stage and diverse search: stage 1's candidates, one block ids | dists | counts for the current call's nq x C
     Buffer<uint32_t> d_rerank;
     // exact search within lists: a chunk's running lists | segment prefix; its locks | query flags
     Buffer<unsigned long long> d_within;
@@ -909,6 +911,8 @@ int validate_batch(const Handle* h, const void* q, size_t nq, int fmt, uint32_t 
 
 constexpr const char* kMaxSearchRule = "max_search must be >= 1 (the reference panics on 0, src/index/mod.rs:1019)";
 constexpr const char* kExactKRule = "num_neighbors exceeds GRANNE_B200_EXACT_MAX_K (1024)";
+constexpr const char* kBadCandidatesRule =
+    "a candidate list is longer than its stride, not ascending by distance, or holds an id >= Index::len";
 
 int validate_search(const Handle* h, const void* q, size_t nq, int fmt, uint32_t max_search, uint32_t k,
                     const void* ids, const void* dists, bool id_formats = true) {
@@ -1078,6 +1082,8 @@ int error_from_bits(int bits) {
     if (bits & gb::kStatusBadSegment)
         return fail(GRANNE_B200_ERR_INVALID_ARGUMENT,
                     "a range search segment's length differs from its query's count (it is padded)");
+    if (bits & gb::kStatusBadCandidates)
+        return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, kBadCandidatesRule);
     return GRANNE_B200_OK;
 }
 
@@ -1698,6 +1704,98 @@ int enqueue_rerank(Handle* h, Workspace* w, const void* d_queries, size_t nq, ui
             return launch_warps<gb::rerank_kernel<Dist>>(h, grid, smem, stream, h->rerank, a);
         }
     });
+}
+
+// ---- diverse search: select_neighbors over candidate lists (diverse_kernels.cuh) ----------------------------------
+constexpr const char* kDiverseStrideRule = "the candidate stride exceeds GRANNE_B200_DIVERSE_MAX_CANDIDATES (1024)";
+
+// validate_search's rules with max_search <= GRANNE_B200_DIVERSE_MAX_CANDIDATES as part of the call's own rule.
+int validate_diverse(const Handle* h, const void* q, size_t nq, int fmt, uint32_t max_search, uint32_t k,
+                     const void* ids, const void* dists) {
+    const char* rule = max_search == 0 ? kMaxSearchRule
+                       : max_search > GRANNE_B200_DIVERSE_MAX_CANDIDATES
+                           ? "max_search exceeds GRANNE_B200_DIVERSE_MAX_CANDIDATES (1024)"
+                           : nullptr;
+    return validate_batch(h, q, nq, fmt, k, ids, dists, rule);
+}
+
+// The rules of the standalone selection that read no handle, in the order they are reported: the handle is null;
+// stride > GRANNE_B200_DIVERSE_MAX_CANDIDATES; nq above the batch limit; with nq > 0, a null candidate array (ids and
+// distances only when stride > 0) or a null output (when k > 0).
+int validate_select(const Handle* h, const void* ids, const void* dists, const void* counts, size_t nq,
+                    uint32_t stride, uint32_t k, const void* out_ids, const void* out_dists) {
+    int rc = validate_batch(h, counts, nq, GRANNE_B200_QUERY_RAW_F32, k, out_ids, out_dists,
+                            stride > GRANNE_B200_DIVERSE_MAX_CANDIDATES ? kDiverseStrideRule : nullptr);
+    if (rc) return rc;
+    if (nq > 0 && stride > 0 && (!ids || !dists)) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "null buffer");
+    return GRANNE_B200_OK;
+}
+
+// The host check of nq caller lists in host memory: each count <= stride, its ids < Index::len and its distances
+// ascending (no NaN).
+int check_candidate_lists(const Handle* h, const uint32_t* ids, const float* dists, const uint32_t* counts, size_t nq,
+                          uint32_t stride) {
+    for (size_t q = 0; q < nq; ++q) {
+        if (counts[q] > stride) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, kBadCandidatesRule);
+        const uint32_t* id = ids + q * stride;
+        const float* d = dists + q * stride;
+        for (uint32_t t = 0; t < counts[q]; ++t)
+            if (id[t] >= h->index_len || d[t] != d[t] || (t > 0 && !(d[t - 1] <= d[t])))
+                return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, kBadCandidatesRule);
+    }
+    return GRANNE_B200_OK;
+}
+
+// Enqueues select_neighbors(list_q, k) for nq lists of up to `stride` candidates (device memory) over h's own container
+// into `out` (ids | dists | counts in search_batch's layout) on `stream`.  `check`: the lists come from a caller, and
+// the kernel checks them (kStatusBadCandidates).  Uses work counter word 7, which the call zeroed.
+int enqueue_select(Handle* h, Workspace* w, const uint32_t* ids, const float* dists, const uint32_t* counts,
+                   size_t nq, uint32_t stride, uint32_t k, bool check, const QueryOut& out, cudaStream_t stream) {
+    const gb::DeviceIndex& d = h->dev;
+    const EngineTiles eng = engine_tiles(d);
+    gb::DiverseArgs a{};
+    a.cand_ids = ids;
+    a.cand_dists = dists;
+    a.cand_counts = counts;
+    a.cand_stride = stride;
+    a.nq = nq;
+    a.num_neighbors = k;
+    a.check = check;
+    a.len = h->index_len;
+    a.out_ids = out.ids;
+    a.out_dists = out.dists;
+    a.out_counts = out.counts;
+    a.work_counter = w->d_counters.get() + 7;
+    a.error_flag = w->d_error;
+    a.tiles = eng.tiles;
+    const size_t smem = gb::diverse_list_offset(eng.base_smem) + gb::diverse_list_bytes(stride);
+    return DistDispatch::call(d, [&](auto e) {
+        constexpr auto kern = gb::diverse_kernel<typename decltype(e)::type>;
+        int occ = 0;
+        const int err = resident_ctas<kern>(h, smem, &occ);
+        if (err) return err;
+        if (occ < 1) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "diverse selection exceeds shared memory");
+        const unsigned grid = (unsigned)std::min<unsigned long long>(nq, (unsigned long long)occ * h->num_sms);
+        return launch_warps<kern>(h, grid, smem, stream, d, a);
+    });
+}
+
+// Enqueues one diverse search on `stream`: stage 1 is the query call's search with k = max_search (any query format;
+// QUERY_ID_EXCLUDING drops the element itself from its candidates) into the workspace's candidate block, stage 2 is
+// enqueue_select over those lists into the caller's outputs.  Stage 1 writes out.stats as search does.
+int enqueue_diverse(Handle* h, Workspace* w, const void* d_queries, size_t nq, int fmt, uint32_t max_search,
+                    uint32_t k, const QueryOut& out, bool host_checked, cudaStream_t stream) {
+    int rc = w->d_rerank.grow(2 * nq * max_search + nq, stream);
+    if (rc) return rc;
+    uint32_t* cand_ids = w->d_rerank.get();
+    float* cand_dists = reinterpret_cast<float*>(cand_ids + nq * max_search);
+    uint32_t* cand_counts = cand_ids + 2 * nq * max_search;
+    if ((rc = enqueue_query(h, w, d_queries, nq, fmt, max_search, {cand_ids, cand_dists, cand_counts, out.stats},
+                            host_checked, stream, [&](const void* q, int f, uint32_t kk, const QueryOut& o) {
+                                return enqueue_search(h, w, q, nq, f, max_search, kk, o, stream);
+                            })))
+        return rc;
+    return enqueue_select(h, w, cand_ids, cand_dists, cand_counts, nq, max_search, k, false, out, stream);
 }
 
 // ---- exact search within candidate lists (within_kernels.cuh) -----------------------------------------------------
@@ -2644,6 +2742,64 @@ int granne_b200_search_rerank_batch_device(granne_b200_index* h, const float* d_
     return device_batch(h, cuda_stream, true, [&](Workspace* w, cudaStream_t stream) {
         return enqueue_rerank(h, w, d_queries, nq, max_search, num_candidates, num_neighbors,
                               {d_out_ids, d_out_dists, d_out_counts, d_out_stats}, stream);
+    });
+}
+
+int granne_b200_search_diverse_batch(granne_b200_index* h, const void* queries, size_t nq, int query_format,
+                                     uint32_t max_search, uint32_t num_neighbors, uint32_t* out_ids, float* out_dists,
+                                     uint32_t* out_counts, uint64_t* out_stats) {
+    int rc = validate_diverse(h, queries, nq, query_format, max_search, num_neighbors, out_ids, out_dists);
+    if (rc || nq == 0) return rc;
+    if ((rc = check_host_query_ids(h, queries, nq, query_format))) return rc;
+    return host_batch(h, queries, nq, query_format, num_neighbors, out_ids, out_dists, out_counts, out_stats,
+                      [&](Workspace* w, cudaStream_t stream, const QueryOut& out) {
+                          return enqueue_diverse(h, w, w->d_queries.get(), nq, query_format, max_search,
+                                                 num_neighbors, out, true, stream);
+                      });
+}
+
+int granne_b200_search_diverse_batch_device(granne_b200_index* h, const void* d_queries, size_t nq, int query_format,
+                                            uint32_t max_search, uint32_t num_neighbors, uint32_t* d_out_ids,
+                                            float* d_out_dists, uint32_t* d_out_counts, uint64_t* d_out_stats,
+                                            void* cuda_stream) {
+    int rc = validate_diverse(h, d_queries, nq, query_format, max_search, num_neighbors, d_out_ids, d_out_dists);
+    if (rc || nq == 0) return rc;
+    return device_batch(h, cuda_stream, true, [&](Workspace* w, cudaStream_t stream) {
+        return enqueue_diverse(h, w, d_queries, nq, query_format, max_search, num_neighbors,
+                               {d_out_ids, d_out_dists, d_out_counts, d_out_stats}, false, stream);
+    });
+}
+
+int granne_b200_select_neighbors_batch(granne_b200_index* h, const uint32_t* cand_ids, const float* cand_dists,
+                                       const uint32_t* cand_counts, size_t nq, uint32_t stride,
+                                       uint32_t num_neighbors, uint32_t* out_ids, float* out_dists,
+                                       uint32_t* out_counts) {
+    int rc = validate_select(h, cand_ids, cand_dists, cand_counts, nq, stride, num_neighbors, out_ids, out_dists);
+    if (rc || nq == 0) return rc;
+    if ((rc = check_candidate_lists(h, cand_ids, cand_dists, cand_counts, nq, stride))) return rc;
+    // the counts go up as the call's 4-byte query rows, the lists as its inputs
+    return host_batch(h, cand_counts, nq, GRANNE_B200_QUERY_ID, num_neighbors, out_ids, out_dists, out_counts, nullptr,
+                      [&](Workspace* w, cudaStream_t stream, const QueryOut& out) {
+                          const HostInput in[] = {{cand_ids, nq * stride * 4}, {cand_dists, nq * stride * 4}};
+                          return with_call_inputs(stream, in, [&](const void* const* d) {
+                              return enqueue_select(h, w, static_cast<const uint32_t*>(d[0]),
+                                                    static_cast<const float*>(d[1]),
+                                                    reinterpret_cast<const uint32_t*>(w->d_queries.get()), nq, stride,
+                                                    num_neighbors, false, out, stream);
+                          });
+                      });
+}
+
+int granne_b200_select_neighbors_batch_device(granne_b200_index* h, const uint32_t* d_cand_ids,
+                                              const float* d_cand_dists, const uint32_t* d_cand_counts, size_t nq,
+                                              uint32_t stride, uint32_t num_neighbors, uint32_t* d_out_ids,
+                                              float* d_out_dists, uint32_t* d_out_counts, void* cuda_stream) {
+    int rc = validate_select(h, d_cand_ids, d_cand_dists, d_cand_counts, nq, stride, num_neighbors, d_out_ids,
+                             d_out_dists);
+    if (rc || nq == 0) return rc;
+    return device_batch(h, cuda_stream, true, [&](Workspace* w, cudaStream_t stream) {
+        return enqueue_select(h, w, d_cand_ids, d_cand_dists, d_cand_counts, nq, stride, num_neighbors, true,
+                              {d_out_ids, d_out_dists, d_out_counts, nullptr}, stream);
     });
 }
 
@@ -3972,6 +4128,142 @@ int granne_b200_multi_search_rerank_batch(granne_b200_multi* m, const float* que
                                                                   query_format, max_search, num_candidates,
                                                                   num_neighbors, ids, ds, c, nullptr);
                        });
+}
+
+}  // extern "C"
+
+namespace {
+
+// The diverse search of a RANGE_PARTITIONED handle (arguments checked, nq > 0).  The candidates are the shards'
+// max_search lists merged by (distance, global id), as granne_b200_multi_search_batch merges them, without the query's
+// own global id for QUERY_ID_EXCLUDING.  select_neighbors then runs over the global container: the merged candidates'
+// element rows are read from the shards that own them and staged on part 0's device as a temporary container (f32 rows
+// re-laid out by permute_rows_f32_kernel, i8 rows padded by pad_rows_i8_kernel; a SumEmbeddings shard's materialised
+// rows as angular f32 rows, whose f32 angular distances are its own), and the lists select there.
+int multi_diverse_partitioned(granne_b200_multi* m, const void* queries, size_t nq, int fmt, uint32_t ms, uint32_t k,
+                              uint64_t* out_ids, float* out_dists, uint32_t* out_counts) {
+    return guarded([&] {
+        const uint64_t* gids = by_id(fmt) ? static_cast<const uint64_t*>(queries) : nullptr;
+        std::vector<uint8_t> id_rows;
+        const void* rows = queries;
+        int qfmt = fmt;
+        int rc;
+        if (gids) {
+            MultiIds mi;
+            if ((rc = multi_ids(m, gids, nq, &mi)) || (rc = multi_id_rows(m, mi, nq, &id_rows))) return rc;
+            rows = id_rows.data();
+            qfmt = GRANNE_B200_QUERY_ELEMENT;
+        }
+        std::vector<uint64_t> cand(nq * ms);
+        std::vector<float> cd(nq * ms);
+        std::vector<uint32_t> cc(nq);
+        if ((rc = multi_batch(m, rows, nq, qfmt, ms, cand.data(), cd.data(), cc.data(),
+                              [&](size_t i, size_t, const void* q, size_t cnt, uint32_t* ids, float* ds, uint32_t* c) {
+                                  return granne_b200_search_batch(m->parts[i], q, cnt, qfmt, ms, ms, ids, ds, c,
+                                                                  nullptr);
+                              })))
+            return rc;
+        // the lists as rows of the gathered container, each merged candidate once
+        std::map<uint64_t, uint32_t> row_of;
+        std::vector<uint64_t> gid_of;
+        std::vector<uint32_t> lid(nq * ms, gb::kUnusedId);
+        for (size_t q = 0; q < nq; ++q) {
+            uint32_t r = 0;
+            for (uint32_t j = 0; j < cc[q]; ++j) {
+                const uint64_t g = cand[q * ms + j];
+                if (fmt == GRANNE_B200_QUERY_ID_EXCLUDING && g == gids[q]) continue;
+                const auto it = row_of.emplace(g, (uint32_t)gid_of.size()).first;
+                if (it->second == gid_of.size()) gid_of.push_back(g);
+                lid[q * ms + r] = it->second;
+                cd[q * ms + r] = cd[q * ms + j];
+                ++r;
+            }
+            cc[q] = r;
+        }
+        const uint64_t n = gid_of.size();
+        const int kind = m->kind == GRANNE_B200_ANGULAR_INT ? GRANNE_B200_ANGULAR_INT : GRANNE_B200_ANGULAR;
+        const size_t row = query_row_bytes(m->kind, m->dim, GRANNE_B200_QUERY_ELEMENT);
+        std::vector<uint8_t> host_rows(std::max<uint64_t>(n, 1) * row);
+        std::vector<uint32_t> local;
+        std::vector<uint64_t> at;
+        std::vector<uint8_t> part_rows;
+        for (size_t s = 0; s < m->parts.size(); ++s) {
+            local.clear();
+            at.clear();
+            for (uint64_t r = 0; r < n; ++r)
+                if (gid_of[r] >= m->base[s] && gid_of[r] - m->base[s] < m->parts[s]->index_len &&
+                    (s + 1 == m->parts.size() || gid_of[r] < m->base[s + 1])) {
+                    local.push_back((uint32_t)(gid_of[r] - m->base[s]));
+                    at.push_back(r);
+                }
+            if (local.empty()) continue;
+            part_rows.resize(local.size() * row);
+            if ((rc = granne_b200_get_elements(m->parts[s], local.data(), local.size(), part_rows.data()))) return rc;
+            for (size_t j = 0; j < at.size(); ++j)
+                std::memcpy(host_rows.data() + at[j] * row, part_rows.data() + j * row, row);
+        }
+        std::vector<uint32_t> sel(nq * k);
+        std::vector<uint32_t> sc(nq, 0);
+        if (n > 0) {
+            DeviceGuard on(m->parts[0]->device);
+            GB_CUDA(on.err);
+            Buffer<uint8_t> d_rows;
+            if ((rc = d_rows.grow(n * row, nullptr))) return rc;
+            GB_CUDA(cudaMemcpy(d_rows.get(), host_rows.data(), n * row, cudaMemcpyHostToDevice));
+            DeviceGuard guard;
+            std::unique_ptr<Handle> t;
+            if ((rc = new_handle(&guard, m->parts[0]->device, kind, nullptr, 0, nullptr, 0, d_rows.get(), n, m->dim,
+                                 &t)))
+                return rc;
+            t->index_len = n;
+            rc = granne_b200_select_neighbors_batch(t.get(), lid.data(), cd.data(), cc.data(), nq, ms, k, sel.data(),
+                                                    out_dists, sc.data());
+            GB_CUDA(cudaDeviceSynchronize());  // the temporary handle's work is done before it is freed
+            if (rc) return rc;
+        } else {
+            std::fill(out_dists, out_dists + nq * k, std::numeric_limits<float>::infinity());
+        }
+        for (size_t q = 0; q < nq; ++q)
+            for (uint32_t j = 0; j < k; ++j)
+                out_ids[q * k + j] = j < sc[q] ? gid_of[sel[q * k + j]] : ~0ull;
+        if (out_counts) std::memcpy(out_counts, sc.data(), nq * 4);
+        return (int)GRANNE_B200_OK;
+    });
+}
+
+}  // namespace
+
+extern "C" {
+
+// REPLICATED: each device runs granne_b200_search_diverse_batch on its slice of the queries (by id: the global ids are
+// its local ids, so QUERY_ID_EXCLUDING drops the element itself on the device).  RANGE_PARTITIONED:
+// multi_diverse_partitioned.
+int granne_b200_multi_search_diverse_batch(granne_b200_multi* m, const void* queries, size_t nq, int query_format,
+                                           uint32_t max_search, uint32_t num_neighbors, uint64_t* out_ids,
+                                           float* out_dists, uint32_t* out_counts) {
+    if (!m) return fail(GRANNE_B200_ERR_INVALID_ARGUMENT, "multi handle is null");
+    int rc = validate_diverse(m->parts[0], queries, nq, query_format, max_search, num_neighbors, out_ids, out_dists);
+    if (rc || nq == 0) return rc;
+    if (m->mode == GRANNE_B200_MODE_RANGE_PARTITIONED)
+        return multi_diverse_partitioned(m, queries, nq, query_format, max_search, num_neighbors, out_ids, out_dists,
+                                         out_counts);
+    return guarded([&] {
+        std::vector<uint32_t> local;
+        const void* rows = queries;
+        if (by_id(query_format)) {
+            const uint64_t* gids = static_cast<const uint64_t*>(queries);
+            MultiIds mi;
+            const int e = multi_ids(m, gids, nq, &mi);
+            if (e) return e;
+            local.assign(gids, gids + nq);  // every id is < Index::len here
+            rows = local.data();
+        }
+        return multi_batch(m, rows, nq, query_format, num_neighbors, out_ids, out_dists, out_counts,
+                           [&](size_t i, size_t, const void* q, size_t cnt, uint32_t* ids, float* ds, uint32_t* c) {
+                               return granne_b200_search_diverse_batch(m->parts[i], q, cnt, query_format, max_search,
+                                                                       num_neighbors, ids, ds, c, nullptr);
+                           });
+    });
 }
 
 }  // extern "C"

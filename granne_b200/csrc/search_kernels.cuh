@@ -1539,6 +1539,14 @@ __device__ __forceinline__ void load_element_to_qs(const DeviceIndex& ix, WarpCt
     __syncwarp();
 }
 
+// ElementContainer::get(id) -> the query slot (c.qs / q registers) of the distance engine (the builder's
+// select_neighbors and add_and_limit, and diverse_kernel).
+template <class Dist>
+__device__ __forceinline__ void set_query_from_element(const DeviceIndex& ix, WarpCtx& c, Dist& dist, uint32_t id) {
+    load_element_to_qs(ix, c, id);
+    dist.load_query(ix, c);
+}
+
 // ------------------------------------------------------------------------------------------------------------------
 // query construction (the `Elements::Element` the reference's callers build)
 // ------------------------------------------------------------------------------------------------------------------

@@ -68,7 +68,8 @@ extern "C" {
                                        reports ERR_OUT_OF_RANGE.  Accepted by search_batch, exact_search_batch,
                                        exact_search_within_batch, search_filtered_batch,
                                        exact_search_filtered_batch, exact_range_count and exact_range_search (host
-                                       and device forms, and their multi-handle forms);
+                                       and device forms, and their multi-handle forms) and search_diverse_batch (host
+                                       and device forms, and its multi-handle form);
                                        search_batch_device_gather and the two-stage calls reject it as an unknown
                                        format. */
 #define GRANNE_B200_QUERY_ID_EXCLUDING 3 /* QUERY_ID without the element itself: the call's result for the same query
@@ -427,6 +428,55 @@ int granne_b200_search_rerank_batch_device(granne_b200_index* h, const float* d_
                                            uint32_t* d_out_ids, float* d_out_dists, uint32_t* d_out_counts,
                                            uint64_t* d_out_stats, void* cuda_stream);
 
+/* ---- diverse search: the neighbours granne would link the query to -------------------------------------------------
+ * NOT a reference function: GranneBuilder::select_neighbors (src/index/mod.rs:849-883) applied to a query's search
+ * list, i.e. what index_element (:805-846) links an inserted element to.  For a query q:
+ *   1. C = granne_b200_search_batch(h, q, max_search, max_search): at most max_search (id, distance) candidates in
+ *      (distance, id) order; QUERY_ID_EXCLUDING drops the element itself (index_element's filter(id != idx), :822);
+ *   2. if |C| <= k the result is C unpruned (:856-858); otherwise the candidates are walked in order and candidate j is
+ *      kept when d(q, j) <= dist_to_element(s, get(j)) for every s kept before it, until k are kept (:864-880).
+ * The result is up to k ids with their stage-1 distance bits, in candidate order, and a count; the k nearest that are
+ * not near-duplicates of nearer ones, so on clustered data the answers differ from one another.  Output layout as
+ * granne_b200_search_batch (padded with 0xFFFFFFFF / +inf); out_stats (may be NULL) holds stage 1's counters.  The
+ * pair distances are the handle's own, bit for bit.  Costs stage 1 plus at most k x |C| pair distances per query.
+ *   queries        every format of granne_b200_search_batch (QUERY_ID / QUERY_ID_EXCLUDING included)
+ *   max_search     1..GRANNE_B200_DIVERSE_MAX_CANDIDATES
+ * ERR_INVALID_ARGUMENT, in this order, before any device call: the handle is NULL; an unknown query format;
+ * max_search == 0 or above GRANNE_B200_DIVERSE_MAX_CANDIDATES; nq above the batch limit; a NULL queries or output
+ * buffer.  Then (host call) an id >= num_elements is ERR_OUT_OF_RANGE.  A NaN distance in either stage returns
+ * ERR_NOT_FINITE (the query gets count 0). */
+#define GRANNE_B200_DIVERSE_MAX_CANDIDATES 1024
+int granne_b200_search_diverse_batch(granne_b200_index* h, const void* queries, size_t nq, int query_format,
+                                     uint32_t max_search, uint32_t num_neighbors, uint32_t* out_ids, float* out_dists,
+                                     uint32_t* out_counts, uint64_t* out_stats);
+/* Same with DEVICE pointers on cuda_stream (NULL = the default stream), asynchronous like
+ * granne_b200_search_batch_device; errors are reported by granne_b200_stream_status. */
+int granne_b200_search_diverse_batch_device(granne_b200_index* h, const void* d_queries, size_t nq, int query_format,
+                                            uint32_t max_search, uint32_t num_neighbors, uint32_t* d_out_ids,
+                                            float* d_out_dists, uint32_t* d_out_counts, uint64_t* d_out_stats,
+                                            void* cuda_stream);
+/* select_neighbors(list_q, k) over nq caller lists, the rule of granne_b200_search_diverse_batch's step 2: it composes
+ * with the output of every query call (exact_search_batch(q, C) gives the exact diverse answer, the filtered calls a
+ * diverse filtered one, exact_search_within_batch a diverse ranking of caller candidates).  List q is
+ * cand_ids / cand_dists[q * stride, q * stride + cand_counts[q]): ids < granne_b200_len(h), distances ascending (taken
+ * as given; the reference requires the order, :860-863).  Outputs as granne_b200_search_diverse_batch.
+ * ERR_INVALID_ARGUMENT, in this order, before any device call: the handle is NULL; stride above
+ * GRANNE_B200_DIVERSE_MAX_CANDIDATES; nq above the batch limit; with nq > 0, cand_counts NULL, an output NULL with
+ * k > 0, or cand_ids / cand_dists NULL with stride > 0; then (host call) a count > stride, an id >= granne_b200_len(h),
+ * or a list whose distances are not ascending (a NaN included).  nq == 0, k == 0 and empty lists are valid.  A NaN
+ * pair distance returns ERR_NOT_FINITE. */
+int granne_b200_select_neighbors_batch(granne_b200_index* h, const uint32_t* cand_ids, const float* cand_dists,
+                                       const uint32_t* cand_counts, size_t nq, uint32_t stride,
+                                       uint32_t num_neighbors, uint32_t* out_ids, float* out_dists,
+                                       uint32_t* out_counts);
+/* Same with DEVICE pointers on cuda_stream, asynchronous; it takes the (ids, dists, counts) outputs of any device query
+ * call as they are (stride = that call's k).  The kernel checks the lists: a bad list gets count 0 and padding, and
+ * granne_b200_stream_status reports ERR_INVALID_ARGUMENT. */
+int granne_b200_select_neighbors_batch_device(granne_b200_index* h, const uint32_t* d_cand_ids,
+                                              const float* d_cand_dists, const uint32_t* d_cand_counts, size_t nq,
+                                              uint32_t stride, uint32_t num_neighbors, uint32_t* d_out_ids,
+                                              float* d_out_dists, uint32_t* d_out_counts, void* cuda_stream);
+
 /* The device-pointer calls keep one workspace per distinct caller stream (status words, per-warp visited tables) until
  * granne_b200_close.  A caller that retires a stream returns its workspace with this call (it synchronises the stream;
  * an error raised by its last batches is reported by the next granne_b200_stream_status). */
@@ -434,7 +484,8 @@ int granne_b200_release_stream(granne_b200_index* h, void* cuda_stream);
 
 /* After synchronising a stream used with granne_b200_search_batch_device: GRANNE_B200_OK, or the first error
  * (ERR_NOT_FINITE / ERR_CAPACITY, or ERR_INVALID_ARGUMENT for a bad candidate list of
- * granne_b200_exact_search_within_batch_device or a range search segment whose length is not its count, or
+ * granne_b200_exact_search_within_batch_device or granne_b200_select_neighbors_batch_device, or a range search segment
+ * whose length is not its count, or
  * ERR_OUT_OF_RANGE for an element id >= num_elements of a
  * GRANNE_B200_QUERY_ID* call or of granne_b200_get_elements_device) any query of the calls issued since the previous
  * check raised. */
@@ -554,6 +605,16 @@ int granne_b200_multi_set_rerank_embeddings(granne_b200_multi* m, const void* co
 int granne_b200_multi_search_rerank_batch(granne_b200_multi* m, const float* queries, size_t nq, int query_format,
                                           uint32_t max_search, uint32_t num_candidates, uint32_t num_neighbors,
                                           uint64_t* out_ids, float* out_dists, uint32_t* out_counts);
+/* granne_b200_search_diverse_batch over a multi handle, with u64 GLOBAL ids like granne_b200_multi_search_batch (every
+ * query format; an id must lie in some part's [shard_base, shard_base + Index::len)).  REPLICATED slices the queries
+ * over the devices.  RANGE_PARTITIONED: the candidates are the shards' max_search lists merged by (distance, global id)
+ * as granne_b200_multi_search_batch merges them (without the query's own global id for QUERY_ID_EXCLUDING), and
+ * select_neighbors runs over the global container: the candidates' element rows are gathered onto part 0's device and
+ * selected there (a SumEmbeddings shard's materialised rows as angular f32 rows, whose distances are the same bits).
+ * Argument rules as granne_b200_search_diverse_batch; no stats. */
+int granne_b200_multi_search_diverse_batch(granne_b200_multi* m, const void* queries, size_t nq, int query_format,
+                                           uint32_t max_search, uint32_t num_neighbors, uint64_t* out_ids,
+                                           float* out_dists, uint32_t* out_counts);
 
 /* Host-only helpers (no device needed): the loader's view of an index image.
  * granne_b200_inspect_index replaces io::read_layer_sizes + Index::num_layers/layer_len on raw bytes
